@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- CenterTrack per-frame inference hot path on B200 (contract: see DESIGN.md section 6).
+"""bench.py -- CenterTrack per-frame inference hot path on H100 (contract: see DESIGN.md section 6).
 
   python bench.py --gpus N --steps K --warmup W [--batch B] [--config CFG] [--precision P] [--impl reference]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
@@ -51,7 +51,7 @@ def _peaks():
 
 
 class ClockSampler(threading.Thread):
-  """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+  """nvidia-smi clocks / throttle reasons during the timed region."""
   Q = ('index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,'
        'clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,'
        'clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap')
@@ -226,9 +226,7 @@ def _op_group(kind, pl, L):
   if kind != 'conv':
     return kind
   if pl.a_mode in (L.CT_A_DCN, L.CT_A_DCN_WIN):
-    # window DCN with one N tile of <= 128 channels runs the persistent kernel (conv_tc.cu conv_forward_tc, CTB_DCN_PERSIST)
-    persist = pl.a_mode == L.CT_A_DCN_WIN and pl.C_out <= 128 and os.environ.get('CTB_DCN_PERSIST', '1') != '0'
-    return 'dcn_persist' if persist else 'dcn_tc'
+    return 'dcn_tc'
   return {L.CT_ENGINE_TCGEN05: 'conv_tc', L.CT_ENGINE_TCGEN05_HALO: 'conv_halo', L.CT_ENGINE_SIMT: 'conv_simt',
           L.CT_ENGINE_TCGEN05_X3: 'conv_tc'}[pl.engine]
 
@@ -359,7 +357,7 @@ def accurate_engine_leg(model, cfg, B, H, W, opt, dev, tracking, host_img, host_
   par = parity_at_bench_shape(r, cfg, B, H, W, 'bf16x3', wt)
   return {'engine': 'bf16x3', 'value': B / (ms / 1000.0), 'unit': 'frames/s', 'ms_per_step': ms, 'steps': steps,
           'warmup': warmup, 'what': 'same step (splat + network + decode + association, one CUDA graph, inputs resident) '
-          'on the tcgen05 engine with bf16 hi/lo split operands and fp32 activations',
+          'on the wgmma engine with bf16 hi/lo split operands and fp32 activations',
           'parity_worst': par['worst'] if par else None, 'tolerance': 'north_star: fp32 heat-maps / offsets within 1e-3'}
 
 
@@ -416,6 +414,30 @@ def stock_pytorch_leg(sd, heads, B, H, W, dev, wt, steps=3, warmup=2):
   return res
 
 
+def dump_outputs(out_dir, runner, tracking, max_elems=1 << 20):
+  """What the timed step returned in its last iteration, as DIR/<name>.npy: the packed detection records and (device
+  tracking) the track tables and per-stream track counts a caller receives, plus the head maps the step decoded.  Float
+  tensors are written as float32, integer ones as float64; an array of more than `max_elems` elements is replaced by a
+  fixed seeded sample of that many (<name>_sample.npy, flat indices from np.random.RandomState(0)), which keeps the
+  whole dump under 64 MB."""
+  os.makedirs(out_dir, exist_ok=True)
+  arrays = [('records', runner.rec)]
+  if tracking:
+    arrays += [('tracks', runner.tracker.tracks), ('track_counts', runner.tracker.counts)]
+  arrays += [('head_' + k, v) for k, v in sorted(runner.eng.outputs.items())]
+  total = 0
+  for name, t in arrays:
+    a = t.detach().cpu().numpy()                          # the copy waits for the step that wrote `t`
+    a = a.astype(np.float32) if t.dtype.is_floating_point else a.astype(np.float64)
+    if a.size > max_elems:
+      idx = np.sort(np.random.RandomState(0).randint(0, a.size, max_elems))
+      a, name = a.reshape(-1)[idx], name + '_sample'
+    total += a.nbytes
+    if total > 64 << 20:
+      raise RuntimeError('--dump-outputs: more than 64 MB of outputs (%d arrays)' % len(arrays))
+    np.save(os.path.join(out_dir, name + '.npy'), a)
+
+
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--gpus', type=int, default=1)
@@ -430,6 +452,8 @@ def main():
   ap.add_argument('--no-latency', action='store_true')
   ap.add_argument('--no-gpu-baseline', action='store_true', help='skip the stock-PyTorch-on-the-same-GPU context leg')
   ap.add_argument('--no-accurate', action='store_true', help='skip the bf16x3 (<= 1e-3) engine leg of the default run')
+  ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                  help='after the timed steps, write what the last timed step computed as DIR/<name>.npy')
   ap.add_argument('--host-tracking', action='store_true',
                   help='round-1 mode: pre_hm supplied by the host, no association on the device')
   args = ap.parse_args()
@@ -469,7 +493,7 @@ def main():
   tracking = not args.host_tracking
   runner = StreamRunner(model, B, H, W, K=K, precision=args.precision, device=dev, opt=opt, device_tracking=tracking)
   # synthetic inputs: 2 distinct frames per stream (+ pre_hm in host-tracking mode); inputs alone are 2 x B x 3-4 MB
-  # and one step streams ~0.3 GB of activations per frame, so nothing but the 40 MB of weights can live in the 126 MB L2
+  # and one step streams ~0.3 GB of activations per frame, so little but the 40 MB of weights can live in the 50 MB L2
   img, pre, hm = wt.synthetic_inputs(2, H, W, seed=317 + rank)
   g = torch.Generator().manual_seed(rank)
   host_img = [(img[s:s + 1] + 0.05 * torch.randn(B, 3, H, W, generator=g)).pin_memory() for s in range(2)]
@@ -510,6 +534,8 @@ def main():
     dist.all_reduce(t, op=dist.ReduceOp.MAX)
     ms = float(t.item())
   clocks = sampler.summary() if rank == 0 else None
+  if args.dump_outputs and rank == 0:
+    dump_outputs(args.dump_outputs, runner, tracking)
   ms_per_step = ms / args.steps
   value = world * B * args.steps / (ms / 1000.0)
 
@@ -543,8 +569,9 @@ def main():
     return
 
   # ---------------- roofline: per-kernel time inside the step, measured live ----------------
-  # `traffic`: dram__bytes_read.sum + dram__bytes_write.sum from the committed ncu --set full capture of one step at
-  # 32 frames/step (profiles/), scaled by frames per step; null for configs without a capture.
+  # `traffic`: dram__bytes_read.sum + dram__bytes_write.sum per frame from profiles/traffic.json (written by
+  # tools/ncu_summary.py from an ncu capture of one step, where Nsight Compute runs), scaled by frames per step; null
+  # when that file does not exist.
   eng = runner.eng
   method, op_ms, decode_ms, tracker_ms = per_op_times(runner, L)
   raw_sum = sum(op_ms) + decode_ms + (tracker_ms or 0.0)
@@ -581,10 +608,10 @@ def main():
             'share_of_step': ms / sum_ms, 'gflop_per_step': fl / 1e9, 'launches': n}
 
   # one entry per kernel FUNCTION; the headline is the function with the largest share of the step
-  fn = {'conv_halo_kernel': merged(['conv_halo']), 'dcn_persist_kernel': merged(['dcn_persist']),
+  fn = {'conv_halo_kernel': merged(['conv_halo']),
         'conv_tc_kernel': merged(['dcn_tc', 'conv_tc']), 'conv_simt_kernel': merged(['conv_simt'])}
   fn = {k: v for k, v in fn.items() if v}
-  dcn = merged(['dcn_persist', 'dcn_tc'])                   # all 16 DCNv2 main launches, whichever kernel ran them
+  dcn = merged(['dcn_tc'])                                  # all 16 DCNv2 main launches
   tc = merged(['conv_tc'])                                  # plain gather launches of conv_tc_kernel
   halo = fn.get('conv_halo_kernel')
   simt = fn.get('conv_simt_kernel')
@@ -674,7 +701,7 @@ def main():
                      'step': ('prior heat-map splat from device-resident tracks + network + decode + greedy association '
                               '(one CUDA graph)') if tracking else 'network + decode, pre_hm given (one CUDA graph)',
                      'l2': 'no flush: per-step inputs %.0f MB in 3 rotating slots + ~%.1f GB of activations per '
-                           'step exceed the 126 MB L2' % (2 * B * 3 * H * W * 4 / 1e6, 0.29 * B * H * W / 262144.),
+                           'step exceed the 50 MB L2' % (2 * B * 3 * H * W * 4 / 1e6, 0.29 * B * H * W / 262144.),
                      'cuda_graph': True},
           'e2e': {'value': e2e, 'unit': 'frames/s', 'h2d_bytes_per_step': runner.h2d_bytes_per_step,
                   'd2h_bytes_per_step': runner.d2h_bytes_per_step,

@@ -17,7 +17,7 @@ CT_F32, CT_BF16 = 0, 1
 CT_A_CONV, CT_A_DCN, CT_A_DCN_WIN = 0, 1, 2
 CT_OUT_NHWC, CT_OUT_NHWC_F32, CT_OUT_NCHW_F32, CT_OUT_NHWC_S2D = 0, 1, 2, 3
 CT_HEAD_NONE, CT_HEAD_SIGMOID, CT_HEAD_DEPTH = 0, 1, 2
-CT_ENGINE_SIMT, CT_ENGINE_TCGEN05, CT_ENGINE_TCGEN05_HALO, CT_ENGINE_TCGEN05_X3 = 0, 1, 2, 3
+CT_ENGINE_SIMT, CT_ENGINE_TCGEN05, CT_ENGINE_TCGEN05_HALO, CT_ENGINE_TCGEN05_X3 = 0, 1, 2, 3   # names kept for ABI stability: wgmma engines on sm_90a
 CT_ROLE_RAW, CT_ROLE_REG, CT_ROLE_WH, CT_ROLE_LTRB, CT_ROLE_LTRB_AMODAL, CT_ROLE_HPS = range(6)
 CT_DECODE_MAX_HEADS = 12
 CT_REC_SCORE, CT_REC_CLS, CT_REC_XS, CT_REC_YS, CT_REC_BBOX, CT_REC_IND, CT_REC_HEADS = 0, 1, 2, 3, 4, 8, 9
@@ -75,24 +75,37 @@ EXPORTS = ['ct_packed_weight_bytes', 'ct_pack_weights', 'ct_conv_forward', 'ct_s
            'ct_warp_affine_normalize', 'ct_last_error', 'ct_abi_version', 'ct_launch_count',
            'ct_reset_launch_count', 'ct_debug_trace', 'ct_debug_watch']
 
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
-              '-shared', '-Xcompiler', '-fPIC']
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17', '-Xcompiler', '-fPIC']
 
 
 def build(force=False, verbose=False):
-  """Compile libctb200.so in-tree for sm_100a (nvcc cross-compiles without a GPU)."""
+  """Compile libctb200.so in-tree for sm_90a (nvcc cross-compiles without a GPU).  The translation units are
+  compiled in parallel into a temporary directory, then linked."""
   srcs = [os.path.join(CSRC, s) for s in SOURCES]
-  deps = srcs + [os.path.join(CSRC, h) for h in ('common.cuh', 'conv_common.cuh')] + \
+  deps = srcs + [os.path.join(CSRC, h) for h in ('common.cuh', 'conv_common.cuh', 'wgmma.cuh')] + \
       [os.path.join(_HERE, '..', 'include', 'ctb200.h')]
   if not force and os.path.exists(LIB_PATH) and \
       all(os.path.getmtime(LIB_PATH) >= os.path.getmtime(d) for d in deps):
     return LIB_PATH
-  cmd = ['nvcc'] + NVCC_FLAGS + (['-Xptxas', '-v'] if verbose else []) + ['-o', LIB_PATH] + srcs
-  r = subprocess.run(cmd, capture_output=True, text=True)
-  if r.returncode != 0:
-    raise RuntimeError('nvcc failed:\n' + r.stdout + r.stderr)
-  if verbose:
-    print(r.stderr)
+  import shutil
+  import tempfile
+  with tempfile.TemporaryDirectory(prefix='ctb_build_') as tmp:
+    objs = [os.path.join(tmp, os.path.basename(s) + '.o') for s in srcs]
+    procs = [subprocess.Popen(['nvcc'] + NVCC_FLAGS + (['-Xptxas', '-v'] if verbose else []) + ['-c', s, '-o', o],
+                              stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+             for s, o in zip(srcs, objs)]
+    logs = [p.communicate()[0] for p in procs]
+    for s, p, log in zip(srcs, procs, logs):
+      if p.returncode != 0:
+        raise RuntimeError('nvcc failed on %s:\n%s' % (os.path.basename(s), log))
+    if verbose:
+      print(''.join(logs))
+    tmp_lib = os.path.join(tmp, 'libctb200.so')
+    r = subprocess.run(['nvcc', '-gencode', 'arch=compute_90a,code=sm_90a', '-shared', '-o', tmp_lib] + objs,
+                       capture_output=True, text=True)
+    if r.returncode != 0:
+      raise RuntimeError('nvcc link failed:\n' + r.stdout + r.stderr)
+    shutil.move(tmp_lib, LIB_PATH)
   return LIB_PATH
 
 
@@ -107,7 +120,7 @@ def lib():
   if not os.path.exists(LIB_PATH):
     raise RuntimeError(
         'centertrack_b200: %s not found. Build it with `python -c "import __graft_entry__ as g; '
-        'g.build()"` (nvcc, sm_100a). There is no CPU fallback.' % LIB_PATH)
+        'g.build()"` (nvcc, sm_90a). There is no CPU fallback.' % LIB_PATH)
   L = C.CDLL(LIB_PATH)
   L.ct_last_error.restype = C.c_char_p
   L.ct_packed_weight_bytes.restype = C.c_int64

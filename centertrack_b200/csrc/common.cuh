@@ -1,4 +1,4 @@
-// Shared helpers for libctb200 (sm_100a only).
+// Shared helpers for libctb200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -32,6 +32,18 @@ inline int fail(int code, const char* fmt, const char* a = "", long b = 0, long 
                        (long)_e, (long)__LINE__);                                  \
   } while (0)
 
+// SM count of the current device (grid caps of the grid-stride kernels), cached per device
+inline int device_sm_count() {
+  static thread_local int sms_of[64] = {0};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 64 && sms_of[dev]) return sms_of[dev];
+  int sms = 0;
+  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
+  if (dev < 64) sms_of[dev] = sms;
+  return sms;
+}
+
 inline int after_launch() {
   ++g_launches;
   cudaError_t e = cudaPeekAtLastError();
@@ -45,7 +57,7 @@ inline int after_launch() {
 // ---- programmatic dependent launch (PDL): a kernel launched with the attribute may start while its predecessor in
 // the stream is still running; it must execute pdl_wait() before touching anything the predecessor produces (or
 // writing anything the predecessor may still read).  What runs before the wait -- shared-memory carve-up, mbarrier
-// init, TMEM allocation, the halo engine's weight load -- overlaps the predecessor's tail.  pdl_trigger() lets the
+// init, the halo engine's weight load -- overlaps the predecessor's tail.  pdl_trigger() lets the
 // NEXT kernel of the stream do the same with us.  CTB_PDL=0 launches everything stream-serialised (no overlap).
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }

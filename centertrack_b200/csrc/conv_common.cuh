@@ -1,4 +1,4 @@
-// Device-side pieces shared by the SIMT (fp32-exact) and tcgen05 (bf16) implicit-GEMM engines:
+// Device-side pieces shared by the SIMT (fp32-exact) and wgmma (bf16) implicit-GEMM engines:
 // output-pixel decomposition, conv window addressing and DCNv2 bilinear sampling.
 #pragma once
 #include "common.cuh"

@@ -1,7 +1,7 @@
 // fp32-accumulate SIMT implicit-GEMM convolution / DCNv2 ("precise" engine).
 // One kernel covers every conv-like layer of the path (see ctb200.h: ct_conv_forward).  It is the
 // reference-accuracy CUDA path (fp32 activations -> matches the reference within 1e-3 end to end)
-// and the on-device cross-check for the tcgen05 engine (same packing order k = tap*C_in + c).
+// and the on-device cross-check for the wgmma engine (same packing order k = tap*C_in + c).
 //
 // Tile: 64 output pixels x 64 output channels per CTA, K step 16, 256 threads, 4x4 outputs/thread.
 #include "conv_common.cuh"

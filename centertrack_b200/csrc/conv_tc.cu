@@ -1,35 +1,33 @@
-// tcgen05 implicit-GEMM convolution / DCNv2 for sm_100a (bf16 operands, fp32 accumulate in TMEM).
+// wgmma implicit-GEMM convolution / DCNv2 for sm_90a (bf16 operands, fp32 accumulate in registers).
 //
-//   D[128 pixels x n_tile channels] (TMEM)  +=  A[128 x 64] (smem, gathered)  x  B[n_tile x 64]^T (smem)
+//   D[128 pixels x n_tile channels]  +=  A[128 x 64] (smem, gathered)  x  B[n_tile x 64]^T (smem)
 //
-// * No im2row buffer in HBM: producer warps gather each 64-wide K slice (tap-major, k = tap*C_in + c)
-//   of the A operand straight into the 128B-swizzled K-major shared-memory layout the UMMA smem
-//   descriptor expects.  For CT_A_DCN the gather is the DCNv2 bilinear sample x mask (the reference's
+// * No im2row buffer in HBM: each warpgroup gathers its 64 rows of every 64-wide K slice (tap-major,
+//   k = tap*C_in + c) of the A operand straight into the 128B-swizzled K-major shared-memory layout the
+//   wgmma descriptor expects.  For CT_A_DCN the gather is the DCNv2 bilinear sample x mask (the reference's
 //   `columns` tensor never exists).
 // * Weights are pre-packed on the host as ready-made swizzled tile images, so one TMA bulk copy
 //   (cp.async.bulk, mbarrier complete_tx) per K slice brings the B tile.
-// * One elected thread issues tcgen05.mma (M=128, N=n_tile, K=16) x4 per slice; tcgen05.commit
-//   releases the smem stage back to the producers and finally signals the epilogue.
-// * Epilogue: tcgen05.ld (32 lanes x 16 columns per warp), + folded-BN shift, + residual, ReLU,
-//   then bf16 NHWC / fp32 NHWC (DCN offsets, sigmoid on the mask channels) / fp32 NCHW (heads,
-//   sigmoid / depth transform) stores.
-//
-// CTA = 288 threads: warps 0-7 producers then epilogue (warp w reads TMEM lanes 32(w%4).., warps 0-3 the even
-// 16-column chunks, warps 4-7 the odd ones), warp 8 = TMEM allocator + MMA issuer.  Eight producer warps
-// (two per SM sub-partition) because the gather is latency-bound: more warps = more loads in flight.
-// Two CTAs are co-resident per SM so one CTA's epilogue overlaps another's main loop.
+// * CTA = 256 threads = two warpgroups.  Warpgroup w gathers rows 64w..64w+63 and issues wgmma
+//   (M=64, N=n_tile, K=16) x4 per slice on them; the MMAs of slice s run while the warpgroup gathers slice s+1
+//   (wgmma.wait_group 1), and one arrival per warp on the stage's empty barrier releases the weight tile.
+// * Epilogue: the register accumulator goes through shared memory 32 columns at a time (row per thread), then
+//   + folded-BN shift, + residual, ReLU, bf16 NHWC / fp32 NHWC (DCN offsets, sigmoid on the mask channels) /
+//   fp32 NCHW (heads, sigmoid / depth transform) stores.
 #include "conv_common.cuh"
+#include "wgmma.cuh"
 #include <cuda.h>
 #include <stdlib.h>
 
 namespace ctb {
 
-constexpr int TC_BM = 128;           // output pixels per CTA (UMMA M)
+constexpr int TC_BM = 128;           // output pixels per CTA
 constexpr int TC_BK = 64;            // K elements per pipeline stage (one 128B swizzle atom of bf16)
-constexpr int TC_THREADS = 288;        // 8 producer/epilogue warps + 1 MMA warp
+constexpr int TC_THREADS = 256;      // two warpgroups: gather + MMA + epilogue
 constexpr int TC_PRODUCERS = 256;
-constexpr int TC_NROW = TC_BM * 8 / TC_PRODUCERS;   // A-tile rows per producer thread per K slice (4)
+constexpr int TC_NROW = TC_BM * 8 / TC_PRODUCERS;   // A-tile rows per thread per K slice (4, 16 rows apart)
 constexpr int A_STAGE_BYTES = TC_BM * 128;
+constexpr int TC_EPI_PITCH = 36;     // floats per row of the 32-column epilogue staging tile (16-byte reads conflict-free)
 
 struct TcArgs {
   ConvGeom g;
@@ -39,14 +37,12 @@ struct TcArgs {
   const __nv_bfloat16* residual;
   const float* om;
   void* out;
-  int n_tile, k_slices, stages, tmem_cols, a_mode;
+  int n_tile, k_slices, stages, a_mode;
   int tiles_x, tiles_y;         // > 0: an M tile is an 8 (y) x 16 (x) pixel patch of one image (L1 reuse of the
                                 // 3x3 / bilinear footprints); 0: 128 consecutive pixels in b,y,x order
   int win_m, win_pw, win_ph;    // CT_A_DCN_WIN: offset margin (px) and the staged window (pixels) of one 8x16 patch
   uint32_t win_bytes;           // bytes of one 64-channel window (= TMA box)
-  int fence_mma;                // 1: the generic->async proxy fence is executed by the MMA thread after the full-barrier
-                                // wait instead of by every producer (fence.proxy.async compiles to MEMBAR.ALL.CTA +
-                                // FENCE.VIEW.ASYNC, and the MEMBAR drains the producer's prefetched global loads)
+  uint32_t region0;             // bytes of the stage area (also holds the epilogue staging tile)
 };
 
 // CT_A_DCN_WIN sampling record (16 bytes): global fall-back offset of the clamped top-left corner (channel 0 of the
@@ -80,7 +76,7 @@ __device__ __forceinline__ int tc_pixel(const TcArgs& a, int mt, int r) {
 }
 
 // Optional timeline of the middle CTA (ct_debug_trace): clock64() stamps -- 0 start, 1 rows set up, 2 DCN table built,
-// 8+s producer warp 0 finished slice s, 4 MMA warp committed, 5 epilogue saw the accumulator, 6 epilogue done.
+// 8+s thread 0 finished gathering slice s, 5 accumulator complete, 6 epilogue done.
 __device__ unsigned long long* g_tc_trace = nullptr;
 // The pointer is read ONCE per thread at kernel entry (tc_trace_ptr): a stamp that re-read the global cost the stamping
 // thread a dependent load per slice even with tracing off.
@@ -103,9 +99,6 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 }
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
@@ -134,27 +127,8 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
       "l"(src), "r"(bytes), "r"(bar)
       : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_mma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                       uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void named_sync(int id, int n) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
 }
 __device__ __forceinline__ uint4 ldg_nc16(const void* p) {
   uint4 r;
@@ -164,16 +138,35 @@ __device__ __forceinline__ uint4 ldg_nc16(const void* p) {
 __device__ __forceinline__ void sts16(uint32_t addr, uint4 v) {
   asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
-
-// K-major, 128B-swizzled smem operand descriptor (cute::UMMA::SmemDescriptor):
-//   [0,14) start>>4 | [16,30) LBO>>4 (=1, unused for swizzled K-major) | [32,46) SBO>>4 (=64: 8 rows x 128B)
-//   [46,48) version=1 | [61,64) layout = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t make_sdesc(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+__device__ __forceinline__ void sts_f2(uint32_t addr, float x, float y) {
+  asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
 }
-// kind::f16 instruction descriptor (cute::UMMA::InstrDescriptor): D=f32, A=B=bf16, K-major both.
-__device__ __forceinline__ uint32_t make_idesc(int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
+__device__ __forceinline__ void lds_f16(uint32_t addr, float (&v)[16]) {
+#pragma unroll
+  for (int j4 = 0; j4 < 4; ++j4)
+    asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];"
+                 : "=f"(v[4 * j4]), "=f"(v[4 * j4 + 1]), "=f"(v[4 * j4 + 2]), "=f"(v[4 * j4 + 3])
+                 : "r"(addr + 16u * j4));
+}
+
+// Columns [c0, c0 + 32) of a warpgroup's m64 accumulator -> rows `row0 + 0..63` of the fp32 staging tile
+// [rows][TC_EPI_PITCH] at `stg` (see wgmma.cuh for the fragment layout).
+template <int M>
+__device__ __forceinline__ void stage_acc_chunk(const float (&d)[M], int c0, uint32_t stg, int row0) {
+  const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
+  const uint32_t r = (uint32_t)(row0 + 16 * w + (l >> 2));
+#pragma unroll
+  for (int i = 0; i < M / 4; ++i) {
+    if (i * 8 < c0 || i * 8 >= c0 + 32) continue;      // resolved at compile time once c0 is
+    const uint32_t col = (uint32_t)(i * 8 - c0 + 2 * (l & 3));
+    sts_f2(stg + (r * TC_EPI_PITCH + col) * 4u, d[4 * i], d[4 * i + 1]);
+    sts_f2(stg + ((r + 8u) * TC_EPI_PITCH + col) * 4u, d[4 * i + 2], d[4 * i + 3]);
+  }
+}
+
+// K-major, 128B-swizzled smem operand descriptor: SBO = 1024 (8 rows x 128 B), LBO unused (1).
+__device__ __forceinline__ uint64_t make_sdesc(uint32_t smem_addr) {
+  return wg_desc(smem_addr, 16u, 1024u, 1u);
 }
 
 // Per (tap, output pixel) DCNv2 sampling record, built once per CTA: clamped top-left corner as a 32-bit element
@@ -182,30 +175,6 @@ __device__ __forceinline__ uint32_t make_idesc(int n) {
 // weights already multiplied by the modulation mask and zeroed for corners / samples outside the image.
 struct __align__(16) DcnEntry { int off, dxo, dyo, pad; float w00, w01, w10, w11; };   // 32 bytes
 
-// bf16x2 word -> two fp32 lanes of one 64-bit register (lo = x << 16, hi = x & 0xffff0000: one ALU op each), then
-// packed fp32 math (FMUL2 / FFMA2): 8 channels x 1 corner = 8 unpack + 4 packed FMAs.
-__device__ __forceinline__ unsigned long long bf2_to_f2(uint32_t x) {
-  unsigned long long r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "r"(x << 16), "r"(x & 0xffff0000u));
-  return r;
-}
-__device__ __forceinline__ unsigned long long dup_f2(float w) {
-  unsigned long long r;
-  asm("mov.b64 %0, {%1, %1};" : "=l"(r) : "r"(__float_as_uint(w)));
-  return r;
-}
-__device__ __forceinline__ void scale8(unsigned long long (&acc)[4], uint4 v, float w) {
-  const unsigned long long ww = dup_f2(w);
-  const uint32_t x[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-  for (int q = 0; q < 4; ++q) asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(acc[q]) : "l"(bf2_to_f2(x[q])), "l"(ww));
-}
-__device__ __forceinline__ void blend8(unsigned long long (&acc)[4], uint4 v, float w) {
-  const unsigned long long ww = dup_f2(w);
-  const uint32_t x[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-  for (int q = 0; q < 4; ++q) asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc[q]) : "l"(bf2_to_f2(x[q])), "l"(ww));
-}
 __device__ __forceinline__ uint32_t bmul2(uint32_t a, uint32_t b) {
   uint32_t d;
   asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
@@ -220,17 +189,6 @@ __device__ __forceinline__ uint32_t dup_bf2(float w) {      // {bf16(w), bf16(w)
   uint32_t d;
   asm("cvt.rn.bf16x2.f32 %0, %1, %1;" : "=r"(d) : "f"(w));
   return d;
-}
-__device__ __forceinline__ uint4 pack8(const unsigned long long (&acc)[4]) {
-  uint32_t o[4];
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    uint32_t lo, hi;
-    asm("mov.b64 {%0, %1}, %2;" : "=r"(lo), "=r"(hi) : "l"(acc[q]));
-    const __nv_bfloat162 h = __floats2bfloat162_rn(__uint_as_float(lo), __uint_as_float(hi));
-    o[q] = *reinterpret_cast<const uint32_t*>(&h);
-  }
-  return make_uint4(o[0], o[1], o[2], o[3]);
 }
 
 // ---- bf16x3 ("X3") engine: fp32 activations, every operand split into bf16 hi + bf16 lo = x - hi (both exact in
@@ -256,33 +214,32 @@ __device__ __forceinline__ float4 ldg_nc_f4(const float* p) {
   return r;
 }
 
-template <bool X3>
-__global__ void __launch_bounds__(TC_THREADS, X3 ? 1 : 2)
+template <bool X3, int N>
+__global__ void __launch_bounds__(TC_THREADS, (!X3 && N <= 64) ? 2 : 1)
 conv_tc_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
   // SWIZZLE_128B operands need 1024B-aligned stage bases: align by hand (launch adds 1 KB of slack)
   unsigned char* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
   const ConvGeom& g = a.g;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = tid >> 7;                 // warpgroup: GEMM rows 64 wg .. 64 wg + 63
   unsigned long long* const trace = tc_trace_ptr();
   const int S = a.stages;
-  const uint32_t b_tile_bytes = (uint32_t)a.n_tile * 128u;                    // one bf16 weight tile of a K slice
-  const uint32_t b_stage_bytes = X3 ? 2u * b_tile_bytes : b_tile_bytes;       // X3: [hi][lo]
+  constexpr uint32_t b_tile_bytes = (uint32_t)N * 128u;                       // one bf16 weight tile of a K slice
+  constexpr uint32_t b_stage_bytes = X3 ? 2u * b_tile_bytes : b_tile_bytes;   // X3: [hi][lo]
   constexpr uint32_t a_stage_bytes = X3 ? 2u * A_STAGE_BYTES : A_STAGE_BYTES; // X3: [hi 16 KB][lo 16 KB]
   const float* xf = reinterpret_cast<const float*>(a.x);
 
-  // carve shared memory
+  // carve shared memory: [stages | epilogue staging][barriers][DCN table / window]
   const uint32_t smem_base = smem_u32(smem);
   const uint32_t sA = smem_base;
   const uint32_t sB = sA + S * a_stage_bytes;
-  const uint32_t off_bar = S * a_stage_bytes + S * b_stage_bytes;
-  const uint32_t bars = smem_base + off_bar;           // full[S], empty[S], tmem_full, win_full
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + off_bar + (2 * S + 2) * 8);
-  DcnEntry* dcn_tab = reinterpret_cast<DcnEntry*>(smem + off_bar + (2 * S + 2) * 8 + 16);  // 16B aligned
+  const uint32_t off_bar = a.region0;
+  const uint32_t bars = smem_base + off_bar;           // full[S], empty[S], win_full
+  DcnEntry* dcn_tab = reinterpret_cast<DcnEntry*>(smem + off_bar + (2 * S + 1) * 8 + 24);  // 16B aligned
   auto full_bar = [&](int s) { return bars + 8u * s; };
   auto empty_bar = [&](int s) { return bars + 8u * (S + s); };
-  const uint32_t tmem_full_bar = bars + 8u * (2 * S);
-  const uint32_t win_bar = bars + 8u * (2 * S + 1);
+  const uint32_t win_bar = bars + 8u * (2 * S);
   const bool win = !X3 && a.a_mode == CT_A_DCN_WIN;
   // CT_A_DCN_WIN: [table 9 x 128 x 16 B][window, 128B aligned]
   DcnWinEntry* win_tab = reinterpret_cast<DcnWinEntry*>(dcn_tab);
@@ -290,491 +247,481 @@ conv_tc_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
 
   const int mt = blockIdx.x;
   const int nt = blockIdx.y;
-  const int n0 = nt * a.n_tile;
+  const int n0 = nt * N;
   if (tid == 0) tc_stamp(trace, 0);
   pdl_trigger();                       // the next kernel of the stream may start its own prologue now
 
   if (tid == 0) {
-    for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), TC_PRODUCERS / 32); mbar_init(empty_bar(s), 1); }
-    mbar_init(tmem_full_bar, 1);
+    for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), TC_THREADS / 32); }
     mbar_init(win_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 8) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32((const void*)tmem_slot)),
-                 "r"((uint32_t)a.tmem_cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  if (tid == 0) tc_stamp(trace, 7);
   pdl_wait();                          // everything below reads what the previous kernel wrote
 
-  if (warp < 8) {
-    // =========================== A producers ===========================
-    const int q = tid & 7;                 // 16-byte chunk (8 channels) inside the 64-wide K slice
-    const int r0 = tid >> 3;               // rows r0 + 32*i, i < TC_NROW
-    const uint32_t swz = (uint32_t)((q ^ (r0 & 7)) << 4);
-    const int HWo = g.OH * g.OW;
-    int row_off[TC_NROW], row_iy[TC_NROW], row_ix[TC_NROW];   // element offset / coords of the window's top-left input pixel
-    if (a.a_mode != CT_A_CONV) {
-      // DCN rows come from the sampling table
+  // =========================== A gather (both warpgroups) ===========================
+  const int q = tid & 7;                   // 16-byte chunk (8 channels) inside the 64-wide K slice
+  const int rb = wg * 64 + ((tid & 127) >> 3);   // rows rb + 16*i, i < TC_NROW
+  const uint32_t swz = (uint32_t)((q ^ (rb & 7)) << 4);
+  const int HWo = g.OH * g.OW;
+  int row_off[TC_NROW], row_iy[TC_NROW], row_ix[TC_NROW];   // element offset / coords of the window's top-left input pixel
+  if (a.a_mode != CT_A_CONV) {
+    // DCN rows come from the sampling table
 #pragma unroll
-      for (int i = 0; i < TC_NROW; ++i) { row_off[i] = 0; row_iy[i] = -100000; row_ix[i] = -100000; }
-    } else if (a.tiles_x != 0) {
+    for (int i = 0; i < TC_NROW; ++i) { row_off[i] = 0; row_iy[i] = -100000; row_ix[i] = -100000; }
+  } else if (a.tiles_x != 0) {
 #pragma unroll
-      for (int i = 0; i < TC_NROW; ++i) {
-        const int p = tc_pixel(a, mt, r0 + 32 * i);   // DCN rows come from its table
-        if (p < g.P_out) {
-          const int b = p / HWo, r = p - b * HWo;
-          const int oy = r / g.OW, ox = r - oy * g.OW;
-          row_iy[i] = oy * g.stride - g.pad;
-          row_ix[i] = ox * g.stride - g.pad_w;
-          row_off[i] = (b * g.H * g.W + row_iy[i] * g.W + row_ix[i]) * g.ld_in;
-        } else {
-          row_off[i] = 0; row_iy[i] = -100000; row_ix[i] = -100000;
+    for (int i = 0; i < TC_NROW; ++i) {
+      const int p = tc_pixel(a, mt, rb + 16 * i);
+      if (p < g.P_out) {
+        const int b = p / HWo, r = p - b * HWo;
+        const int oy = r / g.OW, ox = r - oy * g.OW;
+        row_iy[i] = oy * g.stride - g.pad;
+        row_ix[i] = ox * g.stride - g.pad_w;
+        row_off[i] = (b * g.H * g.W + row_iy[i] * g.W + row_ix[i]) * g.ld_in;
+      } else {
+        row_off[i] = 0; row_iy[i] = -100000; row_ix[i] = -100000;
+      }
+    }
+  } else {
+    // linear tiles: one division pair for the first row, the other rows (+16 pixels each) by carry propagation
+    int p = mt * TC_BM + rb;
+    int b = p / HWo, r = p - b * HWo;
+    int oy = r / g.OW, ox = r - oy * g.OW;
+#pragma unroll
+    for (int i = 0; i < TC_NROW; ++i) {
+      if (p < g.P_out) {
+        row_iy[i] = oy * g.stride - g.pad;
+        row_ix[i] = ox * g.stride - g.pad_w;
+        row_off[i] = (b * g.H * g.W + row_iy[i] * g.W + row_ix[i]) * g.ld_in;
+      } else {
+        row_off[i] = 0; row_iy[i] = -100000; row_ix[i] = -100000;
+      }
+      p += 16; ox += 16;
+      while (ox >= g.OW) { ox -= g.OW; ++oy; }
+      while (oy >= g.OH) { oy -= g.OH; ++b; }
+    }
+  }
+  if (tid == 0) tc_stamp(trace, 1);
+  int win_x0 = 0, win_y0 = 0, win_b = 0;
+  if (win) {
+    // window origin of this 8x16 patch: one kernel-halo pixel + the offset margin to the top/left
+    const int tpi = a.tiles_x * a.tiles_y;
+    win_b = mt / tpi;
+    const int t = mt - win_b * tpi;
+    const int ty = t / a.tiles_x, tx = t - ty * a.tiles_x;
+    win_y0 = ty * 8 - 1 - a.win_m;
+    win_x0 = tx * 16 - 1 - a.win_m;
+    if (tid == 0) {                                   // first 64-channel chunk of the window: TMA, zero fill outside
+      mbar_arrive_expect_tx(win_bar, a.win_bytes);      // count 1: this arrival + the TMA's bytes complete the phase
+      tma_4d(s_win, &tmap, 0, win_x0, win_y0, win_b, win_bar);
+    }
+    // Two threads per row (taps 0-4 and 5-8).  The 27 offset / mask floats of a row sit in one 128-byte line of `om`;
+    // each thread loads only the 16-byte chunks its taps need.
+    const int trow = tid & (TC_BM - 1), thalf = tid >> 7;            // thalf 0: taps 0..4, thalf 1: taps 5..8
+    const int tap0 = thalf ? 5 : 0, tap1 = thalf ? 9 : 5;
+    const int tp = tc_pixel(a, mt, trow);
+    const bool ok = tp < g.P_out;
+    {
+      int oy = 0, ox = 0, img = 0;
+      float om[28];
+#pragma unroll
+      for (int j = 0; j < 28; ++j) om[j] = 0.f;
+      if (ok) {
+        const int bb = tp / HWo, r = tp - bb * HWo;
+        oy = r / g.OW; ox = r - oy * g.OW; img = bb * g.H * g.W;
+        const float4* omp = reinterpret_cast<const float4*>(a.om + (size_t)tp * g.ld_om);
+        // floats [2 tap0, 2 tap1) and [18 + tap0, 18 + tap1): chunks 0-2, 4-5 (thalf 0) / 2-6 (thalf 1)
+#pragma unroll
+        for (int j = 0; j < 7; ++j) {
+          const bool need = thalf ? (j >= 2) : (j <= 2 || j == 4 || j == 5);
+          if (need) {
+            const float4 t4 = __ldg(omp + j);
+            om[4 * j] = t4.x; om[4 * j + 1] = t4.y; om[4 * j + 2] = t4.z; om[4 * j + 3] = t4.w;
+          }
         }
+      }
+#pragma unroll
+      for (int tap = 0; tap < 9; ++tap) {
+        if (tap < tap0 || tap >= tap1) continue;
+        DcnWinEntry e; e.goff = 0; e.meta = WIN_IN; e.w01 = 0u; e.w23 = 0u;
+        if (ok) {
+          const float py = (float)(oy - 1 + tap / 3) + om[2 * tap];
+          const float px = (float)(ox - 1 + tap % 3) + om[2 * tap + 1];
+          if (py > -1.f && py < (float)g.H && px > -1.f && px < (float)g.W) {
+            const float y0f = floorf(py), x0f = floorf(px);
+            const int y0 = (int)y0f, x0 = (int)x0f;
+            const float ly = py - y0f, lx = px - x0f, hy = 1.f - ly, hx = 1.f - lx, m = om[18 + tap];
+            const bool y0ok = y0 >= 0, y1ok = y0 + 1 <= g.H - 1, x0ok = x0 >= 0, x1ok = x0 + 1 <= g.W - 1;
+            const int yc = max(y0, 0), xc = max(x0, 0);
+            e.goff = (img + yc * g.W + xc) * g.ld_in;
+            const bool dx = x0ok && x1ok, dy = y0ok && y1ok;
+            const bool inside = y0 >= win_y0 && y0 + 1 <= win_y0 + a.win_ph - 1 && x0 >= win_x0 && x0 + 1 <= win_x0 + a.win_pw - 1;
+            const uint32_t woff16 = (uint32_t)((yc - win_y0) * a.win_pw + (xc - win_x0)) * 8u;   // 128 B per pixel
+            e.meta = (inside ? (woff16 | WIN_IN) : 0u) | (dx ? WIN_DX : 0u) | (dy ? WIN_DY : 0u);
+            const float w00 = (y0ok && x0ok) ? hy * hx * m : 0.f, w01 = (y0ok && x1ok) ? hy * lx * m : 0.f;
+            const float w10 = (y1ok && x0ok) ? ly * hx * m : 0.f, w11 = (y1ok && x1ok) ? ly * lx * m : 0.f;
+            const __nv_bfloat162 wa = __floats2bfloat162_rn(w00, w01), wb = __floats2bfloat162_rn(w10, w11);
+            e.w01 = *reinterpret_cast<const uint32_t*>(&wa);
+            e.w23 = *reinterpret_cast<const uint32_t*>(&wb);
+          }
+        }
+        win_tab[tap * TC_BM + trow] = e;
+      }
+    }
+    named_sync(1, TC_PRODUCERS);
+    if (tid == 0) tc_stamp(trace, 2);
+  }
+  if (a.a_mode == CT_A_DCN) {
+    // per (tap,row) sampling records, computed once per CTA (row = tid, threads 0..127)
+    const int p = tid < TC_BM ? tc_pixel(a, mt, tid) : g.P_out;
+    const bool ok = p < g.P_out;
+    if (tid < TC_BM) {
+      int oy = 0, ox = 0, img = 0;
+      float om[28];
+      if (ok) {
+        const int bb = p / HWo, r = p - bb * HWo;
+        oy = r / g.OW; ox = r - oy * g.OW; img = bb * g.H * g.W;
+        const float4* omp = reinterpret_cast<const float4*>(a.om + (size_t)p * g.ld_om);
+#pragma unroll
+        for (int j = 0; j < 7; ++j) {
+          const float4 t = __ldg(omp + j);
+          om[4 * j] = t.x; om[4 * j + 1] = t.y; om[4 * j + 2] = t.z; om[4 * j + 3] = t.w;
+        }
+      }
+#pragma unroll
+      for (int tap = 0; tap < 9; ++tap) {
+        DcnEntry e; e.off = 0; e.dxo = 0; e.dyo = 0; e.pad = 0; e.w00 = e.w01 = e.w10 = e.w11 = 0.f;
+        if (ok) {
+          const float py = (float)(oy - 1 + tap / 3) + om[2 * tap];
+          const float px = (float)(ox - 1 + tap % 3) + om[2 * tap + 1];
+          if (py > -1.f && py < (float)g.H && px > -1.f && px < (float)g.W) {
+            const float y0f = floorf(py), x0f = floorf(px);
+            const int y0 = (int)y0f, x0 = (int)x0f;
+            const float ly = py - y0f, lx = px - x0f, hy = 1.f - ly, hx = 1.f - lx, m = om[18 + tap];
+            const bool y0ok = y0 >= 0, y1ok = y0 + 1 <= g.H - 1, x0ok = x0 >= 0, x1ok = x0 + 1 <= g.W - 1;
+            e.off = (img + max(y0, 0) * g.W + max(x0, 0)) * g.ld_in;
+            e.dxo = (x0ok && x1ok) ? g.ld_in : 0;
+            e.dyo = (y0ok && y1ok) ? g.W * g.ld_in : 0;
+            e.w00 = (y0ok && x0ok) ? hy * hx * m : 0.f;
+            e.w01 = (y0ok && x1ok) ? hy * lx * m : 0.f;
+            e.w10 = (y1ok && x0ok) ? ly * hx * m : 0.f;
+            e.w11 = (y1ok && x1ok) ? ly * lx * m : 0.f;
+          }
+        }
+        dcn_tab[tap * TC_BM + tid] = e;
+      }
+    }
+    named_sync(1, TC_PRODUCERS);
+    if (tid == 0) tc_stamp(trace, 2);
+  }
+  const int cin8 = g.C_in >> 3;
+  const int ntaps = g.KH * g.KW;
+  const size_t w_slice_elems = (size_t)(X3 ? 2 : 1) * N * TC_BK;
+  const __nv_bfloat16* wt = a.w + (size_t)nt * a.k_slices * w_slice_elems;
+
+  // ---- per-slice protocol.  begin: wait until both warpgroups' MMAs of the slice that last used the stage are done
+  // (empty barrier, one arrival per warp), then thread 0 requests the weight tile.  end: the warpgroup's A rows are
+  // made visible to the async proxy, the warpgroup synchronises, waits for the weight tile and issues its MMAs; after
+  // those of the PREVIOUS slice have completed (wait_group 1) each warp releases that slice's stage.
+  float acc[N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+  auto begin_stage = [&](int s) {
+    const int stage = s % S;
+    const uint32_t ph = (uint32_t)(s / S) & 1u;
+    mbar_wait(empty_bar(stage), ph ^ 1u);
+    if (tid == 0) {
+      mbar_arrive_expect_tx(full_bar(stage), b_stage_bytes);
+      bulk_g2s(sB + stage * b_stage_bytes, wt + (size_t)s * w_slice_elems, b_stage_bytes, full_bar(stage));
+    }
+    return stage;
+  };
+  auto end_stage = [&](int s, int stage) {
+    fence_proxy_async();                 // generic-proxy smem writes -> visible to the tensor-core (async) proxy
+    named_sync(2 + wg, 128);
+    mbar_wait(full_bar(stage), (uint32_t)(s / S) & 1u);
+    if (tid == 0) tc_stamp(trace, 8 + s);
+    const uint32_t a_base = sA + stage * a_stage_bytes + (uint32_t)wg * (64u * 128u);
+    const uint64_t ad = make_sdesc(a_base);
+    const uint64_t bd = make_sdesc(sB + stage * b_stage_bytes);
+    wg_fence();
+    if constexpr (X3) {
+      const uint64_t ad_lo = make_sdesc(a_base + A_STAGE_BYTES);
+      const uint64_t bd_lo = make_sdesc(sB + stage * b_stage_bytes + b_tile_bytes);
+#pragma unroll
+      for (int k = 0; k < TC_BK / 16; ++k) {      // small cross terms first, then the hi x hi term
+        Wgmma<N>::mma(acc, ad_lo + 2ull * k, bd + 2ull * k, (s > 0 || k > 0) ? 1u : 0u);
+        Wgmma<N>::mma(acc, ad + 2ull * k, bd_lo + 2ull * k, 1u);
+        Wgmma<N>::mma(acc, ad + 2ull * k, bd + 2ull * k, 1u);
       }
     } else {
-      // linear tiles: one division pair for the first row, the other rows (+32 pixels each) by carry propagation
-      int p = mt * TC_BM + r0;
-      int b = p / HWo, r = p - b * HWo;
-      int oy = r / g.OW, ox = r - oy * g.OW;
 #pragma unroll
-      for (int i = 0; i < TC_NROW; ++i) {
-        if (p < g.P_out) {
-          row_iy[i] = oy * g.stride - g.pad;
-          row_ix[i] = ox * g.stride - g.pad_w;
-          row_off[i] = (b * g.H * g.W + row_iy[i] * g.W + row_ix[i]) * g.ld_in;
-        } else {
-          row_off[i] = 0; row_iy[i] = -100000; row_ix[i] = -100000;
-        }
-        p += 32; ox += 32;
-        while (ox >= g.OW) { ox -= g.OW; ++oy; }
-        while (oy >= g.OH) { oy -= g.OH; ++b; }
-      }
+      for (int k = 0; k < TC_BK / 16; ++k)
+        Wgmma<N>::mma(acc, ad + 2ull * k, bd + 2ull * k, (s > 0 || k > 0) ? 1u : 0u);
     }
-    if (tid == 0) tc_stamp(trace, 1);
-    int win_x0 = 0, win_y0 = 0, win_b = 0;
-    if (win) {
-      // window origin of this 8x16 patch: one kernel-halo pixel + the offset margin to the top/left
-      const int tpi = a.tiles_x * a.tiles_y;
-      win_b = mt / tpi;
-      const int t = mt - win_b * tpi;
-      const int ty = t / a.tiles_x, tx = t - ty * a.tiles_x;
-      win_y0 = ty * 8 - 1 - a.win_m;
-      win_x0 = tx * 16 - 1 - a.win_m;
-      if (tid == 0) {                                   // first 64-channel chunk of the window: TMA, zero fill outside
-        mbar_arrive_expect_tx(win_bar, a.win_bytes);      // count 1: this arrival + the TMA's bytes complete the phase
-        tma_4d(s_win, &tmap, 0, win_x0, win_y0, win_b, win_bar);
-      }
-      // Two threads per row (taps 0-4 and 5-8) so that all eight producer warps build the table.  The 27 offset / mask
-      // floats of a row sit in one 128-byte line of `om`; each thread loads only the 16-byte chunks its taps need.
-      const int trow = tid & (TC_BM - 1), thalf = tid >> 7;            // thalf 0: taps 0..4, thalf 1: taps 5..8
-      const int tap0 = thalf ? 5 : 0, tap1 = thalf ? 9 : 5;
-      const int tp = tc_pixel(a, mt, trow);
-      const bool ok = tp < g.P_out;
-      {
-        int oy = 0, ox = 0, img = 0;
-        float om[28];
-#pragma unroll
-        for (int j = 0; j < 28; ++j) om[j] = 0.f;
-        if (ok) {
-          const int bb = tp / HWo, r = tp - bb * HWo;
-          oy = r / g.OW; ox = r - oy * g.OW; img = bb * g.H * g.W;
-          const float4* omp = reinterpret_cast<const float4*>(a.om + (size_t)tp * g.ld_om);
-          // floats [2 tap0, 2 tap1) and [18 + tap0, 18 + tap1): chunks 0-2, 4-5 (thalf 0) / 2-6 (thalf 1)
-#pragma unroll
-          for (int j = 0; j < 7; ++j) {
-            const bool need = thalf ? (j >= 2) : (j <= 2 || j == 4 || j == 5);
-            if (need) {
-              const float4 t4 = __ldg(omp + j);
-              om[4 * j] = t4.x; om[4 * j + 1] = t4.y; om[4 * j + 2] = t4.z; om[4 * j + 3] = t4.w;
-            }
-          }
-        }
-#pragma unroll
-        for (int tap = 0; tap < 9; ++tap) {
-          if (tap < tap0 || tap >= tap1) continue;
-          DcnWinEntry e; e.goff = 0; e.meta = WIN_IN; e.w01 = 0u; e.w23 = 0u;
-          if (ok) {
-            const float py = (float)(oy - 1 + tap / 3) + om[2 * tap];
-            const float px = (float)(ox - 1 + tap % 3) + om[2 * tap + 1];
-            if (py > -1.f && py < (float)g.H && px > -1.f && px < (float)g.W) {
-              const float y0f = floorf(py), x0f = floorf(px);
-              const int y0 = (int)y0f, x0 = (int)x0f;
-              const float ly = py - y0f, lx = px - x0f, hy = 1.f - ly, hx = 1.f - lx, m = om[18 + tap];
-              const bool y0ok = y0 >= 0, y1ok = y0 + 1 <= g.H - 1, x0ok = x0 >= 0, x1ok = x0 + 1 <= g.W - 1;
-              const int yc = max(y0, 0), xc = max(x0, 0);
-              e.goff = (img + yc * g.W + xc) * g.ld_in;
-              const bool dx = x0ok && x1ok, dy = y0ok && y1ok;
-              const bool inside = y0 >= win_y0 && y0 + 1 <= win_y0 + a.win_ph - 1 && x0 >= win_x0 && x0 + 1 <= win_x0 + a.win_pw - 1;
-              const uint32_t woff16 = (uint32_t)((yc - win_y0) * a.win_pw + (xc - win_x0)) * 8u;   // 128 B per pixel
-              e.meta = (inside ? (woff16 | WIN_IN) : 0u) | (dx ? WIN_DX : 0u) | (dy ? WIN_DY : 0u);
-              const float w00 = (y0ok && x0ok) ? hy * hx * m : 0.f, w01 = (y0ok && x1ok) ? hy * lx * m : 0.f;
-              const float w10 = (y1ok && x0ok) ? ly * hx * m : 0.f, w11 = (y1ok && x1ok) ? ly * lx * m : 0.f;
-              const __nv_bfloat162 wa = __floats2bfloat162_rn(w00, w01), wb = __floats2bfloat162_rn(w10, w11);
-              e.w01 = *reinterpret_cast<const uint32_t*>(&wa);
-              e.w23 = *reinterpret_cast<const uint32_t*>(&wb);
-            }
-          }
-          win_tab[tap * TC_BM + trow] = e;
-        }
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (tid == 0) tc_stamp(trace, 2);
+    wg_commit();
+    wg_wait<1>();
+    wg_fence_operand(acc);
+    if (s > 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty_bar((s - 1) % S));
     }
-    if (a.a_mode == CT_A_DCN) {
-      // per (tap,row) sampling records, computed once per CTA (row = tid, threads 0..127)
-      const int p = tid < TC_BM ? tc_pixel(a, mt, tid) : g.P_out;
-      const bool ok = p < g.P_out;
-      if (tid < TC_BM) {
-        int oy = 0, ox = 0, img = 0;
-        float om[28];
-        if (ok) {
-          const int bb = p / HWo, r = p - bb * HWo;
-          oy = r / g.OW; ox = r - oy * g.OW; img = bb * g.H * g.W;
-          const float4* omp = reinterpret_cast<const float4*>(a.om + (size_t)p * g.ld_om);
-#pragma unroll
-          for (int j = 0; j < 7; ++j) {
-            const float4 t = __ldg(omp + j);
-            om[4 * j] = t.x; om[4 * j + 1] = t.y; om[4 * j + 2] = t.z; om[4 * j + 3] = t.w;
-          }
-        }
-#pragma unroll
-        for (int tap = 0; tap < 9; ++tap) {
-          DcnEntry e; e.off = 0; e.dxo = 0; e.dyo = 0; e.pad = 0; e.w00 = e.w01 = e.w10 = e.w11 = 0.f;
-          if (ok) {
-            const float py = (float)(oy - 1 + tap / 3) + om[2 * tap];
-            const float px = (float)(ox - 1 + tap % 3) + om[2 * tap + 1];
-            if (py > -1.f && py < (float)g.H && px > -1.f && px < (float)g.W) {
-              const float y0f = floorf(py), x0f = floorf(px);
-              const int y0 = (int)y0f, x0 = (int)x0f;
-              const float ly = py - y0f, lx = px - x0f, hy = 1.f - ly, hx = 1.f - lx, m = om[18 + tap];
-              const bool y0ok = y0 >= 0, y1ok = y0 + 1 <= g.H - 1, x0ok = x0 >= 0, x1ok = x0 + 1 <= g.W - 1;
-              e.off = (img + max(y0, 0) * g.W + max(x0, 0)) * g.ld_in;
-              e.dxo = (x0ok && x1ok) ? g.ld_in : 0;
-              e.dyo = (y0ok && y1ok) ? g.W * g.ld_in : 0;
-              e.w00 = (y0ok && x0ok) ? hy * hx * m : 0.f;
-              e.w01 = (y0ok && x1ok) ? hy * lx * m : 0.f;
-              e.w10 = (y1ok && x0ok) ? ly * hx * m : 0.f;
-              e.w11 = (y1ok && x1ok) ? ly * lx * m : 0.f;
-            }
-          }
-          dcn_tab[tap * TC_BM + tid] = e;
-        }
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (tid == 0) tc_stamp(trace, 2);
-    }
-    const int cin8 = g.C_in >> 3;
-    const int ntaps = g.KH * g.KW;
-    const size_t w_slice_elems = (size_t)(X3 ? 2 : 1) * a.n_tile * TC_BK;
-    const __nv_bfloat16* wt = a.w + (size_t)nt * a.k_slices * w_slice_elems;
+  };
 
-    if (win) {
-      // ---- DCN sampled from a shared-memory window (CT_A_DCN_WIN).  K order = (64-channel chunk, tap, channel): one K
-      // slice is one tap of one chunk, so the window of a chunk serves nine slices.  Per slice a thread blends its
-      // four rows' 8-channel column: 16 LDS.128 (four corners x four rows) instead of 16 L1/L2 round trips; records
-      // whose 2x2 footprint leaves the window (offset beyond the margin) take the global path.
-      const int nchunks = g.C_in >> 6;
-      const uint32_t pitch = (uint32_t)a.win_pw * 128u;
-      const int gdx = g.ld_in, gdy = g.W * g.ld_in;
-      int s = 0;
-      for (int ch = 0; ch < nchunks; ++ch) {
-        mbar_wait(win_bar, (uint32_t)ch & 1u);
-        for (int tap = 0; tap < 9; ++tap, ++s) {
-          const int stage = s % S;
-          const uint32_t ph = (uint32_t)(s / S) & 1u;
-          mbar_wait(empty_bar(stage), ph ^ 1u);
-          if (tid == 0) {
-            mbar_expect_tx(full_bar(stage), b_stage_bytes);
-            bulk_g2s(sB + stage * b_stage_bytes, wt + (size_t)s * w_slice_elems, b_stage_bytes, full_bar(stage));
-          }
-          const DcnWinEntry* tab = win_tab + tap * TC_BM + r0;
-          uint4 e4[TC_NROW], v[TC_NROW][4];
+  if (win) {
+    // ---- DCN sampled from a shared-memory window (CT_A_DCN_WIN).  K order = (64-channel chunk, tap, channel): one K
+    // slice is one tap of one chunk, so the window of a chunk serves nine slices.  Per slice a thread blends its
+    // four rows' 8-channel column: 16 LDS.128 (four corners x four rows) instead of 16 L1/L2 round trips; records
+    // whose 2x2 footprint leaves the window (offset beyond the margin) take the global path.
+    const int nchunks = g.C_in >> 6;
+    const uint32_t pitch = (uint32_t)a.win_pw * 128u;
+    const int gdx = g.ld_in, gdy = g.W * g.ld_in;
+    int s = 0;
+    for (int ch = 0; ch < nchunks; ++ch) {
+      mbar_wait(win_bar, (uint32_t)ch & 1u);
+      for (int tap = 0; tap < 9; ++tap, ++s) {
+        const int stage = begin_stage(s);
+        const DcnWinEntry* tab = win_tab + tap * TC_BM + rb;
+        uint4 e4[TC_NROW], v[TC_NROW][4];
 #pragma unroll
-          for (int i = 0; i < TC_NROW; ++i) e4[i] = *reinterpret_cast<const uint4*>(&tab[32 * i]);
+        for (int i = 0; i < TC_NROW; ++i) e4[i] = *reinterpret_cast<const uint4*>(&tab[16 * i]);
 #pragma unroll
-          for (int i = 0; i < TC_NROW; ++i) {
-            const uint32_t meta = e4[i].y;
-            if (meta & WIN_IN) {
-              const uint32_t base = s_win + ((meta & 0xffffu) << 4) + (uint32_t)(q << 4);
-              const uint32_t dx = (meta & WIN_DX) ? 128u : 0u, dy = (meta & WIN_DY) ? pitch : 0u;
-              v[i][0] = lds16(base); v[i][1] = lds16(base + dx);
-              v[i][2] = lds16(base + dy); v[i][3] = lds16(base + dy + dx);
-            } else {
-              const __nv_bfloat16* p00 = a.x + ((int)e4[i].x + (ch << 6) + (q << 3));
-              const int dx = (meta & WIN_DX) ? gdx : 0, dy = (meta & WIN_DY) ? gdy : 0;
-              v[i][0] = ldg_nc16(p00); v[i][1] = ldg_nc16(p00 + dx);
-              v[i][2] = ldg_nc16(p00 + dy); v[i][3] = ldg_nc16(p00 + dy + dx);
-            }
-          }
-          const uint32_t dst = sA + stage * A_STAGE_BYTES + (uint32_t)r0 * 128u + swz;
-#pragma unroll
-          for (int i = 0; i < TC_NROW; ++i) {
-            const uint32_t w0 = __byte_perm(e4[i].z, 0, 0x1010), w1 = __byte_perm(e4[i].z, 0, 0x3232);   // {w,w} pairs
-            const uint32_t w2 = __byte_perm(e4[i].w, 0, 0x1010), w3 = __byte_perm(e4[i].w, 0, 0x3232);
-            uint4 o;
-            o.x = bmul2(v[i][0].x, w0); o.y = bmul2(v[i][0].y, w0); o.z = bmul2(v[i][0].z, w0); o.w = bmul2(v[i][0].w, w0);
-            o.x = bfma2(v[i][1].x, w1, o.x); o.y = bfma2(v[i][1].y, w1, o.y); o.z = bfma2(v[i][1].z, w1, o.z); o.w = bfma2(v[i][1].w, w1, o.w);
-            o.x = bfma2(v[i][2].x, w2, o.x); o.y = bfma2(v[i][2].y, w2, o.y); o.z = bfma2(v[i][2].z, w2, o.z); o.w = bfma2(v[i][2].w, w2, o.w);
-            o.x = bfma2(v[i][3].x, w3, o.x); o.y = bfma2(v[i][3].y, w3, o.y); o.z = bfma2(v[i][3].z, w3, o.z); o.w = bfma2(v[i][3].w, w3, o.w);
-            sts16(dst + i * 4096u, o);
-          }
-          if (!a.fence_mma) fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(full_bar(stage));
-          if (tid == 0) tc_stamp(trace, 8 + s);
-        }
-        if (ch + 1 < nchunks) {                       // every producer is done with this chunk's window: refill it
-          asm volatile("bar.sync 1, 256;" ::: "memory");
-          if (tid == 0) {
-            mbar_arrive_expect_tx(win_bar, a.win_bytes);      // count 1: this arrival + the TMA's bytes complete the phase
-            tma_4d(s_win, &tmap, (ch + 1) << 6, win_x0, win_y0, win_b, win_bar);
+        for (int i = 0; i < TC_NROW; ++i) {
+          const uint32_t meta = e4[i].y;
+          if (meta & WIN_IN) {
+            const uint32_t base = s_win + ((meta & 0xffffu) << 4) + (uint32_t)(q << 4);
+            const uint32_t dx = (meta & WIN_DX) ? 128u : 0u, dy = (meta & WIN_DY) ? pitch : 0u;
+            v[i][0] = lds16(base); v[i][1] = lds16(base + dx);
+            v[i][2] = lds16(base + dy); v[i][3] = lds16(base + dy + dx);
+          } else {
+            const __nv_bfloat16* p00 = a.x + ((int)e4[i].x + (ch << 6) + (q << 3));
+            const int dx = (meta & WIN_DX) ? gdx : 0, dy = (meta & WIN_DY) ? gdy : 0;
+            v[i][0] = ldg_nc16(p00); v[i][1] = ldg_nc16(p00 + dx);
+            v[i][2] = ldg_nc16(p00 + dy); v[i][3] = ldg_nc16(p00 + dy + dx);
           }
         }
-      }
-    } else if constexpr (X3) {
-      // ---- bf16x3 producers: fp32 activations, each 8-channel chunk = two 16-byte loads, split into hi / lo tiles
-      auto begin_stage = [&](int s) {
-        const int stage = s % S;
-        const uint32_t ph = (uint32_t)(s / S) & 1u;
-        mbar_wait(empty_bar(stage), ph ^ 1u);
-        if (tid == 0) {
-          mbar_expect_tx(full_bar(stage), b_stage_bytes);
-          bulk_g2s(sB + stage * b_stage_bytes, wt + (size_t)s * w_slice_elems, b_stage_bytes, full_bar(stage));
-        }
-        return stage;
-      };
-      auto end_stage = [&](int s, int stage) {
-        if (!a.fence_mma) fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(full_bar(stage));
-        if (tid == 0) tc_stamp(trace, 8 + s);
-      };
-      if (a.a_mode == CT_A_DCN) {
-        float4 va[2][4][2], vb[2][4][2];
-        auto load_half = [&](int tap, int c, int half, float4 (&v)[2][4][2]) {
-          const DcnEntry* tab = dcn_tab + (tap < ntaps ? tap : 0) * TC_BM + r0 + 64 * half;
+        const uint32_t dst = sA + stage * A_STAGE_BYTES + (uint32_t)rb * 128u + swz;
 #pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            const int4 o = *reinterpret_cast<const int4*>(&tab[32 * j]);     // off, dxo, dyo
-            const float* p00 = xf + (o.x + c);
-            v[j][0][0] = ldg_nc_f4(p00);             v[j][0][1] = ldg_nc_f4(p00 + 4);
-            v[j][1][0] = ldg_nc_f4(p00 + o.y);       v[j][1][1] = ldg_nc_f4(p00 + o.y + 4);
-            v[j][2][0] = ldg_nc_f4(p00 + o.z);       v[j][2][1] = ldg_nc_f4(p00 + o.z + 4);
-            v[j][3][0] = ldg_nc_f4(p00 + o.z + o.y); v[j][3][1] = ldg_nc_f4(p00 + o.z + o.y + 4);
-          }
-        };
-        auto blend_half = [&](int tap, int stage, int half, const float4 (&v)[2][4][2]) {
-          const bool live = tap < ntaps;
-          const DcnEntry* tab = dcn_tab + (live ? tap : 0) * TC_BM + r0 + 64 * half;
-          const uint32_t dst = sA + stage * a_stage_bytes + (uint32_t)(r0 + 64 * half) * 128u + swz;
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            const float4 w = *reinterpret_cast<const float4*>(&tab[32 * j].w00);
-            const float ww[4] = {w.x, w.y, w.z, w.w};
-            float4 acc[2];
-#pragma unroll
-            for (int h2 = 0; h2 < 2; ++h2) {
-              acc[h2] = make_float4(ww[0] * v[j][0][h2].x, ww[0] * v[j][0][h2].y, ww[0] * v[j][0][h2].z, ww[0] * v[j][0][h2].w);
-#pragma unroll
-              for (int cn = 1; cn < 4; ++cn) {
-                acc[h2].x = fmaf(ww[cn], v[j][cn][h2].x, acc[h2].x); acc[h2].y = fmaf(ww[cn], v[j][cn][h2].y, acc[h2].y);
-                acc[h2].z = fmaf(ww[cn], v[j][cn][h2].z, acc[h2].z); acc[h2].w = fmaf(ww[cn], v[j][cn][h2].w, acc[h2].w);
-              }
-            }
-            uint4 hi, lo;
-            split8(acc[0], acc[1], hi, lo);
-            if (!live) { hi = make_uint4(0, 0, 0, 0); lo = hi; }
-            sts16(dst + j * 4096u, hi);
-            sts16(dst + A_STAGE_BYTES + j * 4096u, lo);
-          }
-        };
-        int tap = q / cin8, cq = q - tap * cin8;
-        load_half(tap, cq << 3, 0, va);
-        for (int s = 0; s < a.k_slices; ++s) {
-          load_half(tap, cq << 3, 1, vb);
-          const int stage = begin_stage(s);
-          blend_half(tap, stage, 0, va);
-          int ntap = tap, ncq = cq + 8;
-          while (ncq >= cin8) { ncq -= cin8; ++ntap; }
-          if (s + 1 < a.k_slices) load_half(ntap, ncq << 3, 0, va);
-          blend_half(tap, stage, 1, vb);
-          tap = ntap; cq = ncq;
-          end_stage(s, stage);
-        }
-      } else {
-        int ltap = q / cin8, lcq = q - ltap * cin8;
-        auto load_slice = [&](bool in_range, float4 (&v)[TC_NROW][2]) {
-#pragma unroll
-          for (int i = 0; i < TC_NROW; ++i) { v[i][0] = make_float4(0.f, 0.f, 0.f, 0.f); v[i][1] = v[i][0]; }
-          if (in_range && ltap < ntaps) {
-            const int ky = ltap / g.KW, kx = ltap - ky * g.KW;
-            const int tap_off = (ky * g.W + kx) * g.ld_in + (lcq << 3);
-#pragma unroll
-            for (int i = 0; i < TC_NROW; ++i)
-              if ((unsigned)(row_iy[i] + ky) < (unsigned)g.H && (unsigned)(row_ix[i] + kx) < (unsigned)g.W) {
-                const float* pp = xf + (row_off[i] + tap_off);
-                v[i][0] = ldg_nc_f4(pp); v[i][1] = ldg_nc_f4(pp + 4);
-              }
-          }
-          lcq += 8;
-          while (lcq >= cin8) { lcq -= cin8; ++ltap; }
-        };
-        auto store_slice = [&](int s, const float4 (&v)[TC_NROW][2]) {
-          const int stage = begin_stage(s);
-          const uint32_t dst = sA + stage * a_stage_bytes + (uint32_t)r0 * 128u + swz;
-#pragma unroll
-          for (int i = 0; i < TC_NROW; ++i) {
-            uint4 hi, lo;
-            split8(v[i][0], v[i][1], hi, lo);
-            sts16(dst + i * 4096u, hi);
-            sts16(dst + A_STAGE_BYTES + i * 4096u, lo);
-          }
-          end_stage(s, stage);
-        };
-        const int KS = a.k_slices;
-        float4 v0[TC_NROW][2], v1[TC_NROW][2], v2[TC_NROW][2];
-        load_slice(0 < KS, v0);
-        load_slice(1 < KS, v1);
-        load_slice(2 < KS, v2);
-        for (int s = 0; s < KS; s += 3) {
-          store_slice(s, v0);
-          load_slice(s + 3 < KS, v0);
-          if (s + 1 < KS) { store_slice(s + 1, v1); load_slice(s + 4 < KS, v1); }
-          if (s + 2 < KS) { store_slice(s + 2, v2); load_slice(s + 5 < KS, v2); }
-        }
-      }
-    } else if (a.a_mode == CT_A_DCN) {
-      // Software-pipelined by half slices (2 of the thread's 4 rows): the 8 corner loads of the next half are in
-      // flight while the current half is blended (the gather is latency-bound -- memory-level parallelism first --
-      // and the blend is issue-bound: packed FFMA2, one-op bf16 unpack).  A slice whose tap index runs past the
-      // kernel (K padding) samples tap 0 with its result zeroed.
-      uint4 va[2][4], vb[2][4];
-      auto load_half = [&](int tap, int c, int half, uint4 (&v)[2][4]) {
-        const DcnEntry* tab = dcn_tab + (tap < ntaps ? tap : 0) * TC_BM + r0 + 64 * half;
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-          const int4 o = *reinterpret_cast<const int4*>(&tab[32 * j]);     // off, dxo, dyo
-          const __nv_bfloat16* p00 = a.x + (o.x + c);
-          v[j][0] = ldg_nc16(p00);
-          v[j][1] = ldg_nc16(p00 + o.y);
-          v[j][2] = ldg_nc16(p00 + o.z);
-          v[j][3] = ldg_nc16(p00 + o.z + o.y);
-        }
-      };
-      auto blend_half = [&](int tap, int stage, int half, const uint4 (&v)[2][4]) {
-        const bool live = tap < ntaps;
-        const DcnEntry* tab = dcn_tab + (live ? tap : 0) * TC_BM + r0 + 64 * half;
-        const uint32_t dst = sA + stage * A_STAGE_BYTES + (uint32_t)(r0 + 64 * half) * 128u + swz;
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-          // packed bf16 blend, same rounding points as the window sampler (weights to bf16, fma chain 00,01,10,11)
-          const float4 w = *reinterpret_cast<const float4*>(&tab[32 * j].w00);
-          const uint32_t w0 = dup_bf2(w.x), w1 = dup_bf2(w.y), w2 = dup_bf2(w.z), w3 = dup_bf2(w.w);
+        for (int i = 0; i < TC_NROW; ++i) {
+          const uint32_t w0 = __byte_perm(e4[i].z, 0, 0x1010), w1 = __byte_perm(e4[i].z, 0, 0x3232);   // {w,w} pairs
+          const uint32_t w2 = __byte_perm(e4[i].w, 0, 0x1010), w3 = __byte_perm(e4[i].w, 0, 0x3232);
           uint4 o;
-          o.x = bmul2(v[j][0].x, w0); o.y = bmul2(v[j][0].y, w0); o.z = bmul2(v[j][0].z, w0); o.w = bmul2(v[j][0].w, w0);
-          o.x = bfma2(v[j][1].x, w1, o.x); o.y = bfma2(v[j][1].y, w1, o.y); o.z = bfma2(v[j][1].z, w1, o.z); o.w = bfma2(v[j][1].w, w1, o.w);
-          o.x = bfma2(v[j][2].x, w2, o.x); o.y = bfma2(v[j][2].y, w2, o.y); o.z = bfma2(v[j][2].z, w2, o.z); o.w = bfma2(v[j][2].w, w2, o.w);
-          o.x = bfma2(v[j][3].x, w3, o.x); o.y = bfma2(v[j][3].y, w3, o.y); o.z = bfma2(v[j][3].z, w3, o.z); o.w = bfma2(v[j][3].w, w3, o.w);
-          sts16(dst + j * 4096u, live ? o : make_uint4(0, 0, 0, 0));
+          o.x = bmul2(v[i][0].x, w0); o.y = bmul2(v[i][0].y, w0); o.z = bmul2(v[i][0].z, w0); o.w = bmul2(v[i][0].w, w0);
+          o.x = bfma2(v[i][1].x, w1, o.x); o.y = bfma2(v[i][1].y, w1, o.y); o.z = bfma2(v[i][1].z, w1, o.z); o.w = bfma2(v[i][1].w, w1, o.w);
+          o.x = bfma2(v[i][2].x, w2, o.x); o.y = bfma2(v[i][2].y, w2, o.y); o.z = bfma2(v[i][2].z, w2, o.z); o.w = bfma2(v[i][2].w, w2, o.w);
+          o.x = bfma2(v[i][3].x, w3, o.x); o.y = bfma2(v[i][3].y, w3, o.y); o.z = bfma2(v[i][3].z, w3, o.z); o.w = bfma2(v[i][3].w, w3, o.w);
+          sts16(dst + i * 2048u, o);
+        }
+        end_stage(s, stage);
+      }
+      if (ch + 1 < nchunks) {                       // every thread is done with this chunk's window: refill it
+        named_sync(1, TC_PRODUCERS);
+        if (tid == 0) {
+          mbar_arrive_expect_tx(win_bar, a.win_bytes);      // count 1: this arrival + the TMA's bytes complete the phase
+          tma_4d(s_win, &tmap, (ch + 1) << 6, win_x0, win_y0, win_b, win_bar);
+        }
+      }
+    }
+  } else if constexpr (X3) {
+    // ---- bf16x3 producers: fp32 activations, each 8-channel chunk = two 16-byte loads, split into hi / lo tiles
+    if (a.a_mode == CT_A_DCN) {
+      float4 va[2][4][2], vb[2][4][2];
+      auto load_half = [&](int tap, int c, int half, float4 (&v)[2][4][2]) {
+        const DcnEntry* tab = dcn_tab + (tap < ntaps ? tap : 0) * TC_BM + rb + 32 * half;
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const int4 o = *reinterpret_cast<const int4*>(&tab[16 * j]);     // off, dxo, dyo
+          const float* p00 = xf + (o.x + c);
+          v[j][0][0] = ldg_nc_f4(p00);             v[j][0][1] = ldg_nc_f4(p00 + 4);
+          v[j][1][0] = ldg_nc_f4(p00 + o.y);       v[j][1][1] = ldg_nc_f4(p00 + o.y + 4);
+          v[j][2][0] = ldg_nc_f4(p00 + o.z);       v[j][2][1] = ldg_nc_f4(p00 + o.z + 4);
+          v[j][3][0] = ldg_nc_f4(p00 + o.z + o.y); v[j][3][1] = ldg_nc_f4(p00 + o.z + o.y + 4);
         }
       };
-      // (tap, channel group) of this thread's 8-channel column in slice s, advanced incrementally (no division)
+      auto blend_half = [&](int tap, int stage, int half, const float4 (&v)[2][4][2]) {
+        const bool live = tap < ntaps;
+        const DcnEntry* tab = dcn_tab + (live ? tap : 0) * TC_BM + rb + 32 * half;
+        const uint32_t dst = sA + stage * a_stage_bytes + (uint32_t)(rb + 32 * half) * 128u + swz;
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const float4 w = *reinterpret_cast<const float4*>(&tab[16 * j].w00);
+          const float ww[4] = {w.x, w.y, w.z, w.w};
+          float4 acc4[2];
+#pragma unroll
+          for (int h2 = 0; h2 < 2; ++h2) {
+            acc4[h2] = make_float4(ww[0] * v[j][0][h2].x, ww[0] * v[j][0][h2].y, ww[0] * v[j][0][h2].z, ww[0] * v[j][0][h2].w);
+#pragma unroll
+            for (int cn = 1; cn < 4; ++cn) {
+              acc4[h2].x = fmaf(ww[cn], v[j][cn][h2].x, acc4[h2].x); acc4[h2].y = fmaf(ww[cn], v[j][cn][h2].y, acc4[h2].y);
+              acc4[h2].z = fmaf(ww[cn], v[j][cn][h2].z, acc4[h2].z); acc4[h2].w = fmaf(ww[cn], v[j][cn][h2].w, acc4[h2].w);
+            }
+          }
+          uint4 hi, lo;
+          split8(acc4[0], acc4[1], hi, lo);
+          if (!live) { hi = make_uint4(0, 0, 0, 0); lo = hi; }
+          sts16(dst + j * 2048u, hi);
+          sts16(dst + A_STAGE_BYTES + j * 2048u, lo);
+        }
+      };
       int tap = q / cin8, cq = q - tap * cin8;
       load_half(tap, cq << 3, 0, va);
       for (int s = 0; s < a.k_slices; ++s) {
-        const int stage = s % S;
-        const uint32_t ph = (uint32_t)(s / S) & 1u;
         load_half(tap, cq << 3, 1, vb);
-        mbar_wait(empty_bar(stage), ph ^ 1u);
-        if (tid == 0) {
-          mbar_expect_tx(full_bar(stage), b_stage_bytes);
-          bulk_g2s(sB + stage * b_stage_bytes, wt + (size_t)s * a.n_tile * TC_BK, b_stage_bytes, full_bar(stage));
-        }
+        const int stage = begin_stage(s);
         blend_half(tap, stage, 0, va);
         int ntap = tap, ncq = cq + 8;
         while (ncq >= cin8) { ncq -= cin8; ++ntap; }
         if (s + 1 < a.k_slices) load_half(ntap, ncq << 3, 0, va);
         blend_half(tap, stage, 1, vb);
         tap = ntap; cq = ncq;
-        if (!a.fence_mma) fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(full_bar(stage));      // one arrival per producer warp
-        if (tid == 0) tc_stamp(trace, 8 + s);
+        end_stage(s, stage);
       }
     } else {
-      // Plain convolution gather, register-prefetched three K slices ahead (12 independent 16-byte loads in flight
-      // per thread): one slice's loads alone leave the loop bound by the L2 round trip (~1700 cycles per slice
-      // measured with tools/tc_trace.py).  (tap, channel group) advance incrementally with the load order.
       int ltap = q / cin8, lcq = q - ltap * cin8;
-      auto load_slice = [&](bool in_range, uint4 (&v)[TC_NROW]) {
+      auto load_slice = [&](bool in_range, float4 (&v)[TC_NROW][2]) {
 #pragma unroll
-        for (int i = 0; i < TC_NROW; ++i) v[i] = make_uint4(0, 0, 0, 0);
+        for (int i = 0; i < TC_NROW; ++i) { v[i][0] = make_float4(0.f, 0.f, 0.f, 0.f); v[i][1] = v[i][0]; }
         if (in_range && ltap < ntaps) {
           const int ky = ltap / g.KW, kx = ltap - ky * g.KW;
-          const int tap_off = (ky * g.W + kx) * g.ld_in + (lcq << 3);      // same for every row of the slice
+          const int tap_off = (ky * g.W + kx) * g.ld_in + (lcq << 3);
 #pragma unroll
           for (int i = 0; i < TC_NROW; ++i)
-            if ((unsigned)(row_iy[i] + ky) < (unsigned)g.H && (unsigned)(row_ix[i] + kx) < (unsigned)g.W)
-              v[i] = ldg_nc16(a.x + (row_off[i] + tap_off));
+            if ((unsigned)(row_iy[i] + ky) < (unsigned)g.H && (unsigned)(row_ix[i] + kx) < (unsigned)g.W) {
+              const float* pp = xf + (row_off[i] + tap_off);
+              v[i][0] = ldg_nc_f4(pp); v[i][1] = ldg_nc_f4(pp + 4);
+            }
         }
         lcq += 8;
         while (lcq >= cin8) { lcq -= cin8; ++ltap; }
       };
-      auto store_slice = [&](int s, const uint4 (&v)[TC_NROW]) {
-        const int stage = s % S;
-        const uint32_t ph = (uint32_t)(s / S) & 1u;
-        mbar_wait(empty_bar(stage), ph ^ 1u);
-        if (tid == 0) {
-          mbar_expect_tx(full_bar(stage), b_stage_bytes);
-          bulk_g2s(sB + stage * b_stage_bytes, wt + (size_t)s * a.n_tile * TC_BK, b_stage_bytes, full_bar(stage));
-        }
-        const uint32_t dst = sA + stage * A_STAGE_BYTES + (uint32_t)r0 * 128u + swz;
+      auto store_slice = [&](int s, const float4 (&v)[TC_NROW][2]) {
+        const int stage = begin_stage(s);
+        const uint32_t dst = sA + stage * a_stage_bytes + (uint32_t)rb * 128u + swz;
 #pragma unroll
-        for (int i = 0; i < TC_NROW; ++i) sts16(dst + i * 4096u, v[i]);
-        if (!a.fence_mma) fence_proxy_async();          // generic-proxy smem writes -> visible to the tensor-core (async) proxy
-        __syncwarp();
-        if (lane == 0) mbar_arrive(full_bar(stage));      // one arrival per producer warp (256 arrivals on one
-                                                          // shared-memory word serialise)
-        if (tid == 0) tc_stamp(trace, 8 + s);
+        for (int i = 0; i < TC_NROW; ++i) {
+          uint4 hi, lo;
+          split8(v[i][0], v[i][1], hi, lo);
+          sts16(dst + i * 2048u, hi);
+          sts16(dst + A_STAGE_BYTES + i * 2048u, lo);
+        }
+        end_stage(s, stage);
       };
       const int KS = a.k_slices;
-      uint4 v0[TC_NROW], v1[TC_NROW], v2[TC_NROW];
+      float4 v0[TC_NROW][2], v1[TC_NROW][2];
       load_slice(0 < KS, v0);
       load_slice(1 < KS, v1);
-      load_slice(2 < KS, v2);
-      for (int s = 0; s < KS; s += 3) {
+      for (int s = 0; s < KS; s += 2) {
         store_slice(s, v0);
-        load_slice(s + 3 < KS, v0);
-        if (s + 1 < KS) { store_slice(s + 1, v1); load_slice(s + 4 < KS, v1); }
-        if (s + 2 < KS) { store_slice(s + 2, v2); load_slice(s + 5 < KS, v2); }
+        load_slice(s + 2 < KS, v0);
+        if (s + 1 < KS) { store_slice(s + 1, v1); load_slice(s + 3 < KS, v1); }
       }
     }
-
-    // =========================== epilogue ===========================
-    mbar_wait(tmem_full_bar, 0);
-    tc_fence_after();
-    if (tid == 0) tc_stamp(trace, 5);
-    const int wq = warp & 3, chalf = warp >> 2;      // TMEM lane quarter, column-chunk parity
-    const int row = wq * 32 + lane;
-    const int p = tc_pixel(a, mt, row);
-    const bool p_ok = p < g.P_out;
-    const uint32_t t_lane = tmem_base + ((uint32_t)(wq * 32) << 16);
-    for (int col = chalf * 16; col < a.n_tile; col += 32) {
-      uint32_t r[16];
-      tc_ld16(t_lane + (uint32_t)col, r);
-      const int o0 = n0 + col;
-      if (!p_ok || o0 >= g.C_out) continue;
-      float v[16];
+  } else if (a.a_mode == CT_A_DCN) {
+    // Software-pipelined by half slices (2 of the thread's 4 rows): the 8 corner loads of the next half are in
+    // flight while the current half is blended.  A slice whose tap index runs past the kernel (K padding) samples
+    // tap 0 with its result zeroed.
+    uint4 va[2][4], vb[2][4];
+    auto load_half = [&](int tap, int c, int half, uint4 (&v)[2][4]) {
+      const DcnEntry* tab = dcn_tab + (tap < ntaps ? tap : 0) * TC_BM + rb + 32 * half;
 #pragma unroll
-      for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]);
+      for (int j = 0; j < 2; ++j) {
+        const int4 o = *reinterpret_cast<const int4*>(&tab[16 * j]);     // off, dxo, dyo
+        const __nv_bfloat16* p00 = a.x + (o.x + c);
+        v[j][0] = ldg_nc16(p00);
+        v[j][1] = ldg_nc16(p00 + o.y);
+        v[j][2] = ldg_nc16(p00 + o.z);
+        v[j][3] = ldg_nc16(p00 + o.z + o.y);
+      }
+    };
+    auto blend_half = [&](int tap, int stage, int half, const uint4 (&v)[2][4]) {
+      const bool live = tap < ntaps;
+      const DcnEntry* tab = dcn_tab + (live ? tap : 0) * TC_BM + rb + 32 * half;
+      const uint32_t dst = sA + stage * A_STAGE_BYTES + (uint32_t)(rb + 32 * half) * 128u + swz;
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        // packed bf16 blend, same rounding points as the window sampler (weights to bf16, fma chain 00,01,10,11)
+        const float4 w = *reinterpret_cast<const float4*>(&tab[16 * j].w00);
+        const uint32_t w0 = dup_bf2(w.x), w1 = dup_bf2(w.y), w2 = dup_bf2(w.z), w3 = dup_bf2(w.w);
+        uint4 o;
+        o.x = bmul2(v[j][0].x, w0); o.y = bmul2(v[j][0].y, w0); o.z = bmul2(v[j][0].z, w0); o.w = bmul2(v[j][0].w, w0);
+        o.x = bfma2(v[j][1].x, w1, o.x); o.y = bfma2(v[j][1].y, w1, o.y); o.z = bfma2(v[j][1].z, w1, o.z); o.w = bfma2(v[j][1].w, w1, o.w);
+        o.x = bfma2(v[j][2].x, w2, o.x); o.y = bfma2(v[j][2].y, w2, o.y); o.z = bfma2(v[j][2].z, w2, o.z); o.w = bfma2(v[j][2].w, w2, o.w);
+        o.x = bfma2(v[j][3].x, w3, o.x); o.y = bfma2(v[j][3].y, w3, o.y); o.z = bfma2(v[j][3].z, w3, o.z); o.w = bfma2(v[j][3].w, w3, o.w);
+        sts16(dst + j * 2048u, live ? o : make_uint4(0, 0, 0, 0));
+      }
+    };
+    // (tap, channel group) of this thread's 8-channel column in slice s, advanced incrementally (no division)
+    int tap = q / cin8, cq = q - tap * cin8;
+    load_half(tap, cq << 3, 0, va);
+    for (int s = 0; s < a.k_slices; ++s) {
+      load_half(tap, cq << 3, 1, vb);
+      const int stage = begin_stage(s);
+      blend_half(tap, stage, 0, va);
+      int ntap = tap, ncq = cq + 8;
+      while (ncq >= cin8) { ncq -= cin8; ++ntap; }
+      if (s + 1 < a.k_slices) load_half(ntap, ncq << 3, 0, va);
+      blend_half(tap, stage, 1, vb);
+      tap = ntap; cq = ncq;
+      end_stage(s, stage);
+    }
+  } else {
+    // Plain convolution gather, register-prefetched two K slices ahead (8 independent 16-byte loads in flight per
+    // thread) while the MMAs of the previous slice run.  (tap, channel group) advance incrementally with the load order.
+    int ltap = q / cin8, lcq = q - ltap * cin8;
+    auto load_slice = [&](bool in_range, uint4 (&v)[TC_NROW]) {
+#pragma unroll
+      for (int i = 0; i < TC_NROW; ++i) v[i] = make_uint4(0, 0, 0, 0);
+      if (in_range && ltap < ntaps) {
+        const int ky = ltap / g.KW, kx = ltap - ky * g.KW;
+        const int tap_off = (ky * g.W + kx) * g.ld_in + (lcq << 3);      // same for every row of the slice
+#pragma unroll
+        for (int i = 0; i < TC_NROW; ++i)
+          if ((unsigned)(row_iy[i] + ky) < (unsigned)g.H && (unsigned)(row_ix[i] + kx) < (unsigned)g.W)
+            v[i] = ldg_nc16(a.x + (row_off[i] + tap_off));
+      }
+      lcq += 8;
+      while (lcq >= cin8) { lcq -= cin8; ++ltap; }
+    };
+    auto store_slice = [&](int s, const uint4 (&v)[TC_NROW]) {
+      const int stage = begin_stage(s);
+      const uint32_t dst = sA + stage * A_STAGE_BYTES + (uint32_t)rb * 128u + swz;
+#pragma unroll
+      for (int i = 0; i < TC_NROW; ++i) sts16(dst + i * 2048u, v[i]);
+      end_stage(s, stage);
+    };
+    const int KS = a.k_slices;
+    uint4 v0[TC_NROW], v1[TC_NROW];
+    load_slice(0 < KS, v0);
+    load_slice(1 < KS, v1);
+    for (int s = 0; s < KS; s += 2) {
+      store_slice(s, v0);
+      load_slice(s + 2 < KS, v0);
+      if (s + 1 < KS) { store_slice(s + 1, v1); load_slice(s + 3 < KS, v1); }
+    }
+  }
+  wg_wait<0>();
+  wg_fence_operand(acc);
+  if (tid == 0) tc_stamp(trace, 5);
+  __syncthreads();                     // every MMA has read its stage: the stage area becomes the staging tile
+
+  // =========================== epilogue ===========================
+  // 32 accumulator columns at a time through shared memory; thread (warp w, lane l) then owns GEMM row 32 (w % 4) + l
+  // and the 16-column half w / 4 of the chunk.
+  const uint32_t stg = sA;
+  const int wq = warp & 3, chalf = warp >> 2;
+  const int row = wq * 32 + lane;
+  const int p = tc_pixel(a, mt, row);
+  const bool p_ok = p < g.P_out;
+#pragma unroll
+  for (int c0 = 0; c0 < N; c0 += 32) {
+    stage_acc_chunk(acc, c0, stg, wg * 64);
+    __syncthreads();
+    const int col = c0 + chalf * 16;
+    const int o0 = n0 + col;
+    if (col < N && p_ok && o0 < g.C_out) {
+      float v[16];
+      lds_f16(stg + ((uint32_t)row * TC_EPI_PITCH + (uint32_t)chalf * 16u) * 4u, v);
       if (a.shift) {
         if (o0 + 16 <= g.C_out && (reinterpret_cast<size_t>(a.shift + o0) & 15) == 0) {   // four 16-byte loads
           const float4* sh4 = reinterpret_cast<const float4*>(a.shift + o0);
@@ -807,9 +754,9 @@ conv_tc_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
       } else if (g.out_mode == CT_OUT_NHWC) {
         if (a.residual) {
           const uint4* rp = reinterpret_cast<const uint4*>(a.residual + (size_t)p * g.ld_res + o0);
-          const uint4 ra = ldg_nc16(rp), rb = ldg_nc16(rp + 1);
+          const uint4 ra = ldg_nc16(rp), rb2 = ldg_nc16(rp + 1);
           const __nv_bfloat162* ha = reinterpret_cast<const __nv_bfloat162*>(&ra);
-          const __nv_bfloat162* hb = reinterpret_cast<const __nv_bfloat162*>(&rb);
+          const __nv_bfloat162* hb = reinterpret_cast<const __nv_bfloat162*>(&rb2);
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
             const float2 fa = __bfloat1622float2(ha[j]), fb = __bfloat1622float2(hb[j]);
@@ -865,371 +812,9 @@ conv_tc_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
           if (o0 + j < g.C_out) op[(size_t)j * HWo] = v[j];
       }
     }
-  } else if (lane == 0) {
-    // =========================== MMA issuer (one thread) ===========================
-    const uint32_t idesc = make_idesc(a.n_tile);
-    for (int s = 0; s < a.k_slices; ++s) {
-      const int stage = s % S;
-      const uint32_t ph = (uint32_t)(s / S) & 1u;
-      mbar_wait(full_bar(stage), ph);
-      if (a.fence_mma) fence_proxy_async();      // the producers' st.shared (acquired through the barrier) -> async proxy
-      tc_fence_after();
-      const uint64_t ad = make_sdesc(sA + stage * a_stage_bytes);
-      const uint64_t bd = make_sdesc(sB + stage * b_stage_bytes);
-      if constexpr (X3) {
-        const uint64_t ad_lo = make_sdesc(sA + stage * a_stage_bytes + A_STAGE_BYTES);
-        const uint64_t bd_lo = make_sdesc(sB + stage * b_stage_bytes + b_tile_bytes);
-#pragma unroll
-        for (int k = 0; k < TC_BK / 16; ++k) {      // small cross terms first, then the hi x hi term
-          tc_mma(tmem_base, ad_lo + 2ull * k, bd + 2ull * k, idesc, (s > 0 || k > 0) ? 1u : 0u);
-          tc_mma(tmem_base, ad + 2ull * k, bd_lo + 2ull * k, idesc, 1u);
-          tc_mma(tmem_base, ad + 2ull * k, bd + 2ull * k, idesc, 1u);
-        }
-      } else {
-#pragma unroll
-        for (int k = 0; k < TC_BK / 16; ++k)
-          tc_mma(tmem_base, ad + 2ull * k, bd + 2ull * k, idesc, (s > 0 || k > 0) ? 1u : 0u);
-      }
-      tc_commit(empty_bar(stage));     // frees this smem stage when the MMAs above have read it
-    }
-    tc_commit(tmem_full_bar);           // accumulator complete -> epilogue
-    tc_stamp(trace, 4);
+    __syncthreads();
   }
-
-  tc_fence_before();
-  __syncthreads();
   if (tid == 0) tc_stamp(trace, 6);
-  if (warp == 8) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)a.tmem_cols)
-                 : "memory");
-  }
-}
-
-// =====================================================================================================================
-// Persistent DCNv2 kernel (CT_A_DCN_WIN layers with a single N tile, bf16 NHWC output): one CTA per SM walks its share
-// of the 8x16-pixel output patches.  What the per-tile kernel above spends outside its slice loop -- TMEM allocation,
-// barrier init, the sampling-table build behind an L2 round trip for `om`, the window TMA, the epilogue: 12 k of 30 k
-// cycles per tile (tools/tc_trace.py) -- is taken off the critical path:
-//   * the window of unit u+2 (unit = tile x 64-channel chunk) is requested when unit u is finished: two windows in
-//     flight, a whole unit (9 slices) of latency cover;
-//   * the sampling table of tile t+1 is built by the producers one tap per slice while they sample tile t
-//     (its `om` values fetched one slice ahead), into the other of two table buffers;
-//   * two TMEM accumulators: four dedicated epilogue warps drain tile t while the producers / MMA work on tile t+1.
-//   * the window is requested ROW BY ROW, two rows per slice of the previous unit: one 43 KB request occupied the TMA
-//     unit for ~5000 cycles and the per-slice weight copies queued behind it (a 5000-cycle bubble at every tile
-//     boundary in the first version of this kernel, profiles/r02_tc_trace_persist.txt).
-//   * every TMA request (weight tile per slice, window rows) is issued by a DEDICATED warp: issuing a bulk copy costs the
-//     issuing thread hundreds of cycles, and with the requests on producer thread 0 its warp was the slowest of every
-//     slice (A written 1700 cycles after the stage was acquired, fine-grained trace in profiles/r02_tc_trace_persist.txt).
-// Warps 0-15 producers (sampling + table), warp 16 MMA issuer, warps 17-20 epilogue, warp 21 TMA issuer.
-// =====================================================================================================================
-constexpr int DP_PWARPS = 16;            // producer warps: a slice is a latency chain per warp (table LDS -> 16 LDS -> blend ->
-                                         // STS -> fence -> arrive, ~1100-1500 cycles with 4 rows per thread): 16 warps x 2 rows
-constexpr int DP_PRODUCERS = DP_PWARPS * 32;
-constexpr int DP_NROW = TC_BM * 8 / DP_PRODUCERS;     // A-tile rows per producer thread per K slice (2)
-constexpr int DP_THREADS = DP_PRODUCERS + 32 + 128 + 32 + 128;   // + MMA warp + 4 epilogue warps + TMA warp + 4 table warps
-constexpr int DP_SA = 3;                 // A/B stages
-
-__device__ __forceinline__ void dp_tile_origin(const TcArgs& a, int tile, int& b, int& ty, int& tx) {
-  const int tpi = a.tiles_x * a.tiles_y;
-  b = tile / tpi;
-  const int t = tile - b * tpi;
-  ty = t / a.tiles_x;
-  tx = t - ty * a.tiles_x;
-}
-
-__global__ void __launch_bounds__(DP_THREADS, 1)
-dcn_persist_kernel(const TcArgs a, const int tiles_total, const __grid_constant__ CUtensorMap tmap) {
-  extern __shared__ __align__(1024) unsigned char smem_dyn[];
-  unsigned char* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
-  const ConvGeom& g = a.g;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  unsigned long long* const trace = tc_trace_ptr();
-  const uint32_t b_tile_bytes = (uint32_t)a.n_tile * 128u;
-  const uint32_t win_stride = (a.win_bytes + 127u) & ~127u;
-  const uint32_t smem_base = smem_u32(smem);
-  const uint32_t sA = smem_base;
-  const uint32_t sB = sA + DP_SA * A_STAGE_BYTES;
-  const uint32_t sWin = sB + DP_SA * b_tile_bytes;                       // 1024-aligned (both terms are)
-  const uint32_t off_tab = DP_SA * A_STAGE_BYTES + DP_SA * b_tile_bytes + 2u * win_stride;
-  DcnWinEntry* tabs = reinterpret_cast<DcnWinEntry*>(smem + off_tab);    // [2][9][128]
-  const uint32_t off_bar = off_tab + 2u * 9u * TC_BM * 16u;
-  const uint32_t bars = smem_base + off_bar;
-  auto full_bar = [&](int s) { return bars + 8u * s; };
-  auto empty_bar = [&](int s) { return bars + 8u * (DP_SA + s); };
-  auto win_full = [&](int i) { return bars + 8u * (2 * DP_SA + i); };
-  auto acc_full = [&](int i) { return bars + 8u * (2 * DP_SA + 2 + i); };
-  auto acc_empty = [&](int i) { return bars + 8u * (2 * DP_SA + 4 + i); };
-  auto win_empty = [&](int i) { return bars + 8u * (2 * DP_SA + 6 + i); };
-  auto tab_full = [&](int i) { return bars + 8u * (2 * DP_SA + 8 + i); };
-  auto tab_empty = [&](int i) { return bars + 8u * (2 * DP_SA + 10 + i); };
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + off_bar + 8 * (2 * DP_SA + 12));
-
-  pdl_trigger();
-  if (tid == 0) {
-    for (int s = 0; s < DP_SA; ++s) { mbar_init(full_bar(s), DP_PWARPS + 1); mbar_init(empty_bar(s), 1); }   // 16 producer warps + the TMA warp's expect_tx arrival
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(win_full(i), 1); mbar_init(acc_full(i), 1); mbar_init(acc_empty(i), 4); mbar_init(win_empty(i), DP_PWARPS);
-      mbar_init(tab_full(i), 4); mbar_init(tab_empty(i), DP_PWARPS);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == DP_PWARPS) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32((const void*)tmem_slot)),
-                 "r"((uint32_t)a.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();
-
-  const int G = gridDim.x;
-  const int nchunks = g.C_in >> 6;
-  const int HWo = g.OH * g.OW;
-  int n_my = 0;                                                          // tiles of this CTA
-  if ((int)blockIdx.x < tiles_total) n_my = (tiles_total - 1 - (int)blockIdx.x) / G + 1;
-  const int n_units = n_my * nchunks;
-
-  if (warp < DP_PWARPS) {
-    // ======================================= producers =======================================
-    const int q = tid & 7, r0 = tid >> 3;                                // rows r0 + 64 i, i < DP_NROW
-    const uint32_t swz = (uint32_t)((q ^ (r0 & 7)) << 4);
-    const uint32_t pitch = (uint32_t)a.win_pw * 128u;
-    const int gdx = g.ld_in, gdy = g.W * g.ld_in;
-    // Nothing but the slice loop lives here: `fence.proxy.async` compiles to MEMBAR.ALL.CTA + FENCE.VIEW.ASYNC, and the
-    // MEMBAR waits for every outstanding load of the thread, so a prefetch of the next tile's `om` floats in flight across
-    // it cost the warp a full L2 round trip per slice.  The records are built by the table warps below.
-    int s = 0;
-    for (int t = 0; t < n_my; ++t) {
-      const DcnWinEntry* tab_cur = tabs + (t & 1) * 9 * TC_BM;
-      mbar_wait(tab_full(t & 1), (uint32_t)(t >> 1) & 1u);
-      for (int ch = 0; ch < nchunks; ++ch) {
-        const int u = t * nchunks + ch;
-        const uint32_t s_win = sWin + (uint32_t)(u & 1) * win_stride;
-        mbar_wait(win_full(u & 1), (uint32_t)(u >> 1) & 1u);
-        for (int tap = 0; tap < 9; ++tap, ++s) {
-          const int stage = s % DP_SA;
-          const uint32_t ph = (uint32_t)(s / DP_SA) & 1u;
-          mbar_wait(empty_bar(stage), ph ^ 1u);
-          if (tid == 0 && s < 60) tc_stamp(trace, 16 + 4 * s);
-          const DcnWinEntry* tab = tab_cur + tap * TC_BM + r0;
-          uint4 e4[DP_NROW], v[DP_NROW][4];
-#pragma unroll
-          for (int i = 0; i < DP_NROW; ++i) e4[i] = *reinterpret_cast<const uint4*>(&tab[64 * i]);
-#pragma unroll
-          for (int i = 0; i < DP_NROW; ++i) {
-            const uint32_t meta = e4[i].y;
-            if (meta & WIN_IN) {
-              const uint32_t base = s_win + ((meta & 0xffffu) << 4) + (uint32_t)(q << 4);
-              const uint32_t dx = (meta & WIN_DX) ? 128u : 0u, dy = (meta & WIN_DY) ? pitch : 0u;
-              v[i][0] = lds16(base); v[i][1] = lds16(base + dx);
-              v[i][2] = lds16(base + dy); v[i][3] = lds16(base + dy + dx);
-            } else {
-              const __nv_bfloat16* p00 = a.x + ((int)e4[i].x + (ch << 6) + (q << 3));
-              const int dx = (meta & WIN_DX) ? gdx : 0, dy = (meta & WIN_DY) ? gdy : 0;
-              v[i][0] = ldg_nc16(p00); v[i][1] = ldg_nc16(p00 + dx);
-              v[i][2] = ldg_nc16(p00 + dy); v[i][3] = ldg_nc16(p00 + dy + dx);
-            }
-          }
-          const uint32_t dst = sA + stage * A_STAGE_BYTES + (uint32_t)r0 * 128u + swz;
-#pragma unroll
-          for (int i = 0; i < DP_NROW; ++i) {
-            const uint32_t w0 = __byte_perm(e4[i].z, 0, 0x1010), w1 = __byte_perm(e4[i].z, 0, 0x3232);
-            const uint32_t w2 = __byte_perm(e4[i].w, 0, 0x1010), w3 = __byte_perm(e4[i].w, 0, 0x3232);
-            uint4 o;
-            o.x = bmul2(v[i][0].x, w0); o.y = bmul2(v[i][0].y, w0); o.z = bmul2(v[i][0].z, w0); o.w = bmul2(v[i][0].w, w0);
-            o.x = bfma2(v[i][1].x, w1, o.x); o.y = bfma2(v[i][1].y, w1, o.y); o.z = bfma2(v[i][1].z, w1, o.z); o.w = bfma2(v[i][1].w, w1, o.w);
-            o.x = bfma2(v[i][2].x, w2, o.x); o.y = bfma2(v[i][2].y, w2, o.y); o.z = bfma2(v[i][2].z, w2, o.z); o.w = bfma2(v[i][2].w, w2, o.w);
-            o.x = bfma2(v[i][3].x, w3, o.x); o.y = bfma2(v[i][3].y, w3, o.y); o.z = bfma2(v[i][3].z, w3, o.z); o.w = bfma2(v[i][3].w, w3, o.w);
-            sts16(dst + i * 8192u, o);
-          }
-          if (!a.fence_mma) fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(full_bar(stage));
-          if (tid == 0 && s < 60) tc_stamp(trace, 16 + 4 * s + 1);
-        }
-        if (lane == 0) mbar_arrive(win_empty(u & 1));                    // this warp is done with the unit's window
-      }
-      if (lane == 0) mbar_arrive(tab_empty(t & 1));                      // ... and with the tile's table
-    }
-  } else if (warp >= DP_PWARPS + 6) {
-    // ======================================= table warps: one thread per A-tile row =======================================
-    // Records of tile t into table t & 1, up to two tiles ahead of the producers.  A record is (global offset of corner 00,
-    // window offset | flags, 4 bf16 corner weights with the modulation mask folded in); see conv_tc_kernel's window path.
-    const int trow = tid - (DP_PWARPS + 6) * 32;
-    for (int t = 0; t < n_my; ++t) {
-      const int tile = (int)blockIdx.x + t * G;
-      int b, ty, tx;
-      dp_tile_origin(a, tile, b, ty, tx);
-      const int oy = ty * 8 + (trow >> 4), ox = tx * 16 + (trow & 15);
-      const bool ok = oy < g.OH && ox < g.OW;
-      const int img = b * g.H * g.W;
-      const int wy0 = ty * 8 - 1 - a.win_m, wx0 = tx * 16 - 1 - a.win_m;
-      float omv[28];
-#pragma unroll
-      for (int j = 0; j < 28; ++j) omv[j] = 0.f;
-      if (ok) {
-        const float4* om4 = reinterpret_cast<const float4*>(a.om + (size_t)((b * g.OH + oy) * g.OW + ox) * g.ld_om);
-#pragma unroll
-        for (int j = 0; j < 7; ++j) {
-          const float4 f = __ldg(om4 + j);
-          omv[4 * j] = f.x; omv[4 * j + 1] = f.y; omv[4 * j + 2] = f.z; omv[4 * j + 3] = f.w;
-        }
-      }
-      if (t >= 2) mbar_wait(tab_empty(t & 1), (uint32_t)((t - 2) >> 1) & 1u);
-      DcnWinEntry* tab = tabs + (t & 1) * 9 * TC_BM + trow;
-#pragma unroll
-      for (int tap = 0; tap < 9; ++tap) {
-        DcnWinEntry e; e.goff = 0; e.meta = WIN_IN; e.w01 = 0u; e.w23 = 0u;
-        if (ok) {
-          const float py = (float)(oy - 1 + tap / 3) + omv[2 * tap];
-          const float px = (float)(ox - 1 + tap % 3) + omv[2 * tap + 1];
-          const float m = omv[18 + tap];
-          if (py > -1.f && py < (float)g.H && px > -1.f && px < (float)g.W) {
-            const float y0f = floorf(py), x0f = floorf(px);
-            const int y0 = (int)y0f, x0 = (int)x0f;
-            const float ly = py - y0f, lx = px - x0f, hy = 1.f - ly, hx = 1.f - lx;
-            const bool y0ok = y0 >= 0, y1ok = y0 + 1 <= g.H - 1, x0ok = x0 >= 0, x1ok = x0 + 1 <= g.W - 1;
-            const int yc = max(y0, 0), xc = max(x0, 0);
-            e.goff = (img + yc * g.W + xc) * g.ld_in;
-            const bool ddx = x0ok && x1ok, ddy = y0ok && y1ok;
-            const bool inside = y0 >= wy0 && y0 + 1 <= wy0 + a.win_ph - 1 && x0 >= wx0 && x0 + 1 <= wx0 + a.win_pw - 1;
-            const uint32_t woff16 = (uint32_t)((yc - wy0) * a.win_pw + (xc - wx0)) * 8u;
-            e.meta = (inside ? (woff16 | WIN_IN) : 0u) | (ddx ? WIN_DX : 0u) | (ddy ? WIN_DY : 0u);
-            const float w00 = (y0ok && x0ok) ? hy * hx * m : 0.f, w01 = (y0ok && x1ok) ? hy * lx * m : 0.f;
-            const float w10 = (y1ok && x0ok) ? ly * hx * m : 0.f, w11 = (y1ok && x1ok) ? ly * lx * m : 0.f;
-            const __nv_bfloat162 wa = __floats2bfloat162_rn(w00, w01), wb = __floats2bfloat162_rn(w10, w11);
-            e.w01 = *reinterpret_cast<const uint32_t*>(&wa);
-            e.w23 = *reinterpret_cast<const uint32_t*>(&wb);
-          }
-        }
-        tab[tap * TC_BM] = e;
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tab_full(t & 1));
-    }
-  } else if (warp == DP_PWARPS + 5) {
-    // ======================================= TMA issuer =======================================
-    if (lane == 0 && n_my > 0) {
-    // window of unit u, rows [ry0, ry1): one TMA request per row (tid 0 only); the first request arms the barrier
-    auto issue_window_rows = [&](int u, int ry0, int ry1) {
-      const int t = u / nchunks, ch = u - t * nchunks;
-      int b, ty, tx;
-      dp_tile_origin(a, (int)blockIdx.x + t * G, b, ty, tx);
-      if (ry0 == 0) mbar_arrive_expect_tx(win_full(u & 1), a.win_bytes);
-      const uint32_t row_bytes = (uint32_t)a.win_pw * 128u;
-      for (int ry = ry0; ry < ry1 && ry < a.win_ph; ++ry)
-        tma_4d(sWin + (uint32_t)(u & 1) * win_stride + (uint32_t)ry * row_bytes, &tmap, ch << 6, tx * 16 - 1 - a.win_m,
-               ty * 8 - 1 - a.win_m + ry, b, win_full(u & 1));
-    };
-      issue_window_rows(0, 0, a.win_ph);
-      int s = 0;
-      for (int u = 0; u < n_units; ++u) {
-        const int ch = u % nchunks;
-        for (int tap = 0; tap < 9; ++tap, ++s) {
-          const int stage = s % DP_SA;
-          const uint32_t ph = (uint32_t)(s / DP_SA) & 1u;
-          mbar_wait(empty_bar(stage), ph ^ 1u);
-          mbar_arrive_expect_tx(full_bar(stage), b_tile_bytes);        // the weight tile first: the MMA of this slice waits for it
-          bulk_g2s(sB + stage * b_tile_bytes, a.w + (size_t)(ch * 9 + tap) * a.n_tile * TC_BK, b_tile_bytes, full_bar(stage));
-          // next unit's window into the other buffer, three rows per slice from tap 3 on: issuing a request costs this
-          // thread ~100+ cycles, and 15 of them ahead of the first weight tiles of a unit stalled every tile boundary by
-          // ~4000 cycles.  This warp runs at most DP_SA slices ahead of the producers, so by tap 3 they have released
-          // the buffer (unit u - 1) and the wait below does not block.
-          if (u + 1 < n_units && tap >= 3) {
-            if (tap == 3 && u >= 1) mbar_wait(win_empty((u + 1) & 1), (uint32_t)((u - 1) >> 1) & 1u);
-            issue_window_rows(u + 1, 3 * (tap - 3), 3 * (tap - 3) + 3);
-          }
-        }
-      }
-    }
-  } else if (warp == DP_PWARPS) {
-    // ======================================= MMA issuer =======================================
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc(a.n_tile);
-      int s = 0;
-      for (int t = 0; t < n_my; ++t) {
-        const int ai = t & 1;
-        mbar_wait(acc_empty(ai), ((uint32_t)(t >> 1) & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(ai * a.n_tile);
-        for (int sl = 0; sl < 9 * nchunks; ++sl, ++s) {
-          const int stage = s % DP_SA;
-          const uint32_t ph = (uint32_t)(s / DP_SA) & 1u;
-          mbar_wait(full_bar(stage), ph);
-          if (a.fence_mma) fence_proxy_async();
-          tc_fence_after();
-          if (s < 60) tc_stamp(trace, 16 + 4 * s + 2);
-          const uint64_t ad = make_sdesc(sA + stage * A_STAGE_BYTES);
-          const uint64_t bd = make_sdesc(sB + stage * b_tile_bytes);
-#pragma unroll
-          for (int k = 0; k < TC_BK / 16; ++k)
-            tc_mma(d_tmem, ad + 2ull * k, bd + 2ull * k, idesc, (sl > 0 || k > 0) ? 1u : 0u);
-          tc_commit(empty_bar(stage));
-          if (s < 60) tc_stamp(trace, 16 + 4 * s + 3);
-        }
-        tc_commit(acc_full(ai));
-      }
-    }
-  } else {
-    // ======================================= epilogue warps 17..20 (warp id % 4 = TMEM lane quarter) =======================================
-    const int wq = warp & 3;                          // TMEM lane quarter this warp may read (warp id % 4)
-    const int row = wq * 32 + lane;
-    for (int t = 0; t < n_my; ++t) {
-      const int ai = t & 1;
-      int b, ty, tx;
-      dp_tile_origin(a, (int)blockIdx.x + t * G, b, ty, tx);
-      const int oy = ty * 8 + (row >> 4), ox = tx * 16 + (row & 15);
-      const bool p_ok = oy < g.OH && ox < g.OW;
-      const size_t p = ((size_t)b * g.OH + oy) * g.OW + ox;
-      mbar_wait(acc_full(ai), (uint32_t)(t >> 1) & 1u);
-      tc_fence_after();
-      const uint32_t t_lane = tmem_base + ((uint32_t)(wq * 32) << 16) + (uint32_t)(ai * a.n_tile);
-      for (int col = 0; col < a.n_tile; col += 16) {
-        uint32_t r[16];
-        tc_ld16(t_lane + (uint32_t)col, r);
-        if (!p_ok || col >= g.C_out) continue;
-        float v[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]);
-        if (a.shift) {
-          const float4* sh4 = reinterpret_cast<const float4*>(a.shift + col);
-#pragma unroll
-          for (int j4 = 0; j4 < 4; ++j4) {
-            const float4 sh = __ldg(sh4 + j4);
-            v[4 * j4] += sh.x; v[4 * j4 + 1] += sh.y; v[4 * j4 + 2] += sh.z; v[4 * j4 + 3] += sh.w;
-          }
-        }
-        if (g.relu) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
-        }
-        uint4 oa, ob;
-        __nv_bfloat162* pa = reinterpret_cast<__nv_bfloat162*>(&oa);
-        __nv_bfloat162* pb = reinterpret_cast<__nv_bfloat162*>(&ob);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          pa[j] = __floats2bfloat162_rn(v[2 * j], v[2 * j + 1]);
-          pb[j] = __floats2bfloat162_rn(v[8 + 2 * j], v[8 + 2 * j + 1]);
-        }
-        uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(a.out) + p * g.ld_out + col);
-        op[0] = oa; op[1] = ob;
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(acc_empty(ai));
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == DP_PWARPS) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)a.tmem_cols) : "memory");
-  }
 }
 
 typedef CUresult (*TmapEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -1242,12 +827,35 @@ int tc_set_trace(void* buf) {
   return cudaMemcpyToSymbol(g_tc_trace, &p, sizeof(p)) == cudaSuccess ? CT_OK : CT_ERR_CUDA;
 }
 
+template <bool X3, int N>
+static int launch_tc(dim3 grid, size_t smem, cudaStream_t st, const TcArgs& a, const CUtensorMap& tmap) {
+  int dev = 0;
+  cudaGetDevice(&dev);
+  static thread_local unsigned long long attr_set_mask = 0;      // the attribute is per device
+  if (dev >= 64 || !((attr_set_mask >> dev) & 1ull)) {
+    CT_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<X3, N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024)));
+    if (dev < 64) attr_set_mask |= 1ull << dev;
+  }
+  CT_CUDA_OK(launch_kernel(conv_tc_kernel<X3, N>, grid, dim3(TC_THREADS), smem, st, true, a, tmap));
+  return after_launch();
+}
+
+template <bool X3>
+static int launch_tc_n(int n_tile, dim3 grid, size_t smem, cudaStream_t st, const TcArgs& a, const CUtensorMap& tmap) {
+  switch (n_tile) {
+#define CTB_TC_CASE(n) case n: return launch_tc<X3, n>(grid, smem, st, a, tmap);
+    CTB_TC_CASE(16) CTB_TC_CASE(32) CTB_TC_CASE(48) CTB_TC_CASE(64) CTB_TC_CASE(80) CTB_TC_CASE(96) CTB_TC_CASE(112)
+    CTB_TC_CASE(128) CTB_TC_CASE(144) CTB_TC_CASE(160) CTB_TC_CASE(176) CTB_TC_CASE(192) CTB_TC_CASE(208)
+    CTB_TC_CASE(224) CTB_TC_CASE(240) CTB_TC_CASE(256)
+#undef CTB_TC_CASE
+  }
+  return fail(CT_ERR_INVALID, "conv_tc: unsupported n_tile%s (%ld)", "", (long)n_tile);
+}
+
 int conv_forward_tc(const ct_conv_desc* d, cudaStream_t st) {
   const bool x3 = d->engine == CT_ENGINE_TCGEN05_X3;     // fp32 activations, bf16 hi/lo split operands
   TcArgs a;
   a.g = make_geom(d);
-  static const int fence_mma_env = getenv("CTB_TC_FENCE_MMA") ? atoi(getenv("CTB_TC_FENCE_MMA")) : 1;
-  a.fence_mma = fence_mma_env;
   const ConvGeom& g = a.g;
   if (g.C_in % 8 != 0 || g.ld_in % 8 != 0)
     return fail(CT_ERR_INVALID, "conv_tc: C_in and ld_in must be multiples of 8%s (%ld,%ld)", "", g.C_in, g.ld_in);
@@ -1287,58 +895,38 @@ int conv_forward_tc(const ct_conv_desc* d, cudaStream_t st) {
   a.win_pw = 16 + 2 * a.win_m + 3;
   a.win_ph = 8 + 2 * a.win_m + 3;
   a.win_bytes = (uint32_t)(a.win_pw * a.win_ph * 128);
-  int cols = 32;
-  while (cols < n_tile) cols <<= 1;
-  a.tmem_cols = cols;
   const size_t stage_bytes = (size_t)(x3 ? 2 : 1) * (A_STAGE_BYTES + n_tile * 128);
+  const size_t staging = (size_t)TC_BM * TC_EPI_PITCH * 4;      // <= one stage (16 KB + n_tile x 128 B)
+  auto region0_for = [&](int stg) { return ((size_t)stg * stage_bytes > staging ? (size_t)stg * stage_bytes : staging); };
   auto smem_for = [&](int stg) {
-    return (size_t)stg * stage_bytes + (2 * stg + 2) * 8 + 32 +
+    return region0_for(stg) + (2 * stg + 1) * 8 + 32 +
            (d->a_mode == CT_A_DCN ? 9 * TC_BM * sizeof(DcnEntry) : 0) +
            (win ? 9 * TC_BM * sizeof(DcnWinEntry) + 128 + a.win_bytes : 0) + 1024;
   };
-  int stages = 4;                                   // keep >= 2 CTAs per SM when the tile allows it
-  if (smem_for(stages) > 112 * 1024) stages = 3;
+  // The MMAs of a slice overlap the gather of the next one, so two stages keep the tensor cores fed; a third covers
+  // the weight-tile copy.  Narrow tiles keep two CTAs per SM (<= 113 KB each).
+  int stages = 3;
+  if (smem_for(stages) > 113 * 1024 && smem_for(2) <= 113 * 1024) stages = 2;
   if (d->a_mode == CT_A_DCN) {
-    // the DCN gather, not the MMA, paces the pipeline: fewer stages leave more of the SM's 228 KB to L1, which
+    // the DCN gather, not the MMA, paces the pipeline: fewer stages leave more of the SM's shared memory to L1, which
     // the bilinear corner reads (each input pixel is touched ~36 times) depend on
     static const int dcn_stages = getenv("CTB_TC_DCN_STAGES") ? atoi(getenv("CTB_TC_DCN_STAGES")) : 2;
     if (dcn_stages >= 2 && dcn_stages < stages) stages = dcn_stages;
   }
   if (win) {
-    // two CTAs per SM: table 18 KB + window 43 KB + stages x (16 KB + n_tile x 128 B) must stay under ~113 KB
     static const int win_stages = getenv("CTB_TC_WIN_STAGES") ? atoi(getenv("CTB_TC_WIN_STAGES")) : 0;
     stages = 2;
-    if (smem_for(2) > 113 * 1024) {                  // one CTA per SM anyway (wide N tile): deepen the pipeline instead
-      stages = 4;
-      while (stages > 2 && smem_for(stages) > 200 * 1024) --stages;
-    }
     if (win_stages >= 2) stages = win_stages;
-    if (smem_for(stages) > 200 * 1024)
-      return fail(CT_ERR_UNSUPPORTED, "conv_tc: DCN window does not fit in shared memory%s (%ld)", "", (long)smem_for(stages));
   }
-  if (x3) {                                         // one CTA per SM (register-heavy producers): as deep as fits
-    stages = 4;
-    while (stages > 2 && smem_for(stages) > 200 * 1024) --stages;
-    if (d->a_mode == CT_A_DCN && stages > 3) stages = 3;
-    if (smem_for(stages) > 224 * 1024)
-      return fail(CT_ERR_UNSUPPORTED, "conv_tc x3: tile does not fit in shared memory%s (%ld)", "", (long)n_tile);
-  }
+  while (stages > 2 && smem_for(stages) > 227 * 1024) --stages;
+  if (smem_for(stages) > 227 * 1024)
+    return fail(CT_ERR_UNSUPPORTED, "conv_tc: tile does not fit in shared memory%s (%ld)", "", (long)smem_for(stages));
   if (stages > a.k_slices) stages = a.k_slices;
   a.stages = stages;
+  a.region0 = (uint32_t)region0_for(stages);
   const size_t smem = smem_for(stages);
-  {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    static thread_local unsigned long long attr_set_mask = 0;      // the attribute is per device
-    if (dev >= 64 || !((attr_set_mask >> dev) & 1ull)) {
-      CT_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(200 * 1024)));
-      CT_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024)));
-      if (dev < 64) attr_set_mask |= 1ull << dev;
-    }
-  }
   const int n_tiles = (g.C_out + n_tile - 1) / n_tile;
-  // Optional 2-D pixel patches (CTB_TC_TILE2D=1) when they tile the map exactly.  Measured on B200: no gain -- the
-  // DCN gather at 128x128 went 150 -> 156 us, level1 184 -> 207 us -- the gather is not L1-capacity bound; off.
+  // Optional 2-D pixel patches (CTB_TC_TILE2D=1) when they tile the map exactly; off by default.
   static const int tile2d_env = getenv("CTB_TC_TILE2D") ? atoi(getenv("CTB_TC_TILE2D")) : 0;
   a.tiles_x = a.tiles_y = 0;
   int m_tiles = (g.P_out + TC_BM - 1) / TC_BM;
@@ -1364,49 +952,8 @@ int conv_forward_tc(const ct_conv_desc* d, cudaStream_t st) {
                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (cr != CUDA_SUCCESS) return fail(CT_ERR_CUDA, "conv_tc: cuTensorMapEncodeTiled failed%s (%ld)", "", (long)cr);
   }
-  static const int persist_env = getenv("CTB_DCN_PERSIST") ? atoi(getenv("CTB_DCN_PERSIST")) : 1;
-  if (win && persist_env && n_tiles == 1 && g.out_mode == CT_OUT_NHWC && d->residual == nullptr && g.C_out % 16 == 0 &&
-      g.C_out == n_tile && ((uintptr_t)d->shift & 15) == 0) {
-    // persistent form: one CTA per SM, two windows + two tables + two accumulators (see dcn_persist_kernel)
-    const size_t win_stride = ((size_t)a.win_bytes + 127) & ~(size_t)127;
-    const size_t psmem = (size_t)DP_SA * (A_STAGE_BYTES + n_tile * 128) + 2 * win_stride + 2 * 9 * TC_BM * sizeof(DcnWinEntry) +
-                         8 * (2 * DP_SA + 12) + 16 + 1024;
-    if (psmem <= 227 * 1024) {
-      int cols2 = 32;
-      while (cols2 < 2 * n_tile) cols2 <<= 1;
-      a.tmem_cols = cols2;
-      int dev = 0, sms = 148;
-      cudaGetDevice(&dev);
-      static thread_local unsigned long long pattr_mask = 0;
-      static thread_local int sms_of[64] = {0};
-      if (dev >= 64 || !((pattr_mask >> dev) & 1ull)) {
-        CT_CUDA_OK(cudaFuncSetAttribute(dcn_persist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024)));
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        if (dev < 64) { pattr_mask |= 1ull << dev; sms_of[dev] = sms; }
-      } else {
-        sms = sms_of[dev];
-      }
-      const int pgrid = m_tiles < sms ? m_tiles : sms;
-      CUtensorMap tmap_row;                                  // same tensor, one window ROW per request
-      {
-        TmapEncodeFn enc = tmap_encode_fn();
-        const cuuint64_t dims[4] = {(cuuint64_t)g.C_in, (cuuint64_t)g.W, (cuuint64_t)g.H, (cuuint64_t)g.B};
-        const cuuint64_t strides[3] = {(cuuint64_t)g.ld_in * 2, (cuuint64_t)g.W * g.ld_in * 2, (cuuint64_t)g.H * g.W * g.ld_in * 2};
-        const cuuint32_t box[4] = {64, (cuuint32_t)a.win_pw, 1, 1};
-        const cuuint32_t estr[4] = {1, 1, 1, 1};
-        const CUresult cr = enc(&tmap_row, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(d->x), dims, strides, box, estr,
-                                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (cr != CUDA_SUCCESS) return fail(CT_ERR_CUDA, "conv_tc: cuTensorMapEncodeTiled failed%s (%ld)", "", (long)cr);
-      }
-      CT_CUDA_OK(launch_kernel(dcn_persist_kernel, dim3(pgrid), dim3(DP_THREADS), psmem, st, true, a, m_tiles, tmap_row));
-      return after_launch();
-    }
-  }
   dim3 grid(m_tiles, n_tiles);
-  if (x3) CT_CUDA_OK(launch_kernel(conv_tc_kernel<true>, grid, dim3(TC_THREADS), smem, st, true, a, tmap));
-  else CT_CUDA_OK(launch_kernel(conv_tc_kernel<false>, grid, dim3(TC_THREADS), smem, st, true, a, tmap));
-  return after_launch();
+  return x3 ? launch_tc_n<true>(n_tile, grid, smem, st, a, tmap) : launch_tc_n<false>(n_tile, grid, smem, st, a, tmap);
 }
 
 }  // namespace ctb

@@ -455,7 +455,8 @@ extern "C" int ct_pack_stem_input_f32(const float* img, const float* pre_img, co
 
 static inline int ew_blocks(size_t total) {
   size_t b = (total + 255) / 256;
-  return (int)(b < 148 * 16 ? (b ? b : 1) : 148 * 16);
+  const size_t cap = (size_t)device_sm_count() * 16;
+  return (int)(b < cap ? (b ? b : 1) : cap);
 }
 
 extern "C" int ct_maxpool2(const void* x, void* out, int32_t dtype, int32_t B, int32_t H, int32_t W,
@@ -526,7 +527,7 @@ extern "C" int ct_upsample_add(const void* x, const void* skip, const float* w, 
     // all phases of an input pixel in one CTA (L1 reuse of the taps); grid: a few CTAs per SM, grid-stride over pixels
     const int per_cta = (256 / cv) / (f * f);
     long gx = ((long)B * H * W + per_cta - 1) / per_cta;
-    if (gx > 148 * 8) gx = 148 * 8;
+    if (gx > device_sm_count() * 8) gx = device_sm_count() * 8;
     if (dtype == CT_F32)
       upsample_add_warp_kernel<float><<<(int)gx, 256, 0, st>>>(
           (const float*)x, (const float*)skip, w, (float*)out, B, H, W, C, f, ld_in, ld_skip, ld_out);
@@ -540,7 +541,7 @@ extern "C" int ct_upsample_add(const void* x, const void* skip, const float* w, 
     // phase kernel: grid.y = f*f phases, grid.x sized so that all phases together fill the GPU a few times over
     const int slots = 256 / cv;
     int gx = (int)(((size_t)B * H * W + slots - 1) / slots);
-    const int cap = (148 * 8 + f * f - 1) / (f * f);
+    const int cap = (device_sm_count() * 8 + f * f - 1) / (f * f);
     if (gx > cap) gx = cap;
     if (gx < 1) gx = 1;
     dim3 grid(gx, f * f);

@@ -321,7 +321,8 @@ using namespace ctb;
 
 static inline int sw_blocks(size_t total) {
   size_t b = (total + 255) / 256;
-  return (int)(b < 148 * 16 ? (b ? b : 1) : 148 * 16);
+  const size_t cap = (size_t)device_sm_count() * 16;
+  return (int)(b < cap ? (b ? b : 1) : cap);
 }
 
 extern "C" int ct_flip_merge(const float* in2, float* out, int32_t C, int32_t H, int32_t W, const int32_t* perm,

@@ -39,7 +39,7 @@ class DCN(nn.Module):
     self.bias = nn.Parameter(torch.zeros(out_channels))
     self.conv_offset_mask = nn.Conv2d(in_channels, deformable_groups * 3 * kh * kw, kernel_size=(kh, kw),
                                       stride=1, padding=1, bias=True)
-    self.precision = 'bf16'     # 'bf16' (tcgen05) or 'fp32' (SIMT, reference accuracy)
+    self.precision = 'bf16'     # 'bf16' (wgmma) or 'fp32' (SIMT, reference accuracy)
     self._packed = None
     self.reset_parameters()
 
@@ -57,7 +57,8 @@ class DCN(nn.Module):
     return super(DCN, self)._load_from_state_dict(*args, **kwargs)
 
   def _pack(self, device, P):
-    key = (self.precision, str(device), P >= 148 * 128)
+    sms = torch.cuda.get_device_properties(device).multi_processor_count
+    key = (self.precision, str(device), P >= sms * 128)
     if self._packed is not None and self._packed[0] == key:
       return self._packed[1]
     lib = L.lib()
@@ -72,7 +73,7 @@ class DCN(nn.Module):
                                   C.c_void_p(dst.data_ptr())), 'ct_pack_weights')
       return dst.to(device)
     nt_main = min(256, (self.out_channels + 15) // 16 * 16)
-    if eng == L.CT_ENGINE_TCGEN05 and nt_main > 64 and P < 148 * 128:
+    if eng == L.CT_ENGINE_TCGEN05 and nt_main > 64 and P < sms * 128:
       nt_main = 64
     packed = dict(
         n_om=32, n_main=nt_main,
@@ -84,7 +85,7 @@ class DCN(nn.Module):
 
   def forward(self, x):
     if not x.is_cuda:
-      raise RuntimeError('centertrack_b200.DCN runs on a B200 only (no CPU fallback); got a %s tensor'
+      raise RuntimeError('centertrack_b200.DCN runs on an H100 only (no CPU fallback); got a %s tensor'
                          % x.device)
     lib = L.lib()
     B, Cin, H, W = x.shape

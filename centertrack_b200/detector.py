@@ -72,7 +72,7 @@ class Detector(object):
   def _init_device_model(opt):
     """detector.py:26-36: pick the device, build the network, load the checkpoint.  No CPU fallback."""
     if opt.gpus[0] < 0 or not torch.cuda.is_available():
-      raise RuntimeError('centertrack_b200.Detector needs a CUDA device (B200, sm_100a); there is no '
+      raise RuntimeError('centertrack_b200.Detector needs a CUDA device (H100, sm_90a); there is no '
                          'CPU fallback (got --gpus %s)' % getattr(opt, 'gpus_str', opt.gpus))
     opt.device = torch.device('cuda')
     print('Creating model...')

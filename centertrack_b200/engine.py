@@ -15,8 +15,8 @@ on NHWC activations:
     1x1 per head writing the reference-layout fp32 NCHW map (sigmoid / depth transform of
     detector.py:300-308 optionally fused).
 
-precision='bf16'   : bf16 activations, tcgen05 engines (fast path)
-precision='bf16x3' : fp32 activations, tcgen05 gather engine with bf16 hi/lo split operands (three MMAs per product
+precision='bf16'   : bf16 activations, wgmma engines (fast path)
+precision='bf16x3' : fp32 activations, wgmma gather engine with bf16 hi/lo split operands (three MMAs per product
                      term, fp32 accumulate): the tensor-core path that stays within 1e-3 of the reference
 precision='fp32'   : fp32 activations, SIMT engine (reference-accuracy path, <= 1e-3 of the reference)
 """
@@ -105,7 +105,7 @@ class DLA34Engine(object):
     self.engine = {'bf16': L.CT_ENGINE_TCGEN05, 'fp32': L.CT_ENGINE_SIMT, 'bf16x3': L.CT_ENGINE_TCGEN05_X3}[precision]
     self.x3 = (precision == "bf16x3")
     self.dcn_window = bool(int(__import__('os').environ.get('CTB_DCN_WINDOW', '1')))
-    # the persistent window kernel (CTB_DCN_PERSIST, default on) also wins on 128 -> 128 at 64x64 (100 vs 124 us)
+    # CTB_DCN_PERSIST=0: the 128 -> 128 DCN takes the global-memory gather instead of the window sampler
     self.dcn_window_all = bool(int(__import__('os').environ.get('CTB_DCN_PERSIST', '1')))
     self.ntile_cap = int(__import__('os').environ.get('CTB_NTILE_CAP', '256'))
     self.gather_128 = bool(int(__import__('os').environ.get('CTB_GATHER_128', '0')))   # experiment: level3's 3x3 on the gather engine
@@ -118,7 +118,7 @@ class DLA34Engine(object):
     self.head_descs = {}   # head -> final ConvDesc (to toggle the fused activation)
     self.algo_flops = {}   # op name -> flops of the reference layer, where the launch shape carries structural zeros
     self.s2d_named = set() # named intermediates stored space-to-depth ([B, H/2, W/2, (sy, sx, 16)])
-    self.n_sm = 148
+    self.n_sm = torch.cuda.get_device_properties(self.device).multi_processor_count if self.device.type == 'cuda' else 132
     self.debug_sync = bool(int(__import__('os').environ.get('CTB_DEBUG_SYNC', '0')))
     self.use_halo = use_halo and precision == 'bf16'
     # level1 as a 2x2 stride-1 halo convolution over level0's output written space-to-depth (see _build)
@@ -204,7 +204,7 @@ class DLA34Engine(object):
       halo = C_in * 2 * (8 + k - 1 + (1 if C_in == 8 else 0)) * (16 + k - 1) + 1024 * max(1, C_in // 64)
       cpad = (C_out + 15) // 16 * 16
       for nt in ([48] if sum3 else [c for c in (128, 96, 80, 64, 48, 32, 16) if c <= cpad and (c == cpad or cpad % c == 0 or c >= 64)]):
-        if nblk * nt * 32 + 2 * halo + 4096 <= 224 * 1024 and (nt >= 32 or cpad <= 16):
+        if nblk * nt * 32 + 2 * halo + 4096 + 18432 <= 224 * 1024 and (nt >= 32 or cpad <= 16):   # + epilogue staging
           engine, n_tile = L.CT_ENGINE_TCGEN05_HALO, nt
           break
     d = L.ConvDesc()

@@ -234,7 +234,7 @@ class _B200Net(nn.Module):
     """-> [ {head: [B,c,H/4,W/4] fp32} ]  (list of num_stacks=1; base_model.py:73-91).  Raw head
     outputs (no sigmoid), like the reference module."""
     if not x.is_cuda:
-      raise RuntimeError('centertrack_b200 model runs on a B200 only (no CPU fallback); input is on %s'
+      raise RuntimeError('centertrack_b200 model runs on an H100 only (no CPU fallback); input is on %s'
                          % x.device)
     B, _, H, W = x.shape
     eng = self.engine_for(B, H, W, x.device)
@@ -254,7 +254,7 @@ class DLASegB200(_B200Net):
   def __init__(self, num_layers, heads, head_convs, opt=None):
     super(DLASegB200, self).__init__()
     if num_layers != 34:
-      raise NotImplementedError('only DLA-34 (arch dla_34) is on the B200 hot path')
+      raise NotImplementedError('only DLA-34 (arch dla_34) is on the H100 hot path')
     node_type = self._common_init(heads, opt)
     self.base = _dla34_backbone(opt)
     self.dla_up, self.ida_up = _dlaup_neck(node_type)
@@ -280,7 +280,7 @@ class GenericNetworkB200(_B200Net):
     backbone = getattr(opt, 'backbone', 'dla34') if opt is not None else 'dla34'
     neck = getattr(opt, 'neck', 'dlaup') if opt is not None else 'dlaup'
     if backbone != 'dla34' or neck != 'dlaup':
-      raise NotImplementedError('generic arch: only --backbone dla34 --neck dlaup is on the B200 hot path '
+      raise NotImplementedError('generic arch: only --backbone dla34 --neck dlaup is on the H100 hot path '
                                 '(got %s / %s)' % (backbone, neck))
     print('Using generic model with backbone {} and neck {}'.format(backbone, neck))
     node_type = self._common_init(heads, opt)
@@ -304,7 +304,7 @@ class GenericNetworkB200(_B200Net):
 
 def _unsupported(name):
   def make(*a, **k):
-    raise NotImplementedError('arch %r is outside the B200 hot path (dla_34, or generic with --backbone dla34 '
+    raise NotImplementedError('arch %r is outside the H100 hot path (dla_34, or generic with --backbone dla34 '
                               '--neck dlaup): it has no imgpre2feats, i.e. no tracking inputs' % name)
   return make
 

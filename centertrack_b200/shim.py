@@ -1,13 +1,13 @@
 """install(): make the reference's import names resolve to this package, so the reference's own
 `src/demo.py` / `src/test.py` (which do `from detector import Detector`, `from opts import opts`, ...) run
-unchanged on the B200 path.  See INTEGRATION.md.
+unchanged on the H100 path.  See INTEGRATION.md.
 
     import centertrack_b200.shim as shim; shim.install()        # before importing the reference scripts
     # or, DCN only (keep the reference's PyTorch graph, swap its absent CUDA extension):
     shim.install_dcn_only()
 
 How it works.  A `sys.meta_path` finder placed FIRST answers, lazily and only for the leaf modules this package
-replaces, with the B200 implementation:
+replaces, with the H100 implementation:
 
     detector                          -> centertrack_b200.detector      (Detector)
     model.model                       -> centertrack_b200.model         (create_model / load_model / save_model)
@@ -117,7 +117,7 @@ def install_dcn_only():
 
 
 def install():
-  """-> {reference module name: B200 module} of the names that are always replaced."""
+  """-> {reference module name: product module} of the names that are always replaced."""
   _install(_ALWAYS)
   return {name: importlib.import_module(target) for name, target in _ALWAYS.items()}
 

@@ -3,8 +3,8 @@
 The reference's default init collapses the 64-channel feature to ~1e-5 (SURVEY hazard H3), and no
 pretrained checkpoint is available offline, so goldens and benchmarks use a variance-preserving
 He-fan-in init that is a pure function of (state-dict key, shape, seed): the SAME tensors can be
-materialised for the reference model (in the build container, to generate goldens) and for the B200
-model (on the GPU box, where /root/reference does not exist).
+materialised for the reference model (in the build container, to generate goldens) and for the H100
+model (on the GPU machine, where no reference checkout exists).
 
 BatchNorm running statistics come from data/bn_calib_seed<seed>.npz -- the batch statistics each BN
 saw on one synthetic frame pair, recorded once by oracle/calibrate.py (what training-mode BN would have

@@ -1,4 +1,4 @@
-/* ctb200.h -- C ABI of libctb200.so: the B200 (sm_100a) implementation of CenterTrack's
+/* ctb200.h -- C ABI of libctb200.so: the H100 (sm_90a) implementation of CenterTrack's
  * per-frame inference hot path.  Plain C: raw device pointers, sizes, a cudaStream_t passed
  * as void*; every entry point returns 0 on success or a negative ct_status and never throws.
  * No ownership transfer: the caller (the Python shims in centertrack_b200/, which allocate
@@ -48,7 +48,7 @@ typedef enum { CT_F32 = 0, CT_BF16 = 1 } ct_dtype;
 typedef enum {
   CT_A_CONV = 0,  /* plain KxK window, stride/pad */
   CT_A_DCN = 1,   /* 3x3 s1 p1 modulated-deformable bilinear sampling driven by `om` */
-  CT_A_DCN_WIN = 2 /* the same operator on the bf16 tcgen05 engine with the input neighbourhood of each 8x16-pixel
+  CT_A_DCN_WIN = 2 /* the same operator on the bf16 wgmma engine with the input neighbourhood of each 8x16-pixel
                       output patch staged in shared memory by TMA (samples displaced by more than the margin fall
                       back to global memory).  Needs C_in % 64 == 0 and weights packed 64-channel-chunk-major:
                       ct_pack_weights(engine, w', C_out, 64, 3 * C_in / 64, 3, ...) with
@@ -74,8 +74,8 @@ typedef enum {           /* per-launch transform applied to the fp32 NCHW head o
 
 typedef enum {
   CT_ENGINE_SIMT = 0,          /* fp32 FFMA implicit GEMM (reference accuracy; fp32 or bf16 activations) */
-  CT_ENGINE_TCGEN05 = 1,       /* tcgen05 implicit GEMM, A gathered per tap (any stride, DCN) */
-  CT_ENGINE_TCGEN05_HALO = 2,  /* tcgen05, TMA-loaded halo tile, taps by descriptor shift: stride-1 'same'
+  CT_ENGINE_TCGEN05 = 1,       /* wgmma implicit GEMM, A gathered per tap (any stride, DCN) */
+  CT_ENGINE_TCGEN05_HALO = 2,  /* wgmma, TMA-loaded halo tile, taps by descriptor shift: stride-1 'same'
                                   convs with C_in in {8,16,32,48,64,128,192,256} whose weights fit in smem */
   CT_ENGINE_TCGEN05_X3 = 3     /* the gather engine on fp32 activations (dtype CT_F32) with bf16 hi/lo split operands:
                                   D += A_hi B_hi + A_hi B_lo + A_lo B_hi, fp32 accumulate -- ~1e-5 per layer, the
@@ -102,7 +102,7 @@ typedef struct {
   int32_t sig_from;      /* CT_OUT_NHWC_F32: sigmoid applied to channels >= sig_from (DCN mask) */
   float   depth_scale;
   int32_t ld_om;         /* CT_A_DCN: pixel stride of `om` (fp32 NHWC, >= 27) */
-  int32_t n_tile;        /* tcgen05: output-channel tile (multiple of 16, <= 256); 0 = auto */
+  int32_t n_tile;        /* wgmma engines: output-channel tile (multiple of 16, <= 256); 0 = auto */
   int32_t epilogue_sum3; /* HALO engine, C_out == 48: out16 = sum over present groups g (bit g set) of
                             relu(acc[16g..16g+15] + shift) -- the three DLA stems (dla.py:307-311) */
   int32_t pad_w1;        /* 0: horizontal padding = pad; else horizontal padding + 1 (the (k,1) / (1,k) convs of
@@ -120,10 +120,10 @@ int64_t ct_packed_weight_bytes(int32_t engine, int32_t C_out, int32_t C_in, int3
                                int32_t n_tile);
 /* Host-side packing.  w_oihw: fp32 [C_out, C_in, KH, KW] (already BN-scale-folded).
  * SIMT engine : fp32 [KH*KW*C_in (k = tap*C_in + c)][C_out padded to 64].
- * tcgen05     : bf16 tiles [n_tiles][k_slices][n_tile rows x 64 k] in the 128B-swizzled
+ * wgmma       : bf16 tiles [n_tiles][k_slices][n_tile rows x 64 k] in the 128B-swizzled
  *               shared-memory image the MMA descriptor expects (one bulk copy per tile).
- * tcgen05 x3  : the same with two tiles per K slice: [hi = bf16(w)][lo = bf16(w - hi)].
- * tcgen05 halo: bf16 [n_tiles][K=16 blocks][2 K-cores][n_tile/8][8 rows][8] (un-swizzled K-major core
+ * wgmma x3    : the same with two tiles per K slice: [hi = bf16(w)][lo = bf16(w - hi)].
+ * wgmma halo  : bf16 [n_tiles][K=16 blocks][2 K-cores][n_tile/8][8 rows][8] (un-swizzled K-major core
  *               matrices); block = (tap, 16 channels), or (ky, tap pair) when C_in == 8. */
 int ct_pack_weights(int32_t engine, const float* w_oihw, int32_t C_out, int32_t C_in, int32_t KH,
                     int32_t KW, int32_t n_tile, void* dst);

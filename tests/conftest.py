@@ -12,7 +12,7 @@ GOLDEN = os.path.join(ROOT, 'tests', 'golden')
 
 
 def pytest_configure(config):
-  config.addinivalue_line('markers', 'gpu: needs a CUDA device (B200); run with -m gpu on the GPU box')
+  config.addinivalue_line('markers', 'gpu: needs a CUDA device (H100); run with -m gpu on a GPU machine')
 
 
 @pytest.fixture(scope='session')
@@ -22,6 +22,6 @@ def golden_dir():
 
 @pytest.fixture(scope='session')
 def built_lib():
-  """Path of libctb200.so, building it (nvcc, sm_100a) if needed."""
+  """Path of libctb200.so, building it (nvcc, sm_90a) if needed."""
   from centertrack_b200 import _lib
   return _lib.build()

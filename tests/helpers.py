@@ -23,13 +23,30 @@ def make_opt(cfg, extra=()):
 
 
 def make_model(cfg, seed=317, extra=()):
-  """B200 model with the deterministic synthetic weights (same tensors the goldens were made with)."""
+  """Product model with the deterministic synthetic weights (same tensors the goldens were made with)."""
   from centertrack_b200.model import create_model
   opt = make_opt(cfg, extra)
   m = create_model(opt.arch, opt.heads, opt.head_conv, opt=opt)
   sd = wt.make_state_dict(m.state_dict(), seed, rename=getattr(m, 'RENAME', ()))
   m.load_state_dict(sd)
   return opt, m, sd
+
+
+def load_generic_golden(golden_dir):
+  """The --arch generic goldens (oracle/gen_golden.py::gen_generic): the hc256 and hc64 tags are stored in two files
+  so that each stays under 1 MB."""
+  g = _NpzDict()
+  for f in ('net_generic_coco_tracking_64x96.npz', 'net_generic_coco_tracking_64x96_hc64.npz'):
+    z = np.load(os.path.join(golden_dir, f))
+    g.update({k: z[k] for k in z.files})
+  return g
+
+
+class _NpzDict(dict):
+  """A dict of arrays with np.load's `.files`."""
+  @property
+  def files(self):
+    return list(self.keys())
 
 
 def decode_inputs(kind, B, C, H, W, seed):

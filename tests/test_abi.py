@@ -1,4 +1,4 @@
-"""The C-ABI library builds for sm_100a, loads without a GPU, and exports every symbol the public
+"""The C-ABI library builds for sm_90a, loads without a GPU, and exports every symbol the public
 header declares (no compute calls here)."""
 import ctypes
 import os
@@ -34,20 +34,21 @@ def test_python_binding_lists_match_header(built_lib):
   _lib.lib()     # argtypes/restype wiring must not raise
 
 
-def test_sass_is_blackwell_native(built_lib):
-  """tcgen05.mma / tcgen05.ld / TMA bulk copy must be in the SASS (UTCHMMA / LDTM / UBLKCP / UTMALDG tensor loads / UTCBAR commits)."""
+def test_sass_is_hopper_native(built_lib):
+  """wgmma / TMA bulk copy / mbarrier must be in the SASS (HGMMA + WARPGROUP fences / UBLKCP / UTMALDG tensor loads /
+  SYNCS mbarrier transactions)."""
   import shutil
   import subprocess
   if shutil.which('cuobjdump') is None:
     import pytest
     pytest.skip('cuobjdump not available')
   sass = subprocess.run(['cuobjdump', '-sass', built_lib], capture_output=True, text=True).stdout
-  for mnemonic in ('UTCHMMA', 'LDTM', 'UBLKCP', 'UTMALDG', 'UTCBAR'):
+  for mnemonic in ('HGMMA', 'WARPGROUP', 'UBLKCP', 'UTMALDG', 'SYNCS'):
     assert mnemonic in sass, mnemonic
 
 
 def test_host_weight_packing_roundtrip(built_lib):
-  """ct_pack_weights (host code, no GPU): SIMT layout k-major; tcgen05 layout = 128B-swizzled tiles."""
+  """ct_pack_weights (host code, no GPU): SIMT layout k-major; tensor-core layout = 128B-swizzled tiles."""
   import numpy as np
   from centertrack_b200 import _lib as L
   lib = L.lib()
@@ -61,7 +62,7 @@ def test_host_weight_packing_roundtrip(built_lib):
   ref = np.zeros((k * k * I, ldw), np.float32)
   ref[:, :O] = w.transpose(2, 3, 1, 0).reshape(k * k * I, O)
   assert np.array_equal(dst.reshape(-1, ldw), ref)
-  # tcgen05: de-swizzle and compare against bf16-rounded weights
+  # tensor-core engine: de-swizzle and compare against bf16-rounded weights
   n_tile = 32
   n = lib.ct_packed_weight_bytes(L.CT_ENGINE_TCGEN05, O, I, k, k, n_tile)
   ks = (k * k * I + 63) // 64

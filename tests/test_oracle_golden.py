@@ -12,7 +12,7 @@ import torch
 
 import ct_oracle as co
 from centertrack_b200 import synthetic as wt
-from helpers import DECODE_CASES, HOST_CASES, decode_inputs, host_case_inputs, make_opt, make_model
+from helpers import DECODE_CASES, HOST_CASES, decode_inputs, host_case_inputs, load_generic_golden, make_opt, make_model
 
 
 @pytest.mark.parametrize('cfg', ['coco_tracking', 'mot', 'nuscenes_ddd', 'coco_pose', 'coco_tracking_conv',
@@ -359,7 +359,7 @@ def test_generic_arch_oracle_and_product_keys_match_reference_golden(tag, extra,
   """--arch generic --backbone dla34 --neck dlaup (generic_network.py:29-107): state-dict keys of the product module
   equal the reference GenericNetwork's, the head width follows opts.py:295 (64 unless --head_conv), and the oracle
   restatement reproduces the reference's outputs and stages."""
-  g = np.load(os.path.join(golden_dir, 'net_generic_coco_tracking_64x96.npz'))
+  g = load_generic_golden(golden_dir)
   opt, model, sd = make_model('coco_tracking', extra=['--arch', 'generic'] + extra)
   assert sorted(sd.keys()) == list(g[tag + '.keys'])
   assert [opt.head_conv[h][0] for h in opt.heads] == list(g[tag + '.head_conv'])
@@ -378,7 +378,7 @@ def test_generic_arch_is_the_dla34_graph_under_other_names(golden_dir):
   """With --head_conv 256 the reference's GenericNetwork and DLASeg(34) agree exactly on the same tensors (recorded by
   the generator), the generic golden equals the dla_34 golden, and the product hands its engine the very state dict
   the dla_34 module does -- so the device plan that runs is the one the dla_34 GPU tests cover."""
-  g = np.load(os.path.join(golden_dir, 'net_generic_coco_tracking_64x96.npz'))
+  g = load_generic_golden(golden_dir)
   d = np.load(os.path.join(golden_dir, 'net_coco_tracking_64x96.npz'))
   assert np.all(g['hc256.max_abs_diff_vs_dla_34'] == 0)
   for h in ('hm', 'reg', 'wh', 'tracking'):

@@ -1,24 +1,9 @@
-"""Drop-in boundary (SURVEY 8b): `centertrack_b200.shim.install()` under the reference's own scripts.  CPU only."""
+"""Drop-in boundary (SURVEY 8b): `centertrack_b200.shim.install()` without the reference on sys.path.  CPU only."""
 import os
 import subprocess
 import sys
 
-import pytest
-
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.environ.get('CT_REF_ROOT', '/root/reference')
-
-
-@pytest.mark.skipif(not os.path.isdir(os.path.join(REF, 'src', 'lib')), reason='reference checkout not present')
-def test_reference_demo_and_test_scripts_run_unchanged_through_the_shim(tmp_path):
-  """The reference's UNMODIFIED src/demo.py::demo(opt) (3 written frames, --save_video --save_results) and
-  src/test.py::prefetch_test(opt) (fake dataset, real DataLoader worker calling Detector.pre_process) with the shim
-  installed: see tests/shim_driver.py for what is asserted (which modules stay the reference's, which are replaced,
-  ret['generic'] frames, saved results, tracking ids).  Runs in a subprocess because it rewires sys.modules."""
-  r = subprocess.run([sys.executable, os.path.join(ROOT, 'tests', 'shim_driver.py'), REF, str(tmp_path)],
-                     capture_output=True, text=True, timeout=600)
-  assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
-  assert 'SHIM OK' in r.stdout
 
 
 def test_shim_standalone_fallbacks_without_the_reference():

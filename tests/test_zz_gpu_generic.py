@@ -1,10 +1,8 @@
-"""-m gpu: `--arch generic --backbone dla34 --neck dlaup` (generic_network.py:29-107) on the B200 against goldens made
+"""-m gpu: `--arch generic --backbone dla34 --neck dlaup` (generic_network.py:29-107) on the H100 against goldens made
 by the reference's own GenericNetwork (tests/golden/net_generic_coco_tracking_64x96.npz, oracle/gen_golden.py::
 gen_generic).  With --head_conv 256 the plan that runs is launch for launch the dla_34 one (CPU test
 test_generic_arch_is_the_dla34_graph_under_other_names); the arch's own default head width is 64 (opts.py:295): the
-fused first head conv becomes 64 -> 64 x n_heads and the 1x1 heads read 64-channel slices of it.
-
-(Green on the B200: profiles/r02g_pytest_gpu_generic.log.)"""
+fused first head conv becomes 64 -> 64 x n_heads and the 1x1 heads read 64-channel slices of it."""
 import os
 
 import numpy as np
@@ -13,7 +11,7 @@ import torch
 
 import ct_oracle as co
 from centertrack_b200 import synthetic as wt
-from helpers import make_model
+from helpers import load_generic_golden, make_model
 
 pytestmark = pytest.mark.gpu
 STAGES = ['base.level2', 'base.level5', 'dla_up.ida_0.node_1', 'dla_up.ida_2.node_3', 'ida_up.node_2']
@@ -34,7 +32,7 @@ def _run(extra, precision):
 def test_generic_network_matches_reference_golden(tag, extra, precision, golden_dir):
   """fp32 SIMT and bf16x3 tensor-core engines within north_star's 1e-3 of the reference GenericNetwork's fp32 outputs
   (heads and trunk stages), and the CUDA-graph replay bit-identical to the eager launches."""
-  g = np.load(os.path.join(golden_dir, 'net_generic_coco_tracking_64x96.npz'))
+  g = load_generic_golden(golden_dir)
   opt, model, sd, eng, out, (img, pre, hm) = _run(extra, precision)
   for h in opt.heads:
     ref = g['%s.head.%s' % (tag, h)]
@@ -55,7 +53,7 @@ def test_generic_module_forward_and_reference_checkpoint_names(tmp_path, golden_
   """create_model('generic', ...)(x, pre_img, pre_hm)[-1] after a save_model / load_model round trip of a checkpoint
   with the reference GenericNetwork's key names (`backbone.*`, `neck.dla_up.*`, `neck.ida_up.*`, `module.` prefix)."""
   from centertrack_b200.model import create_model, load_model, save_model
-  g = np.load(os.path.join(golden_dir, 'net_generic_coco_tracking_64x96.npz'))
+  g = load_generic_golden(golden_dir)
   opt, model, sd = make_model('coco_tracking', extra=['--arch', 'generic', '--b200_precision', 'fp32'])
   path = str(tmp_path / 'generic.pth')
   torch.save({'epoch': 3, 'state_dict': {'module.' + k: v for k, v in sd.items()}}, path)
@@ -72,7 +70,7 @@ def test_generic_module_forward_and_reference_checkpoint_names(tmp_path, golden_
 
 
 def test_generic_bf16_engine_tracks_the_emulating_oracle():
-  """The benchmarked bf16 tcgen05 engine on the 64-wide heads (halo engine: 3x3 64 -> 256, then 1x1 heads on
+  """The benchmarked bf16 wgmma engine on the 64-wide heads (halo engine: 3x3 64 -> 256, then 1x1 heads on
   64-channel slices with ld 256) against the oracle run with the engine's rounding points, same statistic and bound as
   the dla_34 test (mean |err| <= 0.2 std)."""
   opt, model, sd, eng, out, (img, pre, hm) = _run([], 'bf16')

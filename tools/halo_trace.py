@@ -55,18 +55,17 @@ for (name, B, Cin, Cout, H, W, k, res, nt) in cases:
   n = int((t[:, 4] > 0).sum())
   t0 = t[0, 0]
   print('==== %s : %d items in CTA 0' % (name, n))
-  print('  it   prod_acq  tma_iss | mma_halo mma_acc  mma_done | epi_start epi_done   (cycles since start; item period)')
+  # stamps (conv_halo.cu h_stamp): 0 producer acquired the stage, 1 TMA issued, 2 MMA saw the halo, 4 MMAs complete,
+  # 5 epilogue started, 6 epilogue done
+  print('  it   prod_acq  tma_iss | mma_halo mma_done | epi_start epi_done   (cycles since start; item period)')
   for i in list(range(min(n, 8))) + list(range(max(8, n - 2), n)):
     row = t[i] - t0
     per = (t[i, 4] - t[i - 1, 4]) if i > 0 else 0
-    print('  %3d %9d %8d | %8d %8d %8d | %8d %8d   period %d' % (i, row[0], row[1], row[2], row[3], row[4], row[5], row[6], per))
+    print('  %3d %9d %8d | %8d %8d | %8d %8d   period %d' % (i, row[0], row[1], row[2], row[4], row[5], row[6], per))
   nblk = (k * k * (Cin // 16)) if Cin != 8 else k * ((k + 1) // 2)
   if n > 4:
-    print('  issue phase per MMA: %.0f cycles (nblk %d); period per MMA %.0f' % (np.mean(t[2:n, 4] - t[2:n, 3]) / nblk, nblk, np.mean(np.diff(t[1:n, 4])) / nblk))
-  if n > 4:
     d = t[2:n]
-    print('  first tcgen05.ld after the accumulator is ready: %.0f cycles; rest of the epilogue %.0f' % (
-        np.mean(d[:, 7] - d[:, 5]), np.mean(d[:, 6] - d[:, 7])))
-    print('  mean over items 2..: wait_halo %.0f  wait_acc %.0f  issue %.0f  | epi %.0f | tma_latency(iss->mma_halo of same item) %.0f  period %.0f' % (
-        np.mean(d[:, 2] - np.maximum(t[1:n - 1, 4], d[:, 2] * 0 + t[1:n - 1, 4])), np.mean(d[:, 3] - d[:, 2]), np.mean(d[:, 4] - d[:, 3]),
-        np.mean(d[:, 6] - d[:, 5]), np.mean(d[:, 2] - d[:, 1]), np.mean(np.diff(t[1:n, 4]))))
+    print('  MMA phase per K16 block: %.0f cycles (nblk %d); period per block %.0f' % (
+        np.mean(d[:, 4] - d[:, 2]) / nblk, nblk, np.mean(np.diff(t[1:n, 4])) / nblk))
+    print('  mean over items 2..: MMA phase %.0f | epilogue %.0f | tma_latency(iss->mma_halo of same item) %.0f  period %.0f' % (
+        np.mean(d[:, 4] - d[:, 2]), np.mean(d[:, 6] - d[:, 5]), np.mean(d[:, 2] - d[:, 1]), np.mean(np.diff(t[1:n, 4]))))

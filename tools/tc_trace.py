@@ -57,21 +57,11 @@ for (name, B, Cin, Cout, H, W, k, stride, dcn, nt) in cases:
   torch.cuda.synchronize()
   L.check(lib.ct_debug_trace(None))
   t = tr.cpu().numpy().astype(np.int64)
-  if os.environ.get('CTB_DCN_PERSIST', '1') == '1' and dcn == 'win':      # the persistent window kernel (default on)
-    q = t[16:16 + 240].reshape(60, 4)
-    n = int((q[:, 3] > 0).sum())
-    base = q[0, 0]
-    print('  persistent CTA, per slice (cycles since the first): stage acquired | A written | MMA saw full | MMA committed   [period]')
-    for i in range(min(n, 30)):
-      print('   %2d  %7d %7d %7d %7d   [%d]  A %d  full-after-A %d' % (i, q[i, 0] - base, q[i, 1] - base, q[i, 2] - base, q[i, 3] - base,
-                                                                   (q[i, 1] - q[i - 1, 1]) if i else 0, q[i, 1] - q[i, 0], q[i, 2] - q[i, 1]))
-    continue
   t0 = t[0]
   sl = t[8:]
   n = int((sl > 0).sum())
   d = np.diff(np.concatenate([[t[2] if t[2] > 0 else t[1]], sl[:n]]))
   print('==== %s : k_slices %d' % (name, n))
-  print('  after alloc+sync %d' % (t[7] - t0))
-  print('  rows set up %d | table built %d | first slice done %d | last slice done %d | mma committed %d | epilogue start %d | end %d'
-        % (t[1] - t0, (t[2] - t0) if t[2] > 0 else -1, sl[0] - t0, sl[n - 1] - t0, t[4] - t0, t[5] - t0, t[6] - t0))
+  print('  rows set up %d | table built %d | first slice gathered %d | last slice gathered %d | accumulator complete %d | end %d'
+        % (t[1] - t0, (t[2] - t0) if t[2] > 0 else -1, sl[0] - t0, sl[n - 1] - t0, t[5] - t0, t[6] - t0))
   print('  cycles per slice: first %d, mean %.0f, min %d, max %d' % (d[0], d.mean(), d.min(), d.max()))

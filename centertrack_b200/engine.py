@@ -112,7 +112,8 @@ class DLA34Engine(object):
     self.depth_scale = float(depth_scale)
     self.has_pre_img = has_pre_img and ('base.pre_img_layer.0.weight' in self.sd)
     self.has_pre_hm = has_pre_hm and ('base.pre_hm_layer.0.weight' in self.sd)
-    self.ops = []          # (kind, payload)
+    self.ops = []          # (kind, payload, name)
+    self.specs = []        # one plain record per op (what it reads, computes and writes), parallel to self.ops
     self.keep = []         # device tensors referenced by raw pointers
     self.named = {}        # name -> TV (for per-stage parity tests)
     self.head_descs = {}   # head -> final ConvDesc (to toggle the fused activation)
@@ -240,15 +241,21 @@ class DLA34Engine(object):
       assert (out.H, out.W) == (OH, OW) and out.C == (16 if sum3 else C_out), (name, out.H, out.W, out.C, OH, OW, C_out)
       d.out, d.ld_out = out.ptr, out.ld
       self.named[name] = out
-    self.ops.append(('conv', d, name))
+    self._op('conv', d, name, x=x, w=w, shift=shift, residual=residual, om=om, out=out, k=(kh, kw), stride=stride,
+             pad=(pad, pad_w), out_hw=(OH, OW), a_mode=a_mode, out_mode=out_mode, relu=relu, sig_from=sig_from,
+             sum3=sum3, engine=engine, n_tile=n_tile)
     return d
 
   def _conv_bn(self, name, x, conv, bn, out, k, stride=1, relu=True, residual=None):
     w, shift = self._fold(conv, bn)
     return self._conv(name, x, w, shift, out, k, stride, relu, residual)
 
+  def _op(self, kind, payload, name, **spec):
+    self.ops.append((kind, payload, name))
+    self.specs.append(dict(spec, kind=kind, name=name, desc=payload if kind == 'conv' else None))
+
   def _maxpool(self, x, out):
-    self.ops.append(('pool', (x, out), 'maxpool'))
+    self._op('pool', (x, out), 'maxpool', x=x, out=out)
 
   def _basic_block(self, p, x, out, stride, residual, x_s2d=False):
     """BasicBlock dla.py:38-66: conv1-bn1-relu-conv2-bn2-(+residual)-relu.  x_s2d: x is stored space-to-depth
@@ -308,7 +315,7 @@ class DLA34Engine(object):
 
   def _up_add(self, p, x, skip, out, f):
     w = self._dev(self.sd[p + '.weight'].to(torch.float32).reshape(x.C, 2 * f, 2 * f).permute(1, 2, 0).contiguous())
-    self.ops.append(('up', (x, skip, w, out, f), p))
+    self._op('up', (x, skip, w, out, f), p, x=x, skip=skip, w=self.sd[p + '.weight'].to(torch.float32), out=out, f=f)
     self.named[p] = out
 
   def _ida(self, p, layers, startp, endp, o):
@@ -354,7 +361,7 @@ class DLA34Engine(object):
       # tensor-core stem: pack (img, pre, hm) -> bf16 NHWC [.,8], one 7x7 conv 8 -> 48 (block-diagonal over the
       # three stems) whose epilogue applies ReLU per stem and sums them (dla.py:307-311)
       x8 = TV(self._buf(H, W, 8), 0, 8)
-      self.ops.append(('pack', x8, 'stem.pack'))
+      self._op('pack', x8, 'stem.pack', out=x8)
       w48 = torch.zeros((48, 8, 7, 7), dtype=torch.float64)
       for si, (c0, cn) in enumerate(((0, 3), (3, 3), (6, 1))):
         w48[16 * si:16 * si + 16, c0:c0 + cn] = wst[:, c0:c0 + cn, :].reshape(7, 7, cn, 16).permute(3, 2, 0, 1)
@@ -367,7 +374,7 @@ class DLA34Engine(object):
       # with shift + ReLU per stem; the sum of the three (dla.py:307-311) is folded into level0, whose 3x3 conv reads
       # the 48 channels with its weights tiled three times along the input (conv(a + b + c) = conv over [a|b|c])
       x8 = TV(self._buf(H, W, 8), 0, 8)
-      self.ops.append(('pack32', x8, 'stem.pack'))
+      self._op('pack32', x8, 'stem.pack', out=x8)
       w48 = torch.zeros((48, 8, 7, 7), dtype=torch.float64)
       sh48 = shst.clone()
       for si, (c0, cn) in enumerate(((0, 3), (3, 3), (6, 1))):
@@ -384,7 +391,7 @@ class DLA34Engine(object):
             shm[gi] = 0
         self.stem48_shift[mask] = self._dev(shm.reshape(48).to(f32).contiguous())
     else:
-      self.ops.append(('stem', x0, 'stem'))
+      self._op('stem', x0, 'stem', out=x0, w=self.stem_w.double().cpu(), shift=self.stem_shift.double().cpu())
     self.named['stem'] = x0
 
     # ---- level0 / level1 ----
@@ -425,7 +432,7 @@ class DLA34Engine(object):
     cat2 = self._buf(h2, w2, 128)
     bottom2 = TV(self._buf(h2, w2, 32), 0, 32)
     if s2d:
-      self.ops.append(('pool_s2d', (l1, bottom2), 'maxpool'))
+      self._op('pool_s2d', (l1, bottom2), 'maxpool', x=l1, out=bottom2)
     else:
       self._maxpool(l1, bottom2)
     res2 = TV(self._buf(h2, w2, 64), 0, 64)

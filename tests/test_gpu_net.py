@@ -14,7 +14,8 @@ Tolerances
                 3e-2, heads 6e-2..8e-2 against the emulation; 0.2..0.25 against the fp32 reference, and the
                 CPU emulation deviates from fp32 by exactly as much), so deeper stages get stage-specific
                 bounds and the fp32 comparison asserts correlation >= 0.9 and mean |err| <= 0.4 x std.
-                Every layer individually is within one bf16 rounding of fp32 (tests/test_gpu_conv.py)."""
+                Every launch of the shipped plans, individually, is checked per element against an fp64
+                reference of its own operands in tests/test_gpu_plan_layers.py."""
 import os
 
 import numpy as np

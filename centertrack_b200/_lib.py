@@ -82,7 +82,7 @@ def build(force=False, verbose=False):
   """Compile libctb200.so in-tree for sm_90a (nvcc cross-compiles without a GPU).  The translation units are
   compiled in parallel into a temporary directory, then linked."""
   srcs = [os.path.join(CSRC, s) for s in SOURCES]
-  deps = srcs + [os.path.join(CSRC, h) for h in ('common.cuh', 'conv_common.cuh', 'wgmma.cuh')] + \
+  deps = srcs + [os.path.join(CSRC, h) for h in ('common.cuh', 'conv_common.cuh', 'ptx.cuh', 'wgmma.cuh')] + \
       [os.path.join(_HERE, '..', 'include', 'ctb200.h')]
   if not force and os.path.exists(LIB_PATH) and \
       all(os.path.getmtime(LIB_PATH) >= os.path.getmtime(d) for d in deps):

@@ -26,7 +26,12 @@ extern "C" int ct_debug_trace(void* device_buf) {
   const int r = halo_set_trace(device_buf);
   return r != CT_OK ? r : tc_set_trace(device_buf);
 }
-extern "C" int ct_debug_watch(void* mapped_host_buf) { return halo_set_watch(mapped_host_buf); }
+extern "C" int ct_debug_watch(void* mapped_host_buf) {
+  int r = halo_set_watch(mapped_host_buf);
+  if (r == CT_OK) r = tc_set_watch(mapped_host_buf);
+  if (r == CT_OK) r = decode_set_watch(mapped_host_buf);
+  return r;
+}
 
 static inline int tc_k_slices(int C_in, int KH, int KW) { return (KH * KW * C_in + 63) / 64; }
 
@@ -61,7 +66,7 @@ extern "C" int ct_pack_weights(int32_t engine, const float* w, int32_t C_out, in
     return CT_OK;
   }
   CT_REQUIRE(n_tile > 0 && n_tile % 16 == 0 && n_tile <= 256, "bad n_tile");
-  CT_REQUIRE(C_in % 8 == 0, "C_in must be a multiple of 8 for the tcgen05 engine");
+  CT_REQUIRE(C_in % 8 == 0, "C_in must be a multiple of 8 for the wgmma engines");
   if (engine == CT_ENGINE_TCGEN05_HALO) {
     CT_REQUIRE(C_in == 8 || (C_in % 16 == 0 && C_in <= 64) || (C_in % 64 == 0 && C_in <= 256),
                "halo engine: C_in in {8,16,32,48,64,128,192,256}");
@@ -127,18 +132,18 @@ extern "C" int ct_conv_forward(const ct_conv_desc* d, void* stream) {
   CT_REQUIRE(d->out_mode == CT_OUT_NCHW_F32 || d->ld_out >= (d->epilogue_sum3 ? 16 : d->C_out), "ld_out < C_out");
   if (d->a_mode == CT_A_DCN || d->a_mode == CT_A_DCN_WIN) {
     CT_REQUIRE(d->om != nullptr && d->ld_om >= 27, "DCN needs om with ld_om >= 27");
-    CT_REQUIRE(d->a_mode == CT_A_DCN || d->engine == CT_ENGINE_TCGEN05, "CT_A_DCN_WIN: bf16 tcgen05 engine only");
+    CT_REQUIRE(d->a_mode == CT_A_DCN || d->engine == CT_ENGINE_TCGEN05, "CT_A_DCN_WIN: bf16 wgmma engine only");
     CT_REQUIRE(d->KH == 3 && d->KW == 3 && d->stride == 1 && d->pad == 1, "DCN is 3x3 s1 p1");
   }
   CT_REQUIRE(d->out_mode != CT_OUT_NHWC_S2D || d->engine == CT_ENGINE_TCGEN05_HALO, "CT_OUT_NHWC_S2D: halo engine only");
   cudaStream_t st = (cudaStream_t)stream;
   if (d->engine == CT_ENGINE_SIMT) return conv_forward_simt(d, st);
   if (d->engine == CT_ENGINE_TCGEN05) {
-    CT_REQUIRE(d->dtype == CT_BF16, "tcgen05 engine needs bf16 activations");
+    CT_REQUIRE(d->dtype == CT_BF16, "wgmma engine needs bf16 activations");
     return conv_forward_tc(d, st);
   }
   if (d->engine == CT_ENGINE_TCGEN05_X3) {
-    CT_REQUIRE(d->dtype == CT_F32, "tcgen05 x3 engine runs on fp32 activations");
+    CT_REQUIRE(d->dtype == CT_F32, "wgmma x3 engine runs on fp32 activations");
     return conv_forward_tc(d, st);
   }
   if (d->engine == CT_ENGINE_TCGEN05_HALO) {

@@ -1,7 +1,9 @@
-// Device-side pieces shared by the SIMT (fp32-exact) and wgmma (bf16) implicit-GEMM engines:
-// output-pixel decomposition, conv window addressing and DCNv2 bilinear sampling.
+// Pieces shared by the SIMT (fp32-exact) and wgmma (bf16) implicit-GEMM engines: output-pixel decomposition, conv
+// window addressing and DCNv2 bilinear sampling, and the host-side tensor-map / launch helpers of the wgmma engines.
 #pragma once
 #include "common.cuh"
+#include <cudaTypedefs.h>
+#include <type_traits>
 
 namespace ctb {
 
@@ -64,10 +66,48 @@ __device__ __forceinline__ float head_transform(float v, int head_act, float dep
   return v;
 }
 
-// cuTensorMapEncodeTiled through the runtime's driver entry point (no -lcuda at link time)
-typedef int (*TmapEncodeFnRaw)(void*, int, unsigned, void*, const unsigned long long*, const unsigned long long*,
-                               const unsigned*, const unsigned*, int, int, int, int);
-void* tmap_encode_raw();
+// ---- host side of the tensor-core engines ----
+// TMA descriptor of a bf16 tensor: `rank` dims and box sizes innermost first, rank - 1 byte strides of the outer
+// dims; elements outside the tensor read as zero.  cuTensorMapEncodeTiled is reached through the runtime's driver
+// entry point (no -lcuda at link time).
+inline int encode_tmap_bf16(CUtensorMap* map, const void* ptr, int rank, const cuuint64_t* dims,
+                            const cuuint64_t* strides, const cuuint32_t* box, CUtensorMapSwizzle swizzle) {
+  static const PFN_cuTensorMapEncodeTiled encode = [] {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    const bool ok = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
+                    q == cudaDriverEntryPointSuccess;
+    return ok ? reinterpret_cast<PFN_cuTensorMapEncodeTiled>(p) : nullptr;
+  }();
+  if (!encode) return fail(CT_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable%s", "");
+  const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+  const CUresult cr = encode(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(ptr), dims,
+                             strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
+                             CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return cr == CUDA_SUCCESS ? CT_OK : fail(CT_ERR_CUDA, "cuTensorMapEncodeTiled failed%s (%ld)", "", (long)cr);
+}
+
+// Launches Kernel with programmatic dependent launch and up to 227 KB of dynamic shared memory.  That limit is a
+// per-device attribute of the kernel: it is set on the first launch on each device (per host thread).
+template <auto Kernel, typename... Args>
+int launch_big_smem(dim3 grid, dim3 block, size_t smem, cudaStream_t st, const Args&... args) {
+  int dev = 0;
+  cudaGetDevice(&dev);
+  static thread_local unsigned long long attr_set_mask = 0;
+  if (dev >= 64 || !((attr_set_mask >> dev) & 1ull)) {
+    CT_CUDA_OK(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    if (dev < 64) attr_set_mask |= 1ull << dev;
+  }
+  CT_CUDA_OK(launch_kernel(Kernel, grid, block, smem, st, true, args...));
+  return after_launch();
+}
+
+// f(std::integral_constant<int, n_tile>()) for the N tiles the tensor-core kernels are instantiated for: 16, 32, .., 256
+template <int N = 16, typename F>
+int dispatch_n_tile(int n_tile, F&& f) {
+  if constexpr (N > 256) return fail(CT_ERR_INVALID, "unsupported n_tile%s (%ld)", "", (long)n_tile);
+  else return n_tile == N ? f(std::integral_constant<int, N>()) : dispatch_n_tile<N + 16>(n_tile, f);
+}
 
 int conv_forward_simt(const ct_conv_desc* d, cudaStream_t st);
 int conv_forward_tc(const ct_conv_desc* d, cudaStream_t st);
@@ -76,5 +116,7 @@ int halo_blocks(int C_in, int KH, int KW);
 int halo_set_trace(void* buf);
 int tc_set_trace(void* buf);
 int halo_set_watch(void* mapped_host_buf);
+int tc_set_watch(void* mapped_host_buf);
+int decode_set_watch(void* mapped_host_buf);
 
 }  // namespace ctb

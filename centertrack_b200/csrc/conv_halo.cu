@@ -43,8 +43,7 @@ __device__ __forceinline__ void h_stamp(unsigned long long* t, int it, int k) {
 }
 constexpr int H_THREADS = 288;           // 2 MMA / epilogue warpgroups + TMA warp
 constexpr int H_MMA_WARPS = 8;
-constexpr int H_EPI_PITCH = 36;          // floats per row of the 32-column epilogue staging tile
-constexpr int H_STAGING_BYTES = 2 * 64 * H_EPI_PITCH * 4;
+constexpr int H_STAGING_BYTES = 2 * 64 * EPI_PITCH * 4;
 
 struct HaloArgs {
   ConvGeom g;
@@ -67,67 +66,11 @@ struct HaloArgs {
   uint32_t m_sky, m_skx, m_sc, m_sq, m_alo, m_ahi;
 };
 
-// ---- PTX (same wrappers as conv_tc.cu; kept local so each TU is self-contained) ----
-__device__ __forceinline__ uint32_t h_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void h_mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void h_mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void h_mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-// Watchdog report: when ct_debug_trace's buffer is host-mapped memory, a stuck wait leaves (site code, item,
-// blockIdx, warp) in its last 4 words before trapping, so a protocol bug can be located post mortem.
-__device__ volatile unsigned int* g_halo_dbg = nullptr;
-__device__ __forceinline__ void h_mbar_wait(uint32_t bar, uint32_t parity, int site = 0, int item = 0) {
-  uint32_t done = 0, spins = 0;
-  while (true) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.b32 %0, 1, 0, p;\n\t}"
-        : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-    if (done) break;
-    if (++spins > 4000000u) {
-      volatile unsigned int* d = g_halo_dbg;
-      if (d != nullptr && (threadIdx.x & 31) == 0) {
-        d[0] = (unsigned)site; d[1] = (unsigned)item; d[2] = blockIdx.x; d[3] = threadIdx.x >> 5;
-        __threadfence_system();
-      }
-      __trap();
-    }
-  }
-}
-__device__ __forceinline__ void h_bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
-__device__ __forceinline__ void h_tma_4d(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, int c3,
-                                         uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
-      ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar) : "memory");
-}
-__device__ __forceinline__ void h_tma_3d(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
-      ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(bar) : "memory");
-}
-__device__ __forceinline__ void h_named_sync(int id, int n) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
-}
-__device__ __forceinline__ void h_lds8(uint32_t addr, float (&v)[8]) {
-  asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]) : "r"(addr));
-  asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7]) : "r"(addr + 16u));
-}
-
 template <int N>
 __global__ void __launch_bounds__(H_THREADS, N <= 128 ? 2 : 1)
 conv_halo_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
   extern __shared__ __align__(1024) unsigned char hsm_dyn[];
-  unsigned char* sm = hsm_dyn + ((1024u - (h_smem_u32(hsm_dyn) & 1023u)) & 1023u);
+  unsigned char* sm = hsm_dyn + ((1024u - (smem_u32(hsm_dyn) & 1023u)) & 1023u);
   const ConvGeom& g = a.g;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   unsigned long long* const trace = h_trace_ptr();
@@ -135,7 +78,7 @@ conv_halo_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
   const uint32_t halo_bytes = (uint32_t)a.planes * a.plane_bytes;
 
   // smem: [weights][halo stage 0..S-1][epilogue staging 2 x 64 x 36 fp32][barriers][shift]
-  const uint32_t base = h_smem_u32(sm);
+  const uint32_t base = smem_u32(sm);
   const uint32_t sW = base;
   const uint32_t sH = base + ((a.w_bytes + 1023u) & ~1023u);
   const uint32_t off_stg = ((a.w_bytes + 1023u) & ~1023u) + S * halo_bytes;
@@ -148,9 +91,9 @@ conv_halo_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
 
   pdl_trigger();                       // the next kernel of the stream may start its own prologue now
   if (tid == 0) {
-    h_mbar_init(w_full, 1);
-    for (int s = 0; s < S; ++s) { h_mbar_init(halo_full(s), 1); h_mbar_init(halo_empty(s), H_MMA_WARPS); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_init(w_full, 1);
+    for (int s = 0; s < S; ++s) { mbar_init(halo_full(s), 1); mbar_init(halo_empty(s), H_MMA_WARPS); }
+    mbar_init_fence();
   }
   // folded-BN shift / bias of this CTA's output-channel tile, staged once (read as float4 broadcasts)
   float* s_shift = reinterpret_cast<float*>(sm + off_bar + 256);      // barriers use <= 136 bytes at S = 8
@@ -163,8 +106,8 @@ conv_halo_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
   // the weights are constants: their bulk copy goes out BEFORE waiting for the previous kernel (PDL), so that it
   // overlaps that kernel's tail; everything after the wait reads activations the previous kernel produced
   if (warp == 8 && lane == 0) {
-    h_mbar_expect_tx(w_full, a.w_bytes);
-    h_bulk_g2s(sW, reinterpret_cast<const unsigned char*>(a.w) + (size_t)(blockIdx.x % a.n_tiles_n) * a.w_bytes, a.w_bytes, w_full);
+    mbar_arrive_expect_tx(w_full, a.w_bytes);
+    bulk_g2s(sW, reinterpret_cast<const unsigned char*>(a.w) + (size_t)(blockIdx.x % a.n_tiles_n) * a.w_bytes, a.w_bytes, w_full);
   }
   pdl_wait();
 
@@ -184,19 +127,19 @@ conv_halo_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
       for (int sp = sp0; sp < sp_total; sp += sp_stride, ++it) {
         const int s = it % S;
         const uint32_t ph = (uint32_t)(it / S) & 1u;
-        h_mbar_wait(halo_empty(s), ph ^ 1u, 1, it);
+        mbar_wait(halo_empty(s), ph ^ 1u, 1, it);
         h_stamp(trace, it, 0);
         const int b = sp / per_img, r = sp - b * per_img;
         const int ty = r / a.tiles_x, tx = r - ty * a.tiles_x;
         const int x0 = tx * a.tw - g.pad, y0 = ty * a.th - g.pad;
-        h_mbar_expect_tx(halo_full(s), (uint32_t)(a.planes * a.box_bytes));   // TMA writes the full box (zero fill incl.)
+        mbar_arrive_expect_tx(halo_full(s), (uint32_t)(a.planes * a.box_bytes));   // TMA writes the full box (zero fill incl.)
         if (a.merged_xc) {
-          h_tma_3d(sH + s * halo_bytes, &tmap, x0 * 8, y0, b, halo_full(s));
+          tma_3d(sH + s * halo_bytes, &tmap, x0 * 8, y0, b, halo_full(s));
         } else {
           // un-swizzled: one 8-channel plane per copy; swizzled: one <=64-channel chunk (whole 128-byte rows)
           const int cstep = a.swz ? (a.swz >> 1) : 8;
           for (int p = 0; p < a.planes; ++p)
-            h_tma_4d(sH + s * halo_bytes + p * a.plane_bytes, &tmap, p * cstep, x0, y0, b, halo_full(s));
+            tma_4d(sH + s * halo_bytes + p * a.plane_bytes, &tmap, p * cstep, x0, y0, b, halo_full(s));
         }
         h_stamp(trace, it, 1);
       }
@@ -207,7 +150,7 @@ conv_halo_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
     const int lrow = 32 * (w4 & 1) + lane;       // row of this warpgroup's 64 (epilogue: row per thread)
     const int chalf = w4 >> 1;                   // 16-column half of each 32-column chunk
     const int row = 64 * wg + lrow;              // GEMM row = g*8 + r  ->  pixel (ty*16 + g, tx*8 + r)
-    const uint32_t stg = base + off_stg + (uint32_t)wg * (64u * H_EPI_PITCH * 4u);
+    const uint32_t stg = base + off_stg + (uint32_t)wg * (64u * EPI_PITCH * 4u);
     // B (weights, K-major no-swizzle): core matrices of 8 channels x 16 B, LBO = next 8 k (n_tile x 16 B), SBO = 128 B
     const uint64_t b_desc0 = wg_desc(sW, (uint32_t)N * 16u, 128u, 0u);
     const uint32_t b_step = ((uint32_t)N * 32u) >> 4;               // descriptor start-address units (16 B) per block
@@ -239,13 +182,13 @@ conv_halo_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
       }
     };
     if (use_res && sp0 < sp_total) prefetch_residual(sp0);
-    h_mbar_wait(w_full, 0, 2, 0);
+    mbar_wait(w_full, 0, 2, 0);
     float acc[N / 2];
     int it = 0;
     for (int sp = sp0; sp < sp_total; sp += sp_stride, ++it) {
       const int s = it % S;
       const uint32_t ph = (uint32_t)(it / S) & 1u;
-      h_mbar_wait(halo_full(s), ph, 3, it);
+      mbar_wait(halo_full(s), ph, 3, it);
       if (tid == 0) h_stamp(trace, it, 2);
       // A-descriptor walk (ky, kx|pair, chunk, K-step): warp-uniform adds on the start address; B advances by b_step
       const uint32_t a_lo0 = a.m_alo + (sH >> 4) + ((uint32_t)s * halo_bytes >> 4) + half16;
@@ -266,7 +209,7 @@ conv_halo_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
       wg_wait<0>();
       wg_fence_operand(acc);
       __syncwarp();
-      if (lane == 0) h_mbar_arrive(halo_empty(s));     // this warp's MMAs no longer read the halo stage
+      if (lane == 0) mbar_arrive(halo_empty(s));     // this warp's MMAs no longer read the halo stage
       if (tid == 0) h_stamp(trace, it, 4);
 
       // ---- epilogue of this warpgroup's 64 rows
@@ -282,22 +225,10 @@ conv_halo_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
       for (int j = 0; j < 8; ++j) s8[j] = 0.f;
 #pragma unroll
       for (int c0 = 0; c0 < N; c0 += 32) {
-        h_named_sync(1 + wg, 128);                   // the previous chunk's readers are done with the staging tile
-        {
-          const int t = tid & 127, w = t >> 5, l = t & 31;
-          const uint32_t rr0 = (uint32_t)(16 * w + (l >> 2));
-#pragma unroll
-          for (int i = 0; i < N / 8; ++i) {
-            if (i * 8 < c0 || i * 8 >= c0 + 32) continue;
-            const uint32_t col = (uint32_t)(i * 8 - c0 + 2 * (l & 3));
-            asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(stg + (rr0 * H_EPI_PITCH + col) * 4u),
-                         "f"(acc[4 * i]), "f"(acc[4 * i + 1]) : "memory");
-            asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(stg + ((rr0 + 8u) * H_EPI_PITCH + col) * 4u),
-                         "f"(acc[4 * i + 2]), "f"(acc[4 * i + 3]) : "memory");
-          }
-        }
-        h_named_sync(1 + wg, 128);
-        const uint32_t srow = stg + (uint32_t)lrow * H_EPI_PITCH * 4u;
+        named_sync(1 + wg, 128);                   // the previous chunk's readers are done with the staging tile
+        stage_acc_chunk(acc, c0, stg, 0);
+        named_sync(1 + wg, 128);
+        const uint32_t srow = stg + (uint32_t)lrow * EPI_PITCH * 4u;
         if (a.sum3) {
           // stem: three 16-channel groups, ReLU each (after its folded-BN shift), then sum (dla.py:307-311).
           // Warp half `chalf` produces output channels 8*chalf .. 8*chalf+7 (columns g*16 + 8*chalf + j).
@@ -306,7 +237,7 @@ conv_halo_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
             if (grp * 16 < c0 || grp * 16 >= c0 + 32 || grp * 16 >= N) continue;
             if (!((a.sum3 >> grp) & 1)) continue;          // absent input (pre_img / pre_hm is None)
             float rr[8];
-            h_lds8(srow + (uint32_t)(grp * 16 - c0 + chalf * 8) * 4u, rr);
+            lds_f(srow + (uint32_t)(grp * 16 - c0 + chalf * 8) * 4u, rr);
             const float4* sh4 = reinterpret_cast<const float4*>(s_shift + grp * 16 + chalf * 8);
             const float4 sa = sh4[0], sb = sh4[1];
             s8[0] += fmaxf(rr[0] + sa.x, 0.f); s8[1] += fmaxf(rr[1] + sa.y, 0.f);
@@ -320,11 +251,7 @@ conv_halo_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
         const int o0 = n0 + col;
         if (col >= N || !p_ok || o0 >= g.C_out) continue;
         float v[16];
-#pragma unroll
-        for (int j4 = 0; j4 < 4; ++j4)
-          asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];"
-                       : "=f"(v[4 * j4]), "=f"(v[4 * j4 + 1]), "=f"(v[4 * j4 + 2]), "=f"(v[4 * j4 + 3])
-                       : "r"(srow + (uint32_t)(chalf * 16 + 4 * j4) * 4u));
+        lds_f(srow + (uint32_t)chalf * 64u, v);
         const float4* sh4 = reinterpret_cast<const float4*>(s_shift + col);
 #pragma unroll
         for (int j4 = 0; j4 < 4; ++j4) {
@@ -343,62 +270,15 @@ conv_halo_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
               const uint4* rp = reinterpret_cast<const uint4*>(a.residual + p * g.ld_res + o0);
               ra = __ldg(rp); rb = __ldg(rp + 1);
             }
-            const __nv_bfloat162* ha = reinterpret_cast<const __nv_bfloat162*>(&ra);
-            const __nv_bfloat162* hb = reinterpret_cast<const __nv_bfloat162*>(&rb);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const float2 fa = __bfloat1622float2(ha[j]), fb = __bfloat1622float2(hb[j]);
-              v[2 * j] += fa.x; v[2 * j + 1] += fa.y; v[8 + 2 * j] += fb.x; v[8 + 2 * j + 1] += fb.y;
-            }
+            add_residual_bf16(v, ra, rb);
           }
-          if (g.relu) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
-          }
-          uint4 oa, ob;
-          __nv_bfloat162* pa2 = reinterpret_cast<__nv_bfloat162*>(&oa);
-          __nv_bfloat162* pb2 = reinterpret_cast<__nv_bfloat162*>(&ob);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            pa2[j] = __floats2bfloat162_rn(v[2 * j], v[2 * j + 1]);
-            pb2[j] = __floats2bfloat162_rn(v[8 + 2 * j], v[8 + 2 * j + 1]);
-          }
-          uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(a.out) + p * g.ld_out + o0);
-          op[0] = oa; op[1] = ob;
+          relu16(v, g.relu);
+          store_bf16x16(reinterpret_cast<__nv_bfloat16*>(a.out) + p * g.ld_out + o0, v);
         } else if (g.out_mode == CT_OUT_NHWC_F32) {
-          float* op = reinterpret_cast<float*>(a.out) + p * g.ld_out + o0;
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            if (g.relu) v[j] = fmaxf(v[j], 0.f);
-            const float sg = sigmoidf_fast(v[j]);            // unconditional: keeps the 16 chains interleaved
-            v[j] = (o0 + j >= g.sig_from) ? sg : v[j];
-          }
-          if (o0 + 16 <= g.ld_out && (g.ld_out & 3) == 0) {      // padded row: four 16-byte stores
-#pragma unroll
-            for (int j4 = 0; j4 < 4; ++j4)
-              reinterpret_cast<float4*>(op)[j4] = make_float4(v[4 * j4], v[4 * j4 + 1], v[4 * j4 + 2], v[4 * j4 + 3]);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) if (o0 + j < g.C_out) op[j] = v[j];
-          }
+          store_f32_nhwc16(reinterpret_cast<float*>(a.out) + p * g.ld_out + o0, v, o0, g);
         } else {
-          float* op = reinterpret_cast<float*>(a.out) + ((size_t)b * g.C_out + o0) * HWo + (size_t)oy * g.OW + ox;
-          // transform all 16 values in straight-line code (the activation kind is uniform: hoisted out of the
-          // loop), then the guarded stores -- per-element branches serialise the ex2/rcp chains
-          if (g.relu) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
-          }
-          if (g.head_act == CT_HEAD_SIGMOID) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = sigmoidf_fast(v[j]);
-          } else if (g.head_act == CT_HEAD_DEPTH) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = (__fdividef(1.f, sigmoidf_fast(v[j]) + 1e-6f) - 1.f) * g.depth_scale;
-          }
-#pragma unroll
-          for (int j = 0; j < 16; ++j)
-            if (o0 + j < g.C_out) op[(size_t)j * HWo] = v[j];
+          store_head16(reinterpret_cast<float*>(a.out) + ((size_t)b * g.C_out + o0) * HWo + (size_t)oy * g.OW + ox, HWo,
+                       v, o0, g);
         }
       }
       if (a.sum3 && p_ok) {
@@ -415,44 +295,11 @@ conv_halo_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
 }
 
 // ---- host ----
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-void* tmap_encode_raw();
-static EncodeTiledFn get_encode() { return reinterpret_cast<EncodeTiledFn>(tmap_encode_raw()); }
-void* tmap_encode_raw() {
-  static void* fn = nullptr;
-  if (fn) return fn;
-  void* p = nullptr;
-  cudaDriverEntryPointQueryResult q;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess ||
-      q != cudaDriverEntryPointSuccess)
-    return nullptr;
-  fn = p;
-  return fn;
-}
-
 int halo_set_trace(void* buf) {
   unsigned long long* p = (unsigned long long*)buf;
   return cudaMemcpyToSymbol(g_halo_trace, &p, sizeof(p)) == cudaSuccess ? CT_OK : CT_ERR_CUDA;
 }
-int halo_set_watch(void* mapped_host_buf) {
-  unsigned int* p = (unsigned int*)mapped_host_buf;
-  return cudaMemcpyToSymbol(g_halo_dbg, &p, sizeof(p)) == cudaSuccess ? CT_OK : CT_ERR_CUDA;
-}
-
-template <int N>
-static int launch_halo(int dev, int grid, size_t smem, cudaStream_t st, const HaloArgs& a, const CUtensorMap& tmap) {
-  // the attribute is per device (a process may drive several GPUs from one thread)
-  static thread_local unsigned long long attr_set_mask = 0;
-  if (dev >= 64 || !((attr_set_mask >> dev) & 1ull)) {
-    CT_CUDA_OK(cudaFuncSetAttribute(conv_halo_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    if (dev < 64) attr_set_mask |= 1ull << dev;
-  }
-  CT_CUDA_OK(launch_kernel(conv_halo_kernel<N>, dim3(grid), dim3(H_THREADS), smem, st, true, a, tmap));
-  return after_launch();
-}
+int halo_set_watch(void* mapped_host_buf) { return set_mbar_watch(mapped_host_buf); }
 
 int halo_blocks(int C_in, int KH, int KW) {
   return C_in == 8 ? KH * ((KW + 1) / 2) : KH * KW * (C_in / 16);
@@ -555,18 +402,13 @@ int conv_forward_halo(const ct_conv_desc* d, cudaStream_t st) {
   a.halo_stages = stages;
   const size_t smem = smem_for(stages);
 
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return fail(CT_ERR_CUDA, "conv_halo: cuTensorMapEncodeTiled entry point unavailable%s", "");
   CUtensorMap tmap;
-  const cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult cr;
+  int r;
   if (a.merged_xc) {
     const cuuint64_t dims[3] = {(cuuint64_t)g.W * 8, (cuuint64_t)g.H, (cuuint64_t)g.B};
     const cuuint64_t strides[2] = {(cuuint64_t)g.W * 16, (cuuint64_t)g.H * g.W * 16};
     const cuuint32_t box[3] = {(cuuint32_t)a.pw * 8, (cuuint32_t)a.ph, 1};
-    cr = enc(&tmap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(d->x), dims, strides, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    r = encode_tmap_bf16(&tmap, d->x, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE);
   } else {
     const cuuint64_t dims[4] = {(cuuint64_t)g.C_in, (cuuint64_t)g.W, (cuuint64_t)g.H, (cuuint64_t)g.B};
     const cuuint64_t strides[3] = {(cuuint64_t)g.ld_in * 2, (cuuint64_t)g.W * g.ld_in * 2,
@@ -575,13 +417,10 @@ int conv_forward_halo(const ct_conv_desc* d, cudaStream_t st) {
     const CUtensorMapSwizzle sw = a.swz == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
                                   : a.swz == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
                                   : a.swz == 32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_NONE;
-    cr = enc(&tmap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(d->x), dims, strides, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    r = encode_tmap_bf16(&tmap, d->x, 4, dims, strides, box, sw);
   }
-  if (cr != CUDA_SUCCESS) return fail(CT_ERR_CUDA, "conv_halo: cuTensorMapEncodeTiled failed%s (%ld)", "", (long)cr);
+  if (r != CT_OK) return r;
 
-  int dev = 0;
-  cudaGetDevice(&dev);
   // persistent grid: a multiple of n_tiles_n, at most (SMs x CTAs that fit) and no more than the work
   const int sms = device_sm_count();
   int per_sm = ctas_for(stages);
@@ -592,14 +431,9 @@ int conv_forward_halo(const ct_conv_desc* d, cudaStream_t st) {
   if (groups < 1) groups = 1;
   if (groups > a.tiles_total) groups = a.tiles_total;
   const int grid = (int)(groups * a.n_tiles_n);
-  switch (n_tile) {
-#define CTB_HALO_CASE(n) case n: return launch_halo<n>(dev, grid, smem, st, a, tmap);
-    CTB_HALO_CASE(16) CTB_HALO_CASE(32) CTB_HALO_CASE(48) CTB_HALO_CASE(64) CTB_HALO_CASE(80) CTB_HALO_CASE(96)
-    CTB_HALO_CASE(112) CTB_HALO_CASE(128) CTB_HALO_CASE(144) CTB_HALO_CASE(160) CTB_HALO_CASE(176) CTB_HALO_CASE(192)
-    CTB_HALO_CASE(208) CTB_HALO_CASE(224) CTB_HALO_CASE(240) CTB_HALO_CASE(256)
-#undef CTB_HALO_CASE
-  }
-  return fail(CT_ERR_INVALID, "conv_halo: bad n_tile%s (%ld)", "", n_tile);
+  return dispatch_n_tile(n_tile, [&](auto n) {
+    return launch_big_smem<conv_halo_kernel<decltype(n)::value>>(dim3(grid), dim3(H_THREADS), smem, st, a, tmap);
+  });
 }
 
 }  // namespace ctb

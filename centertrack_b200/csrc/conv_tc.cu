@@ -27,7 +27,6 @@ constexpr int TC_THREADS = 256;      // two warpgroups: gather + MMA + epilogue
 constexpr int TC_PRODUCERS = 256;
 constexpr int TC_NROW = TC_BM * 8 / TC_PRODUCERS;   // A-tile rows per thread per K slice (4, 16 rows apart)
 constexpr int A_STAGE_BYTES = TC_BM * 128;
-constexpr int TC_EPI_PITCH = 36;     // floats per row of the 32-column epilogue staging tile (16-byte reads conflict-free)
 
 struct TcArgs {
   ConvGeom g;
@@ -53,17 +52,6 @@ struct TcArgs {
 struct __align__(16) DcnWinEntry { int goff; uint32_t meta; uint32_t w01, w23; };
 constexpr uint32_t WIN_DX = 1u << 16, WIN_DY = 1u << 17, WIN_IN = 1u << 18;
 
-__device__ __forceinline__ uint4 lds16(uint32_t addr) {
-  uint4 r;
-  asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(addr));
-  return r;
-}
-__device__ __forceinline__ void tma_4d(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, int c3, uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
-      ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar) : "memory");
-}
-
 // output pixel (linear b,y,x index) of GEMM row r of M tile mt; g.P_out when the row is padding
 __device__ __forceinline__ int tc_pixel(const TcArgs& a, int mt, int r) {
   const ConvGeom& g = a.g;
@@ -88,82 +76,6 @@ __device__ __forceinline__ void tc_stamp(unsigned long long* t, int k) {
   if (t != nullptr && k < 256) t[k] = (unsigned long long)clock64();
 }
 
-// ---------------------------------------------------------------------------------------------
-// PTX wrappers
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-  return (uint32_t)__cvta_generic_to_shared(p);
-}
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done = 0;
-  uint32_t spins = 0;
-  while (true) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.b32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (done) break;
-    if (++spins > 20000000u) __trap();   // watchdog: a protocol bug must not hang the GPU
-  }
-}
-__device__ __forceinline__ void fence_proxy_async() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
-      "l"(src), "r"(bytes), "r"(bar)
-      : "memory");
-}
-__device__ __forceinline__ void named_sync(int id, int n) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
-}
-__device__ __forceinline__ uint4 ldg_nc16(const void* p) {
-  uint4 r;
-  asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
-  return r;
-}
-__device__ __forceinline__ void sts16(uint32_t addr, uint4 v) {
-  asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-__device__ __forceinline__ void sts_f2(uint32_t addr, float x, float y) {
-  asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
-}
-__device__ __forceinline__ void lds_f16(uint32_t addr, float (&v)[16]) {
-#pragma unroll
-  for (int j4 = 0; j4 < 4; ++j4)
-    asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];"
-                 : "=f"(v[4 * j4]), "=f"(v[4 * j4 + 1]), "=f"(v[4 * j4 + 2]), "=f"(v[4 * j4 + 3])
-                 : "r"(addr + 16u * j4));
-}
-
-// Columns [c0, c0 + 32) of a warpgroup's m64 accumulator -> rows `row0 + 0..63` of the fp32 staging tile
-// [rows][TC_EPI_PITCH] at `stg` (see wgmma.cuh for the fragment layout).
-template <int M>
-__device__ __forceinline__ void stage_acc_chunk(const float (&d)[M], int c0, uint32_t stg, int row0) {
-  const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
-  const uint32_t r = (uint32_t)(row0 + 16 * w + (l >> 2));
-#pragma unroll
-  for (int i = 0; i < M / 4; ++i) {
-    if (i * 8 < c0 || i * 8 >= c0 + 32) continue;      // resolved at compile time once c0 is
-    const uint32_t col = (uint32_t)(i * 8 - c0 + 2 * (l & 3));
-    sts_f2(stg + (r * TC_EPI_PITCH + col) * 4u, d[4 * i], d[4 * i + 1]);
-    sts_f2(stg + ((r + 8u) * TC_EPI_PITCH + col) * 4u, d[4 * i + 2], d[4 * i + 3]);
-  }
-}
-
 // K-major, 128B-swizzled smem operand descriptor: SBO = 1024 (8 rows x 128 B), LBO unused (1).
 __device__ __forceinline__ uint64_t make_sdesc(uint32_t smem_addr) {
   return wg_desc(smem_addr, 16u, 1024u, 1u);
@@ -174,6 +86,26 @@ __device__ __forceinline__ uint64_t make_sdesc(uint32_t smem_addr) {
 // outside the image, so every load address is valid and the loads need no predicate), and the four bilinear
 // weights already multiplied by the modulation mask and zeroed for corners / samples outside the image.
 struct __align__(16) DcnEntry { int off, dxo, dyo, pad; float w00, w01, w10, w11; };   // 32 bytes
+
+// Bilinear footprint of the sample point (py, px) of an H x W image, from which both sampling records are packed:
+// top-left corner (y0, x0) and its clamp into the image (yc, xc), whether the x+1 / y+1 neighbours exist on both
+// sides (dx, dy), and the four corner weights times the mask, zero for corners outside the image.
+// Returns false (c untouched) when the sample is outside the image altogether (its value is 0).
+struct DcnCorner { int y0, x0, yc, xc; bool dx, dy; float w00, w01, w10, w11; };
+__device__ __forceinline__ bool dcn_corner(float py, float px, int H, int W, float m, DcnCorner& c) {
+  if (!(py > -1.f && py < (float)H && px > -1.f && px < (float)W)) return false;
+  const float y0f = floorf(py), x0f = floorf(px);
+  const int y0 = (int)y0f, x0 = (int)x0f;
+  const float ly = py - y0f, lx = px - x0f, hy = 1.f - ly, hx = 1.f - lx;
+  const bool y0ok = y0 >= 0, y1ok = y0 + 1 <= H - 1, x0ok = x0 >= 0, x1ok = x0 + 1 <= W - 1;
+  c.y0 = y0; c.x0 = x0; c.yc = max(y0, 0); c.xc = max(x0, 0);
+  c.dx = x0ok && x1ok; c.dy = y0ok && y1ok;
+  c.w00 = (y0ok && x0ok) ? hy * hx * m : 0.f;
+  c.w01 = (y0ok && x1ok) ? hy * lx * m : 0.f;
+  c.w10 = (y1ok && x0ok) ? ly * hx * m : 0.f;
+  c.w11 = (y1ok && x1ok) ? ly * lx * m : 0.f;
+  return true;
+}
 
 __device__ __forceinline__ uint32_t bmul2(uint32_t a, uint32_t b) {
   uint32_t d;
@@ -208,12 +140,6 @@ __device__ __forceinline__ void split8(const float4 lo4, const float4 hi4, uint4
   h = make_uint4(hh[0], hh[1], hh[2], hh[3]);
   l = make_uint4(ll[0], ll[1], ll[2], ll[3]);
 }
-__device__ __forceinline__ float4 ldg_nc_f4(const float* p) {
-  float4 r;
-  asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p));
-  return r;
-}
-
 template <bool X3, int N>
 __global__ void __launch_bounds__(TC_THREADS, (!X3 && N <= 64) ? 2 : 1)
 conv_tc_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
@@ -254,7 +180,7 @@ conv_tc_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
   if (tid == 0) {
     for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), TC_THREADS / 32); }
     mbar_init(win_bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_init_fence();
   }
   __syncthreads();
   pdl_wait();                          // everything below reads what the previous kernel wrote
@@ -345,26 +271,17 @@ conv_tc_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
       for (int tap = 0; tap < 9; ++tap) {
         if (tap < tap0 || tap >= tap1) continue;
         DcnWinEntry e; e.goff = 0; e.meta = WIN_IN; e.w01 = 0u; e.w23 = 0u;
-        if (ok) {
-          const float py = (float)(oy - 1 + tap / 3) + om[2 * tap];
-          const float px = (float)(ox - 1 + tap % 3) + om[2 * tap + 1];
-          if (py > -1.f && py < (float)g.H && px > -1.f && px < (float)g.W) {
-            const float y0f = floorf(py), x0f = floorf(px);
-            const int y0 = (int)y0f, x0 = (int)x0f;
-            const float ly = py - y0f, lx = px - x0f, hy = 1.f - ly, hx = 1.f - lx, m = om[18 + tap];
-            const bool y0ok = y0 >= 0, y1ok = y0 + 1 <= g.H - 1, x0ok = x0 >= 0, x1ok = x0 + 1 <= g.W - 1;
-            const int yc = max(y0, 0), xc = max(x0, 0);
-            e.goff = (img + yc * g.W + xc) * g.ld_in;
-            const bool dx = x0ok && x1ok, dy = y0ok && y1ok;
-            const bool inside = y0 >= win_y0 && y0 + 1 <= win_y0 + a.win_ph - 1 && x0 >= win_x0 && x0 + 1 <= win_x0 + a.win_pw - 1;
-            const uint32_t woff16 = (uint32_t)((yc - win_y0) * a.win_pw + (xc - win_x0)) * 8u;   // 128 B per pixel
-            e.meta = (inside ? (woff16 | WIN_IN) : 0u) | (dx ? WIN_DX : 0u) | (dy ? WIN_DY : 0u);
-            const float w00 = (y0ok && x0ok) ? hy * hx * m : 0.f, w01 = (y0ok && x1ok) ? hy * lx * m : 0.f;
-            const float w10 = (y1ok && x0ok) ? ly * hx * m : 0.f, w11 = (y1ok && x1ok) ? ly * lx * m : 0.f;
-            const __nv_bfloat162 wa = __floats2bfloat162_rn(w00, w01), wb = __floats2bfloat162_rn(w10, w11);
-            e.w01 = *reinterpret_cast<const uint32_t*>(&wa);
-            e.w23 = *reinterpret_cast<const uint32_t*>(&wb);
-          }
+        DcnCorner c;
+        if (ok && dcn_corner((float)(oy - 1 + tap / 3) + om[2 * tap], (float)(ox - 1 + tap % 3) + om[2 * tap + 1],
+                             g.H, g.W, om[18 + tap], c)) {
+          e.goff = (img + c.yc * g.W + c.xc) * g.ld_in;
+          const bool inside = c.y0 >= win_y0 && c.y0 + 1 <= win_y0 + a.win_ph - 1 && c.x0 >= win_x0 &&
+                              c.x0 + 1 <= win_x0 + a.win_pw - 1;
+          const uint32_t woff16 = (uint32_t)((c.yc - win_y0) * a.win_pw + (c.xc - win_x0)) * 8u;   // 128 B per pixel
+          e.meta = (inside ? (woff16 | WIN_IN) : 0u) | (c.dx ? WIN_DX : 0u) | (c.dy ? WIN_DY : 0u);
+          const __nv_bfloat162 wa = __floats2bfloat162_rn(c.w00, c.w01), wb = __floats2bfloat162_rn(c.w10, c.w11);
+          e.w01 = *reinterpret_cast<const uint32_t*>(&wa);
+          e.w23 = *reinterpret_cast<const uint32_t*>(&wb);
         }
         win_tab[tap * TC_BM + trow] = e;
       }
@@ -392,22 +309,13 @@ conv_tc_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
 #pragma unroll
       for (int tap = 0; tap < 9; ++tap) {
         DcnEntry e; e.off = 0; e.dxo = 0; e.dyo = 0; e.pad = 0; e.w00 = e.w01 = e.w10 = e.w11 = 0.f;
-        if (ok) {
-          const float py = (float)(oy - 1 + tap / 3) + om[2 * tap];
-          const float px = (float)(ox - 1 + tap % 3) + om[2 * tap + 1];
-          if (py > -1.f && py < (float)g.H && px > -1.f && px < (float)g.W) {
-            const float y0f = floorf(py), x0f = floorf(px);
-            const int y0 = (int)y0f, x0 = (int)x0f;
-            const float ly = py - y0f, lx = px - x0f, hy = 1.f - ly, hx = 1.f - lx, m = om[18 + tap];
-            const bool y0ok = y0 >= 0, y1ok = y0 + 1 <= g.H - 1, x0ok = x0 >= 0, x1ok = x0 + 1 <= g.W - 1;
-            e.off = (img + max(y0, 0) * g.W + max(x0, 0)) * g.ld_in;
-            e.dxo = (x0ok && x1ok) ? g.ld_in : 0;
-            e.dyo = (y0ok && y1ok) ? g.W * g.ld_in : 0;
-            e.w00 = (y0ok && x0ok) ? hy * hx * m : 0.f;
-            e.w01 = (y0ok && x1ok) ? hy * lx * m : 0.f;
-            e.w10 = (y1ok && x0ok) ? ly * hx * m : 0.f;
-            e.w11 = (y1ok && x1ok) ? ly * lx * m : 0.f;
-          }
+        DcnCorner c;
+        if (ok && dcn_corner((float)(oy - 1 + tap / 3) + om[2 * tap], (float)(ox - 1 + tap % 3) + om[2 * tap + 1],
+                             g.H, g.W, om[18 + tap], c)) {
+          e.off = (img + c.yc * g.W + c.xc) * g.ld_in;
+          e.dxo = c.dx ? g.ld_in : 0;
+          e.dyo = c.dy ? g.W * g.ld_in : 0;
+          e.w00 = c.w00; e.w01 = c.w01; e.w10 = c.w10; e.w11 = c.w11;
         }
         dcn_tab[tap * TC_BM + tid] = e;
       }
@@ -721,7 +629,7 @@ conv_tc_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
     const int o0 = n0 + col;
     if (col < N && p_ok && o0 < g.C_out) {
       float v[16];
-      lds_f16(stg + ((uint32_t)row * TC_EPI_PITCH + (uint32_t)chalf * 16u) * 4u, v);
+      lds_f(stg + ((uint32_t)row * EPI_PITCH + (uint32_t)chalf * 16u) * 4u, v);
       if (a.shift) {
         if (o0 + 16 <= g.C_out && (reinterpret_cast<size_t>(a.shift + o0) & 15) == 0) {   // four 16-byte loads
           const float4* sh4 = reinterpret_cast<const float4*>(a.shift + o0);
@@ -736,80 +644,21 @@ conv_tc_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
         }
       }
       if (X3 && g.out_mode == CT_OUT_NHWC) {            // fp32 activations in, fp32 activations out
-        if (a.residual) {
-          const float4* rp = reinterpret_cast<const float4*>(reinterpret_cast<const float*>(a.residual) + (size_t)p * g.ld_res + o0);
-#pragma unroll
-          for (int j4 = 0; j4 < 4; ++j4) {
-            const float4 rr = ldg_nc_f4(reinterpret_cast<const float*>(rp + j4));
-            v[4 * j4] += rr.x; v[4 * j4 + 1] += rr.y; v[4 * j4 + 2] += rr.z; v[4 * j4 + 3] += rr.w;
-          }
-        }
-        if (g.relu) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
-        }
-        float4* op = reinterpret_cast<float4*>(reinterpret_cast<float*>(a.out) + (size_t)p * g.ld_out + o0);
-#pragma unroll
-        for (int j4 = 0; j4 < 4; ++j4) op[j4] = make_float4(v[4 * j4], v[4 * j4 + 1], v[4 * j4 + 2], v[4 * j4 + 3]);
+        const float* res = a.residual ? reinterpret_cast<const float*>(a.residual) + (size_t)p * g.ld_res + o0 : nullptr;
+        store_f32_act16(reinterpret_cast<float*>(a.out) + (size_t)p * g.ld_out + o0, v, res, g.relu);
       } else if (g.out_mode == CT_OUT_NHWC) {
         if (a.residual) {
           const uint4* rp = reinterpret_cast<const uint4*>(a.residual + (size_t)p * g.ld_res + o0);
           const uint4 ra = ldg_nc16(rp), rb2 = ldg_nc16(rp + 1);
-          const __nv_bfloat162* ha = reinterpret_cast<const __nv_bfloat162*>(&ra);
-          const __nv_bfloat162* hb = reinterpret_cast<const __nv_bfloat162*>(&rb2);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float2 fa = __bfloat1622float2(ha[j]), fb = __bfloat1622float2(hb[j]);
-            v[2 * j] += fa.x; v[2 * j + 1] += fa.y; v[8 + 2 * j] += fb.x; v[8 + 2 * j + 1] += fb.y;
-          }
+          add_residual_bf16(v, ra, rb2);
         }
-        if (g.relu) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
-        }
-        uint4 oa, ob;
-        __nv_bfloat162* pa = reinterpret_cast<__nv_bfloat162*>(&oa);
-        __nv_bfloat162* pb = reinterpret_cast<__nv_bfloat162*>(&ob);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          pa[j] = __floats2bfloat162_rn(v[2 * j], v[2 * j + 1]);
-          pb[j] = __floats2bfloat162_rn(v[8 + 2 * j], v[8 + 2 * j + 1]);
-        }
-        uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(a.out) + (size_t)p * g.ld_out + o0);
-        op[0] = oa; op[1] = ob;
+        relu16(v, g.relu);
+        store_bf16x16(reinterpret_cast<__nv_bfloat16*>(a.out) + (size_t)p * g.ld_out + o0, v);
       } else if (g.out_mode == CT_OUT_NHWC_F32) {
-        float* op = reinterpret_cast<float*>(a.out) + (size_t)p * g.ld_out + o0;
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          if (g.relu) v[j] = fmaxf(v[j], 0.f);
-          const float sg = sigmoidf_fast(v[j]);              // unconditional: keeps the 16 chains interleaved
-          v[j] = (o0 + j >= g.sig_from) ? sg : v[j];
-        }
-        if (o0 + 16 <= g.ld_out && (g.ld_out & 3) == 0) {      // padded row: four 16-byte stores
-#pragma unroll
-          for (int j4 = 0; j4 < 4; ++j4)
-            reinterpret_cast<float4*>(op)[j4] = make_float4(v[4 * j4], v[4 * j4 + 1], v[4 * j4 + 2], v[4 * j4 + 3]);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) if (o0 + j < g.C_out) op[j] = v[j];
-        }
+        store_f32_nhwc16(reinterpret_cast<float*>(a.out) + (size_t)p * g.ld_out + o0, v, o0, g);
       } else {
         const int b = p / HWo, rr = p - b * HWo;
-        float* op = reinterpret_cast<float*>(a.out) + ((size_t)b * g.C_out + o0) * HWo + rr;
-        if (g.relu) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
-        }
-        if (g.head_act == CT_HEAD_SIGMOID) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = sigmoidf_fast(v[j]);
-        } else if (g.head_act == CT_HEAD_DEPTH) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = (__fdividef(1.f, sigmoidf_fast(v[j]) + 1e-6f) - 1.f) * g.depth_scale;
-        }
-#pragma unroll
-        for (int j = 0; j < 16; ++j)
-          if (o0 + j < g.C_out) op[(size_t)j * HWo] = v[j];
+        store_head16(reinterpret_cast<float*>(a.out) + ((size_t)b * g.C_out + o0) * HWo + rr, HWo, v, o0, g);
       }
     }
     __syncthreads();
@@ -817,40 +666,11 @@ conv_tc_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
   if (tid == 0) tc_stamp(trace, 6);
 }
 
-typedef CUresult (*TmapEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                 const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                 CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static TmapEncodeFn tmap_encode_fn() { return reinterpret_cast<TmapEncodeFn>(tmap_encode_raw()); }
-
 int tc_set_trace(void* buf) {
   unsigned long long* p = (unsigned long long*)buf;
   return cudaMemcpyToSymbol(g_tc_trace, &p, sizeof(p)) == cudaSuccess ? CT_OK : CT_ERR_CUDA;
 }
-
-template <bool X3, int N>
-static int launch_tc(dim3 grid, size_t smem, cudaStream_t st, const TcArgs& a, const CUtensorMap& tmap) {
-  int dev = 0;
-  cudaGetDevice(&dev);
-  static thread_local unsigned long long attr_set_mask = 0;      // the attribute is per device
-  if (dev >= 64 || !((attr_set_mask >> dev) & 1ull)) {
-    CT_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<X3, N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024)));
-    if (dev < 64) attr_set_mask |= 1ull << dev;
-  }
-  CT_CUDA_OK(launch_kernel(conv_tc_kernel<X3, N>, grid, dim3(TC_THREADS), smem, st, true, a, tmap));
-  return after_launch();
-}
-
-template <bool X3>
-static int launch_tc_n(int n_tile, dim3 grid, size_t smem, cudaStream_t st, const TcArgs& a, const CUtensorMap& tmap) {
-  switch (n_tile) {
-#define CTB_TC_CASE(n) case n: return launch_tc<X3, n>(grid, smem, st, a, tmap);
-    CTB_TC_CASE(16) CTB_TC_CASE(32) CTB_TC_CASE(48) CTB_TC_CASE(64) CTB_TC_CASE(80) CTB_TC_CASE(96) CTB_TC_CASE(112)
-    CTB_TC_CASE(128) CTB_TC_CASE(144) CTB_TC_CASE(160) CTB_TC_CASE(176) CTB_TC_CASE(192) CTB_TC_CASE(208)
-    CTB_TC_CASE(224) CTB_TC_CASE(240) CTB_TC_CASE(256)
-#undef CTB_TC_CASE
-  }
-  return fail(CT_ERR_INVALID, "conv_tc: unsupported n_tile%s (%ld)", "", (long)n_tile);
-}
+int tc_set_watch(void* mapped_host_buf) { return set_mbar_watch(mapped_host_buf); }
 
 int conv_forward_tc(const ct_conv_desc* d, cudaStream_t st) {
   const bool x3 = d->engine == CT_ENGINE_TCGEN05_X3;     // fp32 activations, bf16 hi/lo split operands
@@ -896,7 +716,7 @@ int conv_forward_tc(const ct_conv_desc* d, cudaStream_t st) {
   a.win_ph = 8 + 2 * a.win_m + 3;
   a.win_bytes = (uint32_t)(a.win_pw * a.win_ph * 128);
   const size_t stage_bytes = (size_t)(x3 ? 2 : 1) * (A_STAGE_BYTES + n_tile * 128);
-  const size_t staging = (size_t)TC_BM * TC_EPI_PITCH * 4;      // <= one stage (16 KB + n_tile x 128 B)
+  const size_t staging = (size_t)TC_BM * EPI_PITCH * 4;      // <= one stage (16 KB + n_tile x 128 B)
   auto region0_for = [&](int stg) { return ((size_t)stg * stage_bytes > staging ? (size_t)stg * stage_bytes : staging); };
   auto smem_for = [&](int stg) {
     return region0_for(stg) + (2 * stg + 1) * 8 + 32 +
@@ -941,19 +761,18 @@ int conv_forward_tc(const ct_conv_desc* d, cudaStream_t st) {
     a.tiles_x = (g.OW + 15) / 16;
     a.tiles_y = (g.OH + 7) / 8;
     m_tiles = g.B * a.tiles_x * a.tiles_y;
-    TmapEncodeFn enc = tmap_encode_fn();
-    if (!enc) return fail(CT_ERR_CUDA, "conv_tc: cuTensorMapEncodeTiled entry point unavailable%s", "");
     const cuuint64_t dims[4] = {(cuuint64_t)g.C_in, (cuuint64_t)g.W, (cuuint64_t)g.H, (cuuint64_t)g.B};
     const cuuint64_t strides[3] = {(cuuint64_t)g.ld_in * 2, (cuuint64_t)g.W * g.ld_in * 2, (cuuint64_t)g.H * g.W * g.ld_in * 2};
     const cuuint32_t box[4] = {64, (cuuint32_t)a.win_pw, (cuuint32_t)a.win_ph, 1};
-    const cuuint32_t estr[4] = {1, 1, 1, 1};
-    const CUresult cr = enc(&tmap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(d->x), dims, strides, box, estr,
-                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) return fail(CT_ERR_CUDA, "conv_tc: cuTensorMapEncodeTiled failed%s (%ld)", "", (long)cr);
+    const int r = encode_tmap_bf16(&tmap, d->x, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE);
+    if (r != CT_OK) return r;
   }
   dim3 grid(m_tiles, n_tiles);
-  return x3 ? launch_tc_n<true>(n_tile, grid, smem, st, a, tmap) : launch_tc_n<false>(n_tile, grid, smem, st, a, tmap);
+  return dispatch_n_tile(n_tile, [&](auto n) {
+    constexpr int N = decltype(n)::value;
+    return x3 ? launch_big_smem<conv_tc_kernel<true, N>>(grid, dim3(TC_THREADS), smem, st, a, tmap)
+              : launch_big_smem<conv_tc_kernel<false, N>>(grid, dim3(TC_THREADS), smem, st, a, tmap);
+  });
 }
 
 }  // namespace ctb

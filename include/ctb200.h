@@ -274,8 +274,8 @@ void ct_reset_launch_count(void);
 /* Debug: timeline trace of CTA 0 of the halo conv kernel into device_buf (>= 16 KB of uint64: 8 clock64()
  * stamps per work item, see csrc/conv_halo.cu); NULL switches it off (default). */
 int ct_debug_trace(void* device_buf);
-/* Debug: 4 uint32 of host-MAPPED memory; a stuck mbarrier wait in the halo kernel writes (site, item, block, warp)
- * there before trapping.  NULL = off (default). */
+/* Debug: 4 uint32 of host-MAPPED memory; a stuck mbarrier wait in any kernel of the library (halo and gather
+ * convolutions, decode) writes (site, item, block, warp) there before trapping.  NULL = off (default). */
 int ct_debug_watch(void* mapped_host_buf);
 
 #ifdef __cplusplus

@@ -18,7 +18,8 @@
 // Warp roles (288 threads): warps 0-7 are two warpgroups; warpgroup w issues the wgmma chain (M=64, N=n_tile, K=16
 // per block) of GEMM rows 64w..64w+63 of every tile and then runs that half's epilogue (accumulator -> shared memory,
 // 32 columns at a time -> row-per-thread stores).  Warp 8 is the TMA producer.  Two CTAs per SM where shared memory
-// allows, so one CTA's epilogue overlaps the other's MMAs.
+// allows, so one CTA's epilogue overlaps the other's MMAs; where only one fits and 64 <= N <= 128, the two warpgroups
+// take turns on the tensor cores instead (ping-pong), so one warpgroup's epilogue overlaps the other's MMAs.
 #include "conv_common.cuh"
 #include "wgmma.cuh"
 #include <cuda.h>
@@ -66,8 +67,10 @@ struct HaloArgs {
   uint32_t m_sky, m_skx, m_sc, m_sq, m_alo, m_ahi;
 };
 
-template <int N>
-__global__ void __launch_bounds__(H_THREADS, N <= 128 ? 2 : 1)
+// OVERLAP: the flavour for launches that get one CTA per SM (64 <= N <= 128): the warpgroups' MMA chains alternate (see
+// the item loop) and the register cap is that of one CTA.
+template <int N, bool OVERLAP>
+__global__ void __launch_bounds__(H_THREADS, (N <= 128 && !OVERLAP) ? 2 : 1)
 conv_halo_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
   extern __shared__ __align__(1024) unsigned char hsm_dyn[];
   unsigned char* sm = hsm_dyn + ((1024u - (smem_u32(hsm_dyn) & 1023u)) & 1023u);
@@ -183,11 +186,20 @@ conv_halo_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
     };
     if (use_res && sp0 < sp_total) prefetch_residual(sp0);
     mbar_wait(w_full, 0, 2, 0);
+    // OVERLAP (ping-pong): the two warpgroups' chains take turns on the tensor cores -- warpgroup 0's chain of item it,
+    // then warpgroup 1's, then warpgroup 0's of item it + 1 -- so each warpgroup's epilogue runs while the other's MMAs
+    // do.  Named barrier 3 + w: "warpgroup w may issue", arrived on by the other warpgroup once its chain is complete
+    // (warpgroup 1 also arrives once up front, for warpgroup 0's first chain, and warpgroup 0 consumes its last
+    // arrival after the loop).  The barrier calls in the loop are unconditional: a branch next to the MMAs would make
+    // ptxas serialise them.
+    if constexpr (OVERLAP)
+      if (wg == 1 && sp0 < sp_total) named_arrive(3, 256);
     float acc[N / 2];
     int it = 0;
     for (int sp = sp0; sp < sp_total; sp += sp_stride, ++it) {
       const int s = it % S;
       const uint32_t ph = (uint32_t)(it / S) & 1u;
+      if constexpr (OVERLAP) named_sync(3 + wg, 256);
       mbar_wait(halo_full(s), ph, 3, it);
       if (tid == 0) h_stamp(trace, it, 2);
       // A-descriptor walk (ky, kx|pair, chunk, K-step): warp-uniform adds on the start address; B advances by b_step
@@ -208,6 +220,7 @@ conv_halo_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
       wg_commit();
       wg_wait<0>();
       wg_fence_operand(acc);
+      if constexpr (OVERLAP) named_arrive(3 + (wg ^ 1), 256);
       __syncwarp();
       if (lane == 0) mbar_arrive(halo_empty(s));     // this warp's MMAs no longer read the halo stage
       if (tid == 0) h_stamp(trace, it, 4);
@@ -291,6 +304,8 @@ conv_halo_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
       if (use_res && sp + sp_stride < sp_total) prefetch_residual(sp + sp_stride);
       if (tid == 0) h_stamp(trace, it, 6);
     }
+    if constexpr (OVERLAP)
+      if (wg == 0 && sp0 < sp_total) named_sync(3, 256);
   }
 }
 
@@ -431,8 +446,18 @@ int conv_forward_halo(const ct_conv_desc* d, cudaStream_t st) {
   if (groups < 1) groups = 1;
   if (groups > a.tiles_total) groups = a.tiles_total;
   const int grid = (int)(groups * a.n_tiles_n);
+  // One CTA per SM: no second CTA's MMAs fill this one's epilogue, so its two warpgroups take turns (OVERLAP).  Not
+  // below N = 64: one warpgroup's m64n32 chain alone is bound by its shared-memory operand reads and leaves the tensor
+  // pipe half idle, so the two chains must run together (measured: the 128 -> 128 N = 32 layers 45 % slower in turns).
+  // CTB_HALO_OVERLAP=0: the serial schedule everywhere, for A/B runs; the outputs are bit-identical.
+  static const int overlap_env = getenv("CTB_HALO_OVERLAP") ? atoi(getenv("CTB_HALO_OVERLAP")) : 1;
+  const bool overlap = overlap_env && per_sm == 1 && n_tile >= 64 && n_tile <= 128;
   return dispatch_n_tile(n_tile, [&](auto n) {
-    return launch_big_smem<conv_halo_kernel<decltype(n)::value>>(dim3(grid), dim3(H_THREADS), smem, st, a, tmap);
+    constexpr int NT = decltype(n)::value;
+    if constexpr (NT >= 64 && NT <= 128)
+      if (overlap)
+        return launch_big_smem<conv_halo_kernel<NT, true>>(dim3(grid), dim3(H_THREADS), smem, st, a, tmap);
+    return launch_big_smem<conv_halo_kernel<NT, false>>(dim3(grid), dim3(H_THREADS), smem, st, a, tmap);
   });
 }
 

@@ -71,6 +71,7 @@ __device__ __forceinline__ void tma_4d(uint32_t dst, const CUtensorMap* map, int
 }
 
 __device__ __forceinline__ void named_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void named_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 // ---- vector accesses ----
 __device__ __forceinline__ uint4 lds16(uint32_t addr) {

@@ -1,12 +1,16 @@
 // Per-stream state kept on the device between frames (SURVEY 8f rows 1-3):
 //   ct_track_step    generic_post_process's affine + Tracker.step's greedy displacement association
 //                    (utils/post_process.py:21-91, utils/tracker.py:28-138) on the packed decode records, plus the
-//                    (centre, radius) boxes of Detector._get_additional_inputs (detector.py:254-290) for the NEXT frame
+//                    (centre, radius) boxes of Detector._get_additional_inputs (detector.py:254-290) for the NEXT frame;
+//                    ct_track_step_assoc: the same kernel with --hungarian (scipy's linear_sum_assignment restated,
+//                    one warp) and / or --public_det births (tracker.py:52-72,83-103)
 //   ct_render_tracks the gaussian max-splat of those boxes into pre_hm (image.py:128-154)
 //   ct_flip_merge    Detector._flip_output (detector.py:311-332; model/utils.py:28-50) for --flip_test
 //   ct_warp_affine_normalize   Detector.pre_process's cv2.warpAffine(INTER_LINEAR) + (x/255 - mean)/std + HWC->CHW
 //                    (detector.py:207-226), cv2's fixed-point bilinear restated
 // All HBM-bound byte/index work: one pass over the data, coalesced, no tensor cores.
+#include <math_constants.h>
+
 #include "common.cuh"
 
 namespace ctb {
@@ -39,7 +43,19 @@ constexpr int TF = CT_TRK_FLOATS;
 
 struct TrackArgs {
   ct_track_desc d;
+  ct_track_assoc as;       // all zero: greedy association, private births (ct_track_step)
 };
+
+// bytes of the greedy layout before the association scratch (a multiple of 8: the scratch starts with fp64 arrays)
+__host__ __device__ constexpr size_t trk_base_bytes(size_t K, size_t T) { return (16 * T + 18 * K) * 4; }
+
+// Sort key of one column in a Dijkstra step of the assignment solver: the lowest shortest-path cost wins; among equal
+// costs a free column (row4col == -1) beats an assigned one, the free one at the LARGEST position of `remaining` and the
+// assigned one at the SMALLEST -- what the sequential scan `spc < lowest || (spc == lowest && row4col == -1)` keeps.
+// rank encodes that preference (larger is better), -1 = no candidate.
+constexpr int LSAP_FREE = 1 << 20;
+__device__ __forceinline__ int lsap_rank(bool is_free, int it) { return is_free ? LSAP_FREE + it : LSAP_FREE - 1 - it; }
+__device__ __forceinline__ int lsap_pos(int rank) { return rank >= LSAP_FREE ? rank - LSAP_FREE : LSAP_FREE - 1 - rank; }
 
 __device__ __forceinline__ float aff_f32(const float* t, float x, float y) {
   // np.dot(trans[2x3] f32, [x, y, 1] f32): x*t0 + y*t1 + t2 accumulated left to right in fp32
@@ -65,6 +81,145 @@ __device__ double gaussian_radius_f64(double h, double w) {
   return fmin(r1, fmin(r2, r3));
 }
 
+// Gated cost of (detection i, track j) as the host Tracker builds it (tracker.py _gated_cost + hungarian_assignment):
+// the greedy path's fp32 squared distance, widened to fp64, plus 1e18 when blocked, clamped to exactly 1e18 so that
+// every blocked cell weighs the same.  Recomputed on every read: the T x K matrix is never stored.
+__device__ __forceinline__ double gated_cost(const float* s_old, const float* s_px, const float* s_py, const float* s_isz,
+                                             const float* s_tsz, const float* s_det, int i, int j) {
+  const float* t = s_old + (size_t)j * TF;
+  const float dx = __fsub_rn(t[CT_TRK_CT], s_px[i]), dy = __fsub_rn(t[CT_TRK_CT + 1], s_py[i]);
+  const float dist = __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy));
+  const bool blocked = dist > s_tsz[j] || dist > s_isz[i] || t[CT_TRK_CLASS] != s_det[(size_t)i * TF + CT_TRK_CLASS];
+  const double c = __dadd_rn((double)dist, blocked ? 1e18 : 0.0);
+  return c > 1e18 ? 1e18 : c;
+}
+
+// --hungarian (tracker.py:52-72): the minimum-cost assignment of scipy.optimize.linear_sum_assignment, restated from
+// Crouse's shortest augmenting path algorithm (IEEE TAES 52(4), 2016) with the same choice among equal-cost optima:
+// rows = the smaller side (detections unless N > M), augmented in order, one Dijkstra search per row over the columns
+// in `remaining` (initialised in reverse, swap-removed), fp64 reduced costs ((minVal + c) - u) - v.  Run by ONE warp:
+// each search step is a shuffle min-reduction with the key of lsap_rank; the steps themselves are serial.
+// Results: s_match[det] = track of a kept pair (cost <= 1e16), s_rej[det] = track of a rejected pair, s_taken[track]
+// for both; the pairs are in ascending detection order, which is the order rejected tracks later coast in.
+__device__ void hungarian_assign(const float* s_old, const float* s_px, const float* s_py, const float* s_isz,
+                                 const float* s_tsz, const float* s_det, int N, int M, double* s_u, double* s_v,
+                                 double* s_spc, int* s_path, int* s_c4r, int* s_r4c, int* s_rem, int* s_match,
+                                 int* s_taken, int* s_rej, int* steps_out, int lane) {
+  const bool tr = N > M;                                  // rows are the smaller side
+  const int nr = tr ? M : N, nc = tr ? N : M;
+  for (int j = lane; j < nc; j += 32) { s_v[j] = 0.0; s_r4c[j] = -1; }
+  for (int i = lane; i < nr; i += 32) { s_u[i] = 0.0; s_c4r[i] = -1; }
+  __syncwarp();
+  int steps = 0;
+  for (int cur = 0; cur < nr; ++cur) {
+    for (int it = lane; it < nc; it += 32) { s_rem[it] = nc - 1 - it; s_spc[it] = CUDART_INF; }
+    __syncwarp();
+    double minVal = 0.0;
+    int i = cur, sink = -1, nrem = nc;
+    while (sink < 0) {                                    // terminates: a free column is always among `remaining`
+      ++steps;
+      const double ui = s_u[i];
+      double best = CUDART_INF;
+      int brank = -1;
+      for (int it = lane; it < nrem; it += 32) {
+        const int j = s_rem[it];
+        const double c = tr ? gated_cost(s_old, s_px, s_py, s_isz, s_tsz, s_det, j, i)
+                            : gated_cost(s_old, s_px, s_py, s_isz, s_tsz, s_det, i, j);
+        const double r = __dsub_rn(__dsub_rn(__dadd_rn(minVal, c), ui), s_v[j]);
+        double sp = s_spc[j];
+        if (r < sp) { sp = r; s_spc[j] = r; s_path[j] = i; }
+        const int rk = lsap_rank(s_r4c[j] < 0, it);
+        if (sp < best || (sp == best && rk > brank)) { best = sp; brank = rk; }
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        const double ov = __shfl_xor_sync(0xffffffffu, best, o);
+        const int orank = __shfl_xor_sync(0xffffffffu, brank, o);
+        if (ov < best || (ov == best && orank > brank)) { best = ov; brank = orank; }
+      }
+      const int pos = lsap_pos(brank);
+      const int j = s_rem[pos];
+      minVal = best;
+      const int owner = s_r4c[j];
+      if (owner < 0) sink = j; else i = owner;
+      --nrem;
+      __syncwarp();
+      if (lane == 0) { s_rem[pos] = s_rem[nrem]; s_rem[nrem] = j; }   // reached columns collect at the tail
+      __syncwarp();
+    }
+    // duals: u[cur] += minVal; every other reached row (the owner of a reached column) and every reached column by
+    // minVal - spc[column]
+    for (int k = nrem + lane; k < nc; k += 32) {
+      const int j = s_rem[k];
+      const double dl = __dsub_rn(minVal, s_spc[j]);
+      if (j != sink) s_u[s_r4c[j]] = __dadd_rn(s_u[s_r4c[j]], dl);
+      s_v[j] = __dsub_rn(s_v[j], dl);
+    }
+    if (lane == 0) s_u[cur] = __dadd_rn(s_u[cur], minVal);
+    __syncwarp();
+    if (lane == 0) {                                      // augment back along the path
+      int j = sink;
+      for (;;) {
+        const int r = s_path[j];
+        s_r4c[j] = r;
+        const int prev = s_c4r[r];
+        s_c4r[r] = j;
+        j = prev;
+        if (r == cur) break;
+      }
+    }
+    __syncwarp();
+  }
+  // pairs (det, track); > 1e16 means forced through a blocked cell: rejected
+  for (int r = lane; r < nr; r += 32) {
+    const int det = tr ? s_c4r[r] : r, trk = tr ? r : s_c4r[r];
+    s_taken[trk] = 1;
+    if (gated_cost(s_old, s_px, s_py, s_isz, s_tsz, s_det, det, trk) > 1e16) s_rej[det] = trk;
+    else s_match[det] = trk;
+  }
+  if (steps_out && lane == 0) *steps_out = steps;
+}
+
+// --public_det births (tracker.py:83-103): public detection p = 0..P-1 claims argmin_i dist(pred_i, pub_p) over the
+// unmatched, unclaimed detections (others read as (float)1e18; ties -> lowest i) when that distance is below the
+// detection's box area.  Claimed detections get s_match = -2 and are listed in s_claim in claim order; returns their
+// number.  One warp: the public centres are read 32 at a time and broadcast by shuffles.
+__device__ int public_claims(const float* pc, int P, const float* s_px, const float* s_py, const float* s_isz, int N,
+                             int* s_match, int* s_claim, int lane) {
+  int n = 0;
+  for (int base = 0; base < P && N > 0; base += 32) {
+    float mx = 0.f, my = 0.f;
+    if (base + lane < P) { mx = pc[2 * (base + lane)]; my = pc[2 * (base + lane) + 1]; }
+    const int cnt = P - base < 32 ? P - base : 32;
+    for (int q = 0; q < cnt; ++q) {
+      const float qx = __shfl_sync(0xffffffffu, mx, q), qy = __shfl_sync(0xffffffffu, my, q);
+      float best = CUDART_INF_F;
+      int bi = 0x7fffffff;
+      for (int i = lane; i < N; i += 32) {
+        float v = 1e18f;
+        if (s_match[i] == -1) {
+          const float dx = __fsub_rn(s_px[i], qx), dy = __fsub_rn(s_py[i], qy);
+          v = __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy));
+        }
+        if (v < best) { best = v; bi = i; }               // ascending i per lane: first minimum kept
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (ov < best || (ov == best && oi < bi)) { best = ov; bi = oi; }
+      }
+      // a blocked argmin (only when every candidate is blocked) is never claimed
+      const bool claim = bi < N && best < s_isz[bi] && s_match[bi] == -1;
+      __syncwarp();
+      if (claim && lane == 0) { s_match[bi] = -2; s_claim[n] = bi; }
+      n += claim ? 1 : 0;
+      __syncwarp();
+    }
+  }
+  return n;
+}
+
 __global__ void __launch_bounds__(TRK_THREADS)
 track_step_kernel(const TrackArgs a) {
   extern __shared__ __align__(16) unsigned char tsm[];
@@ -81,9 +236,19 @@ track_step_kernel(const TrackArgs a) {
   int* s_taken = s_match + K;                                   // [T]
   int* s_pos_det = s_taken + T;                                 // [K] output slot of det or -1
   int* s_pos_trk = s_pos_det + K;                               // [T] output slot of a coasting track or -1
+  // association scratch, present only when ct_track_step_assoc enables a mode (ct_track_assoc_smem_bytes)
+  double* s_u = reinterpret_cast<double*>(tsm + trk_base_bytes(K, T));   // [K] row duals
+  double* s_v = s_u + K;                                        // [T] column duals
+  double* s_spc = s_v + T;                                      // [T] shortest-path costs of the current search
+  int* s_path = reinterpret_cast<int*>(s_spc + T);              // [T] predecessor row of a column
+  int* s_c4r = s_path + T;                                      // [K] column of a row or -1
+  int* s_r4c = s_c4r + K;                                       // [T] row of a column or -1
+  int* s_rem = s_r4c + T;                                       // [T] columns not yet reached, then the reached ones
+  int* s_rej = s_rem + T;                                       // [K] track of a det's rejected Hungarian pair or -1
+  int* s_claim = s_rej + K;                                     // [K] detections claimed by public detections, in order
   __shared__ float red_v[TRK_THREADS / 32];
   __shared__ int red_j[TRK_THREADS / 32];
-  __shared__ int s_n, s_total, s_ids;
+  __shared__ int s_n, s_total, s_ids, s_nclaim;
 
   int M = d.counts[b * 2 + 0];
   if (M > T) M = T;
@@ -132,10 +297,21 @@ track_step_kernel(const TrackArgs a) {
   }
   __syncthreads();
 
+  const bool hung = a.as.hungarian != 0, pub = a.as.public_det != 0;
+  if (hung || pub) {
+    for (int i = tid; i < N; i += TRK_THREADS) s_rej[i] = -1;
+    __syncthreads();
+  }
+  if (!hung && tid == 0 && a.as.steps) a.as.steps[b] = 0;
+  const float INF = 3.0e38f;
+  if (hung) {
+    if (warp == 0) hungarian_assign(s_old, s_px, s_py, s_isz, s_tsz, s_det, N, M, s_u, s_v, s_spc, s_path, s_c4r, s_r4c,
+                                    s_rem, s_match, s_taken, s_rej, a.as.steps ? a.as.steps + b : nullptr, lane);
+    __syncthreads();
+  }
   // ---- greedy assignment (tracker.py:129-138): detections in score order take their nearest free, valid track;
   //      argmin ties -> lowest track index
-  const float INF = 3.0e38f;
-  for (int i = 0; i < N && M > 0; ++i) {
+  for (int i = 0; i < N && M > 0 && !hung; ++i) {
     const float px = s_px[i], py = s_py[i], isz = s_isz[i], icls = s_det[(size_t)i * TF + CT_TRK_CLASS];
     float best = INF;
     int bj = 0x7fffffff;
@@ -164,7 +340,22 @@ track_step_kernel(const TrackArgs a) {
     __syncthreads();
   }
 
-  // ---- output order (tracker.py:74-127): matched detections, then new tracks, then coasting tracks
+  // ---- MOT public-detection births (tracker.py:83-103): each public detection, in order, claims its nearest
+  //      unmatched detection if closer than that detection's box area
+  if (pub) {
+    if (warp == 0) {
+      int P = a.as.public_n[b];
+      P = P < 0 ? 0 : (P > a.as.max_public ? a.as.max_public : P);
+      const int n = public_claims(a.as.public_ct + (size_t)b * a.as.max_public * 2, P, s_px, s_py, s_isz, N, s_match,
+                                  s_claim, lane);
+      if (lane == 0) s_nclaim = n;
+    }
+    __syncthreads();
+  }
+
+  // ---- output order (tracker.py:74-127): matched detections, then new tracks, then coasting tracks.  Births and
+  //      coasting walk the reference's `unmatched` lists: the naturally unmatched ascending, then the detections /
+  //      tracks of rejected (forced through a blocked cell) Hungarian pairs in pair order
   if (tid == 0) {
     int pos = 0, ids = id_count;
     for (int i = 0; i < N; ++i) {
@@ -176,24 +367,37 @@ track_step_kernel(const TrackArgs a) {
         if (pos < T) s_pos_det[i] = pos++;
       }
     }
-    for (int i = 0; i < N; ++i) {
-      if (s_match[i] >= 0) continue;
+    auto birth = [&](int i) {
       float* o = s_det + (size_t)i * TF;
       if (o[CT_TRK_SCORE] > d.new_thresh) {
         ++ids;
         o[CT_TRK_ID] = (float)ids; o[CT_TRK_AGE] = 1.f; o[CT_TRK_ACTIVE] = 1.f;
         if (pos < T) s_pos_det[i] = pos++;
       }
-    }
-    for (int j = 0; j < M; ++j) {
-      s_pos_trk[j] = -1;
-      if (s_taken[j]) continue;
+    };
+    auto coast = [&](int j) {
       float* t = s_old + (size_t)j * TF;
       if (t[CT_TRK_AGE] < (float)d.max_age) {
         t[CT_TRK_AGE] += 1.f; t[CT_TRK_ACTIVE] = 0.f;
         if (pos < T) s_pos_trk[j] = pos++;
       }
+    };
+    if (pub) {
+      for (int k = 0; k < s_nclaim; ++k) birth(s_claim[k]);
+    } else {
+      for (int i = 0; i < N; ++i)
+        if (s_match[i] < 0 && !(hung && s_rej[i] >= 0)) birth(i);
+      if (hung)
+        for (int i = 0; i < N; ++i)
+          if (s_rej[i] >= 0) birth(i);
     }
+    for (int j = 0; j < M; ++j) {
+      s_pos_trk[j] = -1;
+      if (!s_taken[j]) coast(j);
+    }
+    if (hung)
+      for (int i = 0; i < N; ++i)
+        if (s_rej[i] >= 0) coast(s_rej[i]);
     s_total = pos;
     s_ids = ids;
   }
@@ -338,19 +542,34 @@ extern "C" int64_t ct_track_smem_bytes(int32_t K, int32_t max_tracks) {
          (int64_t)(2 * (size_t)K + 2 * (size_t)max_tracks) * 4 + 64;
 }
 
-extern "C" int ct_track_step(const ct_track_desc* d, void* stream) {
-  CT_REQUIRE(d && d->records && d->trans_out_inv && d->tracks && d->counts, "null pointer");
+extern "C" int64_t ct_track_assoc_smem_bytes(int32_t K, int32_t max_tracks) {
+  return ct_track_smem_bytes(K, max_tracks) + (int64_t)(8 * ((size_t)K + 2 * (size_t)max_tracks)) +
+         (int64_t)(4 * (3 * (size_t)max_tracks + 3 * (size_t)K));
+}
+
+extern "C" int ct_track_step_assoc(const ct_track_desc* d, const ct_track_assoc* as, void* stream) {
+  CT_REQUIRE(d && as && d->records && d->trans_out_inv && d->tracks && d->counts, "null pointer");
   CT_REQUIRE(d->B > 0 && d->K > 0 && d->F >= CT_REC_HEADS && d->max_tracks >= d->K, "bad shape");
   CT_REQUIRE(d->rec_tracking < 0 || d->rec_tracking + 2 <= d->F, "tracking offset outside the record");
   CT_REQUIRE(d->boxes == nullptr || (d->trans_input != nullptr && d->inp_h > 0 && d->inp_w > 0), "boxes need trans_input");
-  const size_t smem = (size_t)ct_track_smem_bytes(d->K, d->max_tracks);
+  CT_REQUIRE(!as->public_det || (as->public_ct && as->public_n), "public_det needs public_ct and public_n");
+  CT_REQUIRE(!as->public_det || as->max_public > 0, "public_det needs max_public > 0");
+  const bool scratch = as->hungarian || as->public_det;
+  const size_t smem = (size_t)(scratch ? ct_track_assoc_smem_bytes(d->K, d->max_tracks)
+                                       : ct_track_smem_bytes(d->K, d->max_tracks));
   CT_REQUIRE(smem <= 200 * 1024, "track table does not fit in shared memory (lower max_tracks)");
   if (smem > 48 * 1024)
     CT_CUDA_OK(cudaFuncSetAttribute(track_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   TrackArgs a;
   a.d = *d;
+  a.as = *as;
   track_step_kernel<<<d->B, TRK_THREADS, smem, (cudaStream_t)stream>>>(a);
   return after_launch();
+}
+
+extern "C" int ct_track_step(const ct_track_desc* d, void* stream) {
+  const ct_track_assoc greedy = {};
+  return ct_track_step_assoc(d, &greedy, stream);
 }
 
 extern "C" int ct_render_tracks(const float* boxes, int32_t n, float* pre_hm, int32_t B, int32_t H, int32_t W,

@@ -1,12 +1,10 @@
 """Per-stream tracker state kept on the GPU between frames (SURVEY 8f-1): the reference's
-`generic_post_process` affine (utils/post_process.py:21-91), `Tracker.step` greedy association
-(utils/tracker.py:28-138) and the prior heat-map render of `Detector._get_additional_inputs`
-(detector.py:254-290) as two launches on the decode records -- `ct_track_step` and `ct_render_tracks` -- so that a
-stream never returns to the host between frames: records(t) -> tracks(t) -> pre_hm(t+1) are all device-resident and
-CUDA-graph capturable (fixed launch shapes).
-
-Greedy association only: `--hungarian` / `--public_det` streams use the host tracker (centertrack_b200.tracker,
-`Detector.run`); this class refuses them rather than silently tracking differently.
+`generic_post_process` affine (utils/post_process.py:21-91), `Tracker.step` association (utils/tracker.py:28-138:
+greedy, `--hungarian`, `--public_det`) and the prior heat-map render of `Detector._get_additional_inputs`
+(detector.py:254-290) as two launches on the decode records -- `ct_track_step` (`ct_track_step_assoc` for the
+Hungarian / public-detection modes) and `ct_render_tracks` -- so that a stream never returns to the host between
+frames: records(t) -> tracks(t) -> pre_hm(t+1) are all device-resident and CUDA-graph capturable (fixed launch shapes).
+Every mode reproduces the host `Tracker` (centertrack_b200.tracker) row for row.
 Results are rows of CT_TRK_FLOATS fp32 (score, class, ct, tracking, bbox, tracking_id, age, active) in the
 reference's output order (matched detections, new tracks, coasting tracks); `results()` turns a host copy into the
 reference's list of dicts.
@@ -22,12 +20,16 @@ from .image import get_affine_transform
 
 class DeviceTracker(object):
 
-  def __init__(self, opt, B, K, rec_floats, layout, inp_h, inp_w, device, centers=None, scales=None, max_tracks=None):
+  def __init__(self, opt, B, K, rec_floats, layout, inp_h, inp_w, device, centers=None, scales=None, max_tracks=None,
+               max_public_dets=512):
     """centers/scales: per-stream (c, s) of the source rectangle (Detector._input_geometry); default = a source image
-    of exactly the network input size (the synthetic benchmark streams)."""
-    if getattr(opt, 'hungarian', False) or getattr(opt, 'public_det', False):
-      raise NotImplementedError('the device tracker is greedy-only: --hungarian / --public_det run on the host '
-                                '(centertrack_b200.tracker.Tracker via Detector.run)')
+    of exactly the network input size (the synthetic benchmark streams).  max_public_dets: with --public_det, the most
+    public detections one stream may bring per frame (P, the row count of the public_ct buffers step() takes)."""
+    self.hungarian = bool(getattr(opt, 'hungarian', False))
+    self.public_det = bool(getattr(opt, 'public_det', False))
+    self.max_public = int(max_public_dets)
+    if self.public_det and self.max_public <= 0:
+      raise ValueError('--public_det needs max_public_dets > 0')
     self.opt, self.B, self.K, self.F = opt, B, K, rec_floats
     self.inp_h, self.inp_w = inp_h, inp_w
     self.device = torch.device(device)
@@ -58,7 +60,11 @@ class DeviceTracker(object):
     d.trans_out_inv, d.trans_input = self.trans_out_inv.data_ptr(), self.trans_input.data_ptr()
     d.tracks, d.counts, d.boxes = self.tracks.data_ptr(), self.counts.data_ptr(), self.boxes.data_ptr()
     self.desc = d
-    if L.lib().ct_track_smem_bytes(K, self.T) > 200 * 1024:
+    a = L.TrackAssoc()
+    a.hungarian, a.public_det, a.max_public = int(self.hungarian), int(self.public_det), self.max_public
+    self.assoc = a
+    smem = L.lib().ct_track_assoc_smem_bytes if (self.hungarian or self.public_det) else L.lib().ct_track_smem_bytes
+    if smem(K, self.T) > 200 * 1024:
       raise ValueError('track table of %d rows does not fit in shared memory' % self.T)
 
   def reset(self):
@@ -68,11 +74,37 @@ class DeviceTracker(object):
     self.boxes.zero_()
     self.boxes[:, :, 3] = -1.0
 
-  def step(self, records):
-    """records [B,K,F] (ct_decode) -> updates tracks/counts/boxes in place, on the current stream."""
+  def public_buffers(self):
+    """Zeroed device buffers of the shape step() takes with --public_det: public_ct [B,P,2] fp32, public_n [B] int32."""
+    return (torch.zeros((self.B, self.max_public, 2), dtype=torch.float32, device=self.device),
+            torch.zeros((self.B,), dtype=torch.int32, device=self.device))
+
+  def step(self, records, public_ct=None, public_n=None, steps=None):
+    """records [B,K,F] (ct_decode) -> updates tracks/counts/boxes in place, on the current stream.
+    With --public_det: public_ct [B,P,2] fp32 (each stream's public detection centres, image coordinates, first
+    public_n[b] rows used) and public_n [B] int32, device tensors (P = max_public_dets).  The descriptor points at
+    the buffers of this call, so a CUDA graph captured around it keeps reading them.  steps: optional [B] int32
+    device tensor that receives the Dijkstra search steps of each stream's Hungarian solve."""
+    if self.public_det and (public_ct is None or public_n is None):
+      raise ValueError('--public_det: step() needs the public detections (public_ct, public_n)')
     assert records.is_cuda and records.dtype == torch.float32 and tuple(records.shape) == (self.B, self.K, self.F)
     self.desc.records = records.data_ptr()
-    L.check(L.lib().ct_track_step(C.byref(self.desc), L.stream_ptr()), 'ct_track_step')
+    if not (self.hungarian or self.public_det or steps is not None):
+      L.check(L.lib().ct_track_step(C.byref(self.desc), L.stream_ptr()), 'ct_track_step')
+      return
+    a = self.assoc
+    a.public_ct = a.public_n = None
+    if self.public_det:
+      if not (public_ct.is_cuda and public_ct.dtype == torch.float32 and public_ct.is_contiguous() and
+              tuple(public_ct.shape) == (self.B, self.max_public, 2)):
+        raise ValueError('public_ct must be a contiguous fp32 CUDA tensor [%d, %d, 2]' % (self.B, self.max_public))
+      if not (public_n.is_cuda and public_n.dtype == torch.int32 and tuple(public_n.shape) == (self.B,)):
+        raise ValueError('public_n must be an int32 CUDA tensor [%d]' % self.B)
+      a.public_ct, a.public_n = public_ct.data_ptr(), public_n.data_ptr()
+    if steps is not None:
+      assert steps.is_cuda and steps.dtype == torch.int32 and tuple(steps.shape) == (self.B,)
+    a.steps = steps.data_ptr() if steps is not None else None
+    L.check(L.lib().ct_track_step_assoc(C.byref(self.desc), C.byref(a), L.stream_ptr()), 'ct_track_step_assoc')
 
   def render(self, pre_hm):
     """pre_hm [B,1,H,W] fp32 <- splat of the current tracks (what the NEXT frame's network reads)."""

@@ -17,7 +17,9 @@ Two ways to feed the prior heat-map (`--pre_hm`):
   * device_tracking=True (SURVEY 8f-1): the reference's dependency chain closed ON THE DEVICE, inside the same graph:
         pre_hm(t) = splat(tracks(t-1))  ->  network + decode -> records(t)  ->  tracks(t) = Tracker.step(records(t))
     (`DeviceTracker`: ct_render_tracks, ct_track_step).  Exact reference semantics (no stale prior), no host round
-    trip; the host uploads only the frame and downloads the track table (ids, boxes, ages).
+    trip; the host uploads only the frame and downloads the track table (ids, boxes, ages).  Every association mode
+    of the host Tracker runs there: greedy, `--hungarian`, and `--public_det`, whose public detections (the `ct`s of
+    each frame's provided detections) are staged per input slot like the frames and uploaded with them.
 
 The end-to-end form (`step_host`) takes HOST frames: pinned staging, H2D on a copy stream overlapped
 with the previous step's compute, graph replay, D2H of the records (and tracks).
@@ -36,7 +38,9 @@ NS = 3          # input slots
 class StreamRunner(object):
 
   def __init__(self, model, B, H, W, K=100, precision='bf16', device='cuda', use_graph=True, opt=None,
-               device_tracking=False):
+               device_tracking=False, max_public_dets=512):
+    """max_public_dets: with device_tracking and --public_det, the most public detections a stream may bring per
+    frame (more raise ValueError; none is ever dropped)."""
     self.B, self.H, self.W, self.K = B, H, W, K
     self.device = torch.device(device)
     self.model = model
@@ -63,7 +67,12 @@ class StreamRunner(object):
     self._eager(0, first=True)                               # sizes the record buffer
     if device_tracking:
       assert self.opt is not None, 'device tracking needs opt (thresholds, max_age)'
-      self.tracker = DeviceTracker(self.opt, B, K, self.rec.shape[2], self.layout, H, W, self.device)
+      self.tracker = DeviceTracker(self.opt, B, K, self.rec.shape[2], self.layout, H, W, self.device,
+                                   max_public_dets=max_public_dets)
+    self.public = self.tracker is not None and self.tracker.public_det
+    if self.public:                                          # per slot: device (public_ct, public_n) + pinned staging
+      self.pub = [self.tracker.public_buffers() for _ in range(NS)]
+      self.h_pub = [tuple(t.cpu().pin_memory() for t in p) for p in self.pub]
     torch.cuda.synchronize(self.device)
     self.h_rec = [torch.zeros_like(self.rec, device='cpu').pin_memory() for _ in range(2)]
     if self.tracker is not None:
@@ -87,7 +96,7 @@ class StreamRunner(object):
     if self.rec is None:
       self.rec, self.layout = res.records, res.layout
     if self.tracker is not None:
-      self.tracker.step(self.rec)                            # tracks(t)
+      self.tracker.step(self.rec, *(self.pub[slot] if self.public else ()))    # tracks(t)
     return res
 
   def _graph(self, slot):
@@ -123,10 +132,46 @@ class StreamRunner(object):
     if self.tracker is not None:
       self.tracker.reset()
 
-  def load_device_inputs(self, images, pre_hms, slot):
+  def _check_public(self, public_dets):
+    """public_dets: list of B arrays [P_b, 2] (the `ct` of each of the frame's public detections, image coordinates)
+    -> list of B float32 arrays; ValueError when they are missing, unexpected, or more than max_public_dets."""
+    if not self.public:
+      if public_dets is not None:
+        raise ValueError('public detections are only read by device tracking with --public_det')
+      return None
+    if public_dets is None:
+      raise ValueError('--public_det: every step needs the public detections of its frames (public_dets)')
+    if len(public_dets) != self.B:
+      raise ValueError('public_dets: expected %d arrays (one per stream), got %d' % (self.B, len(public_dets)))
+    out = []
+    for b, p in enumerate(public_dets):
+      a = np.asarray(p, np.float32)
+      if a.size == 0:
+        a = a.reshape(0, 2)
+      if a.ndim != 2 or a.shape[1] != 2:
+        raise ValueError('public_dets[%d]: expected [P, 2] centres, got shape %s' % (b, a.shape))
+      if a.shape[0] > self.tracker.max_public:
+        raise ValueError('public_dets[%d]: %d public detections, more than max_public_dets = %d' %
+                         (b, a.shape[0], self.tracker.max_public))
+      out.append(a)
+    return out
+
+  def _fill_public(self, dst, pub):
+    ct, n = dst
+    ct.zero_()
+    for b, a in enumerate(pub):
+      ct[b, :len(a)] = torch.from_numpy(a)
+      n[b] = len(a)
+
+  def load_device_inputs(self, images, pre_hms, slot, public_dets=None):
+    pub = self._check_public(public_dets)
     self.img[slot].copy_(images)
     if pre_hms is not None:
       self.hm[slot].copy_(pre_hms)
+    if pub is not None:
+      self._fill_public(self.h_pub[slot], pub)
+      self.pub[slot][0].copy_(self.h_pub[slot][0])
+      self.pub[slot][1].copy_(self.h_pub[slot][1])
 
   def _launch(self, slot):
     if self.t == 0:
@@ -143,11 +188,15 @@ class StreamRunner(object):
     self.t += 1
     return self.rec
 
-  def step_host(self, images, pre_hms=None):
+  def step_host(self, images, pre_hms=None, public_dets=None):
     """images [B,3,H,W] (and pre_hms [B,1,H,W] unless device_tracking): float32 HOST tensors (what
-    Detector.pre_process / _get_additional_inputs produce).  Returns the records of the PREVIOUS call (None the first
-    time) -- a one-step software pipeline: this step's H2D overlaps the previous step's compute."""
+    Detector.pre_process / _get_additional_inputs produce); with --public_det, public_dets = B arrays [P_b, 2] (the
+    `ct`s of each frame's public detections).  Returns the records of the PREVIOUS call (None the first time) -- a
+    one-step software pipeline: this step's H2D overlaps the previous step's compute."""
+    pub = self._check_public(public_dets)
     slot = self.t % NS
+    if pub is not None:        # the slot's staging was last read by step t-3's upload, which the last fetch() waited for
+      self._fill_public(self.h_pub[slot], pub)
     use_hm = self.tracker is None and pre_hms is not None
     src_img, src_hm = images, pre_hms
     if not images.is_pinned() or (use_hm and not pre_hms.is_pinned()):   # pageable input: stage through pinned memory
@@ -161,6 +210,9 @@ class StreamRunner(object):
       self.img[slot].copy_(src_img, non_blocking=True)
       if use_hm:
         self.hm[slot].copy_(src_hm, non_blocking=True)
+      if pub is not None:
+        self.pub[slot][0].copy_(self.h_pub[slot][0], non_blocking=True)
+        self.pub[slot][1].copy_(self.h_pub[slot][1], non_blocking=True)
       self.ev_in[slot].record(self.copy)
     prev = self.fetch() if self.t > 0 else None
     with torch.cuda.stream(self.compute):
@@ -191,7 +243,8 @@ class StreamRunner(object):
 
   @property
   def h2d_bytes_per_step(self):
-    return self.B * (3 if self.tracker is not None else 4) * self.H * self.W * 4
+    pub = self.B * (self.tracker.max_public * 2 + 1) * 4 if self.public else 0
+    return self.B * (3 if self.tracker is not None else 4) * self.H * self.W * 4 + pub
 
   @property
   def d2h_bytes_per_step(self):

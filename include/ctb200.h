@@ -21,6 +21,7 @@
  *   ct_track_step     generic_post_process's affine (utils/post_process.py:21-91) + Tracker.step's greedy association
  *                     (utils/tracker.py:28-138) + the (centre, radius) boxes of _get_additional_inputs for the next
  *                     frame, per stream, on the device;  ct_render_tracks splats those boxes (image.py:128-154).
+ *                     ct_track_step_assoc adds --hungarian and --public_det association (tracker.py:52-72,83-103).
  *   ct_flip_merge     Detector._flip_output, detector.py:311-332 (flip_tensor / flip_lr / flip_lr_off, model/utils.py:28-50).
  *   ct_warp_affine_normalize   Detector.pre_process's cv2.warpAffine + normalise + HWC->CHW, detector.py:207-226.
  */
@@ -247,8 +248,24 @@ typedef struct {
   float* boxes;               /* out [B,T,5] rows (b, cx, cy, radius, 0) for ct_render_tracks, radius < 0 = skip; or NULL */
 } ct_track_desc;
 
+/* Association mode of ct_track_step_assoc (tracker.py:52-72,83-103).  All zero = ct_track_step. */
+typedef struct {
+  int32_t hungarian;          /* 1: --hungarian, scipy.optimize.linear_sum_assignment's assignment (same tie-breaking) */
+  int32_t public_det;         /* 1: --public_det, tracks are born only where a public detection claims a detection */
+  int32_t max_public;         /* P: row stride of public_ct (> 0 when public_det) */
+  const float* public_ct;     /* [B,P,2] fp32 public detection centres, image coordinates; needed when public_det */
+  const int32_t* public_n;    /* [B] public detections of each stream (clamped to [0, P] on the device) */
+  int32_t* steps;             /* out [B] Dijkstra search steps of this frame's Hungarian solve (0 if none), or NULL */
+} ct_track_assoc;
+
 int64_t ct_track_smem_bytes(int32_t K, int32_t max_tracks);
 int ct_track_step(const ct_track_desc* d, void* stream);
+/* Shared memory of ct_track_step_assoc with hungarian or public_det set (the solver's scratch comes on top). */
+int64_t ct_track_assoc_smem_bytes(int32_t K, int32_t max_tracks);
+/* ct_track_step with the association mode `a`: same kernel, same phases; the greedy, private-birth path is
+ * ct_track_step's.  Unmatched detections / tracks are born / coast in the reference's order (naturally unmatched
+ * ascending, then those of rejected Hungarian pairs in pair order); public births come in public-detection order. */
+int ct_track_step_assoc(const ct_track_desc* d, const ct_track_assoc* a, void* stream);
 /* pre_hm (fp32 [B,1,H,W], zeroed here) <- max-splat of boxes [n,5] (rows with radius < 0 skipped); n is the grid size,
  * so the launch shape does not depend on the data (CUDA-graph capturable). */
 int ct_render_tracks(const float* boxes, int32_t n, float* pre_hm, int32_t B, int32_t H, int32_t W, void* stream);

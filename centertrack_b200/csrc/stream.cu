@@ -3,7 +3,9 @@
 //                    (utils/post_process.py:21-91, utils/tracker.py:28-138) on the packed decode records, plus the
 //                    (centre, radius) boxes of Detector._get_additional_inputs (detector.py:254-290) for the NEXT frame;
 //                    ct_track_step_assoc: the same kernel with --hungarian (scipy's linear_sum_assignment restated,
-//                    one warp) and / or --public_det births (tracker.py:52-72,83-103)
+//                    one warp) and / or --public_det births (tracker.py:52-72,83-103); ct_track_step_payload: also
+//                    the pose / 3D / velocity / attribute fields of generic_post_process (post_process.py:55-89) in a
+//                    payload table beside the track table, and the amodal centre on 3D head sets
 //   ct_render_tracks the gaussian max-splat of those boxes into pre_hm (image.py:128-154)
 //   ct_flip_merge    Detector._flip_output (detector.py:311-332; model/utils.py:28-50) for --flip_test
 //   ct_warp_affine_normalize   Detector.pre_process's cv2.warpAffine(INTER_LINEAR) + (x/255 - mean)/std + HWC->CHW
@@ -44,6 +46,8 @@ constexpr int TF = CT_TRK_FLOATS;
 struct TrackArgs {
   ct_track_desc d;
   ct_track_assoc as;       // all zero: greedy association, private births (ct_track_step)
+  ct_track_payload p;      // read by the payload instantiation only
+  int pay_smem;            // byte offset of the staged payload rows in dynamic shared memory
 };
 
 // bytes of the greedy layout before the association scratch (a multiple of 8: the scratch starts with fp64 arrays)
@@ -220,6 +224,50 @@ __device__ int public_claims(const float* pc, int P, const float* s_px, const fl
   return n;
 }
 
+// The payload row of one detection (ct_track_payload's field order), generic_post_process's fp32 arithmetic
+// (post_process.py:55-89, ddd_utils.py:91-136): r = its record, ct = its (amodal) image centre, P = the stream's calib.
+__device__ __forceinline__ void det_payload(const ct_track_payload& p, const float* r, const float* to,
+                                            const float* ct, const float* P, float* out) {
+  int o = 0;
+  if (p.rec_hps >= 0)
+    for (int k = 0; k < p.hps_floats; k += 2) {
+      const float x = r[p.rec_hps + k], y = r[p.rec_hps + k + 1];
+      out[o++] = aff_f32(to, x, y);
+      out[o++] = aff_f32(to + 3, x, y);
+    }
+  if (p.rec_dep >= 0) out[o++] = r[p.rec_dep];
+  if (p.rec_dim >= 0)
+    for (int k = 0; k < 3; ++k) out[o++] = r[p.rec_dim + k];
+  float alpha = 0.f;
+  // np.arctan2 on float32 operands is atan2f here (within 3 ulp; an fp64 atan2 put the kernel on a stack frame)
+  if (p.rec_rot >= 0) {          // get_alpha: bin 1 when rot[1] > rot[5]; the +-pi/2 is a float32 constant
+    const float* q = r + p.rec_rot;
+    const float hp = (float)(0.5 * CUDART_PI);
+    alpha = q[1] > q[5] ? __fadd_rn(atan2f(q[2], q[3]), -hp) : __fadd_rn(atan2f(q[6], q[7]), hp);
+    out[o++] = alpha;
+  }
+  if (p.rec_rot >= 0 && p.rec_dep >= 0 && p.rec_dim >= 0) {
+    // ddd2locrot: unproject_2d_to_3d in fp32, loc[1] += dim[0] / 2, then alpha2rot_y (alpha is fp64 there)
+    const float dep = r[p.rec_dep];
+    const float z = __fsub_rn(dep, P[11]);
+    const float x = __fdiv_rn(__fsub_rn(__fsub_rn(__fmul_rn(ct[0], dep), P[3]), __fmul_rn(P[2], z)), P[0]);
+    const float y = __fdiv_rn(__fsub_rn(__fsub_rn(__fmul_rn(ct[1], dep), P[7]), __fmul_rn(P[6], z)), P[5]);
+    out[o++] = x;
+    out[o++] = __fadd_rn(y, __fmul_rn(r[p.rec_dim], 0.5f));
+    out[o++] = z;
+    double ry = (double)alpha + (double)atan2f(__fsub_rn(ct[0], P[2]), P[0]);
+    if (ry > CUDART_PI) ry -= 2 * CUDART_PI;
+    if (ry < -CUDART_PI) ry += 2 * CUDART_PI;
+    out[o++] = (float)ry;
+  }
+  if (p.rec_velocity >= 0)
+    for (int k = 0; k < p.velocity_floats; ++k) out[o++] = r[p.rec_velocity + k];
+  if (p.rec_nuscenes_att >= 0)
+    for (int k = 0; k < p.att_floats; ++k) out[o++] = r[p.rec_nuscenes_att + k];
+}
+
+// PAY: also write the payload table (ct_track_step_payload); the 2-D head sets run the <false> instantiation.
+template <bool PAY>
 __global__ void __launch_bounds__(TRK_THREADS)
 track_step_kernel(const TrackArgs a) {
   extern __shared__ __align__(16) unsigned char tsm[];
@@ -255,6 +303,12 @@ track_step_kernel(const TrackArgs a) {
   const int id_count = d.counts[b * 2 + 1];
   float* trk = d.tracks + (size_t)b * T * TF;
   for (int i = tid; i < M * TF; i += TRK_THREADS) s_old[i] = trk[i];
+  // payload rows are permuted in place like the track rows: the old ones are staged before any is written
+  const int Wp = PAY ? a.p.width : 0;
+  float* pay = PAY ? a.p.payload + (size_t)b * T * Wp : nullptr;
+  float* s_oldp = reinterpret_cast<float*>(tsm + a.pay_smem);  // [T][Wp]
+  if constexpr (PAY)
+    for (int i = tid; i < M * Wp; i += TRK_THREADS) s_oldp[i] = pay[i];
   if (tid == 0) s_n = 0;
   __syncthreads();
 
@@ -266,6 +320,7 @@ track_step_kernel(const TrackArgs a) {
   atomicAdd(&s_n, cnt);
   __syncthreads();
   const int N = s_n;                     // records are sorted by score: the kept detections are a prefix
+  const bool amodal = PAY && a.p.rec_rot >= 0 && a.p.rec_dep >= 0 && a.p.rec_dim >= 0;
   for (int i = tid; i < N; i += TRK_THREADS) {
     const float* r = rec + (size_t)i * d.F;
     float* o = s_det + (size_t)i * TF;
@@ -285,8 +340,20 @@ track_step_kernel(const TrackArgs a) {
     o[CT_TRK_BBOX] = aff_f32(to, bl, bt); o[CT_TRK_BBOX + 1] = aff_f32(to + 3, bl, bt);
     o[CT_TRK_BBOX + 2] = aff_f32(to, br, bb); o[CT_TRK_BBOX + 3] = aff_f32(to + 3, br, bb);
     o[CT_TRK_ID] = 0.f; o[CT_TRK_AGE] = 1.f; o[CT_TRK_ACTIVE] = 0.f;
-    s_px[i] = __fadd_rn(ctx, tx);
-    s_py[i] = __fadd_rn(cty, ty);
+    float acx = ctx, acy = cty;
+    if (amodal) {      // post_process.py:76-84: ct becomes the amodal centre after `tracking` was taken from the peak
+      if (a.p.rec_amodel_offset >= 0) {   // numpy's fp32 mean of the two output-grid corners + amodel_offset
+        const float mx = __fadd_rn(__fmul_rn(__fadd_rn(bl, br), 0.5f), r[a.p.rec_amodel_offset]);
+        const float my = __fadd_rn(__fmul_rn(__fadd_rn(bt, bb), 0.5f), r[a.p.rec_amodel_offset + 1]);
+        acx = aff_f32(to, mx, my); acy = aff_f32(to + 3, mx, my);
+      } else {                            // the image box centre
+        acx = __fmul_rn(__fadd_rn(o[CT_TRK_BBOX], o[CT_TRK_BBOX + 2]), 0.5f);
+        acy = __fmul_rn(__fadd_rn(o[CT_TRK_BBOX + 1], o[CT_TRK_BBOX + 3]), 0.5f);
+      }
+      o[CT_TRK_CT] = acx; o[CT_TRK_CT + 1] = acy;
+    }
+    s_px[i] = __fadd_rn(acx, tx);
+    s_py[i] = __fadd_rn(acy, ty);
     s_isz[i] = __fmul_rn(__fsub_rn(o[CT_TRK_BBOX + 2], o[CT_TRK_BBOX]), __fsub_rn(o[CT_TRK_BBOX + 3], o[CT_TRK_BBOX + 1]));
     s_match[i] = -1;
   }
@@ -410,6 +477,16 @@ track_step_kernel(const TrackArgs a) {
   for (int e = tid; e < M * TF; e += TRK_THREADS) {
     const int j = e / TF, f = e - j * TF;
     if (s_pos_trk[j] >= 0) trk[(size_t)s_pos_trk[j] * TF + f] = s_old[e];
+  }
+  if constexpr (PAY) {           // detections: computed from the read-only records; coasting tracks: their staged rows
+    const float* P = a.p.calib ? a.p.calib + b * 12 : nullptr;
+    for (int i = tid; i < N; i += TRK_THREADS)
+      if (s_pos_det[i] >= 0)
+        det_payload(a.p, rec + (size_t)i * d.F, to, s_det + (size_t)i * TF + CT_TRK_CT, P, pay + (size_t)s_pos_det[i] * Wp);
+    for (int e = tid; e < M * Wp; e += TRK_THREADS) {
+      const int j = e / Wp, f = e - j * Wp;
+      if (s_pos_trk[j] >= 0) pay[(size_t)s_pos_trk[j] * Wp + f] = s_oldp[e];
+    }
   }
   if (tid == 0) { d.counts[b * 2 + 0] = total; d.counts[b * 2 + 1] = s_ids; }
   __syncthreads();     // the table rows written above are re-read below by other threads
@@ -547,24 +624,57 @@ extern "C" int64_t ct_track_assoc_smem_bytes(int32_t K, int32_t max_tracks) {
          (int64_t)(4 * (3 * (size_t)max_tracks + 3 * (size_t)K));
 }
 
-extern "C" int ct_track_step_assoc(const ct_track_desc* d, const ct_track_assoc* as, void* stream) {
+extern "C" int64_t ct_track_payload_smem_bytes(int32_t K, int32_t max_tracks, int32_t width, int32_t assoc) {
+  return (assoc ? ct_track_assoc_smem_bytes(K, max_tracks) : ct_track_smem_bytes(K, max_tracks)) +
+         (int64_t)max_tracks * width * 4;
+}
+
+// a record field of `w` floats at `off` (-1 = absent) lies inside the heads part of an F-float record
+static inline bool rec_field_ok(int32_t off, int32_t w, int32_t F) {
+  return off < 0 || (w > 0 && off >= CT_REC_HEADS && off + w <= F);
+}
+
+extern "C" int ct_track_step_payload(const ct_track_desc* d, const ct_track_assoc* as, const ct_track_payload* p,
+                                     void* stream) {
   CT_REQUIRE(d && as && d->records && d->trans_out_inv && d->tracks && d->counts, "null pointer");
   CT_REQUIRE(d->B > 0 && d->K > 0 && d->F >= CT_REC_HEADS && d->max_tracks >= d->K, "bad shape");
   CT_REQUIRE(d->rec_tracking < 0 || d->rec_tracking + 2 <= d->F, "tracking offset outside the record");
   CT_REQUIRE(d->boxes == nullptr || (d->trans_input != nullptr && d->inp_h > 0 && d->inp_w > 0), "boxes need trans_input");
   CT_REQUIRE(!as->public_det || (as->public_ct && as->public_n), "public_det needs public_ct and public_n");
   CT_REQUIRE(!as->public_det || as->max_public > 0, "public_det needs max_public > 0");
+  if (p) {
+    CT_REQUIRE(p->payload, "null payload table");
+    CT_REQUIRE(rec_field_ok(p->rec_hps, p->hps_floats, d->F) && (p->rec_hps < 0 || p->hps_floats % 2 == 0) &&
+               rec_field_ok(p->rec_dep, 1, d->F) && rec_field_ok(p->rec_dim, 3, d->F) &&
+               rec_field_ok(p->rec_rot, 8, d->F) && rec_field_ok(p->rec_amodel_offset, 2, d->F) &&
+               rec_field_ok(p->rec_velocity, p->velocity_floats, d->F) &&
+               rec_field_ok(p->rec_nuscenes_att, p->att_floats, d->F), "payload field outside the record");
+    const bool ddd = p->rec_rot >= 0 && p->rec_dep >= 0 && p->rec_dim >= 0;
+    const int64_t w = (p->rec_hps >= 0 ? p->hps_floats : 0) + (p->rec_dep >= 0 ? 1 : 0) + (p->rec_dim >= 0 ? 3 : 0) +
+                      (p->rec_rot >= 0 ? 1 : 0) + (ddd ? 4 : 0) + (p->rec_velocity >= 0 ? p->velocity_floats : 0) +
+                      (p->rec_nuscenes_att >= 0 ? p->att_floats : 0);
+    CT_REQUIRE(w > 0 && p->width == w, "payload width does not match its fields");
+    CT_REQUIRE(!ddd || p->calib, "rot, dep and dim need calib");
+  }
   const bool scratch = as->hungarian || as->public_det;
-  const size_t smem = (size_t)(scratch ? ct_track_assoc_smem_bytes(d->K, d->max_tracks)
-                                       : ct_track_smem_bytes(d->K, d->max_tracks));
+  const size_t smem = (size_t)ct_track_payload_smem_bytes(d->K, d->max_tracks, p ? p->width : 0, scratch);
   CT_REQUIRE(smem <= 200 * 1024, "track table does not fit in shared memory (lower max_tracks)");
+  auto kernel = p ? track_step_kernel<true> : track_step_kernel<false>;
   if (smem > 48 * 1024)
-    CT_CUDA_OK(cudaFuncSetAttribute(track_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  TrackArgs a;
+    CT_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  TrackArgs a = {};
   a.d = *d;
   a.as = *as;
-  track_step_kernel<<<d->B, TRK_THREADS, smem, (cudaStream_t)stream>>>(a);
+  if (p) a.p = *p;
+  a.pay_smem = (int)(trk_base_bytes(d->K, d->max_tracks) +
+                     (scratch ? ct_track_assoc_smem_bytes(d->K, d->max_tracks) - ct_track_smem_bytes(d->K, d->max_tracks)
+                              : 0));
+  kernel<<<d->B, TRK_THREADS, smem, (cudaStream_t)stream>>>(a);
   return after_launch();
+}
+
+extern "C" int ct_track_step_assoc(const ct_track_desc* d, const ct_track_assoc* as, void* stream) {
+  return ct_track_step_payload(d, as, nullptr, stream);
 }
 
 extern "C" int ct_track_step(const ct_track_desc* d, void* stream) {

@@ -6,8 +6,10 @@ Hungarian / public-detection modes) and `ct_render_tracks` -- so that a stream n
 frames: records(t) -> tracks(t) -> pre_hm(t+1) are all device-resident and CUDA-graph capturable (fixed launch shapes).
 Every mode reproduces the host `Tracker` (centertrack_b200.tracker) row for row.
 Results are rows of CT_TRK_FLOATS fp32 (score, class, ct, tracking, bbox, tracking_id, age, active) in the
-reference's output order (matched detections, new tracks, coasting tracks); `results()` turns a host copy into the
-reference's list of dicts.
+reference's output order (matched detections, new tracks, coasting tracks).  Pose, 3D, velocity and attribute head
+sets also get a parallel payload table [B,T,Wp] (`ct_track_step_payload`) with the fields generic_post_process adds
+for them (hps, dep, dim, alpha, loc, rot_y, velocity, nuscenes_att); on 3D head sets `ct` is the amodal centre, as in
+the reference.  `results()` turns host copies into the reference's list of dicts.
 """
 import ctypes as C
 
@@ -15,16 +17,42 @@ import numpy as np
 import torch
 
 from . import _lib as L
+from .dataset_info import get_dataset
 from .image import get_affine_transform
+
+# widths of the record heads a payload field is computed from, as the reference's heads have them (opts.py)
+_HEAD_WIDTHS = {'dep': 1, 'dim': 3, 'rot': 8, 'amodel_offset': 2}
+
+
+def payload_layout(layout):
+  """Decode record layout {head: (offset, width)} -> the payload row {field: (offset, width)}, in ct_track_payload's
+  order: each field generic_post_process adds for the heads present (post_process.py:55-89).  {} for 2-D head sets."""
+  for k, w in _HEAD_WIDTHS.items():
+    if k in layout and layout[k][1] != w:
+      raise ValueError('%s head with %d channels, expected %d' % (k, layout[k][1], w))
+  fields = []
+  if 'hps' in layout:
+    fields.append(('hps', layout['hps'][1]))
+  fields += [(f, w) for f, head, w in (('dep', 'dep', 1), ('dim', 'dim', 3), ('alpha', 'rot', 1)) if head in layout]
+  if all(k in layout for k in ('rot', 'dep', 'dim')):
+    fields += [('loc', 3), ('rot_y', 1)]
+  fields += [(k, layout[k][1]) for k in ('velocity', 'nuscenes_att') if k in layout]
+  out, off = {}, 0
+  for f, w in fields:
+    out[f] = (off, w)
+    off += w
+  return out
 
 
 class DeviceTracker(object):
 
   def __init__(self, opt, B, K, rec_floats, layout, inp_h, inp_w, device, centers=None, scales=None, max_tracks=None,
-               max_public_dets=512):
+               max_public_dets=512, calibs=None):
     """centers/scales: per-stream (c, s) of the source rectangle (Detector._input_geometry); default = a source image
     of exactly the network input size (the synthetic benchmark streams).  max_public_dets: with --public_det, the most
-    public detections one stream may bring per frame (P, the row count of the public_ct buffers step() takes)."""
+    public detections one stream may bring per frame (P, the row count of the public_ct buffers step() takes).
+    calibs: per-stream [3,4] camera matrices for the 3D head sets (loc, rot_y); default = Detector._get_default_calib
+    of a source image centred on c, with --test_focal_length or the dataset's rest_focal_length."""
     self.hungarian = bool(getattr(opt, 'hungarian', False))
     self.public_det = bool(getattr(opt, 'public_det', False))
     self.max_public = int(max_public_dets)
@@ -63,14 +91,46 @@ class DeviceTracker(object):
     a = L.TrackAssoc()
     a.hungarian, a.public_det, a.max_public = int(self.hungarian), int(self.public_det), self.max_public
     self.assoc = a
-    smem = L.lib().ct_track_assoc_smem_bytes if (self.hungarian or self.public_det) else L.lib().ct_track_smem_bytes
-    if smem(K, self.T) > 200 * 1024:
+    self.payload_layout = payload_layout(layout)
+    self.Wp = sum(w for _, w in self.payload_layout.values())
+    self.payload = self.calib = self.pay = None
+    if self.Wp:
+      self.payload = torch.zeros((B, self.T, self.Wp), dtype=torch.float32, device=self.device)
+      p = L.TrackPayload()
+      p.width, p.payload = self.Wp, self.payload.data_ptr()
+      rec = lambda k: layout[k][0] if k in layout else -1
+      p.rec_hps = rec('hps_refined' if 'hps_refined' in layout else 'hps')      # as decode.views_from_records
+      p.hps_floats = layout['hps'][1] if 'hps' in layout else 0
+      p.rec_dep, p.rec_dim, p.rec_rot, p.rec_amodel_offset = rec('dep'), rec('dim'), rec('rot'), rec('amodel_offset')
+      p.rec_velocity, p.velocity_floats = rec('velocity'), layout.get('velocity', (0, 0))[1]
+      p.rec_nuscenes_att, p.att_floats = rec('nuscenes_att'), layout.get('nuscenes_att', (0, 0))[1]
+      if 'loc' in self.payload_layout:
+        self.calib = torch.from_numpy(self._calibs(opt, calibs, centers, inp_h, inp_w)).to(self.device)
+        p.calib = self.calib.data_ptr()
+      self.pay = p
+    smem = L.lib().ct_track_payload_smem_bytes(K, self.T, self.Wp, int(self.hungarian or self.public_det))
+    if smem > 200 * 1024:
       raise ValueError('track table of %d rows does not fit in shared memory' % self.T)
+
+  def _calibs(self, opt, calibs, centers, inp_h, inp_w):
+    if calibs is not None:
+      out = np.asarray(calibs, np.float32)
+      if out.shape != (self.B, 3, 4):
+        raise ValueError('calibs: expected %d camera matrices [3, 4], got shape %s' % (self.B, out.shape))
+      return np.ascontiguousarray(out)
+    f = opt.test_focal_length if getattr(opt, 'test_focal_length', -1) >= 0 else get_dataset(opt.dataset).rest_focal_length
+    out = np.zeros((self.B, 3, 4), np.float32)
+    for b in range(self.B):
+      cx, cy = (inp_w / 2., inp_h / 2.) if centers is None else (float(centers[b][0]), float(centers[b][1]))
+      out[b] = [[f, 0, cx, 0], [0, f, cy, 0], [0, 0, 1, 0]]      # Detector._get_default_calib(2 cx, 2 cy)
+    return out
 
   def reset(self):
     """Detector.reset_tracking / Tracker.reset for every stream."""
     self.tracks.zero_()
     self.counts.zero_()
+    if self.payload is not None:
+      self.payload.zero_()
     self.boxes.zero_()
     self.boxes[:, :, 3] = -1.0
 
@@ -89,7 +149,7 @@ class DeviceTracker(object):
       raise ValueError('--public_det: step() needs the public detections (public_ct, public_n)')
     assert records.is_cuda and records.dtype == torch.float32 and tuple(records.shape) == (self.B, self.K, self.F)
     self.desc.records = records.data_ptr()
-    if not (self.hungarian or self.public_det or steps is not None):
+    if self.pay is None and not (self.hungarian or self.public_det or steps is not None):
       L.check(L.lib().ct_track_step(C.byref(self.desc), L.stream_ptr()), 'ct_track_step')
       return
     a = self.assoc
@@ -104,7 +164,11 @@ class DeviceTracker(object):
     if steps is not None:
       assert steps.is_cuda and steps.dtype == torch.int32 and tuple(steps.shape) == (self.B,)
     a.steps = steps.data_ptr() if steps is not None else None
-    L.check(L.lib().ct_track_step_assoc(C.byref(self.desc), C.byref(a), L.stream_ptr()), 'ct_track_step_assoc')
+    if self.pay is not None:
+      L.check(L.lib().ct_track_step_payload(C.byref(self.desc), C.byref(a), C.byref(self.pay), L.stream_ptr()),
+              'ct_track_step_payload')
+    else:
+      L.check(L.lib().ct_track_step_assoc(C.byref(self.desc), C.byref(a), L.stream_ptr()), 'ct_track_step_assoc')
 
   def render(self, pre_hm):
     """pre_hm [B,1,H,W] fp32 <- splat of the current tracks (what the NEXT frame's network reads)."""
@@ -114,16 +178,25 @@ class DeviceTracker(object):
 
   @property
   def d2h_bytes(self):
-    return self.tracks.numel() * 4 + self.counts.numel() * 4
+    return self.tracks.numel() * 4 + self.counts.numel() * 4 + (self.payload.numel() * 4 if self.Wp else 0)
 
-  @staticmethod
-  def results(tracks_np, counts_np):
-    """Host copies -> [[{score, class, ct, tracking, bbox, tracking_id, age, active}, ...] per stream]."""
+  def results(self, tracks_np, counts_np, payload_np=None):
+    """Host copies -> [[{score, class, ct, tracking, bbox, tracking_id, age, active}, ...] per stream], plus the payload
+    fields of the head set (payload_np [B,T,Wp], needed when it has any) with the host path's shapes: hps [2J],
+    dep [1], dim [3], alpha, loc [3], rot_y, velocity, nuscenes_att."""
+    if self.Wp and payload_np is None:
+      raise ValueError('results(): this head set has payload fields (%s): pass payload_np' %
+                       ', '.join(self.payload_layout))
     out = []
     for b in range(tracks_np.shape[0]):
-      rows = tracks_np[b, :int(counts_np[b, 0])]
-      out.append([{'score': float(r[L.CT_TRK_SCORE]), 'class': int(r[L.CT_TRK_CLASS]),
-                   'ct': r[L.CT_TRK_CT:L.CT_TRK_CT + 2].copy(), 'tracking': r[L.CT_TRK_TRACKING:L.CT_TRK_TRACKING + 2].copy(),
-                   'bbox': r[L.CT_TRK_BBOX:L.CT_TRK_BBOX + 4].copy(), 'tracking_id': int(r[L.CT_TRK_ID]),
-                   'age': int(r[L.CT_TRK_AGE]), 'active': int(r[L.CT_TRK_ACTIVE])} for r in rows])
+      n = int(counts_np[b, 0])
+      rows = tracks_np[b, :n]
+      res = [{'score': float(r[L.CT_TRK_SCORE]), 'class': int(r[L.CT_TRK_CLASS]),
+              'ct': r[L.CT_TRK_CT:L.CT_TRK_CT + 2].copy(), 'tracking': r[L.CT_TRK_TRACKING:L.CT_TRK_TRACKING + 2].copy(),
+              'bbox': r[L.CT_TRK_BBOX:L.CT_TRK_BBOX + 4].copy(), 'tracking_id': int(r[L.CT_TRK_ID]),
+              'age': int(r[L.CT_TRK_AGE]), 'active': int(r[L.CT_TRK_ACTIVE])} for r in rows]
+      for item, q in zip(res, payload_np[b, :n] if self.Wp else ()):
+        for k, (o, w) in self.payload_layout.items():
+          item[k] = float(q[o]) if k in ('alpha', 'rot_y') else q[o:o + w].copy()
+      out.append(res)
     return out

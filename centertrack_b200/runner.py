@@ -17,7 +17,8 @@ Two ways to feed the prior heat-map (`--pre_hm`):
   * device_tracking=True (SURVEY 8f-1): the reference's dependency chain closed ON THE DEVICE, inside the same graph:
         pre_hm(t) = splat(tracks(t-1))  ->  network + decode -> records(t)  ->  tracks(t) = Tracker.step(records(t))
     (`DeviceTracker`: ct_render_tracks, ct_track_step).  Exact reference semantics (no stale prior), no host round
-    trip; the host uploads only the frame and downloads the track table (ids, boxes, ages).  Every association mode
+    trip; the host uploads only the frame and downloads the track table (ids, boxes, ages), and for pose / 3D head sets
+    the payload table beside it (hps, dep, dim, alpha, loc, rot_y, velocity, nuscenes_att).  Every association mode
     of the host Tracker runs there: greedy, `--hungarian`, and `--public_det`, whose public detections (the `ct`s of
     each frame's provided detections) are staged per input slot like the frames and uploaded with them.
 
@@ -38,9 +39,10 @@ NS = 3          # input slots
 class StreamRunner(object):
 
   def __init__(self, model, B, H, W, K=100, precision='bf16', device='cuda', use_graph=True, opt=None,
-               device_tracking=False, max_public_dets=512):
+               device_tracking=False, max_public_dets=512, calibs=None):
     """max_public_dets: with device_tracking and --public_det, the most public detections a stream may bring per
-    frame (more raise ValueError; none is ever dropped)."""
+    frame (more raise ValueError; none is ever dropped).  calibs: with device_tracking on a 3D head set, one [3,4]
+    camera matrix per stream (DeviceTracker's default otherwise)."""
     self.B, self.H, self.W, self.K = B, H, W, K
     self.device = torch.device(device)
     self.model = model
@@ -68,7 +70,7 @@ class StreamRunner(object):
     if device_tracking:
       assert self.opt is not None, 'device tracking needs opt (thresholds, max_age)'
       self.tracker = DeviceTracker(self.opt, B, K, self.rec.shape[2], self.layout, H, W, self.device,
-                                   max_public_dets=max_public_dets)
+                                   max_public_dets=max_public_dets, calibs=calibs)
     self.public = self.tracker is not None and self.tracker.public_det
     if self.public:                                          # per slot: device (public_ct, public_n) + pinned staging
       self.pub = [self.tracker.public_buffers() for _ in range(NS)]
@@ -78,6 +80,8 @@ class StreamRunner(object):
     if self.tracker is not None:
       self.h_trk = [torch.zeros_like(self.tracker.tracks, device='cpu').pin_memory() for _ in range(2)]
       self.h_cnt = [torch.zeros_like(self.tracker.counts, device='cpu').pin_memory() for _ in range(2)]
+      if self.tracker.payload is not None:
+        self.h_pay = [torch.zeros_like(self.tracker.payload, device='cpu').pin_memory() for _ in range(2)]
     # launches of one step: the network plan + decode (+ memset-free: render + track step)
     self.launches_per_step = self.eng.n_launches + 1 + (2 if device_tracking else 0)
 
@@ -103,7 +107,7 @@ class StreamRunner(object):
     if self.graphs[slot] is None:
       saved = None
       if self.tracker is not None:                           # capture must not disturb live stream state
-        saved = (self.tracker.tracks.clone(), self.tracker.counts.clone(), self.tracker.boxes.clone())
+        saved = [t.clone() for t in self._tracker_state()]
       s = torch.cuda.Stream(device=self.device)
       s.wait_stream(torch.cuda.current_stream())
       with torch.cuda.stream(s):
@@ -114,8 +118,13 @@ class StreamRunner(object):
         self._eager(slot)
       self.graphs[slot] = g
       if saved is not None:
-        self.tracker.tracks.copy_(saved[0]); self.tracker.counts.copy_(saved[1]); self.tracker.boxes.copy_(saved[2])
+        for t, v in zip(self._tracker_state(), saved):
+          t.copy_(v)
     return self.graphs[slot]
+
+  def _tracker_state(self):
+    trk = self.tracker
+    return [trk.tracks, trk.counts, trk.boxes] + ([trk.payload] if trk.payload is not None else [])
 
   def warm(self):
     for s in range(NS):
@@ -222,6 +231,8 @@ class StreamRunner(object):
       if self.tracker is not None:
         self.h_trk[self.t & 1].copy_(self.tracker.tracks, non_blocking=True)
         self.h_cnt[self.t & 1].copy_(self.tracker.counts, non_blocking=True)
+        if self.tracker.payload is not None:
+          self.h_pay[self.t & 1].copy_(self.tracker.payload, non_blocking=True)
       # this step's pre_images slot may be overwritten once this step is done
       self.ev_done[(slot - 1) % NS].record(self.compute)
     self.t += 1
@@ -240,6 +251,14 @@ class StreamRunner(object):
     self.compute.synchronize()
     i = (self.t - 1) & 1
     return self.h_trk[i].numpy().copy(), self.h_cnt[i].numpy().copy()
+
+  def fetch_results(self):
+    """The last submitted step's tracks (device_tracking) as the host path's per-stream lists of dicts
+    (DeviceTracker.results), payload fields included."""
+    self.compute.synchronize()
+    i = (self.t - 1) & 1
+    pay = self.h_pay[i].numpy() if self.tracker.payload is not None else None
+    return self.tracker.results(self.h_trk[i].numpy(), self.h_cnt[i].numpy(), pay)
 
   @property
   def h2d_bytes_per_step(self):

@@ -21,7 +21,8 @@
  *   ct_track_step     generic_post_process's affine (utils/post_process.py:21-91) + Tracker.step's greedy association
  *                     (utils/tracker.py:28-138) + the (centre, radius) boxes of _get_additional_inputs for the next
  *                     frame, per stream, on the device;  ct_render_tracks splats those boxes (image.py:128-154).
- *                     ct_track_step_assoc adds --hungarian and --public_det association (tracker.py:52-72,83-103).
+ *                     ct_track_step_assoc adds --hungarian and --public_det association (tracker.py:52-72,83-103);
+ *                     ct_track_step_payload adds the pose / 3D / velocity / attribute fields (post_process.py:55-89).
  *   ct_flip_merge     Detector._flip_output, detector.py:311-332 (flip_tensor / flip_lr / flip_lr_off, model/utils.py:28-50).
  *   ct_warp_affine_normalize   Detector.pre_process's cv2.warpAffine + normalise + HWC->CHW, detector.py:207-226.
  */
@@ -266,6 +267,32 @@ int64_t ct_track_assoc_smem_bytes(int32_t K, int32_t max_tracks);
  * ct_track_step's.  Unmatched detections / tracks are born / coast in the reference's order (naturally unmatched
  * ascending, then those of rejected Hungarian pairs in pair order); public births come in public-detection order. */
 int ct_track_step_assoc(const ct_track_desc* d, const ct_track_assoc* a, void* stream);
+
+/* Task fields of generic_post_process (post_process.py:55-89) kept beside the track table: payload row r belongs to
+ * track row r, written by the same launch in the same order; coasting tracks keep theirs unchanged.  A row holds, in
+ * this order and each only when its record offset is >= 0:
+ *   hps [hps_floats]        keypoints through the output affine (rec_hps: the refined keypoints when decode refined them)
+ *   dep [1], dim [3]        copied
+ *   alpha [1]               get_alpha(rot)                                          (rec_rot)
+ *   loc [3], rot_y [1]      ddd2locrot(amodal centre, alpha, dim, dep, calib[b])    (rec_rot, rec_dep and rec_dim)
+ *   velocity [velocity_floats], nuscenes_att [att_floats]   copied
+ * With rot, dep and dim all present the track's CT_TRK_CT is the reference's amodal centre (the output-grid box centre
+ * + amodel_offset through the affine, or the image box centre without rec_amodel_offset), and association runs on it;
+ * CT_TRK_TRACKING stays relative to the heat-map peak. */
+typedef struct {
+  int32_t width;              /* Wp: floats per payload row = the sum of the enabled fields' widths */
+  float* payload;             /* in/out [B,T,Wp] */
+  int32_t rec_hps, hps_floats;
+  int32_t rec_dep, rec_dim, rec_rot, rec_amodel_offset;
+  int32_t rec_velocity, velocity_floats;
+  int32_t rec_nuscenes_att, att_floats;
+  const float* calib;         /* [B,3,4] fp32 camera matrices; needed when rot, dep and dim are all present */
+} ct_track_payload;
+
+/* Shared memory of ct_track_step_payload: the table (with the association scratch when assoc != 0) + T payload rows. */
+int64_t ct_track_payload_smem_bytes(int32_t K, int32_t max_tracks, int32_t width, int32_t assoc);
+/* ct_track_step_assoc that also writes the payload table; p == NULL is ct_track_step_assoc. */
+int ct_track_step_payload(const ct_track_desc* d, const ct_track_assoc* a, const ct_track_payload* p, void* stream);
 /* pre_hm (fp32 [B,1,H,W], zeroed here) <- max-splat of boxes [n,5] (rows with radius < 0 skipped); n is the grid size,
  * so the launch shape does not depend on the data (CUDA-graph capturable). */
 int ct_render_tracks(const float* boxes, int32_t n, float* pre_hm, int32_t B, int32_t H, int32_t W, void* stream);

@@ -1,4 +1,5 @@
-"""Cost of the association modes on the device tracker:   python tools/track_modes_time.py [--steps 60] [--rounds 3]
+"""Cost of the association modes on the device tracker:
+    python tools/track_modes_time.py [--steps 60] [--rounds 3] [--config nuscenes_ddd | coco_pose]
 
 1. ct_track_step / ct_track_step_assoc alone at B = 32 streams, K = 100, on crowded synthetic records
    (synthetic.synthetic_track_stream with up to K detections per frame, identity output affine): microseconds per
@@ -6,6 +7,9 @@
    Dijkstra search steps one stream's Hungarian solve took in a frame.
 2. --config mot StreamRunner (960x544, bf16, B = 32, device tracking, one graph replay per step) frames/s with greedy,
    --hungarian and --public_det --hungarian association, the three runners timed alternately.
+With --config nuscenes_ddd | coco_pose: step 1 only, on the same records widened by the head set's payload columns
+(dep, rot, dim, amodel_offset / raw and refined keypoints), timed with the payload table (ct_track_step_payload) and
+without it (the same records read as a 2-D layout).
 Prints the card and its power limit with the numbers.  Needs a GPU."""
 import argparse
 import os
@@ -25,6 +29,18 @@ from helpers import make_model, make_opt               # noqa
 MODES = [('greedy', []), ('hungarian', ['--hungarian']), ('public', ['--public_det']),
          ('public_hungarian', ['--public_det', '--hungarian'])]
 B, K, F = 32, 100, 11
+# record heads after tracking (9, 2) of the payload configs
+PAYLOAD_HEADS = {'nuscenes_ddd': [('dep', 1), ('rot', 8), ('dim', 3), ('amodel_offset', 2)],
+                 'coco_pose': [('hps', 34), ('hps_refined', 34), ('kps_score', 1)]}
+
+
+def payload_layout(config):
+  """(decode layout, F) of the crowded records with the config's payload heads appended."""
+  layout, off = {'tracking': (9, 2)}, F
+  for name, w in PAYLOAD_HEADS.get(config, ()):
+    layout[name] = (off, w)
+    off += w
+  return layout, off
 
 
 def card():
@@ -37,12 +53,15 @@ def card():
   return '%s, power limit %s' % (name, pl or 'unknown')
 
 
-def track_inputs(frames=6):
-  """Per frame: records [B,K,F] on the device and the public detections (public_ct [B,P,2], public_n [B])."""
+def track_inputs(frames=6, Fr=F):
+  """Per frame: records [B,K,Fr] on the device and the public detections (public_ct [B,P,2], public_n [B]); columns
+  past F are seeded random head outputs."""
   streams = [wt.synthetic_track_stream(100 + b, frames=frames, crowd=2 * K) for b in range(B)]
+  rng = np.random.RandomState(7)
   out = []
   for f in range(frames):
-    rec = np.zeros((B, K, F), np.float32)
+    rec = np.zeros((B, K, Fr), np.float32)
+    rec[:, :, F:] = rng.uniform(0.1, 1.0, (B, K, Fr - F))
     pub = np.zeros((B, 512, 2), np.float32)
     n = np.zeros(B, np.int32)
     for b, st in enumerate(streams):
@@ -56,13 +75,15 @@ def track_inputs(frames=6):
   return out
 
 
-def time_track_step(passes=20):
-  frames = track_inputs()
+def time_track_step(passes=20, config=None, payload=False):
+  layout, Fr = payload_layout(config)
+  frames = track_inputs(Fr=Fr)
   res = {}
   for name, extra in MODES:
-    opt = make_opt('coco_tracking', ['--track_thresh', '0.2', '--new_thresh', '0.3', '--max_age', '3'] + extra)
+    opt = make_opt(config or 'coco_tracking', ['--track_thresh', '0.2', '--new_thresh', '0.3', '--max_age', '3'] + extra)
     opt.out_thresh = 0.1
-    trk = DeviceTracker(opt, B, K, F, {'tracking': (9, 2)}, 544, 960, 'cuda')
+    trk = DeviceTracker(opt, B, K, Fr, layout if payload else {'tracking': (9, 2)}, 544, 960, 'cuda')
+    assert (trk.payload is not None) == payload
     trk.trans_out_inv.copy_(torch.tensor([[1., 0., 0., 0., 1., 0.]] * B))
     steps = torch.zeros(B, dtype=torch.int32, device='cuda')
     us, max_steps, max_tracks = [], 0, 0
@@ -121,9 +142,17 @@ def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--steps', type=int, default=60)
   ap.add_argument('--rounds', type=int, default=3)
+  ap.add_argument('--config', choices=sorted(PAYLOAD_HEADS), default=None)
   args = ap.parse_args()
   assert torch.cuda.is_available(), 'needs a GPU'
   print('card:', card())
+  if args.config:
+    print('track step, --config %s, B=%d K=%d, --max_age 3 (T = %d), crowded synthetic records:' % (args.config, B, K, 4 * K))
+    for payload in (False, True):
+      print(' %s payload:' % ('with' if payload else 'without'))
+      for name, (med, lo, st, mt) in time_track_step(config=args.config, payload=payload).items():
+        print('  %-17s median %7.1f us/launch (min %7.1f), max tracks %d' % (name, med, lo, mt))
+    return
   print('track step, B=%d K=%d, --max_age 3 (T = %d), crowded synthetic records:' % (B, K, 4 * K))
   for name, (med, lo, st, mt) in time_track_step().items():
     print('  %-17s median %7.1f us/launch (min %7.1f), max Dijkstra steps in a frame %4d, max tracks %d' %

@@ -13,6 +13,7 @@ CSRC = os.path.join(_HERE, 'csrc')
 SOURCES = ['api.cu', 'conv_simt.cu', 'conv_tc.cu', 'conv_halo.cu', 'elementwise.cu', 'decode.cu', 'stream.cu']
 
 # ---- enums (mirror include/ctb200.h) ----
+CT_OK, CT_ERR_INVALID, CT_ERR_CUDA, CT_ERR_UNSUPPORTED = 0, -1, -2, -3
 CT_F32, CT_BF16 = 0, 1
 CT_A_CONV, CT_A_DCN, CT_A_DCN_WIN = 0, 1, 2
 CT_OUT_NHWC, CT_OUT_NHWC_F32, CT_OUT_NCHW_F32, CT_OUT_NHWC_S2D = 0, 1, 2, 3
@@ -36,6 +37,11 @@ class ConvDesc(C.Structure):
       ('x', C.c_void_p), ('w', C.c_void_p), ('shift', C.c_void_p), ('residual', C.c_void_p),
       ('om', C.c_void_p), ('out', C.c_void_p),
   ]
+
+
+class ConvConfig(C.Structure):
+  _fields_ = [('smem_bytes', C.c_int32), ('stages', C.c_int32), ('tile_w', C.c_int32), ('tile_h', C.c_int32),
+              ('ctas_per_sm', C.c_int32), ('overlap', C.c_int32)]
 
 
 class DecodeHead(C.Structure):
@@ -85,7 +91,7 @@ class TrackPayload(C.Structure):
   ]
 
 
-EXPORTS = ['ct_packed_weight_bytes', 'ct_pack_weights', 'ct_conv_forward', 'ct_stem_forward',
+EXPORTS = ['ct_packed_weight_bytes', 'ct_pack_weights', 'ct_conv_forward', 'ct_conv_config', 'ct_stem_forward',
            'ct_pack_stem_input', 'ct_pack_stem_input_f32', 'ct_maxpool2', 'ct_maxpool2_s2d', 'ct_upsample_add', 'ct_decode_workspace_bytes', 'ct_decode',
            'ct_render_pre_hm', 'ct_track_smem_bytes', 'ct_track_step', 'ct_track_assoc_smem_bytes',
            'ct_track_step_assoc', 'ct_track_payload_smem_bytes', 'ct_track_step_payload', 'ct_render_tracks', 'ct_flip_merge',
@@ -144,6 +150,7 @@ def lib():
   L.ct_packed_weight_bytes.argtypes = [C.c_int32] * 6
   L.ct_pack_weights.argtypes = [C.c_int32, C.c_void_p] + [C.c_int32] * 5 + [C.c_void_p]
   L.ct_conv_forward.argtypes = [C.POINTER(ConvDesc), C.c_void_p]
+  L.ct_conv_config.argtypes = [C.POINTER(ConvDesc), C.POINTER(ConvConfig)]
   L.ct_stem_forward.argtypes = [C.c_void_p] * 6 + [C.c_int32] * 5 + [C.c_void_p]
   L.ct_pack_stem_input.argtypes = [C.c_void_p] * 4 + [C.c_int32] * 3 + [C.c_void_p]
   L.ct_pack_stem_input_f32.argtypes = [C.c_void_p] * 4 + [C.c_int32] * 3 + [C.c_void_p]
@@ -180,6 +187,17 @@ def check(status, what=''):
   if status != 0:
     raise RuntimeError('libctb200 %s failed (%d): %s' %
                        (what, status, lib().ct_last_error().decode('utf-8', 'replace')))
+
+
+def conv_config(d):
+  """The launch configuration ct_conv_forward picks for descriptor d (ConvConfig), or None when the engine cannot
+  serve that shape at that N tile (CT_ERR_UNSUPPORTED: it does not fit in shared memory).  Other errors raise."""
+  cfg = ConvConfig()
+  rc = lib().ct_conv_config(C.byref(d), C.byref(cfg))
+  if rc == CT_ERR_UNSUPPORTED:
+    return None
+  check(rc, 'ct_conv_config')
+  return cfg
 
 
 def stream_ptr():

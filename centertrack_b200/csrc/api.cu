@@ -115,8 +115,9 @@ extern "C" int ct_pack_weights(int32_t engine, const float* w, int32_t C_out, in
   return CT_OK;
 }
 
-extern "C" int ct_conv_forward(const ct_conv_desc* d, void* stream) {
-  CT_REQUIRE(d && d->x && d->w && d->out, "null pointer");
+// The checks every engine shares; each engine's configuration step adds its own.  No pointer is looked at: both
+// ct_conv_config and ct_conv_forward run this.
+static int check_conv_desc(const ct_conv_desc* d) {
   CT_REQUIRE(d->B > 0 && d->H > 0 && d->W > 0 && d->C_in > 0 && d->C_out > 0, "bad shape");
   // `pad` is the top / left padding; fewer output rows / columns than the symmetric count mean less padding at the
   // bottom / right (even kernels: 2x2, pad 1 -> taps {-1, 0}, OH = H).  Accepted by the halo engine only.
@@ -131,24 +132,44 @@ extern "C" int ct_conv_forward(const ct_conv_desc* d, void* stream) {
   CT_REQUIRE(d->ld_in >= d->C_in, "ld_in < C_in");
   CT_REQUIRE(d->out_mode == CT_OUT_NCHW_F32 || d->ld_out >= (d->epilogue_sum3 ? 16 : d->C_out), "ld_out < C_out");
   if (d->a_mode == CT_A_DCN || d->a_mode == CT_A_DCN_WIN) {
-    CT_REQUIRE(d->om != nullptr && d->ld_om >= 27, "DCN needs om with ld_om >= 27");
+    CT_REQUIRE(d->ld_om >= 27, "DCN needs om with ld_om >= 27");
     CT_REQUIRE(d->a_mode == CT_A_DCN || d->engine == CT_ENGINE_TCGEN05, "CT_A_DCN_WIN: bf16 wgmma engine only");
     CT_REQUIRE(d->KH == 3 && d->KW == 3 && d->stride == 1 && d->pad == 1, "DCN is 3x3 s1 p1");
   }
   CT_REQUIRE(d->out_mode != CT_OUT_NHWC_S2D || d->engine == CT_ENGINE_TCGEN05_HALO, "CT_OUT_NHWC_S2D: halo engine only");
+  switch (d->engine) {
+    case CT_ENGINE_SIMT:
+      return CT_OK;
+    case CT_ENGINE_TCGEN05:
+      CT_REQUIRE(d->dtype == CT_BF16, "wgmma engine needs bf16 activations");
+      return CT_OK;
+    case CT_ENGINE_TCGEN05_X3:
+      CT_REQUIRE(d->dtype == CT_F32, "wgmma x3 engine runs on fp32 activations");
+      return CT_OK;
+    case CT_ENGINE_TCGEN05_HALO:
+      CT_REQUIRE(d->dtype == CT_BF16 && d->a_mode == CT_A_CONV, "halo engine: bf16 plain convolutions");
+      return CT_OK;
+    default:
+      return fail(CT_ERR_INVALID, "unknown engine%s %ld", "", (long)d->engine);
+  }
+}
+
+extern "C" int ct_conv_config(const ct_conv_desc* d, struct ct_conv_config* out) {
+  CT_REQUIRE(d && out, "null pointer");
+  const int r = check_conv_desc(d);
+  if (r != CT_OK) return r;
+  if (d->engine == CT_ENGINE_SIMT) return conv_config_simt(d, out);
+  if (d->engine == CT_ENGINE_TCGEN05_HALO) return conv_config_halo(d, out);
+  return conv_config_tc(d, out);
+}
+
+extern "C" int ct_conv_forward(const ct_conv_desc* d, void* stream) {
+  CT_REQUIRE(d && d->x && d->w && d->out, "null pointer");
+  CT_REQUIRE(d->om || (d->a_mode != CT_A_DCN && d->a_mode != CT_A_DCN_WIN), "DCN needs om with ld_om >= 27");
+  const int r = check_conv_desc(d);
+  if (r != CT_OK) return r;
   cudaStream_t st = (cudaStream_t)stream;
   if (d->engine == CT_ENGINE_SIMT) return conv_forward_simt(d, st);
-  if (d->engine == CT_ENGINE_TCGEN05) {
-    CT_REQUIRE(d->dtype == CT_BF16, "wgmma engine needs bf16 activations");
-    return conv_forward_tc(d, st);
-  }
-  if (d->engine == CT_ENGINE_TCGEN05_X3) {
-    CT_REQUIRE(d->dtype == CT_F32, "wgmma x3 engine runs on fp32 activations");
-    return conv_forward_tc(d, st);
-  }
-  if (d->engine == CT_ENGINE_TCGEN05_HALO) {
-    CT_REQUIRE(d->dtype == CT_BF16 && d->a_mode == CT_A_CONV, "halo engine: bf16 plain convolutions");
-    return conv_forward_halo(d, st);
-  }
-  return fail(CT_ERR_INVALID, "unknown engine%s %ld", "", (long)d->engine);
+  if (d->engine == CT_ENGINE_TCGEN05_HALO) return conv_forward_halo(d, st);
+  return conv_forward_tc(d, st);
 }

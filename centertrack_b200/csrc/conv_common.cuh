@@ -109,6 +109,13 @@ int dispatch_n_tile(int n_tile, F&& f) {
   else return n_tile == N ? f(std::integral_constant<int, N>()) : dispatch_n_tile<N + 16>(n_tile, f);
 }
 
+typedef struct ct_conv_config ConvConfig;
+
+// Each engine's configuration step (ct_conv_config: its shape checks and launch configuration, no CUDA call) and its
+// forward, which runs that step and then launches.
+int conv_config_simt(const ct_conv_desc* d, ConvConfig* c);
+int conv_config_tc(const ct_conv_desc* d, ConvConfig* c);
+int conv_config_halo(const ct_conv_desc* d, ConvConfig* c);
 int conv_forward_simt(const ct_conv_desc* d, cudaStream_t st);
 int conv_forward_tc(const ct_conv_desc* d, cudaStream_t st);
 int conv_forward_halo(const ct_conv_desc* d, cudaStream_t st);

@@ -320,8 +320,8 @@ int halo_blocks(int C_in, int KH, int KW) {
   return C_in == 8 ? KH * ((KW + 1) / 2) : KH * KW * (C_in / 16);
 }
 
-int conv_forward_halo(const ct_conv_desc* d, cudaStream_t st) {
-  HaloArgs a;
+// Configuration step: the launch arguments other than the pointers, and the launch configuration.  No CUDA call.
+static int halo_config(const ct_conv_desc* d, HaloArgs& a, ConvConfig& c) {
   a.g = make_geom(d);
   const ConvGeom& g = a.g;
   if (g.stride != 1 || g.pad != g.KH / 2 || g.KH != g.KW || g.OH != g.H || g.OW != g.W)
@@ -331,8 +331,6 @@ int conv_forward_halo(const ct_conv_desc* d, cudaStream_t st) {
   const int n_tile = d->n_tile;
   if (n_tile <= 0 || n_tile % 16 != 0 || n_tile > 256)
     return fail(CT_ERR_INVALID, "conv_halo: bad n_tile%s (%ld)", "", n_tile);
-  if (((uintptr_t)d->x & 15) || ((uintptr_t)d->w & 15) || ((uintptr_t)d->out & 15))
-    return fail(CT_ERR_INVALID, "conv_halo: x/w/out must be 16-byte aligned%s", "");
   a.sum3 = d->epilogue_sum3;
   a.out_s2d = 0;
   if (g.out_mode == CT_OUT_NHWC_S2D) {
@@ -345,12 +343,8 @@ int conv_forward_halo(const ct_conv_desc* d, cudaStream_t st) {
     return fail(CT_ERR_INVALID, "conv_halo: sum3 epilogue needs C_out == n_tile == 48, NHWC output, shift%s", "");
   if (g.out_mode == CT_OUT_NHWC && !a.sum3 && (g.C_out % 16 != 0 || g.ld_out % 8 != 0))
     return fail(CT_ERR_INVALID, "conv_halo: NHWC bf16 output needs C_out %% 16 == 0, ld_out %% 8 == 0%s", "");
-  if (d->residual && (g.out_mode != CT_OUT_NHWC || g.ld_res % 8 != 0 || ((uintptr_t)d->residual & 15)))
-    return fail(CT_ERR_INVALID, "conv_halo: residual only for NHWC bf16 outputs, 16B aligned%s", "");
-  a.w = (const __nv_bfloat16*)d->w;
-  a.shift = d->shift;
-  a.residual = (const __nv_bfloat16*)d->residual;
-  a.out = d->out;
+  if (d->residual && (g.out_mode != CT_OUT_NHWC || g.ld_res % 8 != 0))
+    return fail(CT_ERR_INVALID, "conv_halo: residual only for NHWC bf16 outputs, ld_res %% 8 == 0%s", "");
   a.n_tile = n_tile;
   a.n_tiles_n = (g.C_out + n_tile - 1) / n_tile;
   a.pair_taps = g.C_in == 8;
@@ -415,7 +409,40 @@ int conv_forward_halo(const ct_conv_desc* d, cudaStream_t st) {
     return fail(CT_ERR_UNSUPPORTED, "conv_halo: weights + halo do not fit in shared memory%s (%ld bytes)", "",
                 (long)smem_for(stages));
   a.halo_stages = stages;
-  const size_t smem = smem_for(stages);
+  // the persistent grid is sized for this many CTAs per SM
+  int per_sm = ctas_for(stages);
+  if (n_tile > 128) per_sm = 1;     // wide tiles: one CTA per SM (accumulator registers)
+  // One CTA per SM: no second CTA's MMAs fill this one's epilogue, so its two warpgroups take turns (overlap).  Not
+  // below N = 64: one warpgroup's m64n32 chain alone is bound by its shared-memory operand reads and leaves the tensor
+  // pipe half idle, so the two chains must run together (measured: the 128 -> 128 N = 32 layers 45 % slower in turns).
+  // CTB_HALO_OVERLAP=0: the serial schedule everywhere, for A/B runs; the outputs are bit-identical.
+  static const int overlap_env = getenv("CTB_HALO_OVERLAP") ? atoi(getenv("CTB_HALO_OVERLAP")) : 1;
+  c.smem_bytes = (int32_t)smem_for(stages);
+  c.stages = stages;
+  c.tile_w = a.tw;
+  c.tile_h = a.th;
+  c.ctas_per_sm = per_sm;
+  c.overlap = overlap_env && per_sm == 1 && n_tile >= 64 && n_tile <= 128;
+  return CT_OK;
+}
+
+int conv_config_halo(const ct_conv_desc* d, ConvConfig* c) {
+  HaloArgs a;
+  return halo_config(d, a, *c);
+}
+
+int conv_forward_halo(const ct_conv_desc* d, cudaStream_t st) {
+  HaloArgs a;
+  ConvConfig c;
+  const int rc = halo_config(d, a, c);
+  if (rc != CT_OK) return rc;
+  if (((uintptr_t)d->x & 15) || ((uintptr_t)d->w & 15) || ((uintptr_t)d->out & 15) || ((uintptr_t)d->residual & 15))
+    return fail(CT_ERR_INVALID, "conv_halo: x/w/out/residual must be 16-byte aligned%s", "");
+  a.w = (const __nv_bfloat16*)d->w;
+  a.shift = d->shift;
+  a.residual = (const __nv_bfloat16*)d->residual;
+  a.out = d->out;
+  const ConvGeom& g = a.g;
 
   CUtensorMap tmap;
   int r;
@@ -438,26 +465,17 @@ int conv_forward_halo(const ct_conv_desc* d, cudaStream_t st) {
 
   // persistent grid: a multiple of n_tiles_n, at most (SMs x CTAs that fit) and no more than the work
   const int sms = device_sm_count();
-  int per_sm = ctas_for(stages);
-  if (per_sm < 1) per_sm = 1;
-  if (n_tile > 128) per_sm = 1;     // wide tiles: one CTA per SM (accumulator registers)
-  long want = (long)sms * per_sm;
+  long want = (long)sms * c.ctas_per_sm;
   long groups = want / a.n_tiles_n;
   if (groups < 1) groups = 1;
   if (groups > a.tiles_total) groups = a.tiles_total;
   const int grid = (int)(groups * a.n_tiles_n);
-  // One CTA per SM: no second CTA's MMAs fill this one's epilogue, so its two warpgroups take turns (OVERLAP).  Not
-  // below N = 64: one warpgroup's m64n32 chain alone is bound by its shared-memory operand reads and leaves the tensor
-  // pipe half idle, so the two chains must run together (measured: the 128 -> 128 N = 32 layers 45 % slower in turns).
-  // CTB_HALO_OVERLAP=0: the serial schedule everywhere, for A/B runs; the outputs are bit-identical.
-  static const int overlap_env = getenv("CTB_HALO_OVERLAP") ? atoi(getenv("CTB_HALO_OVERLAP")) : 1;
-  const bool overlap = overlap_env && per_sm == 1 && n_tile >= 64 && n_tile <= 128;
-  return dispatch_n_tile(n_tile, [&](auto n) {
+  return dispatch_n_tile(a.n_tile, [&](auto n) {
     constexpr int NT = decltype(n)::value;
     if constexpr (NT >= 64 && NT <= 128)
-      if (overlap)
-        return launch_big_smem<conv_halo_kernel<NT, true>>(dim3(grid), dim3(H_THREADS), smem, st, a, tmap);
-    return launch_big_smem<conv_halo_kernel<NT, false>>(dim3(grid), dim3(H_THREADS), smem, st, a, tmap);
+      if (c.overlap)
+        return launch_big_smem<conv_halo_kernel<NT, true>>(dim3(grid), dim3(H_THREADS), c.smem_bytes, st, a, tmap);
+    return launch_big_smem<conv_halo_kernel<NT, false>>(dim3(grid), dim3(H_THREADS), c.smem_bytes, st, a, tmap);
   });
 }
 

@@ -140,15 +140,20 @@ static int launch_simt(const ct_conv_desc* d, const ConvGeom& g, cudaStream_t st
   return after_launch();
 }
 
+// No dynamic shared memory and no pipeline: the configuration stays all zero.
+int conv_config_simt(const ct_conv_desc* d, ConvConfig* c) {
+  if (d->C_in % 16 != 0) return fail(CT_ERR_INVALID, "conv_simt: C_in must be a multiple of 16%s (%ld)", "", d->C_in);
+  if (d->ld_in % 4 != 0) return fail(CT_ERR_INVALID, "conv_simt: ld_in %% 4 != 0%s", "");
+  *c = ConvConfig{};
+  return CT_OK;
+}
+
 int conv_forward_simt(const ct_conv_desc* d, cudaStream_t st) {
+  ConvConfig c;
+  const int rc = conv_config_simt(d, &c);
+  if (rc != CT_OK) return rc;
   const ConvGeom g = make_geom(d);
-  if (g.C_in % 16 != 0) return fail(CT_ERR_INVALID, "conv_simt: C_in must be a multiple of 16%s (%ld)", "", g.C_in);
-  if (d->dtype == CT_F32) {
-    if (g.ld_in % 4 != 0) return fail(CT_ERR_INVALID, "conv_simt: ld_in %% 4 != 0%s", "");
-    return launch_simt<float>(d, g, st);
-  }
-  if (g.ld_in % 4 != 0) return fail(CT_ERR_INVALID, "conv_simt: ld_in %% 4 != 0%s", "");
-  return launch_simt<__nv_bfloat16>(d, g, st);
+  return d->dtype == CT_F32 ? launch_simt<float>(d, g, st) : launch_simt<__nv_bfloat16>(d, g, st);
 }
 
 }  // namespace ctb

@@ -672,36 +672,26 @@ int tc_set_trace(void* buf) {
 }
 int tc_set_watch(void* mapped_host_buf) { return set_mbar_watch(mapped_host_buf); }
 
-int conv_forward_tc(const ct_conv_desc* d, cudaStream_t st) {
+// Configuration step: the launch arguments other than the pointers, and the launch configuration.  No CUDA call.
+static int tc_config(const ct_conv_desc* d, TcArgs& a, ConvConfig& c) {
   const bool x3 = d->engine == CT_ENGINE_TCGEN05_X3;     // fp32 activations, bf16 hi/lo split operands
-  TcArgs a;
   a.g = make_geom(d);
   const ConvGeom& g = a.g;
   if (g.C_in % 8 != 0 || g.ld_in % 8 != 0)
     return fail(CT_ERR_INVALID, "conv_tc: C_in and ld_in must be multiples of 8%s (%ld,%ld)", "", g.C_in, g.ld_in);
-  if (((uintptr_t)d->x & 15) || ((uintptr_t)d->w & 15) || ((uintptr_t)d->out & 15))
-    return fail(CT_ERR_INVALID, "conv_tc: x/w/out must be 16-byte aligned%s", "");
-  int n_tile = d->n_tile;
+  const int n_tile = d->n_tile;
   if (n_tile <= 0 || n_tile % 16 != 0 || n_tile > 256)
     return fail(CT_ERR_INVALID, "conv_tc: n_tile must be a multiple of 16 in [16,256]%s (%ld)", "", n_tile);
   if (g.out_mode == CT_OUT_NHWC) {
     if (g.C_out % 16 != 0 || g.ld_out % 8 != 0)
       return fail(CT_ERR_INVALID, "conv_tc: NHWC output needs C_out %% 16 == 0 and ld_out %% 8 == 0%s", "");
-    if (d->residual && (g.ld_res % 8 != 0 || ((uintptr_t)d->residual & 15)))
-      return fail(CT_ERR_INVALID, "conv_tc: residual must be 16B aligned with ld_res %% 8 == 0%s", "");
-  } else if (g.out_mode == CT_OUT_NHWC_F32) {
-    if (d->residual) return fail(CT_ERR_INVALID, "conv_tc: residual unsupported for fp32 outputs%s", "");
+    if (d->residual && g.ld_res % 8 != 0)
+      return fail(CT_ERR_INVALID, "conv_tc: residual needs ld_res %% 8 == 0%s", "");
   } else if (d->residual) {
     return fail(CT_ERR_INVALID, "conv_tc: residual unsupported for fp32 outputs%s", "");
   }
   if ((long long)g.B * g.H * g.W * g.ld_in >= (1ll << 31))
     return fail(CT_ERR_INVALID, "conv_tc: input tensor exceeds 2^31 elements (32-bit offsets)%s", "");
-  a.x = (const __nv_bfloat16*)d->x;
-  a.w = (const __nv_bfloat16*)d->w;
-  a.shift = d->shift;
-  a.residual = (const __nv_bfloat16*)d->residual;
-  a.om = d->om;
-  a.out = d->out;
   a.n_tile = n_tile;
   a.k_slices = (g.K_total + TC_BK - 1) / TC_BK;
   a.a_mode = d->a_mode;
@@ -744,23 +734,47 @@ int conv_forward_tc(const ct_conv_desc* d, cudaStream_t st) {
   if (stages > a.k_slices) stages = a.k_slices;
   a.stages = stages;
   a.region0 = (uint32_t)region0_for(stages);
-  const size_t smem = smem_for(stages);
-  const int n_tiles = (g.C_out + n_tile - 1) / n_tile;
-  // Optional 2-D pixel patches (CTB_TC_TILE2D=1) when they tile the map exactly; off by default.
+  // M tiles: 128 consecutive pixels, or 8 (y) x 16 (x) patches -- always for the window sampler (ragged at the right /
+  // bottom edge), and with CTB_TC_TILE2D=1 (off by default) where they tile the map exactly.
   static const int tile2d_env = getenv("CTB_TC_TILE2D") ? atoi(getenv("CTB_TC_TILE2D")) : 0;
   a.tiles_x = a.tiles_y = 0;
-  int m_tiles = (g.P_out + TC_BM - 1) / TC_BM;
-  if (tile2d_env && g.OW % 16 == 0 && g.OH % 8 == 0) {
-    a.tiles_x = g.OW / 16;
-    a.tiles_y = g.OH / 8;
-    m_tiles = g.B * a.tiles_x * a.tiles_y;
-  }
-  CUtensorMap tmap;
-  memset(&tmap, 0, sizeof(tmap));
-  if (win) {                                         // 8x16 patches (ragged at the right / bottom edge) + their windows
+  if (win || (tile2d_env && g.OW % 16 == 0 && g.OH % 8 == 0)) {
     a.tiles_x = (g.OW + 15) / 16;
     a.tiles_y = (g.OH + 7) / 8;
-    m_tiles = g.B * a.tiles_x * a.tiles_y;
+  }
+  c.smem_bytes = (int32_t)smem_for(stages);
+  c.stages = stages;
+  c.tile_w = a.tiles_x ? 16 : TC_BM;
+  c.tile_h = a.tiles_x ? 8 : 1;
+  c.ctas_per_sm = 0;
+  c.overlap = 0;
+  return CT_OK;
+}
+
+int conv_config_tc(const ct_conv_desc* d, ConvConfig* c) {
+  TcArgs a;
+  return tc_config(d, a, *c);
+}
+
+int conv_forward_tc(const ct_conv_desc* d, cudaStream_t st) {
+  TcArgs a;
+  ConvConfig c;
+  const int rc = tc_config(d, a, c);
+  if (rc != CT_OK) return rc;
+  if (((uintptr_t)d->x & 15) || ((uintptr_t)d->w & 15) || ((uintptr_t)d->out & 15) || ((uintptr_t)d->residual & 15))
+    return fail(CT_ERR_INVALID, "conv_tc: x/w/out/residual must be 16-byte aligned%s", "");
+  a.x = (const __nv_bfloat16*)d->x;
+  a.w = (const __nv_bfloat16*)d->w;
+  a.shift = d->shift;
+  a.residual = (const __nv_bfloat16*)d->residual;
+  a.om = d->om;
+  a.out = d->out;
+  const ConvGeom& g = a.g;
+  const int m_tiles = a.tiles_x ? g.B * a.tiles_x * a.tiles_y : (g.P_out + TC_BM - 1) / TC_BM;
+  const int n_tiles = (g.C_out + a.n_tile - 1) / a.n_tile;
+  CUtensorMap tmap;
+  memset(&tmap, 0, sizeof(tmap));
+  if (a.a_mode == CT_A_DCN_WIN) {                    // the TMA box of one patch's window
     const cuuint64_t dims[4] = {(cuuint64_t)g.C_in, (cuuint64_t)g.W, (cuuint64_t)g.H, (cuuint64_t)g.B};
     const cuuint64_t strides[3] = {(cuuint64_t)g.ld_in * 2, (cuuint64_t)g.W * g.ld_in * 2, (cuuint64_t)g.H * g.W * g.ld_in * 2};
     const cuuint32_t box[4] = {64, (cuuint32_t)a.win_pw, (cuuint32_t)a.win_ph, 1};
@@ -768,10 +782,11 @@ int conv_forward_tc(const ct_conv_desc* d, cudaStream_t st) {
     if (r != CT_OK) return r;
   }
   dim3 grid(m_tiles, n_tiles);
-  return dispatch_n_tile(n_tile, [&](auto n) {
+  const bool x3 = d->engine == CT_ENGINE_TCGEN05_X3;
+  return dispatch_n_tile(a.n_tile, [&](auto n) {
     constexpr int N = decltype(n)::value;
-    return x3 ? launch_big_smem<conv_tc_kernel<true, N>>(grid, dim3(TC_THREADS), smem, st, a, tmap)
-              : launch_big_smem<conv_tc_kernel<false, N>>(grid, dim3(TC_THREADS), smem, st, a, tmap);
+    return x3 ? launch_big_smem<conv_tc_kernel<true, N>>(grid, dim3(TC_THREADS), c.smem_bytes, st, a, tmap)
+              : launch_big_smem<conv_tc_kernel<false, N>>(grid, dim3(TC_THREADS), c.smem_bytes, st, a, tmap);
   });
 }
 

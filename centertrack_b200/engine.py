@@ -150,17 +150,32 @@ class DLA34Engine(object):
     shift = self.sd[bn + '.bias'] - self.sd[bn + '.running_mean'] * s + b * s
     return w * s.view(-1, 1, 1, 1), shift
 
-  def _pick_n_tile(self, P, C_out):
+  @staticmethod
+  def _n_tile_cands(C_out):
+    """N tiles of the gather engines for C_out channels, widest first."""
     cpad = (C_out + 15) // 16 * 16
     cands = [c for c in (256, 128, 64, 32, 16) if c <= max(cpad, 16)]
     if cpad <= 256 and cpad not in cands:
       cands = [cpad] + cands
+    return cands
+
+  def _pick_n_tile(self, P, C_out, cands):
     m_tiles = (P + 127) // 128
     for c in cands:
       if m_tiles * ((C_out + c - 1) // c) >= self.n_sm:
         return c
     small = [c for c in cands if c >= 64]
     return small[-1] if small else cands[0]
+
+  @staticmethod
+  def _first_fit(d, engine, n_tiles):
+    """The first of n_tiles at which the library can configure d's launch on `engine` (ct_conv_config), or None.
+    Leaves d.engine / d.n_tile at the last one tried."""
+    for nt in n_tiles:
+      d.engine, d.n_tile = engine, nt
+      if L.conv_config(d) is not None:
+        return nt
+    return None
 
   def _pack(self, w, n_tile, engine):
     """w: float64 [O,I,kh,kw] -> packed device blob for `engine`."""
@@ -188,28 +203,8 @@ class DLA34Engine(object):
     if out_hw is not None:      # even kernels: padding on the top / left only (ctb200.h, OH / OW)
       OH, OW = out_hw
     P = self.B * OH * OW
-    engine = self.engine
-    n_tile = self._pick_n_tile(P, C_out) if engine in (L.CT_ENGINE_TCGEN05, L.CT_ENGINE_TCGEN05_X3) else 0
-    if engine == L.CT_ENGINE_TCGEN05 and a_mode == L.CT_A_CONV and n_tile > self.ntile_cap:
-      # experiment knob (CTB_NTILE_CAP): 128-wide tiles with two co-resident CTAs measured SLOWER than one 256-wide
-      # CTA on levels 4-5 (conv_tc plain 1.81 vs 1.73 ms per 32-frame step), so the default cap is 256 = no cap
-      n_tile = self.ntile_cap
-    if engine == L.CT_ENGINE_TCGEN05_X3 and n_tile > 128 and a_mode == L.CT_A_DCN:
-      n_tile = 128            # x3 DCN: two 36 KB-table stages of (32 + 2 x n_tile/8) KB must fit
-    if engine == L.CT_ENGINE_TCGEN05 and self.use_halo and a_mode == L.CT_A_CONV and stride == 1 and kh == kw and \
-        (C_in in (16, 32, 48, 64, 128, 192, 256) or (C_in == 8 and sum3)) and \
-        not (self.gather_128 and C_in == 128 and C_out == 128 and kh == 3):
-      k = kh
-      # stride-1 layer whose weights fit in smem: TMA halo tile + descriptor-shifted taps (csrc/conv_halo.cu)
-      nblk = k * ((k + 1) // 2) if C_in == 8 else k * k * (C_in // 16)
-      halo = C_in * 2 * (8 + k - 1 + (1 if C_in == 8 else 0)) * (16 + k - 1) + 1024 * max(1, C_in // 64)
-      cpad = (C_out + 15) // 16 * 16
-      for nt in ([48] if sum3 else [c for c in (128, 96, 80, 64, 48, 32, 16) if c <= cpad and (c == cpad or cpad % c == 0 or c >= 64)]):
-        if nblk * nt * 32 + 2 * halo + 4096 + 18432 <= 224 * 1024 and (nt >= 32 or cpad <= 16):   # + epilogue staging
-          engine, n_tile = L.CT_ENGINE_TCGEN05_HALO, nt
-          break
     d = L.ConvDesc()
-    d.engine, d.dtype, d.a_mode = engine, self.ct_dtype, a_mode
+    d.dtype, d.a_mode = self.ct_dtype, a_mode
     d.epilogue_sum3 = sum3
     d.B, d.H, d.W, d.C_in, d.ld_in, d.C_out = self.B, x.H, x.W, C_in, x.ld, C_out
     d.KH, d.KW = kh, kw
@@ -217,9 +212,7 @@ class DLA34Engine(object):
     d.pad_w1 = 0 if pad_w == pad else pad_w + 1
     d.out_mode, d.relu, d.head_act, d.sig_from = out_mode, int(relu), head_act, sig_from
     d.depth_scale = self.depth_scale
-    d.n_tile = n_tile
     d.x = x.ptr
-    d.w = self._pack(w if w_pack is None else w_pack, n_tile, engine).data_ptr()
     sh = self._dev(shift.to(torch.float32).contiguous())
     d.shift = sh.data_ptr()
     if residual is not None:
@@ -234,13 +227,37 @@ class DLA34Engine(object):
       d.out, d.ld_out = out.data_ptr(), out.shape[-1]
     elif out_mode == L.CT_OUT_NHWC_S2D:
       co = 16 if sum3 else C_out
-      assert engine == L.CT_ENGINE_TCGEN05_HALO and (out.H, out.W, out.C, out.ld) == (OH // 2, OW // 2, 4 * co, 4 * co)
+      assert (out.H, out.W, out.C, out.ld) == (OH // 2, OW // 2, 4 * co, 4 * co)
       d.out, d.ld_out = out.ptr, co
       self.named[name] = out
     else:
       assert (out.H, out.W) == (OH, OW) and out.C == (16 if sum3 else C_out), (name, out.H, out.W, out.C, OH, OW, C_out)
       d.out, d.ld_out = out.ptr, out.ld
       self.named[name] = out
+    n_tile = None
+    if self.engine == L.CT_ENGINE_TCGEN05 and self.use_halo and a_mode == L.CT_A_CONV and stride == 1 and kh == kw and \
+        (C_in in (16, 32, 48, 64, 128, 192, 256) or (C_in == 8 and sum3)) and \
+        not (self.gather_128 and C_in == 128 and C_out == 128 and kh == 3):
+      # stride-1 layer whose weights fit in smem: TMA halo tile + descriptor-shifted taps (csrc/conv_halo.cu)
+      cpad = (C_out + 15) // 16 * 16
+      n_tile = self._first_fit(d, L.CT_ENGINE_TCGEN05_HALO, [48] if sum3 else [
+          c for c in (128, 96, 80, 64, 48, 32, 16)
+          if c <= cpad and (c == cpad or cpad % c == 0 or c >= 64) and (c >= 32 or cpad <= 16)])
+    if n_tile is None:
+      d.engine, d.n_tile = self.engine, 0
+      if self.engine != L.CT_ENGINE_SIMT:
+        cands = self._n_tile_cands(C_out)
+        n_tile = self._pick_n_tile(P, C_out, cands)
+        if self.engine == L.CT_ENGINE_TCGEN05 and a_mode == L.CT_A_CONV and n_tile > self.ntile_cap:
+          # experiment knob (CTB_NTILE_CAP): 128-wide tiles with two co-resident CTAs measured SLOWER than one 256-wide
+          # CTA on levels 4-5 (conv_tc plain 1.81 vs 1.73 ms per 32-frame step), so the default cap is 256 = no cap
+          n_tile = self.ntile_cap
+        # the widest tile not above that one whose stages fit in shared memory (the x3 DCN's do not at N = 256)
+        if self._first_fit(d, self.engine, [c for c in cands if c <= n_tile]) is None:
+          raise ValueError('%s: no N tile of %s fits in shared memory' % (name, cands))
+    engine, n_tile = d.engine, d.n_tile
+    assert out_mode != L.CT_OUT_NHWC_S2D or engine == L.CT_ENGINE_TCGEN05_HALO, name
+    d.w = self._pack(w if w_pack is None else w_pack, n_tile, engine).data_ptr()
     self._op('conv', d, name, x=x, w=w, shift=shift, residual=residual, om=om, out=out, k=(kh, kw), stride=stride,
              pad=(pad, pad_w), out_hw=(OH, OW), a_mode=a_mode, out_mode=out_mode, relu=relu, sig_from=sig_from,
              sum3=sum3, engine=engine, n_tile=n_tile)

@@ -104,7 +104,7 @@ typedef struct {
   int32_t sig_from;      /* CT_OUT_NHWC_F32: sigmoid applied to channels >= sig_from (DCN mask) */
   float   depth_scale;
   int32_t ld_om;         /* CT_A_DCN: pixel stride of `om` (fp32 NHWC, >= 27) */
-  int32_t n_tile;        /* wgmma engines: output-channel tile (multiple of 16, <= 256); 0 = auto */
+  int32_t n_tile;        /* wgmma engines: output-channel tile (multiple of 16, <= 256; required) */
   int32_t epilogue_sum3; /* HALO engine, C_out == 48: out16 = sum over present groups g (bit g set) of
                             relu(acc[16g..16g+15] + shift) -- the three DLA stems (dla.py:307-311) */
   int32_t pad_w1;        /* 0: horizontal padding = pad; else horizontal padding + 1 (the (k,1) / (1,k) convs of
@@ -131,6 +131,21 @@ int ct_pack_weights(int32_t engine, const float* w_oihw, int32_t C_out, int32_t 
                     int32_t KW, int32_t n_tile, void* dst);
 
 int ct_conv_forward(const ct_conv_desc* d, void* stream);
+
+/* Launch configuration ct_conv_forward picks for a descriptor (ct_conv_config). */
+struct ct_conv_config {
+  int32_t smem_bytes;    /* dynamic shared memory per CTA (0: SIMT engine) */
+  int32_t stages;        /* pipeline stages: halo tiles (HALO) or K slices (gather engines) in flight */
+  int32_t tile_w, tile_h;/* output pixels of one work item: 8 x 16 or 32 x 4 (HALO); 16 x 8 patches or 128 x 1
+                            consecutive pixels (gather engines) */
+  int32_t ctas_per_sm;   /* HALO: CTAs per SM the persistent grid is sized for; 0 for the other engines */
+  int32_t overlap;       /* HALO: 1 = the one-CTA-per-SM flavour whose two warpgroups take turns on the tensor cores */
+};
+/* The configuration step of ct_conv_forward alone: validates the descriptor's shape and fills `out`, with no CUDA
+ * call.  Returns the status and ct_last_error() message ct_conv_forward would return for this shape
+ * (CT_ERR_UNSUPPORTED: the tile does not fit in shared memory).  Of the pointer fields of `d` only whether residual
+ * and shift are NULL is read (a layer without residual / shift); the others may be NULL. */
+int ct_conv_config(const ct_conv_desc* d, struct ct_conv_config* out);
 
 /* Three 7x7 stems on reference-layout inputs (fp32 NCHW):
  *   out = relu(bn(conv7(img))) + relu(bn(conv7(pre_img))) + relu(bn(conv7(pre_hm)))

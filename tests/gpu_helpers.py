@@ -9,8 +9,9 @@ from centertrack_b200 import _lib as L
 dev = torch.device('cuda')
 
 
-def run_conv(engine, dtype, x_nchw, w, bias, stride, relu=True, residual=None, a_mode=L.CT_A_CONV, om=None,
-             out_mode=L.CT_OUT_NHWC, n_tile=0, head_act=0, sig_from=1 << 30, ld_pad=0, ch_off=0, sum3=0):
+def conv_desc(engine, dtype, x_nchw, w, bias, stride, relu=True, residual=None, a_mode=L.CT_A_CONV, om=None,
+              out_mode=L.CT_OUT_NHWC, n_tile=0, head_act=0, sig_from=1 << 30, ld_pad=0, ch_off=0, sum3=0):
+  """-> (descriptor, output buffer, the device buffers the descriptor points to) of the launch run_conv makes."""
   lib = L.lib()
   B, Cin, H, W = x_nchw.shape
   O, _, k, _ = w.shape
@@ -64,12 +65,18 @@ def run_conv(engine, dtype, x_nchw, w, bias, stride, relu=True, residual=None, a
     oc = 16 if sum3 else O
     out = torch.zeros((B, OH, OW, oc), dtype=act, device=dev)
     d.out, d.ld_out = out.data_ptr(), oc
-  L.check(lib.ct_conv_forward(C.byref(d), L.stream_ptr()), 'conv')
+  return d, out, (xb, wp, sh, rb if residual is not None else None)
+
+
+def run_conv(*args, **kwargs):
+  d, out, _buffers = conv_desc(*args, **kwargs)
+  L.check(L.lib().ct_conv_forward(C.byref(d), L.stream_ptr()), 'conv')
   torch.cuda.synchronize()
-  if out_mode == L.CT_OUT_NCHW_F32:
+  if d.out_mode == L.CT_OUT_NCHW_F32:
     return out
-  if out_mode == L.CT_OUT_NHWC_S2D:   # undo: [B, OH/2, OW/2, (sy, sx, c)] -> [B, c, OH, OW]
-    return out.reshape(B, OH // 2, OW // 2, 2, 2, oc).permute(0, 5, 1, 3, 2, 4).reshape(B, oc, OH, OW).float()
+  if d.out_mode == L.CT_OUT_NHWC_S2D:   # undo: [B, OH/2, OW/2, (sy, sx, c)] -> [B, c, OH, OW]
+    B, h, w, c4 = out.shape
+    return out.reshape(B, h, w, 2, 2, c4 // 4).permute(0, 5, 1, 3, 2, 4).reshape(B, c4 // 4, 2 * h, 2 * w).float()
   return out.permute(0, 3, 1, 2).float()
 
 

@@ -16,8 +16,8 @@ pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 
-# (name, B, C_in, C_out, H, W, k, residual, n_tile, output).  Every shape takes the overlapped path (one CTA per SM,
-# 64 <= N <= 128: asserted below); the sizes give the persistent CTAs (132 on an H100 SXM) a mix of 1 and 2 work items,
+# (name, B, C_in, C_out, H, W, k, residual, n_tile, output).  Every shape takes the overlapped path (asserted below from
+# the library's configuration); the sizes give the persistent CTAs (132 on an H100 SXM) a mix of 1 and 2 work items,
 # and 8-9 (heads.0) or 3-4 (3x3 64 -> 160) items.
 CASES = [
     ('heads.0 3x3 64->1024 nt128', 1, 64, 1024, 176, 104, 3, False, 128, 'nhwc'),
@@ -34,17 +34,6 @@ CASES = [
 ]
 
 
-def _ctas_per_sm(C_in, k, n_tile, wide):
-  """CTAs per SM of a halo launch, by conv_forward_halo's shared-memory formula (2 halo stages)."""
-  nblk = k * k * (C_in // 16)
-  swz = 128 if C_in > 64 else C_in * 2
-  planes = (C_in * 2 + swz - 1) // swz
-  tw, th = (32, 4) if wide else (8, 16)
-  plane = ((tw + k - 1) * (th + k - 1) * swz + 1023) // 1024 * 1024
-  smem = (nblk * n_tile * 32 + 1023) // 1024 * 1024 + 2 * planes * plane + 2 * 64 * 36 * 4 + 256 + 2048
-  return min(2, 227 * 1024 // smem)
-
-
 def _inputs(case, seed):
   name, B, Cin, Cout, H, W, k, res, nt, out = case
   g = torch.Generator().manual_seed(seed)
@@ -55,16 +44,21 @@ def _inputs(case, seed):
   return x, w, b, r
 
 
-def _run(case, seed):
-  from gpu_helpers import run_conv
+def _conv_args(case, seed):
+  """(args, keyword args) of gpu_helpers.run_conv / conv_desc for this case."""
   name, B, Cin, Cout, H, W, k, res, nt, out = case
   x, w, b, r = _inputs(case, seed)
   kw = {'nhwc': {}, 's2d': dict(out_mode=L.CT_OUT_NHWC_S2D),
         'f32_nhwc': dict(out_mode=L.CT_OUT_NHWC_F32, sig_from=18),
         'nchw_sigmoid': dict(out_mode=L.CT_OUT_NCHW_F32, head_act=1), 'nchw': dict(out_mode=L.CT_OUT_NCHW_F32)}[out]
   relu = out in ('nhwc', 's2d')
-  return run_conv(L.CT_ENGINE_TCGEN05_HALO, L.CT_BF16, x.cuda(), w, b, 1, relu, r.cuda() if res else None,
-                  n_tile=nt, **kw)
+  return (L.CT_ENGINE_TCGEN05_HALO, L.CT_BF16, x.cuda(), w, b, 1, relu, r.cuda() if res else None), dict(kw, n_tile=nt)
+
+
+def _run(case, seed):
+  from gpu_helpers import run_conv
+  args, kw = _conv_args(case, seed)
+  return run_conv(*args, **kw)
 
 
 def dump_cases(path):
@@ -105,9 +99,11 @@ def _in_process(fn, path, overlap):
 
 
 def test_one_cta_halo_shapes_bit_identical_to_serial(tmp_path):
-  for c in CASES:
-    assert _ctas_per_sm(c[2], c[6], c[8], c[9].startswith('nchw') and c[6] == 1 and c[5] % 32 == 0) == 1, c[0]
-    assert 64 <= c[8] <= 128, c[0]
+  from gpu_helpers import conv_desc
+  for i, c in enumerate(CASES):
+    args, kw = _conv_args(c, 500 + i)
+    cfg = L.conv_config(conv_desc(*args, **kw)[0])
+    assert cfg.ctas_per_sm == 1 and cfg.overlap == 1, c[0]
   got = _in_process('dump_cases', tmp_path / 'overlap.pt', '1')
   serial = _in_process('dump_cases', tmp_path / 'serial.pt', '0')
   for i, c in enumerate(CASES):

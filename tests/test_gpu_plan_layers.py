@@ -4,7 +4,7 @@ The engine is built as the product builds it (synthetic calibrated checkpoint, r
 replay runs with the fused activations, and then every op's output is recomputed in fp64 from the buffers as they are
 after the replay.  That is valid because the plan never writes in place: every buffer still holds what its consumer
 read -- which the test asserts first by checking that no two ops write overlapping bytes.  Each layer therefore runs at
-the (engine, N tile, halo stages, tile shape, ld / offset) its plan selects for that batch and resolution.
+the (engine, N tile, stages, tile shape, ld / offset) its plan selects for that batch and resolution.
 """
 import pytest
 import torch
@@ -53,22 +53,6 @@ def _unshuffle(t):
   B, h, w, c4 = t.shape
   c = c4 // 4
   return t.reshape(B, h, w, 2, 2, c).permute(0, 5, 1, 3, 2, 4).reshape(B, c, 2 * h, 2 * w).double()
-
-
-def _halo_stages(c_in, kh, kw, n, wide):
-  """Halo stages the kernel picks for this layer (conv_halo.cu::conv_forward_halo), for the coverage table."""
-  swz = 128 if c_in > 64 else (c_in * 2 if c_in in (16, 32, 64) else 0)
-  planes = (c_in * 2 + swz - 1) // swz if swz else c_in // 8
-  tw, th = (32, 4) if wide else (8, 16)
-  pw, ph = tw + kw - 1 + (1 if c_in == 8 else 0), th + kh - 1
-  plane = (pw * ph * (swz or 16) + 1023) // 1024 * 1024
-  nblk = kh * ((kw + 1) // 2) if c_in == 8 else kh * kw * (c_in // 16)
-  smem = lambda s: (nblk * n * 32 + 1023) // 1024 * 1024 + s * planes * plane + 2 * 64 * 36 * 4 + 256 + 2048
-  ctas = lambda s: min(2, (227 * 1024) // smem(s))
-  for s in (4, 3):
-    if smem(s) <= 227 * 1024 and ctas(s) == ctas(2):
-      return s
-  return 2
 
 
 def _out_ranges(eng):
@@ -242,12 +226,12 @@ def _coverage_row(eng, sp):
   d = sp['desc']
   kern = KERNEL[sp['engine']]
   kh, kw = sp['k']
-  wide = kern == 'halo' and kh == 1 and kw == 1 and sp['out_mode'] == L.CT_OUT_NCHW_F32 and \
-      (d.C_in in (16, 32, 64) or d.C_in > 64) and \
-      d.OW % 32 == 0 and d.OH % 4 == 0
+  cfg = L.conv_config(d)             # the launch configuration the library picked for this op
+  assert cfg is not None, sp['name']
+  launch = ('%dx%d' % (cfg.tile_w, cfg.tile_h), cfg.stages, cfg.overlap) if kern != 'simt' else ('-', '-', '-')
   return (kern, sp['n_tile'], d.C_in, '%dx%d' % (kh, kw), A_MODE[sp['a_mode']], OUT_MODE[sp['out_mode']],
           int(sp['residual'] is not None), int(sp['out_mode'] == L.CT_OUT_NHWC_S2D or sp['name'] in eng.s2d_named),
-          int(bool(sp['sum3'])), int(wide), _halo_stages(d.C_in, kh, kw, sp['n_tile'], wide) if kern == 'halo' else '-')
+          int(bool(sp['sum3']))) + launch
 
 
 COVERAGE = {}
@@ -299,10 +283,10 @@ def test_plan_layers_within_bounds(case, monkeypatch):
 
 
 def test_zz_plan_coverage_table():
-  """Print which (kernel, N, C_in, k, a_mode, out_mode, residual, s2d, sum3, wide tile, halo stages) the plans above
+  """Print which (kernel, N, C_in, k, a_mode, out_mode, residual, s2d, sum3, tile, stages, overlap) the plans above
   ran (runs after them in file order)."""
   if not COVERAGE:
     pytest.skip('no plan audited in this session')
-  print('\nkernel     N   C_in k    a_mode  out_mode  res s2d sum3 wide stages  configs')
+  print('\nkernel     N   C_in k    a_mode  out_mode  res s2d sum3 tile   stages overlap  configs')
   for row in sorted(COVERAGE, key=lambda r: tuple(str(v) for v in r)):
-    print('%-9s %4d %5d %-4s %-7s %-9s %3d %3d %4d %4d %6s  %s' % (row + (','.join(sorted(COVERAGE[row])),)))
+    print('%-9s %4d %5d %-4s %-7s %-9s %3d %3d %4d %-6s %6s %7s  %s' % (row + (','.join(sorted(COVERAGE[row])),)))

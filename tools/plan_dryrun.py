@@ -7,6 +7,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, 'tests'))
 import helpers as th                                   # noqa
+from centertrack_b200 import _lib as L                 # noqa
 from centertrack_b200 import engine as E               # noqa
 
 for cfg, (H, W) in (('coco_tracking', (64, 96)), ('coco_pose', (64, 64))):
@@ -16,6 +17,8 @@ for cfg, (H, W) in (('coco_tracking', (64, 96)), ('coco_pose', (64, 64))):
     print(cfg, prec, len(e.ops), 'ops')
     for kind, d, name in e.ops:
       if name in ('base.level0', 'base.level1') and kind == 'conv':
-        print('   %-12s engine %d  k %dx%d s%d pad %d  C %d -> %d  %dx%d -> %dx%d  out_mode %d ld_out %d n_tile %d'
+        c = L.conv_config(d)
+        print('   %-12s engine %d  k %dx%d s%d pad %d  C %d -> %d  %dx%d -> %dx%d  out_mode %d ld_out %d n_tile %d  '
+              'smem %d stages %d tile %dx%d ctas/SM %d overlap %d'
               % (name, d.engine, d.KH, d.KW, d.stride, d.pad, d.C_in, d.C_out, d.H, d.W, d.OH, d.OW, d.out_mode, d.ld_out,
-                 d.n_tile))
+                 d.n_tile, c.smem_bytes, c.stages, c.tile_w, c.tile_h, c.ctas_per_sm, c.overlap))

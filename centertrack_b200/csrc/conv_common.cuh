@@ -30,33 +30,28 @@ inline ConvGeom make_geom(const ct_conv_desc* d) {
   return g;
 }
 
-// Modulated-deformable sampling parameters of one (output pixel, tap):  SURVEY.md Appendix B.
+// Modulated-deformable sampling of one (output pixel, tap):  SURVEY.md Appendix B.
 //   py = y - 1 + i + dy_k,  px = x - 1 + j + dx_k ;  S = 0 unless -1 < py < H and -1 < px < W ;
 //   bilinear over the integer neighbours that lie inside the image; the whole sample times mask.
-struct DcnTap {
-  int off[4];     // element offsets (relative to the image base) of the 4 corner pixels
-  float w[4];     // bilinear weight x mask, 0 for corners outside the image
-};
-
-__device__ __forceinline__ DcnTap dcn_tap(const float* __restrict__ om_px, int tap, int oy, int ox,
-                                          int H, int W, int ld_in) {
-  DcnTap t;
-  const float dy = om_px[2 * tap], dx = om_px[2 * tap + 1], m = om_px[18 + tap];
-  const float py = (float)(oy - 1 + tap / 3) + dy;
-  const float px = (float)(ox - 1 + tap % 3) + dx;
-  const bool valid = (py > -1.f) && (py < (float)H) && (px > -1.f) && (px < (float)W);
+// dcn_corner gives the footprint of (py, px) in an H x W image, from which every engine samples: top-left corner
+// (y0, x0) and its clamp into the image (yc, xc), whether the x+1 / y+1 neighbours exist on both sides (dx, dy), and
+// the four corner weights times the mask, zero for corners outside the image.  A corner of non-zero weight is the
+// pixel (yc, xc) stepped by dy / dx where it lies below / right of the top-left one.  Returns false (c untouched)
+// when the sample is outside the image altogether (its value is 0).
+struct DcnCorner { int y0, x0, yc, xc; bool dx, dy; float w00, w01, w10, w11; };
+__device__ __forceinline__ bool dcn_corner(float py, float px, int H, int W, float m, DcnCorner& c) {
+  if (!(py > -1.f && py < (float)H && px > -1.f && px < (float)W)) return false;
   const float y0f = floorf(py), x0f = floorf(px);
-  const float ly = py - y0f, lx = px - x0f, hy = 1.f - ly, hx = 1.f - lx;
   const int y0 = (int)y0f, x0 = (int)x0f;
-  const bool y0ok = valid && y0 >= 0 && y0 <= H - 1, y1ok = valid && y0 + 1 >= 0 && y0 + 1 <= H - 1;
-  const bool x0ok = x0 >= 0 && x0 <= W - 1, x1ok = x0 + 1 >= 0 && x0 + 1 <= W - 1;
-  const int yc0 = min(max(y0, 0), H - 1), yc1 = min(max(y0 + 1, 0), H - 1);
-  const int xc0 = min(max(x0, 0), W - 1), xc1 = min(max(x0 + 1, 0), W - 1);
-  t.off[0] = (yc0 * W + xc0) * ld_in; t.w[0] = (y0ok && x0ok) ? hy * hx * m : 0.f;
-  t.off[1] = (yc0 * W + xc1) * ld_in; t.w[1] = (y0ok && x1ok) ? hy * lx * m : 0.f;
-  t.off[2] = (yc1 * W + xc0) * ld_in; t.w[2] = (y1ok && x0ok) ? ly * hx * m : 0.f;
-  t.off[3] = (yc1 * W + xc1) * ld_in; t.w[3] = (y1ok && x1ok) ? ly * lx * m : 0.f;
-  return t;
+  const float ly = py - y0f, lx = px - x0f, hy = 1.f - ly, hx = 1.f - lx;
+  const bool y0ok = y0 >= 0, y1ok = y0 + 1 <= H - 1, x0ok = x0 >= 0, x1ok = x0 + 1 <= W - 1;
+  c.y0 = y0; c.x0 = x0; c.yc = max(y0, 0); c.xc = max(x0, 0);
+  c.dx = x0ok && x1ok; c.dy = y0ok && y1ok;
+  c.w00 = (y0ok && x0ok) ? hy * hx * m : 0.f;
+  c.w01 = (y0ok && x1ok) ? hy * lx * m : 0.f;
+  c.w10 = (y1ok && x0ok) ? ly * hx * m : 0.f;
+  c.w11 = (y1ok && x1ok) ? ly * lx * m : 0.f;
+  return true;
 }
 
 // Apply the per-channel epilogue transform of fp32 head planes.

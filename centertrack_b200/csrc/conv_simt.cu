@@ -72,12 +72,19 @@ conv_simt_kernel(ConvGeom g, const T* __restrict__ x, const float* __restrict__ 
         if (iy >= 0 && iy < g.H && ix >= 0 && ix < g.W)
           av = Vec4<T>::ld(xb + ((size_t)iy * g.W + ix) * g.ld_in + c);
       } else {
-        const DcnTap s = dcn_tap(om_px, tap, aoy, aox, g.H, g.W, g.ld_in);
+        DcnCorner s;
+        if (dcn_corner((float)(aoy - 1 + tap / 3) + om_px[2 * tap], (float)(aox - 1 + tap % 3) + om_px[2 * tap + 1],
+                       g.H, g.W, om_px[18 + tap], s)) {
+          const int dx = s.dx ? g.ld_in : 0, dy = s.dy ? g.W * g.ld_in : 0;
+          const int off[4] = {0, dx, dy, dy + dx};
+          const float wq[4] = {s.w00, s.w01, s.w10, s.w11};
+          const T* p00 = xb + (s.yc * g.W + s.xc) * g.ld_in + c;
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          if (s.w[q] != 0.f) {
-            const float4 v = Vec4<T>::ld(xb + s.off[q] + c);
-            av.x += s.w[q] * v.x; av.y += s.w[q] * v.y; av.z += s.w[q] * v.z; av.w += s.w[q] * v.w;
+          for (int q = 0; q < 4; ++q) {
+            if (wq[q] != 0.f) {
+              const float4 v = Vec4<T>::ld(p00 + off[q]);
+              av.x += wq[q] * v.x; av.y += wq[q] * v.y; av.z += wq[q] * v.z; av.w += wq[q] * v.w;
+            }
           }
         }
       }

@@ -87,24 +87,40 @@ __device__ __forceinline__ uint64_t make_sdesc(uint32_t smem_addr) {
 // weights already multiplied by the modulation mask and zeroed for corners / samples outside the image.
 struct __align__(16) DcnEntry { int off, dxo, dyo, pad; float w00, w01, w10, w11; };   // 32 bytes
 
-// Bilinear footprint of the sample point (py, px) of an H x W image, from which both sampling records are packed:
-// top-left corner (y0, x0) and its clamp into the image (yc, xc), whether the x+1 / y+1 neighbours exist on both
-// sides (dx, dy), and the four corner weights times the mask, zero for corners outside the image.
-// Returns false (c untouched) when the sample is outside the image altogether (its value is 0).
-struct DcnCorner { int y0, x0, yc, xc; bool dx, dy; float w00, w01, w10, w11; };
-__device__ __forceinline__ bool dcn_corner(float py, float px, int H, int W, float m, DcnCorner& c) {
-  if (!(py > -1.f && py < (float)H && px > -1.f && px < (float)W)) return false;
-  const float y0f = floorf(py), x0f = floorf(px);
-  const int y0 = (int)y0f, x0 = (int)x0f;
-  const float ly = py - y0f, lx = px - x0f, hy = 1.f - ly, hx = 1.f - lx;
-  const bool y0ok = y0 >= 0, y1ok = y0 + 1 <= H - 1, x0ok = x0 >= 0, x1ok = x0 + 1 <= W - 1;
-  c.y0 = y0; c.x0 = x0; c.yc = max(y0, 0); c.xc = max(x0, 0);
-  c.dx = x0ok && x1ok; c.dy = y0ok && y1ok;
-  c.w00 = (y0ok && x0ok) ? hy * hx * m : 0.f;
-  c.w01 = (y0ok && x1ok) ? hy * lx * m : 0.f;
-  c.w10 = (y1ok && x0ok) ? ly * hx * m : 0.f;
-  c.w11 = (y1ok && x1ok) ? ly * lx * m : 0.f;
-  return true;
+// Sampling footprint of output pixel p (g.P_out: a padding row) for taps [tap0, tap1), the common part of both
+// sampling tables: loads the 16-byte chunks of p's offset / mask row that those taps read, then calls
+// f(tap, in, c, img) per tap.  in: the sample lies inside the image and c holds its footprint; img: the first pixel
+// of p's image.
+template <class F>
+__device__ __forceinline__ void dcn_row(const TcArgs& a, int p, int tap0, int tap1, F&& f) {
+  const ConvGeom& g = a.g;
+  const bool ok = p < g.P_out;
+  int oy = 0, ox = 0, img = 0;
+  float om[28];
+#pragma unroll
+  for (int j = 0; j < 28; ++j) om[j] = 0.f;
+  if (ok) {
+    const int HWo = g.OH * g.OW;
+    const int bb = p / HWo, r = p - bb * HWo;
+    oy = r / g.OW; ox = r - oy * g.OW; img = bb * g.H * g.W;
+    const float4* omp = reinterpret_cast<const float4*>(a.om + (size_t)p * g.ld_om);
+    // offsets: floats [2 tap0, 2 tap1), masks: [18 + tap0, 18 + tap1)
+#pragma unroll
+    for (int j = 0; j < 7; ++j) {
+      if ((4 * j < 2 * tap1 && 4 * j + 4 > 2 * tap0) || (4 * j < 18 + tap1 && 4 * j + 4 > 18 + tap0)) {
+        const float4 t4 = __ldg(omp + j);
+        om[4 * j] = t4.x; om[4 * j + 1] = t4.y; om[4 * j + 2] = t4.z; om[4 * j + 3] = t4.w;
+      }
+    }
+  }
+#pragma unroll
+  for (int tap = 0; tap < 9; ++tap) {
+    if (tap < tap0 || tap >= tap1) continue;
+    DcnCorner c;
+    const bool in = ok && dcn_corner((float)(oy - 1 + tap / 3) + om[2 * tap], (float)(ox - 1 + tap % 3) + om[2 * tap + 1],
+                                     g.H, g.W, om[18 + tap], c);
+    f(tap, in, c, img);
+  }
 }
 
 __device__ __forceinline__ uint32_t bmul2(uint32_t a, uint32_t b) {
@@ -140,6 +156,213 @@ __device__ __forceinline__ void split8(const float4 lo4, const float4 hi4, uint4
   h = make_uint4(hh[0], hh[1], hh[2], hh[3]);
   l = make_uint4(ll[0], ll[1], ll[2], ll[3]);
 }
+
+// Packed bf16 blend of four corner columns with {w,w} weight pairs: mul for corner 00, then fma for 01, 10, 11.
+__device__ __forceinline__ uint4 blend_bf2(const uint4 (&v)[4], uint32_t w0, uint32_t w1, uint32_t w2, uint32_t w3) {
+  uint4 o;
+  o.x = bmul2(v[0].x, w0); o.y = bmul2(v[0].y, w0); o.z = bmul2(v[0].z, w0); o.w = bmul2(v[0].w, w0);
+  o.x = bfma2(v[1].x, w1, o.x); o.y = bfma2(v[1].y, w1, o.y); o.z = bfma2(v[1].z, w1, o.z); o.w = bfma2(v[1].w, w1, o.w);
+  o.x = bfma2(v[2].x, w2, o.x); o.y = bfma2(v[2].y, w2, o.y); o.z = bfma2(v[2].z, w2, o.z); o.w = bfma2(v[2].w, w2, o.w);
+  o.x = bfma2(v[3].x, w3, o.x); o.y = bfma2(v[3].y, w3, o.y); o.z = bfma2(v[3].z, w3, o.z); o.w = bfma2(v[3].w, w3, o.w);
+  return o;
+}
+
+// One row's 8-channel column of the A operand in each activation format: its registers V, a load from global memory,
+// zero, the store into a swizzled A stage of STAGE_BYTES (zeros where !live: K padding), and the DCNv2 blend of the
+// four corner columns with the float weights of a DcnEntry.
+struct OpBf16 {
+  using T = __nv_bfloat16;
+  using V = uint4;
+  static constexpr uint32_t STAGE_BYTES = A_STAGE_BYTES;
+  static __device__ __forceinline__ V load(const T* p) { return ldg_nc16(p); }
+  static __device__ __forceinline__ V zero() { return make_uint4(0, 0, 0, 0); }
+  static __device__ __forceinline__ void store(uint32_t dst, const V& v, bool live = true) {
+    sts16(dst, live ? v : zero());
+  }
+  // same rounding points as the window sampler: weights to bf16, then the packed chain
+  static __device__ __forceinline__ V blend(const V (&v)[4], const float4 w) {
+    return blend_bf2(v, dup_bf2(w.x), dup_bf2(w.y), dup_bf2(w.z), dup_bf2(w.w));
+  }
+};
+// X3: fp32 activations (channels 0-3 and 4-7), stored split into the bf16 hi tile and the lo tile A_STAGE_BYTES after
+struct OpX3 {
+  using T = float;
+  struct V { float4 f[2]; };
+  static constexpr uint32_t STAGE_BYTES = 2u * A_STAGE_BYTES;
+  static __device__ __forceinline__ V load(const T* p) { return {{ldg_nc_f4(p), ldg_nc_f4(p + 4)}}; }
+  static __device__ __forceinline__ V zero() { return {{make_float4(0.f, 0.f, 0.f, 0.f), make_float4(0.f, 0.f, 0.f, 0.f)}}; }
+  static __device__ __forceinline__ void store(uint32_t dst, const V& v, bool live = true) {
+    uint4 hi, lo;
+    split8(v.f[0], v.f[1], hi, lo);
+    if (!live) { hi = make_uint4(0, 0, 0, 0); lo = hi; }
+    sts16(dst, hi);
+    sts16(dst + A_STAGE_BYTES, lo);
+  }
+  // fp32: w0 * v0, then fmaf for corners 1 to 3
+  static __device__ __forceinline__ V blend(const V (&v)[4], const float4 w) {
+    const float ww[4] = {w.x, w.y, w.z, w.w};
+    V o;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      o.f[h] = make_float4(ww[0] * v[0].f[h].x, ww[0] * v[0].f[h].y, ww[0] * v[0].f[h].z, ww[0] * v[0].f[h].w);
+#pragma unroll
+      for (int cn = 1; cn < 4; ++cn) {
+        o.f[h].x = fmaf(ww[cn], v[cn].f[h].x, o.f[h].x); o.f[h].y = fmaf(ww[cn], v[cn].f[h].y, o.f[h].y);
+        o.f[h].z = fmaf(ww[cn], v[cn].f[h].z, o.f[h].z); o.f[h].w = fmaf(ww[cn], v[cn].f[h].w, o.f[h].w);
+      }
+    }
+    return o;
+  }
+};
+
+// The gather role of one thread: the 8-channel column q of GEMM rows rb + 16 i (i < TC_NROW) of every K slice, stored
+// at swizzle swz into the A stages at sA.  The producers below reach the kernel's per-slice protocol through
+// begin_stage(s) -> stage and end_stage(s, stage).
+struct Gather { uint32_t sA, swz; int tid, q, rb, cin8, ntaps; };
+
+// Plain convolution gather, register-prefetched two K slices ahead (8 independent 16-byte loads in flight per
+// thread) while the MMAs of the previous slice run.  (tap, channel group) advance incrementally with the load order.
+// row_off / row_iy / row_ix: element offset and coordinates of each row's top-left input pixel.
+template <class Op, class Begin, class End>
+__device__ __forceinline__ void gather_conv(const TcArgs& a, const Gather& t, const int (&row_off)[TC_NROW],
+                                            const int (&row_iy)[TC_NROW], const int (&row_ix)[TC_NROW],
+                                            Begin&& begin_stage, End&& end_stage) {
+  using T = typename Op::T;
+  using V = typename Op::V;
+  const ConvGeom& g = a.g;
+  int ltap = t.q / t.cin8, lcq = t.q - ltap * t.cin8;
+  auto load_slice = [&](bool in_range, V (&v)[TC_NROW]) {
+#pragma unroll
+    for (int i = 0; i < TC_NROW; ++i) v[i] = Op::zero();
+    if (in_range && ltap < t.ntaps) {
+      const int ky = ltap / g.KW, kx = ltap - ky * g.KW;
+      const int tap_off = (ky * g.W + kx) * g.ld_in + (lcq << 3);      // same for every row of the slice
+#pragma unroll
+      for (int i = 0; i < TC_NROW; ++i)
+        if ((unsigned)(row_iy[i] + ky) < (unsigned)g.H && (unsigned)(row_ix[i] + kx) < (unsigned)g.W)
+          v[i] = Op::load(reinterpret_cast<const T*>(a.x) + (row_off[i] + tap_off));
+    }
+    lcq += 8;
+    while (lcq >= t.cin8) { lcq -= t.cin8; ++ltap; }
+  };
+  auto store_slice = [&](int s, const V (&v)[TC_NROW]) {
+    const int stage = begin_stage(s);
+    const uint32_t dst = t.sA + stage * Op::STAGE_BYTES + (uint32_t)t.rb * 128u + t.swz;
+#pragma unroll
+    for (int i = 0; i < TC_NROW; ++i) Op::store(dst + i * 2048u, v[i]);
+    end_stage(s, stage);
+  };
+  const int KS = a.k_slices;
+  V v0[TC_NROW], v1[TC_NROW];
+  load_slice(0 < KS, v0);
+  load_slice(1 < KS, v1);
+  for (int s = 0; s < KS; s += 2) {
+    store_slice(s, v0);
+    load_slice(s + 2 < KS, v0);
+    if (s + 1 < KS) { store_slice(s + 1, v1); load_slice(s + 3 < KS, v1); }
+  }
+}
+
+// DCNv2 sampled from global memory through the DcnEntry table (CT_A_DCN).  Software-pipelined by half slices (2 of
+// the thread's 4 rows): the 8 corner loads of the next half are in flight while the current half is blended.  A slice
+// whose tap index runs past the kernel (K padding) samples tap 0 with its result zeroed.
+template <class Op, class Begin, class End>
+__device__ __forceinline__ void gather_dcn(const TcArgs& a, const Gather& t, const DcnEntry* dcn_tab,
+                                           Begin&& begin_stage, End&& end_stage) {
+  using T = typename Op::T;
+  using V = typename Op::V;
+  V va[2][4], vb[2][4];
+  auto load_half = [&](int tap, int c, int half, V (&v)[2][4]) {
+    const DcnEntry* tab = dcn_tab + (tap < t.ntaps ? tap : 0) * TC_BM + t.rb + 32 * half;
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int4 o = *reinterpret_cast<const int4*>(&tab[16 * j]);     // off, dxo, dyo
+      const T* p00 = reinterpret_cast<const T*>(a.x) + (o.x + c);
+      v[j][0] = Op::load(p00);
+      v[j][1] = Op::load(p00 + o.y);
+      v[j][2] = Op::load(p00 + o.z);
+      v[j][3] = Op::load(p00 + o.z + o.y);
+    }
+  };
+  auto blend_half = [&](int tap, int stage, int half, const V (&v)[2][4]) {
+    const bool live = tap < t.ntaps;
+    const DcnEntry* tab = dcn_tab + (live ? tap : 0) * TC_BM + t.rb + 32 * half;
+    const uint32_t dst = t.sA + stage * Op::STAGE_BYTES + (uint32_t)(t.rb + 32 * half) * 128u + t.swz;
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const float4 w = *reinterpret_cast<const float4*>(&tab[16 * j].w00);
+      Op::store(dst + j * 2048u, Op::blend(v[j], w), live);
+    }
+  };
+  // (tap, channel group) of this thread's 8-channel column in slice s, advanced incrementally (no division)
+  int tap = t.q / t.cin8, cq = t.q - tap * t.cin8;
+  load_half(tap, cq << 3, 0, va);
+  for (int s = 0; s < a.k_slices; ++s) {
+    load_half(tap, cq << 3, 1, vb);
+    const int stage = begin_stage(s);
+    blend_half(tap, stage, 0, va);
+    int ntap = tap, ncq = cq + 8;
+    while (ncq >= t.cin8) { ncq -= t.cin8; ++ntap; }
+    if (s + 1 < a.k_slices) load_half(ntap, ncq << 3, 0, va);
+    blend_half(tap, stage, 1, vb);
+    tap = ntap; cq = ncq;
+    end_stage(s, stage);
+  }
+}
+
+// DCN sampled from a shared-memory window (CT_A_DCN_WIN, bf16 only).  K order = (64-channel chunk, tap, channel): one
+// K slice is one tap of one chunk, so the window of a chunk serves nine slices.  Per slice a thread blends its four
+// rows' 8-channel column: 16 LDS.128 (four corners x four rows) instead of 16 L1/L2 round trips; records whose 2x2
+// footprint leaves the window (offset beyond the margin) take the global path.  load_window(ch): thread 0 requests
+// chunk ch of the window at s_win, completing win_bar.
+template <class LoadWindow, class Begin, class End>
+__device__ __forceinline__ void gather_window(const TcArgs& a, const Gather& t, const DcnWinEntry* win_tab,
+                                              uint32_t s_win, uint32_t win_bar, LoadWindow&& load_window,
+                                              Begin&& begin_stage, End&& end_stage) {
+  const ConvGeom& g = a.g;
+  const int nchunks = g.C_in >> 6;
+  const uint32_t pitch = (uint32_t)a.win_pw * 128u;
+  const int gdx = g.ld_in, gdy = g.W * g.ld_in;
+  int s = 0;
+  for (int ch = 0; ch < nchunks; ++ch) {
+    mbar_wait(win_bar, (uint32_t)ch & 1u);
+    for (int tap = 0; tap < 9; ++tap, ++s) {
+      const int stage = begin_stage(s);
+      const DcnWinEntry* tab = win_tab + tap * TC_BM + t.rb;
+      uint4 e4[TC_NROW], v[TC_NROW][4];
+#pragma unroll
+      for (int i = 0; i < TC_NROW; ++i) e4[i] = *reinterpret_cast<const uint4*>(&tab[16 * i]);
+#pragma unroll
+      for (int i = 0; i < TC_NROW; ++i) {
+        const uint32_t meta = e4[i].y;
+        if (meta & WIN_IN) {
+          const uint32_t base = s_win + ((meta & 0xffffu) << 4) + (uint32_t)(t.q << 4);
+          const uint32_t dx = (meta & WIN_DX) ? 128u : 0u, dy = (meta & WIN_DY) ? pitch : 0u;
+          v[i][0] = lds16(base); v[i][1] = lds16(base + dx);
+          v[i][2] = lds16(base + dy); v[i][3] = lds16(base + dy + dx);
+        } else {
+          const __nv_bfloat16* p00 = a.x + ((int)e4[i].x + (ch << 6) + (t.q << 3));
+          const int dx = (meta & WIN_DX) ? gdx : 0, dy = (meta & WIN_DY) ? gdy : 0;
+          v[i][0] = ldg_nc16(p00); v[i][1] = ldg_nc16(p00 + dx);
+          v[i][2] = ldg_nc16(p00 + dy); v[i][3] = ldg_nc16(p00 + dy + dx);
+        }
+      }
+      const uint32_t dst = t.sA + stage * A_STAGE_BYTES + (uint32_t)t.rb * 128u + t.swz;
+#pragma unroll
+      for (int i = 0; i < TC_NROW; ++i) {
+        const uint32_t w0 = __byte_perm(e4[i].z, 0, 0x1010), w1 = __byte_perm(e4[i].z, 0, 0x3232);   // {w,w} pairs
+        const uint32_t w2 = __byte_perm(e4[i].w, 0, 0x1010), w3 = __byte_perm(e4[i].w, 0, 0x3232);
+        sts16(dst + i * 2048u, blend_bf2(v[i], w0, w1, w2, w3));
+      }
+      end_stage(s, stage);
+    }
+    if (ch + 1 < nchunks) {                       // every thread is done with this chunk's window: refill it
+      named_sync(1, TC_PRODUCERS);
+      if (t.tid == 0) load_window(ch + 1);
+    }
+  }
+}
+
 template <bool X3, int N>
 __global__ void __launch_bounds__(TC_THREADS, (!X3 && N <= 64) ? 2 : 1)
 conv_tc_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
@@ -153,8 +376,8 @@ conv_tc_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
   const int S = a.stages;
   constexpr uint32_t b_tile_bytes = (uint32_t)N * 128u;                       // one bf16 weight tile of a K slice
   constexpr uint32_t b_stage_bytes = X3 ? 2u * b_tile_bytes : b_tile_bytes;   // X3: [hi][lo]
-  constexpr uint32_t a_stage_bytes = X3 ? 2u * A_STAGE_BYTES : A_STAGE_BYTES; // X3: [hi 16 KB][lo 16 KB]
-  const float* xf = reinterpret_cast<const float*>(a.x);
+  using Op = std::conditional_t<X3, OpX3, OpBf16>;
+  constexpr uint32_t a_stage_bytes = Op::STAGE_BYTES;                         // X3: [hi 16 KB][lo 16 KB]
 
   // carve shared memory: [stages | epilogue staging][barriers][DCN table / window]
   const uint32_t smem_base = smem_u32(smem);
@@ -230,6 +453,10 @@ conv_tc_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
   }
   if (tid == 0) tc_stamp(trace, 1);
   int win_x0 = 0, win_y0 = 0, win_b = 0;
+  auto load_window = [&](int ch) {                    // 64-channel chunk ch of the window: TMA, zero fill outside
+    mbar_arrive_expect_tx(win_bar, a.win_bytes);      // count 1: this arrival + the TMA's bytes complete the phase
+    tma_4d(s_win, &tmap, ch << 6, win_x0, win_y0, win_b, win_bar);
+  };
   if (win) {
     // window origin of this 8x16 patch: one kernel-halo pixel + the offset margin to the top/left
     const int tpi = a.tiles_x * a.tiles_y;
@@ -238,93 +465,44 @@ conv_tc_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
     const int ty = t / a.tiles_x, tx = t - ty * a.tiles_x;
     win_y0 = ty * 8 - 1 - a.win_m;
     win_x0 = tx * 16 - 1 - a.win_m;
-    if (tid == 0) {                                   // first 64-channel chunk of the window: TMA, zero fill outside
-      mbar_arrive_expect_tx(win_bar, a.win_bytes);      // count 1: this arrival + the TMA's bytes complete the phase
-      tma_4d(s_win, &tmap, 0, win_x0, win_y0, win_b, win_bar);
-    }
+    if (tid == 0) load_window(0);
     // Two threads per row (taps 0-4 and 5-8).  The 27 offset / mask floats of a row sit in one 128-byte line of `om`;
     // each thread loads only the 16-byte chunks its taps need.
     const int trow = tid & (TC_BM - 1), thalf = tid >> 7;            // thalf 0: taps 0..4, thalf 1: taps 5..8
-    const int tap0 = thalf ? 5 : 0, tap1 = thalf ? 9 : 5;
-    const int tp = tc_pixel(a, mt, trow);
-    const bool ok = tp < g.P_out;
-    {
-      int oy = 0, ox = 0, img = 0;
-      float om[28];
-#pragma unroll
-      for (int j = 0; j < 28; ++j) om[j] = 0.f;
-      if (ok) {
-        const int bb = tp / HWo, r = tp - bb * HWo;
-        oy = r / g.OW; ox = r - oy * g.OW; img = bb * g.H * g.W;
-        const float4* omp = reinterpret_cast<const float4*>(a.om + (size_t)tp * g.ld_om);
-        // floats [2 tap0, 2 tap1) and [18 + tap0, 18 + tap1): chunks 0-2, 4-5 (thalf 0) / 2-6 (thalf 1)
-#pragma unroll
-        for (int j = 0; j < 7; ++j) {
-          const bool need = thalf ? (j >= 2) : (j <= 2 || j == 4 || j == 5);
-          if (need) {
-            const float4 t4 = __ldg(omp + j);
-            om[4 * j] = t4.x; om[4 * j + 1] = t4.y; om[4 * j + 2] = t4.z; om[4 * j + 3] = t4.w;
-          }
-        }
+    dcn_row(a, tc_pixel(a, mt, trow), thalf ? 5 : 0, thalf ? 9 : 5, [&](int tap, bool in, const DcnCorner& c, int img) {
+      DcnWinEntry e; e.goff = 0; e.meta = WIN_IN; e.w01 = 0u; e.w23 = 0u;
+      if (in) {
+        e.goff = (img + c.yc * g.W + c.xc) * g.ld_in;
+        const bool inside = c.y0 >= win_y0 && c.y0 + 1 <= win_y0 + a.win_ph - 1 && c.x0 >= win_x0 &&
+                            c.x0 + 1 <= win_x0 + a.win_pw - 1;
+        const uint32_t woff16 = (uint32_t)((c.yc - win_y0) * a.win_pw + (c.xc - win_x0)) * 8u;   // 128 B per pixel
+        e.meta = (inside ? (woff16 | WIN_IN) : 0u) | (c.dx ? WIN_DX : 0u) | (c.dy ? WIN_DY : 0u);
+        const __nv_bfloat162 wa = __floats2bfloat162_rn(c.w00, c.w01), wb = __floats2bfloat162_rn(c.w10, c.w11);
+        e.w01 = *reinterpret_cast<const uint32_t*>(&wa);
+        e.w23 = *reinterpret_cast<const uint32_t*>(&wb);
       }
-#pragma unroll
-      for (int tap = 0; tap < 9; ++tap) {
-        if (tap < tap0 || tap >= tap1) continue;
-        DcnWinEntry e; e.goff = 0; e.meta = WIN_IN; e.w01 = 0u; e.w23 = 0u;
-        DcnCorner c;
-        if (ok && dcn_corner((float)(oy - 1 + tap / 3) + om[2 * tap], (float)(ox - 1 + tap % 3) + om[2 * tap + 1],
-                             g.H, g.W, om[18 + tap], c)) {
-          e.goff = (img + c.yc * g.W + c.xc) * g.ld_in;
-          const bool inside = c.y0 >= win_y0 && c.y0 + 1 <= win_y0 + a.win_ph - 1 && c.x0 >= win_x0 &&
-                              c.x0 + 1 <= win_x0 + a.win_pw - 1;
-          const uint32_t woff16 = (uint32_t)((c.yc - win_y0) * a.win_pw + (c.xc - win_x0)) * 8u;   // 128 B per pixel
-          e.meta = (inside ? (woff16 | WIN_IN) : 0u) | (c.dx ? WIN_DX : 0u) | (c.dy ? WIN_DY : 0u);
-          const __nv_bfloat162 wa = __floats2bfloat162_rn(c.w00, c.w01), wb = __floats2bfloat162_rn(c.w10, c.w11);
-          e.w01 = *reinterpret_cast<const uint32_t*>(&wa);
-          e.w23 = *reinterpret_cast<const uint32_t*>(&wb);
-        }
-        win_tab[tap * TC_BM + trow] = e;
-      }
-    }
+      win_tab[tap * TC_BM + trow] = e;
+    });
     named_sync(1, TC_PRODUCERS);
     if (tid == 0) tc_stamp(trace, 2);
   }
   if (a.a_mode == CT_A_DCN) {
     // per (tap,row) sampling records, computed once per CTA (row = tid, threads 0..127)
-    const int p = tid < TC_BM ? tc_pixel(a, mt, tid) : g.P_out;
-    const bool ok = p < g.P_out;
     if (tid < TC_BM) {
-      int oy = 0, ox = 0, img = 0;
-      float om[28];
-      if (ok) {
-        const int bb = p / HWo, r = p - bb * HWo;
-        oy = r / g.OW; ox = r - oy * g.OW; img = bb * g.H * g.W;
-        const float4* omp = reinterpret_cast<const float4*>(a.om + (size_t)p * g.ld_om);
-#pragma unroll
-        for (int j = 0; j < 7; ++j) {
-          const float4 t = __ldg(omp + j);
-          om[4 * j] = t.x; om[4 * j + 1] = t.y; om[4 * j + 2] = t.z; om[4 * j + 3] = t.w;
-        }
-      }
-#pragma unroll
-      for (int tap = 0; tap < 9; ++tap) {
+      dcn_row(a, tc_pixel(a, mt, tid), 0, 9, [&](int tap, bool in, const DcnCorner& c, int img) {
         DcnEntry e; e.off = 0; e.dxo = 0; e.dyo = 0; e.pad = 0; e.w00 = e.w01 = e.w10 = e.w11 = 0.f;
-        DcnCorner c;
-        if (ok && dcn_corner((float)(oy - 1 + tap / 3) + om[2 * tap], (float)(ox - 1 + tap % 3) + om[2 * tap + 1],
-                             g.H, g.W, om[18 + tap], c)) {
+        if (in) {
           e.off = (img + c.yc * g.W + c.xc) * g.ld_in;
           e.dxo = c.dx ? g.ld_in : 0;
           e.dyo = c.dy ? g.W * g.ld_in : 0;
           e.w00 = c.w00; e.w01 = c.w01; e.w10 = c.w10; e.w11 = c.w11;
         }
         dcn_tab[tap * TC_BM + tid] = e;
-      }
+      });
     }
     named_sync(1, TC_PRODUCERS);
     if (tid == 0) tc_stamp(trace, 2);
   }
-  const int cin8 = g.C_in >> 3;
-  const int ntaps = g.KH * g.KW;
   const size_t w_slice_elems = (size_t)(X3 ? 2 : 1) * N * TC_BK;
   const __nv_bfloat16* wt = a.w + (size_t)nt * a.k_slices * w_slice_elems;
 
@@ -377,237 +555,10 @@ conv_tc_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
     }
   };
 
-  if (win) {
-    // ---- DCN sampled from a shared-memory window (CT_A_DCN_WIN).  K order = (64-channel chunk, tap, channel): one K
-    // slice is one tap of one chunk, so the window of a chunk serves nine slices.  Per slice a thread blends its
-    // four rows' 8-channel column: 16 LDS.128 (four corners x four rows) instead of 16 L1/L2 round trips; records
-    // whose 2x2 footprint leaves the window (offset beyond the margin) take the global path.
-    const int nchunks = g.C_in >> 6;
-    const uint32_t pitch = (uint32_t)a.win_pw * 128u;
-    const int gdx = g.ld_in, gdy = g.W * g.ld_in;
-    int s = 0;
-    for (int ch = 0; ch < nchunks; ++ch) {
-      mbar_wait(win_bar, (uint32_t)ch & 1u);
-      for (int tap = 0; tap < 9; ++tap, ++s) {
-        const int stage = begin_stage(s);
-        const DcnWinEntry* tab = win_tab + tap * TC_BM + rb;
-        uint4 e4[TC_NROW], v[TC_NROW][4];
-#pragma unroll
-        for (int i = 0; i < TC_NROW; ++i) e4[i] = *reinterpret_cast<const uint4*>(&tab[16 * i]);
-#pragma unroll
-        for (int i = 0; i < TC_NROW; ++i) {
-          const uint32_t meta = e4[i].y;
-          if (meta & WIN_IN) {
-            const uint32_t base = s_win + ((meta & 0xffffu) << 4) + (uint32_t)(q << 4);
-            const uint32_t dx = (meta & WIN_DX) ? 128u : 0u, dy = (meta & WIN_DY) ? pitch : 0u;
-            v[i][0] = lds16(base); v[i][1] = lds16(base + dx);
-            v[i][2] = lds16(base + dy); v[i][3] = lds16(base + dy + dx);
-          } else {
-            const __nv_bfloat16* p00 = a.x + ((int)e4[i].x + (ch << 6) + (q << 3));
-            const int dx = (meta & WIN_DX) ? gdx : 0, dy = (meta & WIN_DY) ? gdy : 0;
-            v[i][0] = ldg_nc16(p00); v[i][1] = ldg_nc16(p00 + dx);
-            v[i][2] = ldg_nc16(p00 + dy); v[i][3] = ldg_nc16(p00 + dy + dx);
-          }
-        }
-        const uint32_t dst = sA + stage * A_STAGE_BYTES + (uint32_t)rb * 128u + swz;
-#pragma unroll
-        for (int i = 0; i < TC_NROW; ++i) {
-          const uint32_t w0 = __byte_perm(e4[i].z, 0, 0x1010), w1 = __byte_perm(e4[i].z, 0, 0x3232);   // {w,w} pairs
-          const uint32_t w2 = __byte_perm(e4[i].w, 0, 0x1010), w3 = __byte_perm(e4[i].w, 0, 0x3232);
-          uint4 o;
-          o.x = bmul2(v[i][0].x, w0); o.y = bmul2(v[i][0].y, w0); o.z = bmul2(v[i][0].z, w0); o.w = bmul2(v[i][0].w, w0);
-          o.x = bfma2(v[i][1].x, w1, o.x); o.y = bfma2(v[i][1].y, w1, o.y); o.z = bfma2(v[i][1].z, w1, o.z); o.w = bfma2(v[i][1].w, w1, o.w);
-          o.x = bfma2(v[i][2].x, w2, o.x); o.y = bfma2(v[i][2].y, w2, o.y); o.z = bfma2(v[i][2].z, w2, o.z); o.w = bfma2(v[i][2].w, w2, o.w);
-          o.x = bfma2(v[i][3].x, w3, o.x); o.y = bfma2(v[i][3].y, w3, o.y); o.z = bfma2(v[i][3].z, w3, o.z); o.w = bfma2(v[i][3].w, w3, o.w);
-          sts16(dst + i * 2048u, o);
-        }
-        end_stage(s, stage);
-      }
-      if (ch + 1 < nchunks) {                       // every thread is done with this chunk's window: refill it
-        named_sync(1, TC_PRODUCERS);
-        if (tid == 0) {
-          mbar_arrive_expect_tx(win_bar, a.win_bytes);      // count 1: this arrival + the TMA's bytes complete the phase
-          tma_4d(s_win, &tmap, (ch + 1) << 6, win_x0, win_y0, win_b, win_bar);
-        }
-      }
-    }
-  } else if constexpr (X3) {
-    // ---- bf16x3 producers: fp32 activations, each 8-channel chunk = two 16-byte loads, split into hi / lo tiles
-    if (a.a_mode == CT_A_DCN) {
-      float4 va[2][4][2], vb[2][4][2];
-      auto load_half = [&](int tap, int c, int half, float4 (&v)[2][4][2]) {
-        const DcnEntry* tab = dcn_tab + (tap < ntaps ? tap : 0) * TC_BM + rb + 32 * half;
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-          const int4 o = *reinterpret_cast<const int4*>(&tab[16 * j]);     // off, dxo, dyo
-          const float* p00 = xf + (o.x + c);
-          v[j][0][0] = ldg_nc_f4(p00);             v[j][0][1] = ldg_nc_f4(p00 + 4);
-          v[j][1][0] = ldg_nc_f4(p00 + o.y);       v[j][1][1] = ldg_nc_f4(p00 + o.y + 4);
-          v[j][2][0] = ldg_nc_f4(p00 + o.z);       v[j][2][1] = ldg_nc_f4(p00 + o.z + 4);
-          v[j][3][0] = ldg_nc_f4(p00 + o.z + o.y); v[j][3][1] = ldg_nc_f4(p00 + o.z + o.y + 4);
-        }
-      };
-      auto blend_half = [&](int tap, int stage, int half, const float4 (&v)[2][4][2]) {
-        const bool live = tap < ntaps;
-        const DcnEntry* tab = dcn_tab + (live ? tap : 0) * TC_BM + rb + 32 * half;
-        const uint32_t dst = sA + stage * a_stage_bytes + (uint32_t)(rb + 32 * half) * 128u + swz;
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-          const float4 w = *reinterpret_cast<const float4*>(&tab[16 * j].w00);
-          const float ww[4] = {w.x, w.y, w.z, w.w};
-          float4 acc4[2];
-#pragma unroll
-          for (int h2 = 0; h2 < 2; ++h2) {
-            acc4[h2] = make_float4(ww[0] * v[j][0][h2].x, ww[0] * v[j][0][h2].y, ww[0] * v[j][0][h2].z, ww[0] * v[j][0][h2].w);
-#pragma unroll
-            for (int cn = 1; cn < 4; ++cn) {
-              acc4[h2].x = fmaf(ww[cn], v[j][cn][h2].x, acc4[h2].x); acc4[h2].y = fmaf(ww[cn], v[j][cn][h2].y, acc4[h2].y);
-              acc4[h2].z = fmaf(ww[cn], v[j][cn][h2].z, acc4[h2].z); acc4[h2].w = fmaf(ww[cn], v[j][cn][h2].w, acc4[h2].w);
-            }
-          }
-          uint4 hi, lo;
-          split8(acc4[0], acc4[1], hi, lo);
-          if (!live) { hi = make_uint4(0, 0, 0, 0); lo = hi; }
-          sts16(dst + j * 2048u, hi);
-          sts16(dst + A_STAGE_BYTES + j * 2048u, lo);
-        }
-      };
-      int tap = q / cin8, cq = q - tap * cin8;
-      load_half(tap, cq << 3, 0, va);
-      for (int s = 0; s < a.k_slices; ++s) {
-        load_half(tap, cq << 3, 1, vb);
-        const int stage = begin_stage(s);
-        blend_half(tap, stage, 0, va);
-        int ntap = tap, ncq = cq + 8;
-        while (ncq >= cin8) { ncq -= cin8; ++ntap; }
-        if (s + 1 < a.k_slices) load_half(ntap, ncq << 3, 0, va);
-        blend_half(tap, stage, 1, vb);
-        tap = ntap; cq = ncq;
-        end_stage(s, stage);
-      }
-    } else {
-      int ltap = q / cin8, lcq = q - ltap * cin8;
-      auto load_slice = [&](bool in_range, float4 (&v)[TC_NROW][2]) {
-#pragma unroll
-        for (int i = 0; i < TC_NROW; ++i) { v[i][0] = make_float4(0.f, 0.f, 0.f, 0.f); v[i][1] = v[i][0]; }
-        if (in_range && ltap < ntaps) {
-          const int ky = ltap / g.KW, kx = ltap - ky * g.KW;
-          const int tap_off = (ky * g.W + kx) * g.ld_in + (lcq << 3);
-#pragma unroll
-          for (int i = 0; i < TC_NROW; ++i)
-            if ((unsigned)(row_iy[i] + ky) < (unsigned)g.H && (unsigned)(row_ix[i] + kx) < (unsigned)g.W) {
-              const float* pp = xf + (row_off[i] + tap_off);
-              v[i][0] = ldg_nc_f4(pp); v[i][1] = ldg_nc_f4(pp + 4);
-            }
-        }
-        lcq += 8;
-        while (lcq >= cin8) { lcq -= cin8; ++ltap; }
-      };
-      auto store_slice = [&](int s, const float4 (&v)[TC_NROW][2]) {
-        const int stage = begin_stage(s);
-        const uint32_t dst = sA + stage * a_stage_bytes + (uint32_t)rb * 128u + swz;
-#pragma unroll
-        for (int i = 0; i < TC_NROW; ++i) {
-          uint4 hi, lo;
-          split8(v[i][0], v[i][1], hi, lo);
-          sts16(dst + i * 2048u, hi);
-          sts16(dst + A_STAGE_BYTES + i * 2048u, lo);
-        }
-        end_stage(s, stage);
-      };
-      const int KS = a.k_slices;
-      float4 v0[TC_NROW][2], v1[TC_NROW][2];
-      load_slice(0 < KS, v0);
-      load_slice(1 < KS, v1);
-      for (int s = 0; s < KS; s += 2) {
-        store_slice(s, v0);
-        load_slice(s + 2 < KS, v0);
-        if (s + 1 < KS) { store_slice(s + 1, v1); load_slice(s + 3 < KS, v1); }
-      }
-    }
-  } else if (a.a_mode == CT_A_DCN) {
-    // Software-pipelined by half slices (2 of the thread's 4 rows): the 8 corner loads of the next half are in
-    // flight while the current half is blended.  A slice whose tap index runs past the kernel (K padding) samples
-    // tap 0 with its result zeroed.
-    uint4 va[2][4], vb[2][4];
-    auto load_half = [&](int tap, int c, int half, uint4 (&v)[2][4]) {
-      const DcnEntry* tab = dcn_tab + (tap < ntaps ? tap : 0) * TC_BM + rb + 32 * half;
-#pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        const int4 o = *reinterpret_cast<const int4*>(&tab[16 * j]);     // off, dxo, dyo
-        const __nv_bfloat16* p00 = a.x + (o.x + c);
-        v[j][0] = ldg_nc16(p00);
-        v[j][1] = ldg_nc16(p00 + o.y);
-        v[j][2] = ldg_nc16(p00 + o.z);
-        v[j][3] = ldg_nc16(p00 + o.z + o.y);
-      }
-    };
-    auto blend_half = [&](int tap, int stage, int half, const uint4 (&v)[2][4]) {
-      const bool live = tap < ntaps;
-      const DcnEntry* tab = dcn_tab + (live ? tap : 0) * TC_BM + rb + 32 * half;
-      const uint32_t dst = sA + stage * A_STAGE_BYTES + (uint32_t)(rb + 32 * half) * 128u + swz;
-#pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        // packed bf16 blend, same rounding points as the window sampler (weights to bf16, fma chain 00,01,10,11)
-        const float4 w = *reinterpret_cast<const float4*>(&tab[16 * j].w00);
-        const uint32_t w0 = dup_bf2(w.x), w1 = dup_bf2(w.y), w2 = dup_bf2(w.z), w3 = dup_bf2(w.w);
-        uint4 o;
-        o.x = bmul2(v[j][0].x, w0); o.y = bmul2(v[j][0].y, w0); o.z = bmul2(v[j][0].z, w0); o.w = bmul2(v[j][0].w, w0);
-        o.x = bfma2(v[j][1].x, w1, o.x); o.y = bfma2(v[j][1].y, w1, o.y); o.z = bfma2(v[j][1].z, w1, o.z); o.w = bfma2(v[j][1].w, w1, o.w);
-        o.x = bfma2(v[j][2].x, w2, o.x); o.y = bfma2(v[j][2].y, w2, o.y); o.z = bfma2(v[j][2].z, w2, o.z); o.w = bfma2(v[j][2].w, w2, o.w);
-        o.x = bfma2(v[j][3].x, w3, o.x); o.y = bfma2(v[j][3].y, w3, o.y); o.z = bfma2(v[j][3].z, w3, o.z); o.w = bfma2(v[j][3].w, w3, o.w);
-        sts16(dst + j * 2048u, live ? o : make_uint4(0, 0, 0, 0));
-      }
-    };
-    // (tap, channel group) of this thread's 8-channel column in slice s, advanced incrementally (no division)
-    int tap = q / cin8, cq = q - tap * cin8;
-    load_half(tap, cq << 3, 0, va);
-    for (int s = 0; s < a.k_slices; ++s) {
-      load_half(tap, cq << 3, 1, vb);
-      const int stage = begin_stage(s);
-      blend_half(tap, stage, 0, va);
-      int ntap = tap, ncq = cq + 8;
-      while (ncq >= cin8) { ncq -= cin8; ++ntap; }
-      if (s + 1 < a.k_slices) load_half(ntap, ncq << 3, 0, va);
-      blend_half(tap, stage, 1, vb);
-      tap = ntap; cq = ncq;
-      end_stage(s, stage);
-    }
-  } else {
-    // Plain convolution gather, register-prefetched two K slices ahead (8 independent 16-byte loads in flight per
-    // thread) while the MMAs of the previous slice run.  (tap, channel group) advance incrementally with the load order.
-    int ltap = q / cin8, lcq = q - ltap * cin8;
-    auto load_slice = [&](bool in_range, uint4 (&v)[TC_NROW]) {
-#pragma unroll
-      for (int i = 0; i < TC_NROW; ++i) v[i] = make_uint4(0, 0, 0, 0);
-      if (in_range && ltap < ntaps) {
-        const int ky = ltap / g.KW, kx = ltap - ky * g.KW;
-        const int tap_off = (ky * g.W + kx) * g.ld_in + (lcq << 3);      // same for every row of the slice
-#pragma unroll
-        for (int i = 0; i < TC_NROW; ++i)
-          if ((unsigned)(row_iy[i] + ky) < (unsigned)g.H && (unsigned)(row_ix[i] + kx) < (unsigned)g.W)
-            v[i] = ldg_nc16(a.x + (row_off[i] + tap_off));
-      }
-      lcq += 8;
-      while (lcq >= cin8) { lcq -= cin8; ++ltap; }
-    };
-    auto store_slice = [&](int s, const uint4 (&v)[TC_NROW]) {
-      const int stage = begin_stage(s);
-      const uint32_t dst = sA + stage * A_STAGE_BYTES + (uint32_t)rb * 128u + swz;
-#pragma unroll
-      for (int i = 0; i < TC_NROW; ++i) sts16(dst + i * 2048u, v[i]);
-      end_stage(s, stage);
-    };
-    const int KS = a.k_slices;
-    uint4 v0[TC_NROW], v1[TC_NROW];
-    load_slice(0 < KS, v0);
-    load_slice(1 < KS, v1);
-    for (int s = 0; s < KS; s += 2) {
-      store_slice(s, v0);
-      load_slice(s + 2 < KS, v0);
-      if (s + 1 < KS) { store_slice(s + 1, v1); load_slice(s + 3 < KS, v1); }
-    }
-  }
+  const Gather t{sA, swz, tid, q, rb, g.C_in >> 3, g.KH * g.KW};
+  if (win) gather_window(a, t, win_tab, s_win, win_bar, load_window, begin_stage, end_stage);
+  else if (a.a_mode == CT_A_DCN) gather_dcn<Op>(a, t, dcn_tab, begin_stage, end_stage);
+  else gather_conv<Op>(a, t, row_off, row_iy, row_ix, begin_stage, end_stage);
   wg_wait<0>();
   wg_fence_operand(acc);
   if (tid == 0) tc_stamp(trace, 5);

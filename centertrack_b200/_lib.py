@@ -10,7 +10,7 @@ import subprocess
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libctb200.so')
 CSRC = os.path.join(_HERE, 'csrc')
-SOURCES = ['api.cu', 'conv_simt.cu', 'conv_tc.cu', 'conv_halo.cu', 'elementwise.cu', 'decode.cu', 'stream.cu']
+SOURCES = ['api.cu', 'conv_simt.cu', 'conv_tc.cu', 'conv_halo.cu', 'conv_heads.cu', 'elementwise.cu', 'decode.cu', 'stream.cu']
 
 # ---- enums (mirror include/ctb200.h) ----
 CT_OK, CT_ERR_INVALID, CT_ERR_CUDA, CT_ERR_UNSUPPORTED = 0, -1, -2, -3
@@ -24,6 +24,14 @@ CT_DECODE_MAX_HEADS = 12
 CT_REC_SCORE, CT_REC_CLS, CT_REC_XS, CT_REC_YS, CT_REC_BBOX, CT_REC_IND, CT_REC_HEADS = 0, 1, 2, 3, 4, 8, 9
 
 
+CT_MAX_FUSED_HEADS = 12
+
+
+class Head(C.Structure):
+  _fields_ = [('w', C.c_void_p), ('bias', C.c_void_p), ('out', C.c_void_p), ('C_out', C.c_int32),
+              ('n_tile', C.c_int32), ('head_act', C.c_int32), ('reserved', C.c_int32)]
+
+
 class ConvDesc(C.Structure):
   _fields_ = [
       ('engine', C.c_int32), ('dtype', C.c_int32), ('a_mode', C.c_int32),
@@ -35,7 +43,7 @@ class ConvDesc(C.Structure):
       ('sig_from', C.c_int32), ('depth_scale', C.c_float), ('ld_om', C.c_int32),
       ('n_tile', C.c_int32), ('epilogue_sum3', C.c_int32), ('pad_w1', C.c_int32),
       ('x', C.c_void_p), ('w', C.c_void_p), ('shift', C.c_void_p), ('residual', C.c_void_p),
-      ('om', C.c_void_p), ('out', C.c_void_p),
+      ('om', C.c_void_p), ('out', C.c_void_p), ('n_heads', C.c_int32), ('heads', C.POINTER(Head)),
   ]
 
 

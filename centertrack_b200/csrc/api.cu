@@ -159,17 +159,17 @@ extern "C" int ct_conv_config(const ct_conv_desc* d, struct ct_conv_config* out)
   const int r = check_conv_desc(d);
   if (r != CT_OK) return r;
   if (d->engine == CT_ENGINE_SIMT) return conv_config_simt(d, out);
-  if (d->engine == CT_ENGINE_TCGEN05_HALO) return conv_config_halo(d, out);
+  if (d->engine == CT_ENGINE_TCGEN05_HALO) return d->n_heads ? conv_config_heads(d, out) : conv_config_halo(d, out);
   return conv_config_tc(d, out);
 }
 
 extern "C" int ct_conv_forward(const ct_conv_desc* d, void* stream) {
-  CT_REQUIRE(d && d->x && d->w && d->out, "null pointer");
+  CT_REQUIRE(d && d->x && d->w && (d->out || d->n_heads), "null pointer");
   CT_REQUIRE(d->om || (d->a_mode != CT_A_DCN && d->a_mode != CT_A_DCN_WIN), "DCN needs om with ld_om >= 27");
   const int r = check_conv_desc(d);
   if (r != CT_OK) return r;
   cudaStream_t st = (cudaStream_t)stream;
   if (d->engine == CT_ENGINE_SIMT) return conv_forward_simt(d, st);
-  if (d->engine == CT_ENGINE_TCGEN05_HALO) return conv_forward_halo(d, st);
+  if (d->engine == CT_ENGINE_TCGEN05_HALO) return d->n_heads ? conv_forward_heads(d, st) : conv_forward_halo(d, st);
   return conv_forward_tc(d, st);
 }

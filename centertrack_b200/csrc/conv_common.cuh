@@ -111,9 +111,11 @@ typedef struct ct_conv_config ConvConfig;
 int conv_config_simt(const ct_conv_desc* d, ConvConfig* c);
 int conv_config_tc(const ct_conv_desc* d, ConvConfig* c);
 int conv_config_halo(const ct_conv_desc* d, ConvConfig* c);
+int conv_config_heads(const ct_conv_desc* d, ConvConfig* c);
 int conv_forward_simt(const ct_conv_desc* d, cudaStream_t st);
 int conv_forward_tc(const ct_conv_desc* d, cudaStream_t st);
 int conv_forward_halo(const ct_conv_desc* d, cudaStream_t st);
+int conv_forward_heads(const ct_conv_desc* d, cudaStream_t st);
 int halo_blocks(int C_in, int KH, int KW);
 int halo_set_trace(void* buf);
 int tc_set_trace(void* buf);

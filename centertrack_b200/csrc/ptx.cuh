@@ -17,6 +17,11 @@ __device__ __forceinline__ void mbar_init_fence() { asm volatile("fence.mbarrier
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
+// arrive only where `pred` holds, without a branch (a branch between asynchronous MMAs makes ptxas serialise them)
+__device__ __forceinline__ void mbar_arrive_if(uint32_t bar, bool pred) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}"
+               ::"r"(bar), "r"((uint32_t)pred) : "memory");
+}
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
@@ -52,6 +57,17 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int sit
   }
 }
 
+// The same wait with its loop inside one asm block and no watchdog: for waits between asynchronous MMAs, where any
+// branch the compiler sees makes ptxas serialise the MMAs.
+__device__ __forceinline__ void mbar_wait_inline(uint32_t bar, uint32_t parity) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "WAIT_%=:\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+      "@!p bra WAIT_%=;\n\t}"
+      ::"r"(bar), "r"(parity) : "memory");
+}
+
 // ---- async proxy: bulk and tensor (TMA) copies global -> shared, completing on an mbarrier ----
 // generic-proxy shared-memory writes -> visible to the async proxy (tensor cores, TMA)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
@@ -81,6 +97,9 @@ __device__ __forceinline__ uint4 lds16(uint32_t addr) {
 }
 __device__ __forceinline__ void sts16(uint32_t addr, uint4 v) {
   asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+__device__ __forceinline__ void sts32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
 }
 __device__ __forceinline__ void sts_f2(uint32_t addr, float x, float y) {
   asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(addr), "f"(x), "f"(y) : "memory");

@@ -11,9 +11,11 @@ on NHWC activations:
   * DeformConv (dla.py:506-518) = offset/mask 3x3 conv (fp32 NHWC map, sigmoid fused on the mask
     channels) + the DCN implicit GEMM with BN+ReLU fused;
   * IDAUp's `up(proj(x)) + skip` (dla.py:543-545) is one fused depthwise-transposed-conv + add;
-  * all heads' first 3x3 convs (base_model.py:27-38) run as one conv 64 -> 256*n_heads, then one
-    1x1 per head writing the reference-layout fp32 NCHW map (sigmoid / depth transform of
-    detector.py:300-308 optionally fused).
+  * the heads (base_model.py:27-38): when every head is 3x3 + ReLU + 1x1 (bf16 halo plan), ONE launch runs all
+    heads' 3x3 convs and their 1x1s per 128-pixel tile and writes only the reference-layout fp32 NCHW maps
+    (csrc/conv_heads.cu; the 256*n_heads-channel intermediate stays on chip); otherwise all heads' first 3x3 convs
+    run as one conv 64 -> 256*n_heads, then one 1x1 per head.  Either way the sigmoid / depth transform of
+    detector.py:300-308 is optionally fused.  CTB_HEAD_FUSE=0 builds the two-pass plan (same bits).
 
 precision='bf16'   : bf16 activations, wgmma engines (fast path)
 precision='bf16x3' : fp32 activations, wgmma gather engine with bf16 hi/lo split operands (three MMAs per product
@@ -43,6 +45,28 @@ class TV(object):
 
   def tensor(self):
     return self.buf[..., self.off:self.off + self.C]
+
+
+class DeferredTV(TV):
+  """A channel slice of an NHWC buffer that no launch of the plan writes: allocated and filled by holder['fill'] the
+  first time its contents are read.  The fused head launch keeps its 3x3 result on chip; its records in `specs`
+  describe it as the two unfused layers it matches bit for bit, and this is their intermediate."""
+
+  def __init__(self, holder, off, Cn):
+    self.holder, self.off, self.C = holder, off, Cn
+    self.B, self.H, self.W, self.ld = holder['shape']
+
+  @property
+  def buf(self):
+    h = self.holder
+    if h['t'] is None:
+      h['t'] = torch.empty(h['shape'], dtype=h['dtype'], device=h['device'])
+      h['fill'](h['t'])
+    return h['t']
+
+  @property
+  def ptr(self):
+    return TV.ptr.fget(self) if self.holder['t'] is not None else 0
 
 
 def _pow2_at_least(n):
@@ -113,10 +137,13 @@ class DLA34Engine(object):
     self.has_pre_img = has_pre_img and ('base.pre_img_layer.0.weight' in self.sd)
     self.has_pre_hm = has_pre_hm and ('base.pre_hm_layer.0.weight' in self.sd)
     self.ops = []          # (kind, payload, name)
-    self.specs = []        # one plain record per op (what it reads, computes and writes), parallel to self.ops
+    self.specs = []        # one plain record per op (what it reads, computes and writes); the fused head launch has
+                           # the records of the unfused layers it computes bit for bit (_fused_heads)
     self.keep = []         # device tensors referenced by raw pointers
     self.named = {}        # name -> TV (for per-stage parity tests)
     self.head_descs = {}   # head -> final ConvDesc (to toggle the fused activation)
+    self.head_table = None # fused heads: the launch's ct_head table, in the order of head_names
+    self.head_fuse = bool(int(__import__('os').environ.get('CTB_HEAD_FUSE', '1')))
     self.algo_flops = {}   # op name -> flops of the reference layer, where the launch shape carries structural zeros
     self.s2d_named = set() # named intermediates stored space-to-depth ([B, H/2, W/2, (sy, sx, 16)])
     self.n_sm = torch.cuda.get_device_properties(self.device).multi_processor_count if self.device.type == 'cuda' else 132
@@ -190,8 +217,9 @@ class DLA34Engine(object):
 
   def _conv(self, name, x, w, shift, out, k, stride=1, relu=True, residual=None, a_mode=L.CT_A_CONV,
             om=None, out_mode=L.CT_OUT_NHWC, head_act=L.CT_HEAD_NONE, sig_from=1 << 30, c_out=None, sum3=0,
-            w_pack=None, out_hw=None):
-    """Append one conv-like launch.  x: TV; out: TV (NHWC modes) or fp32 tensor (NCHW)."""
+            w_pack=None, out_hw=None, record_only=False):
+    """Append one conv-like launch.  x: TV; out: TV (NHWC modes) or fp32 tensor (NCHW).  record_only: build the
+    descriptor and its record in `specs` without a launch (the unfused layers of the fused head launch)."""
     C_in = x.C
     if w.shape[1] != C_in:      # input channels padded (never happens for DLA-34 tensors)
       raise ValueError('%s: C_in mismatch %d vs %d' % (name, w.shape[1], C_in))
@@ -258,9 +286,13 @@ class DLA34Engine(object):
     engine, n_tile = d.engine, d.n_tile
     assert out_mode != L.CT_OUT_NHWC_S2D or engine == L.CT_ENGINE_TCGEN05_HALO, name
     d.w = self._pack(w if w_pack is None else w_pack, n_tile, engine).data_ptr()
-    self._op('conv', d, name, x=x, w=w, shift=shift, residual=residual, om=om, out=out, k=(kh, kw), stride=stride,
-             pad=(pad, pad_w), out_hw=(OH, OW), a_mode=a_mode, out_mode=out_mode, relu=relu, sig_from=sig_from,
-             sum3=sum3, engine=engine, n_tile=n_tile)
+    spec = dict(x=x, w=w, shift=shift, residual=residual, om=om, out=out, k=(kh, kw), stride=stride,
+                pad=(pad, pad_w), out_hw=(OH, OW), a_mode=a_mode, out_mode=out_mode, relu=relu, sig_from=sig_from,
+                sum3=sum3, engine=engine, n_tile=n_tile)
+    if record_only:
+      self.specs.append(dict(spec, kind='conv', name=name, desc=d))
+    else:
+      self._op('conv', d, name, **spec)
     return d
 
   def _conv_bn(self, name, x, conv, bn, out, k, stride=1, relu=True, residual=None):
@@ -533,6 +565,12 @@ class DLA34Engine(object):
     mid_c = {h: sd[h + '.0.weight'].shape[0] for h in fused}
     ks = {sd[h + '.0.weight'].shape[2] for h in fused}
     assert len(ks) <= 1, 'heads with different first-conv kernel sizes are not supported'
+    if (self.head_fuse and self.use_halo and fused and all(n == 2 for _, n in first) and ks == {3} and feat.C == 64 and
+        len(set(mid_c.values())) == 1 and set(mid_c.values()) <= {64, 256} and
+        len(fused) <= L.CT_MAX_FUSED_HEADS and max(self.heads[h] for h in fused) <= 80):
+      self._fused_heads(feat, fused, mid_c[fused[0]], oh, ow)
+      self.set_fused_activations(False)
+      return
     if fused:
       kh = ks.pop()
       wcat = torch.cat([sd[h + '.0.weight'] for h in fused], 0)
@@ -562,6 +600,46 @@ class DLA34Engine(object):
       self.head_descs[h] = d
     self.set_fused_activations(False)
 
+  def _fused_heads(self, feat, heads, mc, oh, ow):
+    """Every head = 3x3 conv 64 -> mc + ReLU, 1x1 conv mc -> classes: one launch (csrc/conv_heads.cu, n_tile = the mid
+    channels per pass, one 1x1 n_tile for all heads).  Its records in `specs` are the unfused layers (heads.0 and one
+    1x1 per head), whose intermediate is computed on demand by heads.0's own launch."""
+    B, sd, f32 = self.B, self.sd, torch.float32
+    wcat = torch.cat([sd[h + '.0.weight'] for h in heads], 0)
+    bcat = torch.cat([sd[h + '.0.bias'] for h in heads], 0)
+    n2 = max((self.heads[h] + 15) // 16 * 16 for h in heads)
+    holder = dict(shape=(B, oh, ow, wcat.shape[0]), dtype=self.dtype, device=self.device, t=None)
+    mid = DeferredTV(holder, 0, wcat.shape[0])
+    d0 = self._conv('heads.0', feat, wcat, bcat, mid, 3, 1, relu=True, record_only=True)
+
+    def fill(t):
+      d0.out = t.data_ptr()
+      L.check(self.lib.ct_conv_forward(C.byref(d0), L.stream_ptr()), 'heads.0')
+      torch.cuda.synchronize(self.device)
+    holder['fill'] = fill
+    table = (L.Head * len(heads))()
+    for i, h in enumerate(heads):
+      o = torch.empty((B, self.heads[h], oh, ow), dtype=f32, device=self.device)
+      self.outputs[h] = o
+      w2, b2 = sd[h + '.2.weight'], sd[h + '.2.bias']
+      self.head_descs[h] = self._conv(h, DeferredTV(holder, i * mc, mc), w2, b2, o, 1, 1, relu=False,
+                                      out_mode=L.CT_OUT_NCHW_F32, record_only=True)
+      t = table[i]
+      t.w = self._pack(w2, n2, L.CT_ENGINE_TCGEN05_HALO).data_ptr()
+      t.bias = self._dev(b2.to(f32).contiguous()).data_ptr()
+      t.out, t.C_out, t.n_tile = o.data_ptr(), self.heads[h], n2
+    d = L.ConvDesc()
+    C.pointer(d)[0] = d0
+    d.out, d.ld_out, d.out_mode = None, 0, L.CT_OUT_NCHW_F32
+    d.n_tile = 128 if mc == 256 else 64
+    d.w = self._pack(wcat, d.n_tile, L.CT_ENGINE_TCGEN05_HALO).data_ptr()
+    d.n_heads, d.heads = len(heads), C.cast(table, C.POINTER(L.Head))
+    self.head_table, self.head_names = table, list(heads)
+    if L.conv_config(d) is None:
+      raise ValueError('heads: the fused head launch does not fit in shared memory')
+    self.ops.append(('conv', d, 'heads'))
+    self.algo_flops['heads'] = 2.0 * B * oh * ow * (9 * feat.C * wcat.shape[0] + mc * sum(self.heads[h] for h in heads))
+
   # ------------------------------------------------------------------ run
   def set_fused_activations(self, on):
     """on=True: hm/hm_hp sigmoid and the dep transform (detector.py:300-308) run in the head epilogue."""
@@ -572,6 +650,9 @@ class DLA34Engine(object):
       elif on and h == 'dep':
         act = L.CT_HEAD_DEPTH
       d.head_act = act
+    if self.head_table is not None:
+      for i, h in enumerate(self.head_names):
+        self.head_table[i].head_act = self.head_descs[h].head_act
     self.fused_act = on
     self.graph = None
 

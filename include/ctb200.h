@@ -84,6 +84,19 @@ typedef enum {
                                   tensor-core path that meets the reference's fp32 results to 1e-3 end to end */
 } ct_engine;
 
+/* One output head of a fused head launch (ct_conv_desc.n_heads > 0): the head's 1x1 convolution over its mid_c
+ * channels of the shared 3x3 layer, + bias, head_act, written as an fp32 NCHW map. */
+#define CT_MAX_FUSED_HEADS 12
+typedef struct {
+  const void* w;         /* 1x1 weights [C_out, mid_c] packed by ct_pack_weights(CT_ENGINE_TCGEN05_HALO, .., n_tile) */
+  const float* bias;     /* [C_out] */
+  float* out;            /* fp32 [B, C_out, OH, OW] */
+  int32_t C_out;
+  int32_t n_tile;        /* multiple of 16, C_out <= n_tile <= 80 */
+  int32_t head_act;      /* ct_head_act */
+  int32_t reserved;
+} ct_head;
+
 /* One convolution-like layer.  Activations are NHWC with an explicit pixel stride (ld, in
  * elements) so that a producer can write straight into a channel slice of a concat buffer
  * (DLA Root nodes, dla.py:167) and a consumer can read a slice back. */
@@ -115,6 +128,12 @@ typedef struct {
   const void* residual;  /* [P_out, ld_res] same dtype as activations, or NULL */
   const float* om;       /* CT_A_DCN: offsets (ch 0..17, 2k=dy 2k+1=dx) + sigmoid'd mask (18..26) */
   void* out;
+  /* Fused output heads (HALO engine; 0 = an ordinary layer): the layer is the heads' shared 3x3 convolution
+   * C_in = 64 -> C_out = n_heads * mid_c (mid_c = 64 or 256, n_tile = 64 or 128 = the mid channels per pass, relu,
+   * shift = its bias), and each head's 1x1 runs on its mid_c channels in the same launch: the 3x3 result never leaves
+   * the chip.  out_mode = CT_OUT_NCHW_F32, `out` is unused, the head outputs are heads[i].out. */
+  int32_t n_heads;
+  const ct_head* heads;  /* [n_heads] */
 } ct_conv_desc;
 
 /* Size in bytes of the packed weight blob ct_pack_weights produces for this engine/shape. */
@@ -144,7 +163,8 @@ struct ct_conv_config {
 /* The configuration step of ct_conv_forward alone: validates the descriptor's shape and fills `out`, with no CUDA
  * call.  Returns the status and ct_last_error() message ct_conv_forward would return for this shape
  * (CT_ERR_UNSUPPORTED: the tile does not fit in shared memory).  Of the pointer fields of `d` only whether residual
- * and shift are NULL is read (a layer without residual / shift); the others may be NULL. */
+ * and shift are NULL is read (a layer without residual / shift), and the head table of a fused head launch (its
+ * C_out / n_tile); the others may be NULL.  Fused heads: `stages` counts the weight-slice ring. */
 int ct_conv_config(const ct_conv_desc* d, struct ct_conv_config* out);
 
 /* Three 7x7 stems on reference-layout inputs (fp32 NCHW):

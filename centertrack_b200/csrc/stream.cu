@@ -10,6 +10,8 @@
 //   ct_flip_merge    Detector._flip_output (detector.py:311-332; model/utils.py:28-50) for --flip_test
 //   ct_warp_affine_normalize   Detector.pre_process's cv2.warpAffine(INTER_LINEAR) + (x/255 - mean)/std + HWC->CHW
 //                    (detector.py:207-226), cv2's fixed-point bilinear restated
+//   ct_pack_stem_frames        the same warp + normalise of B ragged uint8 frames (and of their previous frames),
+//                    written straight as the tensor-core stem's packed bf16 input
 // All HBM-bound byte/index work: one pass over the data, coalesced, no tensor cores.
 #include <math_constants.h>
 
@@ -552,6 +554,41 @@ __device__ __forceinline__ int sat_int(double v) {        // cv::saturate_cast<i
   return __double2int_rn(v);
 }
 
+// The warped uint8 BGR value of output pixel (x, y): src uint8 [sh, sw, 3] with row pitch sstep bytes, M the inverted
+// (dst -> src) map.  The one copy of the per-pixel warp arithmetic: ct_warp_affine_normalize and ct_pack_stem_frames
+// both call it, so that the fused stem input is byte-identical to the fp32 image packed afterwards.
+__device__ __forceinline__ void warp_bilinear_u8(const unsigned char* __restrict__ img, int sh, int sw, int sstep,
+                                                 const double* M, int x, int y, int p8[3]) {
+  const int AB_BITS = 10, AB_SCALE = 1 << AB_BITS, INTER_BITS = 5, INTER_TAB = 1 << INTER_BITS;
+  const int round_delta = AB_SCALE / INTER_TAB / 2;
+  const int adelta = sat_int(M[0] * x * AB_SCALE), bdelta = sat_int(M[3] * x * AB_SCALE);
+  const int X0 = sat_int((M[1] * y + M[2]) * AB_SCALE) + round_delta;
+  const int Y0 = sat_int((M[4] * y + M[5]) * AB_SCALE) + round_delta;
+  const int X = (X0 + adelta) >> (AB_BITS - INTER_BITS), Y = (Y0 + bdelta) >> (AB_BITS - INTER_BITS);
+  const int sx = X >> INTER_BITS, sy = Y >> INTER_BITS;          // arithmetic shifts: floor
+  // BilinearTab_i: (1-fy|fy) x (1-fx|fx) in 1/32 steps, scaled by 2^15: exact integers (the table's one saturated
+  // entry, fx = fy = 0, yields the same pixel as the exact weight 32768)
+  const int fx = X & (INTER_TAB - 1), fy = Y & (INTER_TAB - 1);
+  const int w[4] = {(32 - fy) * (32 - fx) * 32, (32 - fy) * fx * 32, fy * (32 - fx) * 32, fy * fx * 32};
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    int acc = 0;
+#pragma unroll
+    for (int t = 0; t < 4; ++t) {
+      const int yy = sy + (t >> 1), xx = sx + (t & 1);
+      const int v = ((unsigned)yy < (unsigned)sh && (unsigned)xx < (unsigned)sw) ? img[(size_t)yy * sstep + xx * 3 + c] : 0;
+      acc += v * w[t];
+    }
+    const int pix = (acc + (1 << 14)) >> 15;
+    p8[c] = pix < 0 ? 0 : (pix > 255 ? 255 : pix);
+  }
+}
+
+// ((inp / 255. - mean) / std).astype(float32): float64 arithmetic, one final rounding
+__device__ __forceinline__ float normalize_u8(int v, float mean, float stdv) {
+  return (float)(((double)v / 255.0 - (double)mean) / (double)stdv);
+}
+
 __global__ void warp_affine_norm_kernel(const unsigned char* __restrict__ src, int sh, int sw, int sstep,
                                         float* __restrict__ dst, int B, int oh, int ow,
                                         const double* __restrict__ minv /*[B][6] dst->src*/, float3 mean, float3 stdv) {
@@ -560,39 +597,69 @@ __global__ void warp_affine_norm_kernel(const unsigned char* __restrict__ src, i
     const int b = (int)(i / ((size_t)oh * ow));
     const size_t r = i - (size_t)b * oh * ow;
     const int y = (int)(r / ow), x = (int)(r - (size_t)y * ow);
-    const double* M = minv + b * 6;
-    const int AB_BITS = 10, AB_SCALE = 1 << AB_BITS, INTER_BITS = 5, INTER_TAB = 1 << INTER_BITS;
-    const int round_delta = AB_SCALE / INTER_TAB / 2;
-    const int adelta = sat_int(M[0] * x * AB_SCALE), bdelta = sat_int(M[3] * x * AB_SCALE);
-    const int X0 = sat_int((M[1] * y + M[2]) * AB_SCALE) + round_delta;
-    const int Y0 = sat_int((M[4] * y + M[5]) * AB_SCALE) + round_delta;
-    const int X = (X0 + adelta) >> (AB_BITS - INTER_BITS), Y = (Y0 + bdelta) >> (AB_BITS - INTER_BITS);
-    const int sx = X >> INTER_BITS, sy = Y >> INTER_BITS;          // arithmetic shifts: floor
-    // BilinearTab_i: (1-fy|fy) x (1-fx|fx) in 1/32 steps, scaled by 2^15: exact integers (the table's one saturated
-    // entry, fx = fy = 0, yields the same pixel as the exact weight 32768)
-    const int fx = X & (INTER_TAB - 1), fy = Y & (INTER_TAB - 1);
-    const int w[4] = {(32 - fy) * (32 - fx) * 32, (32 - fy) * fx * 32, fy * (32 - fx) * 32, fy * fx * 32};
-    const unsigned char* img = src + (size_t)b * sh * sstep;
-    float out[3];
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      int acc = 0;
-#pragma unroll
-      for (int t = 0; t < 4; ++t) {
-        const int yy = sy + (t >> 1), xx = sx + (t & 1);
-        const int v = ((unsigned)yy < (unsigned)sh && (unsigned)xx < (unsigned)sw) ? img[(size_t)yy * sstep + xx * 3 + c] : 0;
-        acc += v * w[t];
-      }
-      const int pix = (acc + (1 << 14)) >> 15;
-      const int p8 = pix < 0 ? 0 : (pix > 255 ? 255 : pix);
-      // ((inp / 255. - mean) / std).astype(float32): float64 arithmetic, one final rounding
-      out[c] = (float)p8;
-    }
+    int p8[3];
+    warp_bilinear_u8(src + (size_t)b * sh * sstep, sh, sw, sstep, minv + b * 6, x, y, p8);
     const size_t plane = (size_t)oh * ow;
     float* o = dst + (size_t)b * 3 * plane + (size_t)y * ow + x;
-    o[0] = (float)(((double)out[0] / 255.0 - (double)mean.x) / (double)stdv.x);
-    o[plane] = (float)(((double)out[1] / 255.0 - (double)mean.y) / (double)stdv.y);
-    o[2 * plane] = (float)(((double)out[2] / 255.0 - (double)mean.z) / (double)stdv.z);
+    o[0] = normalize_u8(p8[0], mean.x, stdv.x);
+    o[plane] = normalize_u8(p8[1], mean.y, stdv.y);
+    o[2 * plane] = normalize_u8(p8[2], mean.z, stdv.z);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// ct_pack_stem_frames: the tensor-core stem's input [B,H,W,8] bf16 = (norm(warp(cur_b)) x3, norm(warp(prev_b)) x3,
+// pre_hm, 0) straight from each stream's uint8 frame.  blockIdx.y = stream (its descriptor read once, from the kernel
+// parameters), one 16-byte output pixel per thread and iteration.  The normalisation depends on the 8-bit value only:
+// a 3 x 256 table built per CTA with normalize_u8 gives the same floats without a per-pixel fp64 divide.
+// ------------------------------------------------------------------------------------------------------------------
+struct FramesArgs {
+  ct_frame f[CT_FRAMES_PER_LAUNCH];
+};
+
+constexpr int PACK_THREADS = 256;
+constexpr int PACK_PIX_PER_THREAD = 4;      // pixels per thread: amortises the table build over 1024 pixels per CTA
+
+__global__ void __launch_bounds__(PACK_THREADS)
+pack_stem_frames_kernel(const unsigned char* __restrict__ cur, const unsigned char* __restrict__ prev,
+                        const __grid_constant__ FramesArgs fa, int b0, float3 mean, float3 stdv,
+                        const float* __restrict__ hm, uint4* __restrict__ out, int H, int W) {
+  __shared__ float tab[3][256];
+  for (int i = threadIdx.x; i < 3 * 256; i += PACK_THREADS) {
+    const int c = i >> 8, v = i & 255;
+    tab[c][v] = normalize_u8(v, c == 0 ? mean.x : (c == 1 ? mean.y : mean.z), c == 0 ? stdv.x : (c == 1 ? stdv.y : stdv.z));
+  }
+  __syncthreads();
+  const ct_frame& f = fa.f[blockIdx.y];
+  const int b = b0 + blockIdx.y;
+  const size_t plane = (size_t)H * W;
+  const unsigned char* src = cur + f.offset;
+  const unsigned char* psrc = prev ? prev + f.offset : nullptr;
+  const size_t base = (size_t)blockIdx.x * PACK_THREADS * PACK_PIX_PER_THREAD + threadIdx.x;
+#pragma unroll
+  for (int k = 0; k < PACK_PIX_PER_THREAD; ++k) {
+    const size_t r = base + (size_t)k * PACK_THREADS;
+    if (r >= plane) break;
+    const int y = (int)(r / W), x = (int)(r - (size_t)y * W);
+    float v[8];
+    int p8[3];
+    warp_bilinear_u8(src, f.h, f.w, f.step, f.minv, x, y, p8);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) v[c] = tab[c][p8[c]];
+    if (psrc) {
+      warp_bilinear_u8(psrc, f.h, f.w, f.step, f.minv, x, y, p8);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) v[3 + c] = tab[c][p8[c]];
+    } else {
+      v[3] = v[4] = v[5] = 0.f;
+    }
+    v[6] = hm ? __ldg(hm + (size_t)b * plane + r) : 0.f;
+    v[7] = 0.f;
+    uint4 o;
+    __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&o);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) h[q] = __floats2bfloat162_rn(v[2 * q], v[2 * q + 1]);
+    out[(size_t)b * plane + r] = o;
   }
 }
 
@@ -700,4 +767,30 @@ extern "C" int ct_warp_affine_normalize(const uint8_t* src, int32_t B, int32_t s
       src, src_h, src_w, src_step, dst, B, out_h, out_w, minv, make_float3(mean[0], mean[1], mean[2]),
       make_float3(std[0], std[1], std[2]));
   return after_launch();
+}
+
+extern "C" int ct_pack_stem_frames(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames, int32_t B,
+                                   const float* mean, const float* std, const float* pre_hm, void* out, int32_t H,
+                                   int32_t W, void* stream) {
+  CT_REQUIRE(cur && frames && mean && std && out, "null pointer");
+  CT_REQUIRE(B > 0 && H > 0 && W > 0, "bad shape");
+  for (int32_t b = 0; b < B; ++b)
+    CT_REQUIRE(frames[b].offset >= 0 && frames[b].h > 0 && frames[b].w > 0 && frames[b].step >= 3 * frames[b].w,
+               "bad frame descriptor (offset >= 0, h > 0, w > 0, step >= 3 w)");
+  const size_t plane = (size_t)H * W;
+  const size_t per_cta = (size_t)PACK_THREADS * PACK_PIX_PER_THREAD;
+  CT_REQUIRE((plane + per_cta - 1) / per_cta <= 0x7fffffffu, "output too large");
+  const float3 m = make_float3(mean[0], mean[1], mean[2]), s = make_float3(std[0], std[1], std[2]);
+  // descriptors travel in the kernel parameters (captured by value in a CUDA graph): CT_FRAMES_PER_LAUNCH per launch
+  for (int32_t b0 = 0; b0 < B; b0 += CT_FRAMES_PER_LAUNCH) {
+    const int n = B - b0 < CT_FRAMES_PER_LAUNCH ? B - b0 : CT_FRAMES_PER_LAUNCH;
+    FramesArgs fa = {};
+    memcpy(fa.f, frames + b0, sizeof(ct_frame) * n);
+    dim3 grid((unsigned)((plane + per_cta - 1) / per_cta), (unsigned)n);
+    pack_stem_frames_kernel<<<grid, PACK_THREADS, 0, (cudaStream_t)stream>>>(cur, prev, fa, b0, m, s, pre_hm,
+                                                                             (uint4*)out, H, W);
+    const int rc = after_launch();
+    if (rc != CT_OK) return rc;
+  }
+  return CT_OK;
 }

@@ -51,6 +51,56 @@ def _round_up(v, m):
   return (v + m - 1) // m * m
 
 
+def input_geometry(opt, height, width, scale):
+  """Network input size and the (centre, scale) of the source rectangle mapped onto it, for the three resolution
+  policies of detector.py:175-204: --fix_short (short side fixed, long side rounded up to 64), fixed resolution
+  (default), or keep_res (image size padded up to (size | pad) + 1)."""
+  sh, sw = int(height * scale), int(width * scale)
+  if opt.fix_short > 0:
+    long_side = lambda a, b: _round_up(int(a / b * opt.fix_short), 64)
+    inp_h, inp_w = (opt.fix_short, long_side(width, height)) if height < width else \
+                   (long_side(height, width), opt.fix_short)
+    centre = np.array([width / 2, height / 2], dtype=np.float32)
+    extent = np.array([width, height], dtype=np.float32)
+  elif opt.fix_res:
+    inp_h, inp_w = opt.input_h, opt.input_w
+    centre = np.array([sw / 2., sh / 2.], dtype=np.float32)
+    extent = max(height, width) * 1.0
+  else:
+    inp_h, inp_w = (sh | opt.pad) + 1, (sw | opt.pad) + 1
+    centre = np.array([sw // 2, sh // 2], dtype=np.float32)
+    extent = np.array([inp_w, inp_h], dtype=np.float32)
+  return (sh, sw), centre, extent, inp_w, inp_h
+
+
+def frame_geometry(opt, height, width):
+  """Geometry of one height x width source frame at scale 1 (hazard H5: the reference never forwards `scale`), as
+  Detector.pre_process_device and StreamRunner's frames mode use it: (meta, minv) with meta = pre_process's meta
+  without `calib`, and minv fp64 [6] = meta['trans_input'] inverted exactly as cv::warpAffine inverts it (the dst -> src
+  map ct_warp_affine_normalize / ct_pack_stem_frames sample with)."""
+  _, c, s, inp_w, inp_h = input_geometry(opt, height, width, 1)
+  out_w, out_h = inp_w // opt.down_ratio, inp_h // opt.down_ratio
+  to_input = get_affine_transform(c, s, 0, [inp_w, inp_h])
+  to_output = get_affine_transform(c, s, 0, [out_w, out_h])
+  M = np.asarray(to_input, np.float64).reshape(6).copy()
+  D = M[0] * M[4] - M[1] * M[3]
+  D = 1. / D if D != 0 else 0.
+  A11, A22 = M[4] * D, M[0] * D
+  M[0] = A11; M[1] *= -D; M[3] *= -D; M[4] = A22
+  b1, b2 = -M[0] * M[2] - M[1] * M[5], -M[3] * M[2] - M[4] * M[5]
+  M[2], M[5] = b1, b2
+  meta = dict(c=c, s=s, height=height, width=width, out_height=out_h, out_width=out_w, inp_height=inp_h,
+              inp_width=inp_w, trans_input=to_input, trans_output=to_output)
+  return meta, M
+
+
+def default_calib(focal_length, width, height):
+  """Detector._get_default_calib: the camera matrix of a width x height image with its principal point at the centre."""
+  return np.array([[focal_length, 0, width / 2, 0],
+                   [0, focal_length, height / 2, 0],
+                   [0, 0, 1, 0]])
+
+
 class Detector(object):
 
   def __init__(self, opt):
@@ -168,26 +218,7 @@ class Detector(object):
 
   # ------------------------------------------------------------------------------------ host pre
   def _input_geometry(self, height, width, scale):
-    """Network input size and the (centre, scale) of the source rectangle mapped onto it, for the three resolution
-    policies of detector.py:175-204: --fix_short (short side fixed, long side rounded up to 64), fixed resolution
-    (default), or keep_res (image size padded up to (size | pad) + 1)."""
-    opt = self.opt
-    sh, sw = int(height * scale), int(width * scale)
-    if opt.fix_short > 0:
-      long_side = lambda a, b: _round_up(int(a / b * opt.fix_short), 64)
-      inp_h, inp_w = (opt.fix_short, long_side(width, height)) if height < width else \
-                     (long_side(height, width), opt.fix_short)
-      centre = np.array([width / 2, height / 2], dtype=np.float32)
-      extent = np.array([width, height], dtype=np.float32)
-    elif opt.fix_res:
-      inp_h, inp_w = opt.input_h, opt.input_w
-      centre = np.array([sw / 2., sh / 2.], dtype=np.float32)
-      extent = max(height, width) * 1.0
-    else:
-      inp_h, inp_w = (sh | opt.pad) + 1, (sw | opt.pad) + 1
-      centre = np.array([sw // 2, sh // 2], dtype=np.float32)
-      extent = np.array([inp_w, inp_h], dtype=np.float32)
-    return (sh, sw), centre, extent, inp_w, inp_h
+    return input_geometry(self.opt, height, width, scale)
 
   def _transform_scale(self, image, scale=1):
     """Reference-named helper (detector.py:175): resized image + geometry tuple."""
@@ -223,20 +254,8 @@ class Detector(object):
     geometry stays on the host; `pre_process` itself must remain CPU-only and fork-safe for test.py's DataLoader).
     Returns CUDA `images`."""
     height, width = image.shape[:2]
-    (sh, sw), c, s, inp_w, inp_h = self._input_geometry(height, width, 1)     # hazard H5: scale is not forwarded
-    if (sh, sw) != (height, width):
-      import cv2
-      image = cv2.resize(image, (sw, sh))
-    out_w, out_h = inp_w // self.opt.down_ratio, inp_h // self.opt.down_ratio
-    to_input = get_affine_transform(c, s, 0, [inp_w, inp_h])
-    to_output = get_affine_transform(c, s, 0, [out_w, out_h])
-    M = np.asarray(to_input, np.float64).reshape(6).copy()                   # cv::warpAffine inverts the map like this
-    D = M[0] * M[4] - M[1] * M[3]
-    D = 1. / D if D != 0 else 0.
-    A11, A22 = M[4] * D, M[0] * D
-    M[0] = A11; M[1] *= -D; M[3] *= -D; M[4] = A22
-    b1, b2 = -M[0] * M[2] - M[1] * M[5], -M[3] * M[2] - M[4] * M[5]
-    M[2], M[5] = b1, b2
+    geom, M = frame_geometry(self.opt, height, width)
+    inp_h, inp_w = geom['inp_height'], geom['inp_width']
     dev = self.opt.device
     src = torch.from_numpy(np.ascontiguousarray(image)).to(dev, non_blocking=True)
     minv = torch.from_numpy(M.reshape(1, 6)).to(dev)
@@ -249,8 +268,7 @@ class Detector(object):
     images = torch.cat((out, out.flip(3)), 0) if self.opt.flip_test else out
     calib = np.array(input_meta['calib'], dtype=np.float32) if 'calib' in input_meta \
         else self._get_default_calib(width, height)
-    meta = dict(calib=calib, c=c, s=s, height=height, width=width, out_height=out_h, out_width=out_w,
-                inp_height=inp_h, inp_width=inp_w, trans_input=to_input, trans_output=to_output)
+    meta = dict(calib=calib, **geom)
     meta.update({k: input_meta[k] for k in ('pre_dets', 'cur_dets') if k in input_meta})
     return images, meta
 
@@ -288,9 +306,7 @@ class Detector(object):
     return canvas, pre_inds
 
   def _get_default_calib(self, width, height):
-    return np.array([[self.rest_focal_length, 0, width / 2, 0],
-                     [0, self.rest_focal_length, height / 2, 0],
-                     [0, 0, 1, 0]])
+    return default_calib(self.rest_focal_length, width, height)
 
   def _sigmoid_output(self, output):
     """detector.py:300-308 (kept for callers that run the nn.Module surface themselves; `process`

@@ -411,6 +411,7 @@ class DLA34Engine(object):
       # three stems) whose epilogue applies ReLU per stem and sums them (dla.py:307-311)
       x8 = TV(self._buf(H, W, 8), 0, 8)
       self._op('pack', x8, 'stem.pack', out=x8)
+      self.stem_input = x8.buf                            # what forward_packed reads (ct_pack_stem_frames writes it)
       w48 = torch.zeros((48, 8, 7, 7), dtype=torch.float64)
       for si, (c0, cn) in enumerate(((0, 3), (3, 3), (6, 1))):
         w48[16 * si:16 * si + 16, c0:c0 + cn] = wst[:, c0:c0 + cn, :].reshape(7, 7, cn, 16).permute(3, 2, 0, 1)
@@ -656,13 +657,15 @@ class DLA34Engine(object):
     self.fused_act = on
     self.graph = None
 
-  def _run_one(self, kind, pl, name, img_ptr, pre_ptr, hm_ptr, st):
+  def _run_one(self, kind, pl, name, img_ptr, pre_ptr, hm_ptr, st, mask=None):
     lib = self.lib
+    if mask is None:               # which of (img, pre_img, pre_hm) exist this call (dla.py:308-311)
+      mask = 1 | (2 if pre_ptr.value else 0) | (4 if hm_ptr.value else 0)
     if kind == 'conv':
-      if pl.epilogue_sum3:          # stem: which of (img, pre_img, pre_hm) exist this call (dla.py:308-311)
-        pl.epilogue_sum3 = 1 | (2 if pre_ptr.value else 0) | (4 if hm_ptr.value else 0)
+      if pl.epilogue_sum3:          # stem: the ReLU'd groups it sums
+        pl.epilogue_sum3 = mask
       elif name == 'stem48':
-        pl.shift = self.stem48_shift[1 | (2 if pre_ptr.value else 0) | (4 if hm_ptr.value else 0)].data_ptr()
+        pl.shift = self.stem48_shift[mask].data_ptr()
       rc = lib.ct_conv_forward(C.byref(pl), st)
     elif kind == 'stem':
       rc = lib.ct_stem_forward(img_ptr, pre_ptr, hm_ptr, L.ptr(self.stem_w), L.ptr(self.stem_shift),
@@ -690,10 +693,13 @@ class DLA34Engine(object):
       except Exception as e:
         raise RuntimeError('kernel fault in op %s (%s): %s' % (kind, name, e))
 
-  def _run_ops(self, img_ptr, pre_ptr, hm_ptr):
+  def _run_ops(self, img_ptr, pre_ptr, hm_ptr, mask=None, packed=False):
+    """mask: which stem inputs (bit 0 img, 1 pre_img, 2 pre_hm) are present, by default those whose pointer is set.
+    packed: the stem input is already in stem_input; the pack op is skipped."""
     st = L.stream_ptr()
     for kind, pl, name in self.ops:
-      self._run_one(kind, pl, name, img_ptr, pre_ptr, hm_ptr, st)
+      if not (packed and kind == 'pack'):
+        self._run_one(kind, pl, name, img_ptr, pre_ptr, hm_ptr, st, mask)
 
   @property
   def n_launches(self):
@@ -709,6 +715,17 @@ class DLA34Engine(object):
     pre = pre_images if self.has_pre_img else None
     hm = pre_hms if self.has_pre_hm else None
     self._run_ops(L.ptr(images), L.ptr(pre), L.ptr(hm))
+    return self.outputs
+
+  def forward_packed(self, has_pre, has_hm):
+    """The plan without its pack op, on a stem input the caller wrote into `stem_input` (bf16 NHWC [B,H,W,8],
+    ct_pack_stem_input's layout, e.g. by ct_pack_stem_frames): has_pre / has_hm say whether its pre_img / pre_hm
+    channels are present, as forward's pre_images / pre_hms being given does.  bf16 tensor-core plan only."""
+    if not self.use_halo:
+      raise ValueError('forward_packed: only the bf16 tensor-core plan reads a packed stem input')
+    mask = 1 | (2 if has_pre and self.has_pre_img else 0) | (4 if has_hm and self.has_pre_hm else 0)
+    none = C.c_void_p(0)
+    self._run_ops(none, none, none, mask, packed=True)
     return self.outputs
 
   # CUDA-graph replay: inputs are first copied into the engine's static buffers

@@ -24,12 +24,24 @@ Two ways to feed the prior heat-map (`--pre_hm`):
 
 The end-to-end form (`step_host`) takes HOST frames: pinned staging, H2D on a copy stream overlapped
 with the previous step's compute, graph replay, D2H of the records (and tracks).
+
+Frames mode (`frame_sizes`, `step_frames`) takes the raw uint8 BGR camera frames instead, one source size per stream:
+the three slots hold the B frames ragged (16-byte aligned offsets) in pinned and device memory, and the step warps and
+normalises them on the device exactly as Detector.pre_process_device does (cv2's fixed-point bilinear).  On the bf16
+engine ct_pack_stem_frames writes the stem's packed bf16 input straight from slot t (images) and slot t-1 (pre_images,
+warped again: no fp32 copy is kept); the fp32 and bf16x3 engines warp each stream into the fp32 image slot with
+ct_warp_affine_normalize and run their plan unchanged.  The tracker gets each stream's (c, s) and default calib, so
+tracks, public detections and 3D boxes are in that camera's pixels.
 """
+import ctypes as C
+
 import numpy as np
 import torch
 
 from . import _lib as L
+from .dataset_info import get_dataset
 from .decode import generic_decode
+from .detector import default_calib, frame_geometry
 from .device_tracker import DeviceTracker
 
 
@@ -39,14 +51,20 @@ NS = 3          # input slots
 class StreamRunner(object):
 
   def __init__(self, model, B, H, W, K=100, precision='bf16', device='cuda', use_graph=True, opt=None,
-               device_tracking=False, max_public_dets=512, calibs=None):
+               device_tracking=False, max_public_dets=512, calibs=None, frame_sizes=None):
     """max_public_dets: with device_tracking and --public_det, the most public detections a stream may bring per
     frame (more raise ValueError; none is ever dropped).  calibs: with device_tracking on a 3D head set, one [3,4]
-    camera matrix per stream (DeviceTracker's default otherwise)."""
+    camera matrix per stream (DeviceTracker's default otherwise; in frames mode Detector._get_default_calib of the
+    stream's source size).  frame_sizes: B (height, width) source sizes, fixed for the runner's lifetime, to feed raw
+    uint8 frames with step_frames; each must map to the network input (H, W) under opt's resolution policy
+    (ValueError otherwise)."""
     self.B, self.H, self.W, self.K = B, H, W, K
     self.device = torch.device(device)
     self.model = model
     self.opt = opt if opt is not None else getattr(model, 'opt', None)
+    self.frames_mode = frame_sizes is not None
+    if self.frames_mode:
+      calibs = self._frame_geometry(frame_sizes, calibs)
     self.eng = model.engine_for(B, H, W, self.device, precision)
     self.eng.set_fused_activations(True)
     f32 = torch.float32
@@ -54,6 +72,10 @@ class StreamRunner(object):
     self.hm = [torch.zeros((B, 1, H, W), dtype=f32, device=self.device) for _ in range(NS)]
     self.h_img = [torch.zeros((B, 3, H, W), dtype=f32).pin_memory() for _ in range(NS)]
     self.h_hm = [torch.zeros((B, 1, H, W), dtype=f32).pin_memory() for _ in range(NS)]
+    if self.frames_mode:      # frame slots: B uint8 frames at 16-byte aligned offsets, pinned staging + device
+      self.u8 = [torch.zeros(self.slot_bytes, dtype=torch.uint8, device=self.device) for _ in range(NS)]
+      self.h_u8 = [torch.zeros(self.slot_bytes, dtype=torch.uint8).pin_memory() for _ in range(NS)]
+      self.minv = torch.from_numpy(np.stack([f.minv[:] for f in self.frames])).to(self.device)
     self.rec = None
     self.layout = None
     self.ws = None                                           # private decode workspace (captured by the graphs)
@@ -69,8 +91,11 @@ class StreamRunner(object):
     self._eager(0, first=True)                               # sizes the record buffer
     if device_tracking:
       assert self.opt is not None, 'device tracking needs opt (thresholds, max_age)'
+      geo = {}
+      if self.frames_mode:
+        geo = dict(centers=[m['c'] for m in self._meta], scales=[m['s'] for m in self._meta])
       self.tracker = DeviceTracker(self.opt, B, K, self.rec.shape[2], self.layout, H, W, self.device,
-                                   max_public_dets=max_public_dets, calibs=calibs)
+                                   max_public_dets=max_public_dets, calibs=calibs, **geo)
     self.public = self.tracker is not None and self.tracker.public_det
     if self.public:                                          # per slot: device (public_ct, public_n) + pinned staging
       self.pub = [self.tracker.public_buffers() for _ in range(NS)]
@@ -82,15 +107,73 @@ class StreamRunner(object):
       self.h_cnt = [torch.zeros_like(self.tracker.counts, device='cpu').pin_memory() for _ in range(2)]
       if self.tracker.payload is not None:
         self.h_pay = [torch.zeros_like(self.tracker.payload, device='cpu').pin_memory() for _ in range(2)]
-    # launches of one step: the network plan + decode (+ memset-free: render + track step)
+    # launches of one step: the network plan + decode (+ memset-free: render + track step); frames mode: the pack op
+    # becomes ct_pack_stem_frames (one launch per CT_FRAMES_PER_LAUNCH streams), or B warps come before the plan
     self.launches_per_step = self.eng.n_launches + 1 + (2 if device_tracking else 0)
+    if self.frames_mode:
+      self.launches_per_step += (-(-B // L.CT_FRAMES_PER_LAUNCH) - 1) if self.eng.use_halo else B
+
+  def _frame_geometry(self, frame_sizes, calibs):
+    """Per-stream geometry of frames mode (Detector.pre_process_device's, through detector.frame_geometry): the
+    ct_frame descriptors, the metas, the slot size.  -> the tracker's calibs."""
+    opt, B = self.opt, self.B
+    if opt is None:
+      raise ValueError('frames mode needs opt (the resolution policy and the dataset mean / std)')
+    if len(frame_sizes) != B:
+      raise ValueError('frame_sizes: expected %d (height, width) pairs, got %d' % (B, len(frame_sizes)))
+    if calibs is not None:
+      calibs = np.asarray(calibs, np.float32)
+      if calibs.shape != (B, 3, 4):
+        raise ValueError('calibs: expected %d camera matrices [3, 4], got shape %s' % (B, calibs.shape))
+    ds = get_dataset(opt.dataset)
+    focal = opt.test_focal_length if getattr(opt, 'test_focal_length', -1) >= 0 else ds.rest_focal_length
+    self.mean = np.ascontiguousarray(ds.mean, dtype=np.float32).reshape(3)
+    self.std = np.ascontiguousarray(ds.std, dtype=np.float32).reshape(3)
+    self.frames = (L.Frame * B)()
+    self._meta = []
+    off = 0
+    for b, (h, w) in enumerate(frame_sizes):
+      h, w = int(h), int(w)
+      if h <= 0 or w <= 0:
+        raise ValueError('frame_sizes[%d]: bad size %s' % (b, (h, w)))
+      meta, minv = frame_geometry(opt, h, w)
+      if (meta['inp_height'], meta['inp_width']) != (self.H, self.W):
+        raise ValueError('frame_sizes[%d] = %s maps to a %dx%d network input under this resolution policy, not the '
+                         "runner's %dx%d" % (b, (h, w), meta['inp_height'], meta['inp_width'], self.H, self.W))
+      meta['calib'] = calibs[b] if calibs is not None else default_calib(focal, w, h)
+      self._meta.append(meta)
+      f = self.frames[b]
+      f.offset, f.h, f.w, f.step = off, h, w, 3 * w
+      f.minv[:] = minv.tolist()
+      off += (h * w * 3 + 15) // 16 * 16
+    self.frame_sizes = [(int(h), int(w)) for h, w in frame_sizes]
+    self.slot_bytes = off
+    return calibs if calibs is not None else np.stack([m['calib'] for m in self._meta]).astype(np.float32)
+
+  def meta(self, b):
+    """Frames mode: the meta dict Detector.pre_process returns for stream b's frames (c, s, sizes, trans_input,
+    trans_output, calib) -- what generic_post_process needs when the records are post-processed on the host."""
+    if not self.frames_mode:
+      raise ValueError('meta(): the runner was not built with frame_sizes')
+    return {k: (v.copy() if isinstance(v, np.ndarray) else v) for k, v in self._meta[b].items()}
 
   # one step, eager launches on the current stream
   def _eager(self, slot, first=False):
     if self.tracker is not None:
       self.tracker.render(self.hm[slot])                     # pre_hm(t) from tracks(t-1)
-    pre = self.img[slot] if first else self.img[(slot - 1) % NS]
-    out = dict(self.eng.forward(self.img[slot], pre, self.hm[slot]))
+    prev = slot if first else (slot - 1) % NS
+    if self.frames_mode and self.eng.use_halo:
+      eng = self.eng
+      L.check(L.lib().ct_pack_stem_frames(
+          L.ptr(self.u8[slot]), L.ptr(self.u8[prev] if eng.has_pre_img else None), self.frames, self.B,
+          C.c_void_p(self.mean.ctypes.data), C.c_void_p(self.std.ctypes.data),
+          L.ptr(self.hm[slot] if eng.has_pre_hm else None), L.ptr(eng.stem_input), self.H, self.W, L.stream_ptr()),
+          'ct_pack_stem_frames')
+      out = dict(eng.forward_packed(eng.has_pre_img, eng.has_pre_hm))
+    else:
+      if self.frames_mode:
+        self._warp_frames(slot)
+      out = dict(self.eng.forward(self.img[slot], self.img[prev], self.hm[slot]))
     if self.ws is None:
       cat = out['hm'].shape[1]
       J = out['hm_hp'].shape[1] if ('hm_hp' in out and 'hps' in out) else 0
@@ -102,6 +185,15 @@ class StreamRunner(object):
     if self.tracker is not None:
       self.tracker.step(self.rec, *(self.pub[slot] if self.public else ()))    # tracks(t)
     return res
+
+  def _warp_frames(self, slot):
+    """fp32 and bf16x3 engines: the slot's frames -> its fp32 image, one ct_warp_affine_normalize per stream."""
+    lib, st = L.lib(), L.stream_ptr()
+    src, dst = self.u8[slot].data_ptr(), self.img[slot]
+    for b, f in enumerate(self.frames):
+      L.check(lib.ct_warp_affine_normalize(C.c_void_p(src + f.offset), 1, f.h, f.w, f.step, L.ptr(self.minv[b]),
+                                           C.c_void_p(self.mean.ctypes.data), C.c_void_p(self.std.ctypes.data),
+                                           L.ptr(dst[b]), self.H, self.W, st), 'ct_warp_affine_normalize')
 
   def _graph(self, slot):
     if self.graphs[slot] is None:
@@ -223,6 +315,11 @@ class StreamRunner(object):
         self.pub[slot][0].copy_(self.h_pub[slot][0], non_blocking=True)
         self.pub[slot][1].copy_(self.h_pub[slot][1], non_blocking=True)
       self.ev_in[slot].record(self.copy)
+    return self._submit(slot)
+
+  def _submit(self, slot):
+    """The step of the uploaded slot on the compute stream and the D2H of its results; -> the previous step's
+    records."""
     prev = self.fetch() if self.t > 0 else None
     with torch.cuda.stream(self.compute):
       self.compute.wait_event(self.ev_in[slot])
@@ -237,6 +334,55 @@ class StreamRunner(object):
       self.ev_done[(slot - 1) % NS].record(self.compute)
     self.t += 1
     return prev
+
+  def frame_buffers(self):
+    """Frames mode: numpy views [h_b, w_b, 3] uint8 of the pinned staging the NEXT step_frames uploads, one per stream,
+    for a decoder to write its frames in place; then call step_frames(None).  They may be written once the previous
+    step_frames call has returned (its upload of three steps ago, which last read this staging, has completed by
+    then) and until the next step_frames call."""
+    if not self.frames_mode:
+      raise ValueError('frame_buffers(): the runner was not built with frame_sizes')
+    buf = self.h_u8[self.t % NS].numpy()
+    return [buf[f.offset:f.offset + f.h * f.w * 3].reshape(f.h, f.w, 3) for f in self.frames]
+
+  def step_frames(self, frames, pre_hms=None, public_dets=None):
+    """frames: B uint8 [h_b, w_b, 3] BGR arrays of the sizes given as frame_sizes, or None when they were written
+    through frame_buffers().  pre_hms, public_dets and the return value as in step_host; public detections are in each
+    stream's source pixels, and so are the tracks.  ValueError on a wrong count, dtype or shape, or when the runner
+    was not built with frame_sizes."""
+    if not self.frames_mode:
+      raise ValueError('step_frames: the runner was not built with frame_sizes (use step_host)')
+    pub = self._check_public(public_dets)
+    slot = self.t % NS
+    if frames is not None:
+      if len(frames) != self.B:
+        raise ValueError('frames: expected %d arrays (one per stream), got %d' % (self.B, len(frames)))
+      for b, (a, (h, w)) in enumerate(zip(frames, self.frame_sizes)):
+        if not isinstance(a, np.ndarray) or a.dtype != np.uint8:
+          raise ValueError('frames[%d]: expected a uint8 numpy array, got %s' %
+                           (b, getattr(a, 'dtype', type(a).__name__)))
+        if a.shape != (h, w, 3):
+          raise ValueError('frames[%d]: expected shape %s, got %s' % (b, (h, w, 3), a.shape))
+      # the slot's staging was last read by step t-3's upload, which the last fetch() waited for
+      for a, v in zip(frames, self.frame_buffers()):
+        np.copyto(v, a)
+    if pub is not None:
+      self._fill_public(self.h_pub[slot], pub)
+    use_hm = self.tracker is None and pre_hms is not None
+    src_hm = pre_hms
+    if use_hm and not pre_hms.is_pinned():
+      self.h_hm[slot].copy_(pre_hms)
+      src_hm = self.h_hm[slot]
+    with torch.cuda.stream(self.copy):
+      self.copy.wait_event(self.ev_done[slot])       # slot's old contents were last read as pre_images of step t-2
+      self.u8[slot].copy_(self.h_u8[slot], non_blocking=True)
+      if use_hm:
+        self.hm[slot].copy_(src_hm, non_blocking=True)
+      if pub is not None:
+        self.pub[slot][0].copy_(self.h_pub[slot][0], non_blocking=True)
+        self.pub[slot][1].copy_(self.h_pub[slot][1], non_blocking=True)
+      self.ev_in[slot].record(self.copy)
+    return self._submit(slot)
 
   def fetch(self, copy=True):
     """Blocks until the last submitted step finished; returns its records as numpy [B,K,F].  A copy by default: the
@@ -263,7 +409,10 @@ class StreamRunner(object):
   @property
   def h2d_bytes_per_step(self):
     pub = self.B * (self.tracker.max_public * 2 + 1) * 4 if self.public else 0
-    return self.B * (3 if self.tracker is not None else 4) * self.H * self.W * 4 + pub
+    hm = self.B * self.H * self.W * 4 if self.tracker is None else 0
+    if self.frames_mode:
+      return self.slot_bytes + hm + pub
+    return self.B * 3 * self.H * self.W * 4 + hm + pub
 
   @property
   def d2h_bytes_per_step(self):

@@ -25,6 +25,8 @@
  *                     ct_track_step_payload adds the pose / 3D / velocity / attribute fields (post_process.py:55-89).
  *   ct_flip_merge     Detector._flip_output, detector.py:311-332 (flip_tensor / flip_lr / flip_lr_off, model/utils.py:28-50).
  *   ct_warp_affine_normalize   Detector.pre_process's cv2.warpAffine + normalise + HWC->CHW, detector.py:207-226.
+ *   ct_pack_stem_frames        the same for B ragged uint8 frames and their previous frames, written as the packed
+ *                     input of the tensor-core stem (no fp32 image in between).
  */
 #ifndef CTB200_H_
 #define CTB200_H_
@@ -343,6 +345,25 @@ int ct_flip_merge(const float* in2, float* out, int32_t C, int32_t H, int32_t W,
 int ct_warp_affine_normalize(const uint8_t* src, int32_t B, int32_t src_h, int32_t src_w, int32_t src_step,
                              const double* minv, const float* mean, const float* std, float* dst, int32_t out_h,
                              int32_t out_w, void* stream);
+
+/* One stream's frame inside a buffer of B ragged uint8 BGR frames (StreamRunner's frame slots). */
+typedef struct {
+  int64_t offset;             /* byte offset of the frame in the buffer (StreamRunner aligns it to 16 bytes) */
+  int32_t h, w, step;         /* source rows, columns, row pitch in bytes (>= 3 w) */
+  int32_t reserved;
+  double  minv[6];            /* dst -> src map, inverted exactly as cv::warpAffine inverts it (see above) */
+} ct_frame;
+
+/* Streams per kernel launch of ct_pack_stem_frames (the descriptors travel in the kernel parameters). */
+#define CT_FRAMES_PER_LAUNCH 48
+
+/* out bf16 NHWC [B,H,W,8] = (norm(warp(cur_b)) x3, norm(warp(prev_b)) x3, pre_hm_b, 0): the tensor-core stem's input,
+ * byte-identical to ct_warp_affine_normalize of each stream followed by ct_pack_stem_input.  cur / prev: device buffers
+ * holding each stream's frame at frames[b].offset (the same descriptor is used for both); prev == NULL or
+ * pre_hm == NULL (fp32 [B,1,H,W]) give zeros.  frames: HOST array [B], read during the call and passed to the kernels
+ * by value (a captured CUDA graph keeps them); one launch per CT_FRAMES_PER_LAUNCH streams.  mean / std host fp32[3]. */
+int ct_pack_stem_frames(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames, int32_t B, const float* mean,
+                        const float* std, const float* pre_hm, void* out, int32_t H, int32_t W, void* stream);
 
 /* ---- misc --------------------------------------------------------------------------- */
 const char* ct_last_error(void);

@@ -110,7 +110,8 @@ class Frame(C.Structure):
 EXPORTS = ['ct_packed_weight_bytes', 'ct_pack_weights', 'ct_conv_forward', 'ct_conv_config', 'ct_stem_forward',
            'ct_pack_stem_input', 'ct_pack_stem_input_f32', 'ct_maxpool2', 'ct_maxpool2_s2d', 'ct_upsample_add', 'ct_decode_workspace_bytes', 'ct_decode',
            'ct_render_pre_hm', 'ct_track_smem_bytes', 'ct_track_step', 'ct_track_assoc_smem_bytes',
-           'ct_track_step_assoc', 'ct_track_payload_smem_bytes', 'ct_track_step_payload', 'ct_render_tracks', 'ct_flip_merge',
+           'ct_track_step_assoc', 'ct_track_payload_smem_bytes', 'ct_track_step_payload', 'ct_track_start',
+           'ct_render_tracks', 'ct_flip_merge',
            'ct_warp_affine_normalize', 'ct_pack_stem_frames', 'ct_last_error', 'ct_abi_version', 'ct_launch_count',
            'ct_reset_launch_count', 'ct_debug_trace', 'ct_debug_watch']
 
@@ -186,6 +187,8 @@ def lib():
   L.ct_track_payload_smem_bytes.restype = C.c_int64
   L.ct_track_payload_smem_bytes.argtypes = [C.c_int32] * 4
   L.ct_track_step_payload.argtypes = [C.POINTER(TrackDesc), C.POINTER(TrackAssoc), C.POINTER(TrackPayload), C.c_void_p]
+  L.ct_track_start.argtypes = [C.POINTER(TrackDesc), C.POINTER(TrackPayload), C.c_void_p, C.c_int32, C.c_void_p,
+                               C.c_void_p]
   L.ct_render_tracks.argtypes = [C.c_void_p, C.c_int32, C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p]
   L.ct_flip_merge.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p, C.c_void_p, C.c_void_p]
   L.ct_warp_affine_normalize.argtypes = [C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 4 + [C.c_int32] * 2 + [C.c_void_p]

@@ -268,6 +268,40 @@ __device__ __forceinline__ void det_payload(const ct_track_payload& p, const flo
     for (int k = 0; k < p.att_floats; ++k) out[o++] = r[p.rec_nuscenes_att + k];
 }
 
+// Boxes of the NEXT frame's prior heat-map (detector.py:254-290) from stream b's first `total` track rows `trk`: image
+// -> input coords, clip, radius, centre; rows past `total` and tracks that are not splatted get radius -1.  The one copy
+// of this arithmetic: the track step and ct_track_start both end with it.  Called by all TRK_THREADS threads.
+__device__ __forceinline__ void track_boxes(const ct_track_desc& d, int b, const float* trk, int total, int tid) {
+  if (!d.boxes) return;
+  const int T = d.max_tracks;
+  const double* ti = d.trans_input + b * 6;
+  float* bx = d.boxes + (size_t)b * T * 5;
+  for (int r = tid; r < T; r += TRK_THREADS) {
+    float radius = -1.f, cxo = 0.f, cyo = 0.f;
+    if (r < total) {
+      const float* t = trk + (size_t)r * TF;
+      if (!(t[CT_TRK_SCORE] < d.pre_thresh) && t[CT_TRK_ACTIVE] != 0.f) {
+        const float wmax = (float)(d.inp_w - 1), hmax = (float)(d.inp_h - 1);
+        float x0 = (float)aff_f64(ti, (double)t[CT_TRK_BBOX], (double)t[CT_TRK_BBOX + 1]);
+        float y0 = (float)aff_f64(ti + 3, (double)t[CT_TRK_BBOX], (double)t[CT_TRK_BBOX + 1]);
+        float x1 = (float)aff_f64(ti, (double)t[CT_TRK_BBOX + 2], (double)t[CT_TRK_BBOX + 3]);
+        float y1 = (float)aff_f64(ti + 3, (double)t[CT_TRK_BBOX + 2], (double)t[CT_TRK_BBOX + 3]);
+        x0 = fminf(fmaxf(x0, 0.f), wmax); x1 = fminf(fmaxf(x1, 0.f), wmax);
+        y0 = fminf(fmaxf(y0, 0.f), hmax); y1 = fminf(fmaxf(y1, 0.f), hmax);
+        const float h = __fsub_rn(y1, y0), w = __fsub_rn(x1, x0);
+        if (h > 0.f && w > 0.f) {
+          const double rad = gaussian_radius_f64(ceil((double)h), ceil((double)w));
+          const int ri = (int)rad;                 // int(): truncation
+          radius = (float)(ri > 0 ? ri : 0);
+          cxo = (float)(int)(__fadd_rn(x0, x1) * 0.5f);   // astype(np.int32): truncation
+          cyo = (float)(int)(__fadd_rn(y0, y1) * 0.5f);
+        }
+      }
+    }
+    bx[r * 5 + 0] = (float)b; bx[r * 5 + 1] = cxo; bx[r * 5 + 2] = cyo; bx[r * 5 + 3] = radius; bx[r * 5 + 4] = 0.f;
+  }
+}
+
 // PAY: also write the payload table (ct_track_step_payload); the 2-D head sets run the <false> instantiation.
 template <bool PAY>
 __global__ void __launch_bounds__(TRK_THREADS)
@@ -493,36 +527,32 @@ track_step_kernel(const TrackArgs a) {
   if (tid == 0) { d.counts[b * 2 + 0] = total; d.counts[b * 2 + 1] = s_ids; }
   __syncthreads();     // the table rows written above are re-read below by other threads
   __threadfence_block();
+  track_boxes(d, b, trk, total, tid);
+}
 
-  // ---- boxes of the NEXT frame's prior heat-map (detector.py:254-290): image -> input coords, clip, radius, centre
-  if (d.boxes) {
-    const double* ti = d.trans_input + b * 6;
-    float* bx = d.boxes + (size_t)b * T * 5;
-    for (int r = tid; r < T; r += TRK_THREADS) {
-      float radius = -1.f, cxo = 0.f, cyo = 0.f;
-      if (r < total) {
-        const float* t = trk + (size_t)r * TF;
-        if (!(t[CT_TRK_SCORE] < d.pre_thresh) && t[CT_TRK_ACTIVE] != 0.f) {
-          const float wmax = (float)(d.inp_w - 1), hmax = (float)(d.inp_h - 1);
-          float x0 = (float)aff_f64(ti, (double)t[CT_TRK_BBOX], (double)t[CT_TRK_BBOX + 1]);
-          float y0 = (float)aff_f64(ti + 3, (double)t[CT_TRK_BBOX], (double)t[CT_TRK_BBOX + 1]);
-          float x1 = (float)aff_f64(ti, (double)t[CT_TRK_BBOX + 2], (double)t[CT_TRK_BBOX + 3]);
-          float y1 = (float)aff_f64(ti + 3, (double)t[CT_TRK_BBOX + 2], (double)t[CT_TRK_BBOX + 3]);
-          x0 = fminf(fmaxf(x0, 0.f), wmax); x1 = fminf(fmaxf(x1, 0.f), wmax);
-          y0 = fminf(fmaxf(y0, 0.f), hmax); y1 = fminf(fmaxf(y1, 0.f), hmax);
-          const float h = __fsub_rn(y1, y0), w = __fsub_rn(x1, x0);
-          if (h > 0.f && w > 0.f) {
-            const double rad = gaussian_radius_f64(ceil((double)h), ceil((double)w));
-            const int ri = (int)rad;                 // int(): truncation
-            radius = (float)(ri > 0 ? ri : 0);
-            cxo = (float)(int)(__fadd_rn(x0, x1) * 0.5f);   // astype(np.int32): truncation
-            cyo = (float)(int)(__fadd_rn(y0, y1) * 0.5f);
-          }
-        }
-      }
-      bx[r * 5 + 0] = (float)b; bx[r * 5 + 1] = cxo; bx[r * 5 + 2] = cyo; bx[r * 5 + 3] = radius; bx[r * 5 + 4] = 0.f;
-    }
-  }
+// ct_track_start: stream starts[e][0] begins a new video -- Tracker.reset + init_track(seeds): its T track rows, counts
+// and payload rows are cleared, its starts[e][1] seed rows (already filtered and numbered on the host) written, and its
+// render boxes computed from them by the same code as the track step's.  One CTA per started stream; the seeds of
+// entry e follow those of entries 0..e-1 in `seeds`.
+__global__ void __launch_bounds__(TRK_THREADS)
+track_start_kernel(const ct_track_desc d, float* __restrict__ payload, int Wp, const int* __restrict__ starts,
+                   const float* __restrict__ seeds) {
+  const int e = blockIdx.x, tid = threadIdx.x, T = d.max_tracks;
+  const int b = starts[2 * e];
+  if (b < 0 || b >= d.B) return;
+  auto clamp_n = [&](int n) { return seeds == nullptr ? 0 : (n < 0 ? 0 : (n > T ? T : n)); };
+  size_t off = 0;
+  for (int k = 0; k < e; ++k) off += (size_t)clamp_n(starts[2 * k + 1]);
+  const int n = clamp_n(starts[2 * e + 1]);
+  float* trk = d.tracks + (size_t)b * T * TF;
+  const float* src = seeds ? seeds + off * TF : nullptr;
+  for (int i = tid; i < T * TF; i += TRK_THREADS) trk[i] = i < n * TF ? src[i] : 0.f;
+  if (payload)
+    for (int i = tid; i < T * Wp; i += TRK_THREADS) payload[(size_t)b * T * Wp + i] = 0.f;
+  if (tid == 0) { d.counts[b * 2 + 0] = n; d.counts[b * 2 + 1] = n; }
+  __syncthreads();     // the seed rows written above are re-read below by other threads
+  __threadfence_block();
+  track_boxes(d, b, trk, n, tid);
 }
 
 // splat of the boxes written by track_step_kernel; rows with radius < 0 are skipped.  grid = B*T (fixed: graph-capturable)
@@ -747,6 +777,20 @@ extern "C" int ct_track_step_assoc(const ct_track_desc* d, const ct_track_assoc*
 extern "C" int ct_track_step(const ct_track_desc* d, void* stream) {
   const ct_track_assoc greedy = {};
   return ct_track_step_assoc(d, &greedy, stream);
+}
+
+extern "C" int ct_track_start(const ct_track_desc* d, const ct_track_payload* p, const int32_t* starts,
+                              int32_t n_starts, const float* seeds, void* stream) {
+  CT_REQUIRE(d && d->tracks && d->counts, "null pointer");
+  CT_REQUIRE(d->B > 0 && d->max_tracks > 0, "bad shape");
+  CT_REQUIRE(d->boxes == nullptr || (d->trans_input != nullptr && d->inp_h > 0 && d->inp_w > 0), "boxes need trans_input");
+  CT_REQUIRE(n_starts >= 0 && n_starts <= d->B, "n_starts outside [0, B]");
+  CT_REQUIRE(n_starts == 0 || starts, "null start list");
+  CT_REQUIRE(!p || (p->payload && p->width > 0), "payload table needs payload and width > 0");
+  if (n_starts == 0) return CT_OK;
+  track_start_kernel<<<n_starts, TRK_THREADS, 0, (cudaStream_t)stream>>>(*d, p ? p->payload : nullptr, p ? p->width : 0,
+                                                                          starts, seeds);
+  return after_launch();
 }
 
 extern "C" int ct_render_tracks(const float* boxes, int32_t n, float* pre_hm, int32_t B, int32_t H, int32_t W,

@@ -44,6 +44,64 @@ def payload_layout(layout):
   return out
 
 
+def seed_rows(items, new_thresh):
+  """Tracker.init_track on a fresh tracker (utils/tracker.py:11-22) as track-table rows: the result dicts with
+  score > new_thresh, in input order, get ids 1..n with age = 1 and active = 1; `ct` is the bbox centre when the item has
+  none, computed in float64 as the reference does on its JSON-loaded results.  `tracking` is 0 when absent.
+  -> float32 [n, CT_TRK_FLOATS].  ValueError when a kept item lacks score, class or bbox."""
+  rows = []
+  for item in items:
+    if item['score'] <= new_thresh:
+      continue
+    try:
+      bbox = [float(v) for v in item['bbox'][:4]]
+      cls = item['class']
+    except KeyError as e:
+      raise ValueError('pre_dets: a seed needs score, class and bbox (missing %s)' % e)
+    ct = item['ct'] if 'ct' in item else [(bbox[0] + bbox[2]) / 2, (bbox[1] + bbox[3]) / 2]
+    r = np.zeros(L.CT_TRK_FLOATS, np.float32)
+    r[L.CT_TRK_SCORE], r[L.CT_TRK_CLASS] = item['score'], cls
+    r[L.CT_TRK_CT:L.CT_TRK_CT + 2] = np.asarray(ct, np.float64)[:2]
+    r[L.CT_TRK_TRACKING:L.CT_TRK_TRACKING + 2] = np.asarray(item.get('tracking', (0., 0.)), np.float64)[:2]
+    r[L.CT_TRK_BBOX:L.CT_TRK_BBOX + 4] = bbox
+    r[L.CT_TRK_ID], r[L.CT_TRK_AGE], r[L.CT_TRK_ACTIVE] = len(rows) + 1, 1, 1
+    rows.append(r)
+  return np.stack(rows) if rows else np.zeros((0, L.CT_TRK_FLOATS), np.float32)
+
+
+def plan_starts(B, T, new_thresh, has_payload, starts, pre_dets):
+  """Checks one step's video starts and builds their seeds, before anything is enqueued.  starts: stream indices whose
+  frame is a video's first; pre_dets: {stream: list of result dicts} seeding some of them (or None).
+  -> (streams list, [seed rows float32 [n_i, CT_TRK_FLOATS]] in the same order).  ValueError on a stream out of range
+  or repeated, pre_dets for a stream that does not start, more kept seeds than the T rows of the track table, or
+  pre_dets on a head set with payload fields (their seeds would need those fields)."""
+  streams = []
+  for s in starts:
+    if isinstance(s, (bool, np.bool_)) or not isinstance(s, (int, np.integer)):
+      raise ValueError('starts: stream indices must be integers, got %r' % (s,))
+    s = int(s)
+    if not 0 <= s < B:
+      raise ValueError('starts: stream %d out of range [0, %d)' % (s, B))
+    if s in streams:
+      raise ValueError('starts: stream %d given twice' % s)
+    streams.append(s)
+  pre_dets = pre_dets or {}
+  for s in pre_dets:
+    if s not in streams:
+      raise ValueError('pre_dets: stream %r does not start a video in this step' % (s,))
+  if has_payload and pre_dets:
+    raise ValueError('pre_dets: seeding is not supported on head sets with payload fields (pose, 3D, velocity, '
+                     'attributes); start those streams without pre_dets')
+  seeds = []
+  for s in streams:
+    rows = seed_rows(pre_dets.get(s, ()), new_thresh)
+    if len(rows) > T:
+      raise ValueError('pre_dets[%d]: %d seeds above new_thresh, more than the %d rows of the track table' %
+                       (s, len(rows), T))
+    seeds.append(rows)
+  return streams, seeds
+
+
 class DeviceTracker(object):
 
   def __init__(self, opt, B, K, rec_floats, layout, inp_h, inp_w, device, centers=None, scales=None, max_tracks=None,
@@ -133,6 +191,24 @@ class DeviceTracker(object):
       self.payload.zero_()
     self.boxes.zero_()
     self.boxes[:, :, 3] = -1.0
+
+  def start(self, streams, seeds=None):
+    """Detector.reset_tracking + Tracker.init_track(seeds[b]) on each stream b of `streams` alone, on the current
+    stream: its tracks, counts and payload are cleared, the seeds written (seed_rows), and its boxes rendered from them,
+    so that the next render() splats them.  seeds: {stream: list of result dicts} (pre_dets) or None.  ValueError as
+    plan_starts."""
+    streams, rows = plan_starts(self.B, self.T, self.opt.new_thresh, self.payload is not None, streams, seeds)
+    if not streams:
+      return
+    lst = torch.tensor([[s, len(r)] for s, r in zip(streams, rows)], dtype=torch.int32).to(self.device)
+    seed = torch.from_numpy(np.concatenate(rows)).to(self.device) if sum(map(len, rows)) else None
+    self.start_device(lst, len(streams), seed)
+
+  def start_device(self, start_list, n_starts, seeds=None):
+    """ct_track_start on device buffers: start_list int32 [>= n_starts, 2] rows (stream, seed rows), seeds fp32
+    [sum of n, CT_TRK_FLOATS] in start_list's order (or None).  No checks of the contents: see plan_starts."""
+    L.check(L.lib().ct_track_start(C.byref(self.desc), C.byref(self.pay) if self.pay is not None else None,
+                                   L.ptr(start_list), n_starts, L.ptr(seeds), L.stream_ptr()), 'ct_track_start')
 
   def public_buffers(self):
     """Zeroed device buffers of the shape step() takes with --public_det: public_ct [B,P,2] fp32, public_n [B] int32."""

@@ -32,6 +32,12 @@ engine ct_pack_stem_frames writes the stem's packed bf16 input straight from slo
 warped again: no fp32 copy is kept); the fp32 and bf16x3 engines warp each stream into the fp32 image slot with
 ct_warp_affine_normalize and run their plan unchanged.  The tracker gets each stream's (c, s) and default calib, so
 tracks, public detections and 3D boxes are in that camera's pixels.
+
+Video starts (`starts=`, `pre_dets=` of step_host / step_frames / load_device_inputs): a stream may begin a new video at
+any step, as Detector.reset_tracking + Tracker.init_track(pre_dets) on that stream alone.  A start is rare (once per
+video), so it is not in the graphs: a step that carries starts first runs a short prologue on the compute stream -- the
+started streams' frames copied into the previous slot (their pre_images), then ct_track_start (reset, seeds, render
+boxes) -- and then replays the same graph as any other step.  Steps without starts run exactly what they ran before.
 """
 import ctypes as C
 
@@ -42,7 +48,7 @@ from . import _lib as L
 from .dataset_info import get_dataset
 from .decode import generic_decode
 from .detector import default_calib, frame_geometry
-from .device_tracker import DeviceTracker
+from .device_tracker import DeviceTracker, plan_starts
 
 
 NS = 3          # input slots
@@ -88,6 +94,9 @@ class StreamRunner(object):
     self.t = 0
     self.tracker = None
     self.device_tracking = device_tracking
+    self._starts = [None] * NS                               # per slot: the streams whose frame starts a video
+    self._start_bytes = 0                                    # start list + seed rows uploaded by the last step
+    self.h_start = None                                      # per slot start list / seed staging, made on first use
     self._eager(0, first=True)                               # sizes the record buffer
     if device_tracking:
       assert self.opt is not None, 'device tracking needs opt (thresholds, max_age)'
@@ -264,8 +273,58 @@ class StreamRunner(object):
       ct[b, :len(a)] = torch.from_numpy(a)
       n[b] = len(a)
 
-  def load_device_inputs(self, images, pre_hms, slot, public_dets=None):
+  def _check_starts(self, starts, pre_dets):
+    """starts (stream indices whose frame in this step is a video's first) and pre_dets ({stream: list of result
+    dicts} seeding the tracker of some of them, in each stream's source pixels like the tracks) -> (streams, seed rows)
+    or None.  ValueError (device_tracker.plan_starts) before anything is enqueued; without device tracking a start only
+    switches pre_images, and pre_dets are refused."""
+    if starts is None or len(starts) == 0:
+      if pre_dets:
+        raise ValueError('pre_dets: stream(s) %s do not start a video in this step' % sorted(pre_dets))
+      return None
+    if self.tracker is None:
+      if pre_dets:
+        raise ValueError('pre_dets seed the device tracker: this runner was built without device_tracking')
+      return plan_starts(self.B, 0, 0.0, False, starts, None)
+    trk = self.tracker
+    return plan_starts(self.B, trk.T, self.opt.new_thresh, trk.payload is not None, starts, pre_dets)
+
+  def _stage_starts(self, slot, plan):
+    """The pinned staging of slot's start list (stream, seeds) and seed rows <- plan; -> (entries, seed rows).  The
+    staging was last read by the upload of step t-3, which the last fetch() waited for."""
+    if self.h_start is None:
+      T = self.tracker.T
+      self.h_start = [torch.zeros((self.B, 2), dtype=torch.int32).pin_memory() for _ in range(NS)]
+      self.h_seed = [torch.zeros((self.B * T, L.CT_TRK_FLOATS), dtype=torch.float32).pin_memory() for _ in range(NS)]
+      self.d_start = [torch.zeros((self.B, 2), dtype=torch.int32, device=self.device) for _ in range(NS)]
+      self.d_seed = [torch.zeros((self.B * T, L.CT_TRK_FLOATS), dtype=torch.float32, device=self.device)
+                     for _ in range(NS)]
+    streams, seeds = plan
+    n = 0
+    for e, (s, rows) in enumerate(zip(streams, seeds)):
+      self.h_start[slot][e, 0], self.h_start[slot][e, 1] = s, len(rows)
+      self.h_seed[slot][n:n + len(rows)] = torch.from_numpy(rows)
+      n += len(rows)
+    return len(streams), n
+
+  def _upload_starts(self, slot, plan, non_blocking):
+    """Stages and uploads one step's starts for slot (the current stream is the upload's); -> the bytes uploaded."""
+    self._starts[slot] = None
+    if plan is None:
+      return 0
+    self._starts[slot] = plan[0]
+    if self.tracker is None:
+      return 0
+    e, n = self._stage_starts(slot, plan)
+    self.d_start[slot][:e].copy_(self.h_start[slot][:e], non_blocking=non_blocking)
+    if n:
+      self.d_seed[slot][:n].copy_(self.h_seed[slot][:n], non_blocking=non_blocking)
+    return e * 8 + n * L.CT_TRK_FLOATS * 4
+
+  def load_device_inputs(self, images, pre_hms, slot, public_dets=None, starts=None, pre_dets=None):
+    """Copies step_device's inputs into `slot` on the current stream; starts / pre_dets as in step_host."""
     pub = self._check_public(public_dets)
+    plan = self._check_starts(starts, pre_dets)
     self.img[slot].copy_(images)
     if pre_hms is not None:
       self.hm[slot].copy_(pre_hms)
@@ -273,8 +332,36 @@ class StreamRunner(object):
       self._fill_public(self.h_pub[slot], pub)
       self.pub[slot][0].copy_(self.h_pub[slot][0])
       self.pub[slot][1].copy_(self.h_pub[slot][1])
+    self._start_bytes = self._upload_starts(slot, plan, non_blocking=False)
+
+  def _start_prologue(self, slot, streams):
+    """A step whose frames start new videos on `streams`, before the step itself (graph replay or eager), on the same
+    stream: first-frame pre_images and the tracker start.  Outside the graphs: they stay the same for every step."""
+    if self.t > 0:
+      # pre_images of a started stream = its own frame: overwrite its part of the previous slot, which holds step t-1's
+      # images.  Safe: that slot is read only by this step (as pre_images), after this prologue on the same stream, and
+      # it is next written by the upload of step t+2, which waits for ev_done[prev], recorded after this step.
+      prev = (slot - 1) % NS
+      for b in streams:
+        if self.frames_mode and self.eng.use_halo:          # the pack kernel warps u8[prev] again
+          f = self.frames[b]
+          o, n = f.offset, f.h * f.w * 3
+          self.u8[prev][o:o + n].copy_(self.u8[slot][o:o + n])
+        elif self.frames_mode:                               # the plan reads img[prev]: warp this frame into it
+          f = self.frames[b]
+          L.check(L.lib().ct_warp_affine_normalize(
+              C.c_void_p(self.u8[slot].data_ptr() + f.offset), 1, f.h, f.w, f.step, L.ptr(self.minv[b]),
+              C.c_void_p(self.mean.ctypes.data), C.c_void_p(self.std.ctypes.data), L.ptr(self.img[prev][b]), self.H,
+              self.W, L.stream_ptr()), 'ct_warp_affine_normalize')
+        else:
+          self.img[prev][b].copy_(self.img[slot][b])
+    if self.tracker is not None:                             # reset + seeds + boxes: the step's render splats them
+      self.tracker.start_device(self.d_start[slot], len(streams), self.d_seed[slot])
 
   def _launch(self, slot):
+    streams, self._starts[slot] = self._starts[slot], None
+    if streams:
+      self._start_prologue(slot, streams)
     if self.t == 0:
       self._eager(slot, first=True)                          # first frame of the streams: pre_images = images
     elif self.use_graph:
@@ -289,12 +376,16 @@ class StreamRunner(object):
     self.t += 1
     return self.rec
 
-  def step_host(self, images, pre_hms=None, public_dets=None):
+  def step_host(self, images, pre_hms=None, public_dets=None, starts=None, pre_dets=None):
     """images [B,3,H,W] (and pre_hms [B,1,H,W] unless device_tracking): float32 HOST tensors (what
     Detector.pre_process / _get_additional_inputs produce); with --public_det, public_dets = B arrays [P_b, 2] (the
-    `ct`s of each frame's public detections).  Returns the records of the PREVIOUS call (None the first time) -- a
-    one-step software pipeline: this step's H2D overlaps the previous step's compute."""
+    `ct`s of each frame's public detections).  starts: the streams whose frame in this step is a new video's first
+    (Detector.reset_tracking on those streams alone: the frame is its own pre_images and the stream's tracker restarts
+    empty, or from pre_dets = {stream: list of result dicts} as Tracker.init_track; the other streams are unaffected).
+    Returns the records of the PREVIOUS call (None the first time) -- a one-step software pipeline: this step's H2D
+    overlaps the previous step's compute."""
     pub = self._check_public(public_dets)
+    plan = self._check_starts(starts, pre_dets)
     slot = self.t % NS
     if pub is not None:        # the slot's staging was last read by step t-3's upload, which the last fetch() waited for
       self._fill_public(self.h_pub[slot], pub)
@@ -314,6 +405,7 @@ class StreamRunner(object):
       if pub is not None:
         self.pub[slot][0].copy_(self.h_pub[slot][0], non_blocking=True)
         self.pub[slot][1].copy_(self.h_pub[slot][1], non_blocking=True)
+      self._start_bytes = self._upload_starts(slot, plan, non_blocking=True)
       self.ev_in[slot].record(self.copy)
     return self._submit(slot)
 
@@ -345,14 +437,15 @@ class StreamRunner(object):
     buf = self.h_u8[self.t % NS].numpy()
     return [buf[f.offset:f.offset + f.h * f.w * 3].reshape(f.h, f.w, 3) for f in self.frames]
 
-  def step_frames(self, frames, pre_hms=None, public_dets=None):
+  def step_frames(self, frames, pre_hms=None, public_dets=None, starts=None, pre_dets=None):
     """frames: B uint8 [h_b, w_b, 3] BGR arrays of the sizes given as frame_sizes, or None when they were written
-    through frame_buffers().  pre_hms, public_dets and the return value as in step_host; public detections are in each
-    stream's source pixels, and so are the tracks.  ValueError on a wrong count, dtype or shape, or when the runner
-    was not built with frame_sizes."""
+    through frame_buffers().  pre_hms, public_dets, starts, pre_dets and the return value as in step_host; public
+    detections and pre_dets are in each stream's source pixels, and so are the tracks.  ValueError on a wrong count,
+    dtype or shape, or when the runner was not built with frame_sizes."""
     if not self.frames_mode:
       raise ValueError('step_frames: the runner was not built with frame_sizes (use step_host)')
     pub = self._check_public(public_dets)
+    plan = self._check_starts(starts, pre_dets)
     slot = self.t % NS
     if frames is not None:
       if len(frames) != self.B:
@@ -381,6 +474,7 @@ class StreamRunner(object):
       if pub is not None:
         self.pub[slot][0].copy_(self.h_pub[slot][0], non_blocking=True)
         self.pub[slot][1].copy_(self.h_pub[slot][1], non_blocking=True)
+      self._start_bytes = self._upload_starts(slot, plan, non_blocking=True)
       self.ev_in[slot].record(self.copy)
     return self._submit(slot)
 
@@ -406,13 +500,25 @@ class StreamRunner(object):
     pay = self.h_pay[i].numpy() if self.tracker.payload is not None else None
     return self.tracker.results(self.h_trk[i].numpy(), self.h_cnt[i].numpy(), pay)
 
+  def previous_results(self):
+    """After a step_host / step_frames call: the tracks of the step before it, as fetch_results() gives them.  No wait:
+    the call returned once that step had finished (its records are what the call returned), and its tables are not
+    overwritten before the next call."""
+    if self.t < 2:
+      raise ValueError('previous_results(): fewer than two steps submitted')
+    i = (self.t - 2) & 1
+    pay = self.h_pay[i].numpy() if self.tracker.payload is not None else None
+    return self.tracker.results(self.h_trk[i].numpy(), self.h_cnt[i].numpy(), pay)
+
   @property
   def h2d_bytes_per_step(self):
+    """Bytes uploaded per step: the frames (and pre_hm / public detections); a step that starts videos with device
+    tracking also uploads its start list and seed rows, counted here after that step is submitted."""
     pub = self.B * (self.tracker.max_public * 2 + 1) * 4 if self.public else 0
     hm = self.B * self.H * self.W * 4 if self.tracker is None else 0
     if self.frames_mode:
-      return self.slot_bytes + hm + pub
-    return self.B * 3 * self.H * self.W * 4 + hm + pub
+      return self.slot_bytes + hm + pub + self._start_bytes
+    return self.B * 3 * self.H * self.W * 4 + hm + pub + self._start_bytes
 
   @property
   def d2h_bytes_per_step(self):

@@ -23,6 +23,8 @@
  *                     frame, per stream, on the device;  ct_render_tracks splats those boxes (image.py:128-154).
  *                     ct_track_step_assoc adds --hungarian and --public_det association (tracker.py:52-72,83-103);
  *                     ct_track_step_payload adds the pose / 3D / velocity / attribute fields (post_process.py:55-89).
+ *                     ct_track_start: reset_tracking + Tracker.init_track(pre_dets) on some streams alone
+ *                     (detector.py:97-103, utils/tracker.py:11-22).
  *   ct_flip_merge     Detector._flip_output, detector.py:311-332 (flip_tensor / flip_lr / flip_lr_off, model/utils.py:28-50).
  *   ct_warp_affine_normalize   Detector.pre_process's cv2.warpAffine + normalise + HWC->CHW, detector.py:207-226.
  *   ct_pack_stem_frames        the same for B ragged uint8 frames and their previous frames, written as the packed
@@ -330,6 +332,16 @@ typedef struct {
 int64_t ct_track_payload_smem_bytes(int32_t K, int32_t max_tracks, int32_t width, int32_t assoc);
 /* ct_track_step_assoc that also writes the payload table; p == NULL is ct_track_step_assoc. */
 int ct_track_step_payload(const ct_track_desc* d, const ct_track_assoc* a, const ct_track_payload* p, void* stream);
+/* Start a new video on some streams (Detector.reset_tracking + Tracker.init_track on those streams alone): for each of
+ * the n_starts entries of `starts` (device int32 [n_starts][2] = (stream, seed rows n), distinct streams in [0, B)), the
+ * stream's T track rows, its counts and (p != NULL) its payload rows are zeroed, its n seed rows are written (fp32
+ * [n][CT_TRK_FLOATS] in track-table format, already filtered and numbered: ids 1..n), counts = (n, n), and its T render
+ * boxes are computed from them as ct_track_step computes them.  `seeds` (device) holds the rows of entry 0, then entry 1,
+ * ...; it may be NULL when no entry has seeds.  n is clamped to [0, T] and entries with a stream outside [0, B) are
+ * skipped on the device.  Every other stream is left untouched.  One CTA per entry; n_starts == 0 launches nothing.
+ * Only d->B, max_tracks, pre_thresh, inp_h, inp_w, trans_input, tracks, counts and boxes are read. */
+int ct_track_start(const ct_track_desc* d, const ct_track_payload* p, const int32_t* starts, int32_t n_starts,
+                   const float* seeds, void* stream);
 /* pre_hm (fp32 [B,1,H,W], zeroed here) <- max-splat of boxes [n,5] (rows with radius < 0 skipped); n is the grid size,
  * so the launch shape does not depend on the data (CUDA-graph capturable). */
 int ct_render_tracks(const float* boxes, int32_t n, float* pre_hm, int32_t B, int32_t H, int32_t W, void* stream);

@@ -107,13 +107,21 @@ class Frame(C.Structure):
               ('minv', C.c_double * 6)]
 
 
+CT_FLIP_MAX_HEADS = 12
+
+
+class FlipHead(C.Structure):
+  _fields_ = [('input', C.c_void_p), ('out', C.c_void_p), ('C', C.c_int32), ('reserved', C.c_int32),
+              ('perm', C.c_void_p), ('sign', C.c_void_p)]
+
+
 EXPORTS = ['ct_packed_weight_bytes', 'ct_pack_weights', 'ct_conv_forward', 'ct_conv_config', 'ct_stem_forward',
            'ct_pack_stem_input', 'ct_pack_stem_input_f32', 'ct_maxpool2', 'ct_maxpool2_s2d', 'ct_upsample_add', 'ct_decode_workspace_bytes', 'ct_decode',
            'ct_render_pre_hm', 'ct_track_smem_bytes', 'ct_track_step', 'ct_track_assoc_smem_bytes',
            'ct_track_step_assoc', 'ct_track_payload_smem_bytes', 'ct_track_step_payload', 'ct_track_start',
-           'ct_render_tracks', 'ct_flip_merge',
-           'ct_warp_affine_normalize', 'ct_pack_stem_frames', 'ct_last_error', 'ct_abi_version', 'ct_launch_count',
-           'ct_reset_launch_count', 'ct_debug_trace', 'ct_debug_watch']
+           'ct_render_tracks', 'ct_flip_merge', 'ct_flip_merge_heads', 'ct_mirror_x',
+           'ct_warp_affine_normalize', 'ct_pack_stem_frames', 'ct_pack_stem_frames_flip', 'ct_last_error',
+           'ct_abi_version', 'ct_launch_count', 'ct_reset_launch_count', 'ct_debug_trace', 'ct_debug_watch']
 
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17', '-Xcompiler', '-fPIC']
 
@@ -192,8 +200,11 @@ def lib():
   L.ct_render_tracks.argtypes = [C.c_void_p, C.c_int32, C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p]
   L.ct_flip_merge.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p, C.c_void_p, C.c_void_p]
   L.ct_warp_affine_normalize.argtypes = [C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 4 + [C.c_int32] * 2 + [C.c_void_p]
+  L.ct_flip_merge_heads.argtypes = [C.POINTER(FlipHead)] + [C.c_int32] * 4 + [C.c_void_p]
+  L.ct_mirror_x.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p]
   L.ct_pack_stem_frames.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(Frame), C.c_int32] + [C.c_void_p] * 4 + \
       [C.c_int32] * 2 + [C.c_void_p]
+  L.ct_pack_stem_frames_flip.argtypes = L.ct_pack_stem_frames.argtypes
   L.ct_launch_count.restype = C.c_int64
   L.ct_reset_launch_count.restype = None
   L.ct_debug_trace.argtypes = [C.c_void_p]

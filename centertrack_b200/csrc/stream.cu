@@ -7,11 +7,14 @@
 //                    the pose / 3D / velocity / attribute fields of generic_post_process (post_process.py:55-89) in a
 //                    payload table beside the track table, and the amodal centre on 3D head sets
 //   ct_render_tracks the gaussian max-splat of those boxes into pre_hm (image.py:128-154)
-//   ct_flip_merge    Detector._flip_output (detector.py:311-332; model/utils.py:28-50) for --flip_test
+//   ct_flip_merge    Detector._flip_output (detector.py:311-332; model/utils.py:28-50) for --flip_test;
+//                    ct_flip_merge_heads: every averaged head of B (frame, mirror) pairs in one launch
+//   ct_mirror_x      the mirrored half of a --flip_test batch (detector.py:225-226,285-286)
 //   ct_warp_affine_normalize   Detector.pre_process's cv2.warpAffine(INTER_LINEAR) + (x/255 - mean)/std + HWC->CHW
 //                    (detector.py:207-226), cv2's fixed-point bilinear restated
 //   ct_pack_stem_frames        the same warp + normalise of B ragged uint8 frames (and of their previous frames),
-//                    written straight as the tensor-core stem's packed bf16 input
+//                    written straight as the tensor-core stem's packed bf16 input; ct_pack_stem_frames_flip also
+//                    writes each stream's mirror image (--flip_test)
 // All HBM-bound byte/index work: one pass over the data, coalesced, no tensor cores.
 #include <math_constants.h>
 
@@ -20,22 +23,44 @@
 namespace ctb {
 
 // ------------------------------------------------------------------------------------------------------------------
-// flip merge: out[c,y,x] = 0.5 * (in[0,c,y,x] + sign[c] * in[1,perm[c],y,W-1-x])
+// flip merge of B (frame, mirrored frame) pairs, every averaged head in one launch (blockIdx.y = head):
+//   out[b,c,y,x] = 0.5 * (in[b,c,y,x] + sign[c] * in[B+b,perm[c],y,W-1-x])
+// The descriptors travel in the kernel parameters, so a captured CUDA graph keeps them.
 // ------------------------------------------------------------------------------------------------------------------
-__global__ void flip_merge_kernel(const float* __restrict__ in2, float* __restrict__ out, int C, int H, int W,
-                                  const int* __restrict__ perm, const float* __restrict__ sign) {
-  const size_t total = (size_t)C * H * W;
+struct FlipArgs {
+  ct_flip_head h[CT_FLIP_MAX_HEADS];
+};
+
+__global__ void flip_merge_kernel(const __grid_constant__ FlipArgs fa, int B, int H, int W) {
+  const ct_flip_head& hd = fa.h[blockIdx.y];
+  const int C = hd.C;
   const size_t plane = (size_t)H * W;
+  const size_t img = (size_t)C * plane;
+  const size_t total = (size_t)B * img;
+  const float* __restrict__ in = hd.in;
+  float* __restrict__ out = hd.out;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int c = (int)(i / plane);
-    const size_t r = i - (size_t)c * plane;
+    const int b = (int)(i / img);
+    const size_t q = i - (size_t)b * img;
+    const int c = (int)(q / plane);
+    const size_t r = q - (size_t)c * plane;
     const int y = (int)(r / W), x = (int)(r - (size_t)y * W);
-    const int cs = perm ? perm[c] : c;
-    const float sg = sign ? sign[c] : 1.f;
-    const float a = in2[i];
-    const float b = in2[total + (size_t)cs * plane + (size_t)y * W + (W - 1 - x)];
+    const int cs = hd.perm ? hd.perm[c] : c;
+    const float sg = hd.sign ? hd.sign[c] : 1.f;
+    const float a = in[i];
+    const float m = in[(size_t)(B + b) * img + (size_t)cs * plane + (size_t)y * W + (W - 1 - x)];
     // the reference adds the two maps and halves the sum: (a + s*b) / 2, in that order (division by 2 is exact)
-    out[i] = __fmul_rn(__fadd_rn(a, __fmul_rn(sg, b)), 0.5f);
+    out[i] = __fmul_rn(__fadd_rn(a, __fmul_rn(sg, m)), 0.5f);
+  }
+}
+
+// dst[i,c,y,x] = src[i,c,y,W-1-x]: the mirrored half of a flip-test batch (images, pre_images, pre_hm)
+__global__ void mirror_x_kernel(const float* __restrict__ src, float* __restrict__ dst, size_t rows, int W) {
+  const size_t total = rows * W;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const size_t row = i / W;
+    const int x = (int)(i - row * W);
+    dst[i] = src[row * W + (W - 1 - x)];
   }
 }
 
@@ -642,6 +667,9 @@ __global__ void warp_affine_norm_kernel(const unsigned char* __restrict__ src, i
 // pre_hm, 0) straight from each stream's uint8 frame.  blockIdx.y = stream (its descriptor read once, from the kernel
 // parameters), one 16-byte output pixel per thread and iteration.  The normalisation depends on the 8-bit value only:
 // a 3 x 256 table built per CTA with normalize_u8 gives the same floats without a per-pixel fp64 divide.
+// FLIP (ct_pack_stem_frames_flip): out is [2B,H,W,8] and image B+b is image b mirrored.  The mirrored packed pixel
+// (y, W-1-x) equals the original's (y, x) in all 8 channels (frame, previous frame and pre_hm are all mirrored), so each
+// pixel is warped once and its 16-byte vector stored twice.
 // ------------------------------------------------------------------------------------------------------------------
 struct FramesArgs {
   ct_frame f[CT_FRAMES_PER_LAUNCH];
@@ -650,9 +678,10 @@ struct FramesArgs {
 constexpr int PACK_THREADS = 256;
 constexpr int PACK_PIX_PER_THREAD = 4;      // pixels per thread: amortises the table build over 1024 pixels per CTA
 
+template <bool FLIP>
 __global__ void __launch_bounds__(PACK_THREADS)
 pack_stem_frames_kernel(const unsigned char* __restrict__ cur, const unsigned char* __restrict__ prev,
-                        const __grid_constant__ FramesArgs fa, int b0, float3 mean, float3 stdv,
+                        const __grid_constant__ FramesArgs fa, int b0, int B, float3 mean, float3 stdv,
                         const float* __restrict__ hm, uint4* __restrict__ out, int H, int W) {
   __shared__ float tab[3][256];
   for (int i = threadIdx.x; i < 3 * 256; i += PACK_THREADS) {
@@ -690,6 +719,7 @@ pack_stem_frames_kernel(const unsigned char* __restrict__ cur, const unsigned ch
 #pragma unroll
     for (int q = 0; q < 4; ++q) h[q] = __floats2bfloat162_rn(v[2 * q], v[2 * q + 1]);
     out[(size_t)b * plane + r] = o;
+    if constexpr (FLIP) out[(size_t)(B + b) * plane + (size_t)y * W + (W - 1 - x)] = o;
   }
 }
 
@@ -703,11 +733,36 @@ static inline int sw_blocks(size_t total) {
   return (int)(b < cap ? (b ? b : 1) : cap);
 }
 
+extern "C" int ct_flip_merge_heads(const ct_flip_head* heads, int32_t n_heads, int32_t B, int32_t H, int32_t W,
+                                   void* stream) {
+  CT_REQUIRE(heads, "null pointer");
+  CT_REQUIRE(n_heads > 0 && n_heads <= CT_FLIP_MAX_HEADS, "n_heads outside [1, CT_FLIP_MAX_HEADS]");
+  CT_REQUIRE(B > 0 && H > 0 && W > 0, "bad shape");
+  FlipArgs fa = {};
+  size_t most = 0;
+  for (int32_t i = 0; i < n_heads; ++i) {
+    CT_REQUIRE(heads[i].in && heads[i].out, "null pointer");
+    CT_REQUIRE(heads[i].C > 0, "bad shape");
+    fa.h[i] = heads[i];
+    const size_t n = (size_t)B * heads[i].C * H * W;
+    most = n > most ? n : most;
+  }
+  dim3 grid((unsigned)sw_blocks(most), (unsigned)n_heads);
+  flip_merge_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(fa, B, H, W);
+  return after_launch();
+}
+
 extern "C" int ct_flip_merge(const float* in2, float* out, int32_t C, int32_t H, int32_t W, const int32_t* perm,
                              const float* sign, void* stream) {
-  CT_REQUIRE(in2 && out, "null pointer");
-  CT_REQUIRE(C > 0 && H > 0 && W > 0, "bad shape");
-  flip_merge_kernel<<<sw_blocks((size_t)C * H * W), 256, 0, (cudaStream_t)stream>>>(in2, out, C, H, W, perm, sign);
+  const ct_flip_head h = {in2, out, C, 0, perm, sign};
+  return ct_flip_merge_heads(&h, 1, 1, H, W, stream);
+}
+
+extern "C" int ct_mirror_x(const float* src, float* dst, int32_t n, int32_t C, int32_t H, int32_t W, void* stream) {
+  CT_REQUIRE(src && dst, "null pointer");
+  CT_REQUIRE(n > 0 && C > 0 && H > 0 && W > 0, "bad shape");
+  const size_t rows = (size_t)n * C * H;
+  mirror_x_kernel<<<sw_blocks(rows * W), 256, 0, (cudaStream_t)stream>>>(src, dst, rows, W);
   return after_launch();
 }
 
@@ -813,9 +868,10 @@ extern "C" int ct_warp_affine_normalize(const uint8_t* src, int32_t B, int32_t s
   return after_launch();
 }
 
-extern "C" int ct_pack_stem_frames(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames, int32_t B,
-                                   const float* mean, const float* std, const float* pre_hm, void* out, int32_t H,
-                                   int32_t W, void* stream) {
+template <bool FLIP>
+static int pack_stem_frames(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames, int32_t B,
+                            const float* mean, const float* std, const float* pre_hm, void* out, int32_t H, int32_t W,
+                            void* stream) {
   CT_REQUIRE(cur && frames && mean && std && out, "null pointer");
   CT_REQUIRE(B > 0 && H > 0 && W > 0, "bad shape");
   for (int32_t b = 0; b < B; ++b)
@@ -831,10 +887,22 @@ extern "C" int ct_pack_stem_frames(const uint8_t* cur, const uint8_t* prev, cons
     FramesArgs fa = {};
     memcpy(fa.f, frames + b0, sizeof(ct_frame) * n);
     dim3 grid((unsigned)((plane + per_cta - 1) / per_cta), (unsigned)n);
-    pack_stem_frames_kernel<<<grid, PACK_THREADS, 0, (cudaStream_t)stream>>>(cur, prev, fa, b0, m, s, pre_hm,
-                                                                             (uint4*)out, H, W);
+    pack_stem_frames_kernel<FLIP><<<grid, PACK_THREADS, 0, (cudaStream_t)stream>>>(cur, prev, fa, b0, B, m, s, pre_hm,
+                                                                                   (uint4*)out, H, W);
     const int rc = after_launch();
     if (rc != CT_OK) return rc;
   }
   return CT_OK;
+}
+
+extern "C" int ct_pack_stem_frames(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames, int32_t B,
+                                   const float* mean, const float* std, const float* pre_hm, void* out, int32_t H,
+                                   int32_t W, void* stream) {
+  return pack_stem_frames<false>(cur, prev, frames, B, mean, std, pre_hm, out, H, W, stream);
+}
+
+extern "C" int ct_pack_stem_frames_flip(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames, int32_t B,
+                                        const float* mean, const float* std, const float* pre_hm, void* out, int32_t H,
+                                        int32_t W, void* stream) {
+  return pack_stem_frames<true>(cur, prev, frames, B, mean, std, pre_hm, out, H, W, stream);
 }

@@ -94,6 +94,51 @@ def frame_geometry(opt, height, width):
   return meta, M
 
 
+def flip_plan(outputs, flip_idx, device):
+  """Which heads of `outputs` ({head: [n,c,h,w]}) Detector._flip_output (detector.py:311-332) averages with the
+  mirrored pass, and how: {head: (perm or None, sign or None)} as device tensors; every other head keeps its un-flipped
+  pass.  Shared by Detector (one pair) and StreamRunner (B pairs)."""
+  plan = {}
+  pairs = {}
+  for a, b in flip_idx:
+    pairs[a], pairs[b] = b, a
+  for h, t in outputs.items():
+    c = t.shape[1]
+    if h in ('hm', 'wh', 'dep', 'dim'):
+      plan[h] = (None, None)
+    elif h == 'amodel_offset':                              # flipped copy with its x components negated
+      plan[h] = (None, torch.tensor([-1. if i % 2 == 0 else 1. for i in range(c)], dtype=torch.float32, device=device))
+    elif h == 'hps':                                        # flip_lr_off: mirror, negate x offsets, swap left/right joints
+      perm = [2 * pairs.get(i // 2, i // 2) + (i % 2) for i in range(c)]
+      plan[h] = (torch.tensor(perm, dtype=torch.int32, device=device),
+                 torch.tensor([-1. if i % 2 == 0 else 1. for i in range(c)], dtype=torch.float32, device=device))
+    elif h == 'hm_hp':                                      # flip_lr: mirror, swap left/right joints
+      plan[h] = (torch.tensor([pairs.get(i, i) for i in range(c)], dtype=torch.int32, device=device), None)
+  return plan
+
+
+def flip_output(output, plan, merged):
+  """Device form of detector.py:311-332 on B (frame, mirrored frame) pairs: output {head: [2B,c,h,w]} (frames first,
+  mirrors second), merged {head of plan: [B,c,h,w]} -> {head: merged[head], or the frames' half [0, B) of every other
+  head}.  Every averaged head is merged by one ct_flip_merge_heads launch."""
+  heads = (L.FlipHead * L.CT_FLIP_MAX_HEADS)()
+  res, n = {}, 0
+  dptr = lambda t: t.data_ptr() if t is not None else None
+  for h, t in output.items():
+    n2, c, oh, ow = t.shape
+    if h in plan:
+      perm, sign = plan[h]
+      f = heads[n]
+      f.input, f.out, f.C, f.perm, f.sign = t.data_ptr(), merged[h].data_ptr(), c, dptr(perm), dptr(sign)
+      n += 1
+      res[h] = merged[h]
+    else:
+      res[h] = t[0:n2 // 2]
+  if n:
+    L.check(L.lib().ct_flip_merge_heads(heads, n, n2 // 2, oh, ow, L.stream_ptr()), 'ct_flip_merge_heads')
+  return res
+
+
 def default_calib(focal_length, width, height):
   """Detector._get_default_calib: the camera matrix of a width x height image with its principal point at the centre."""
   return np.array([[focal_length, 0, width / 2, 0],
@@ -324,37 +369,11 @@ class Detector(object):
   def _flip_plan(self, eng):
     """Which heads Detector._flip_output (detector.py:311-332) averages with the mirrored pass, and how:
     {head: (perm or None, sign or None)}; every other head keeps its un-flipped pass."""
-    plan = {}
-    dev = eng.device
-    pairs = {}
-    for a, b in getattr(self, 'flip_idx', None) or get_dataset(self.opt.dataset).flip_idx:
-      pairs[a], pairs[b] = b, a
-    for h, t in eng.outputs.items():
-      c = t.shape[1]
-      if h in ('hm', 'wh', 'dep', 'dim'):
-        plan[h] = (None, None)
-      elif h == 'amodel_offset':                              # flipped copy with its x components negated
-        plan[h] = (None, torch.tensor([-1. if i % 2 == 0 else 1. for i in range(c)], dtype=torch.float32, device=dev))
-      elif h == 'hps':                                        # flip_lr_off: mirror, negate x offsets, swap left/right joints
-        perm = [2 * pairs.get(i // 2, i // 2) + (i % 2) for i in range(c)]
-        plan[h] = (torch.tensor(perm, dtype=torch.int32, device=dev),
-                   torch.tensor([-1. if i % 2 == 0 else 1. for i in range(c)], dtype=torch.float32, device=dev))
-      elif h == 'hm_hp':                                      # flip_lr: mirror, swap left/right joints
-        plan[h] = (torch.tensor([pairs.get(i, i) for i in range(c)], dtype=torch.int32, device=dev), None)
-    return plan
+    return flip_plan(eng.outputs, getattr(self, 'flip_idx', None) or get_dataset(self.opt.dataset).flip_idx, eng.device)
 
   def _flip_output(self, output, plan, merged):
     """Device form of detector.py:311-332 on the post-activation maps of a (frame, mirrored frame) pair."""
-    res = {}
-    for h, t in output.items():
-      if h in plan:
-        perm, sign = plan[h]
-        L.check(L.lib().ct_flip_merge(L.ptr(t), L.ptr(merged[h]), t.shape[1], t.shape[2], t.shape[3], L.ptr(perm),
-                                      L.ptr(sign), L.stream_ptr()), 'ct_flip_merge')
-        res[h] = merged[h]
-      else:
-        res[h] = t[0:1]
-    return res
+    return flip_output(output, plan, merged)
 
   def _process_plan(self, B, H, W, device, has_pre, has_hm):
     """Everything `process` launches for one input signature, built once: engine plan, flip-merge buffers, decode

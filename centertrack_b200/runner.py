@@ -38,6 +38,14 @@ any step, as Detector.reset_tracking + Tracker.init_track(pre_dets) on that stre
 video), so it is not in the graphs: a step that carries starts first runs a short prologue on the compute stream -- the
 started streams' frames copied into the previous slot (their pre_images), then ct_track_start (reset, seeds, render
 boxes) -- and then replays the same graph as any other step.  Steps without starts run exactly what they ran before.
+
+Flip test (`opt.flip_test`, detector.py:225-226,285-286,311-332): the network runs on 2B images, the streams' frames
+[0, B) and their mirrors [B, 2B), inside the same step.  pre_images is the previous step's 2B images, so the previous
+frame's mirror comes free (detector.py:148).  Uploads, the device tracker's render and a caller's pre_hm fill the first
+B images; ct_mirror_x writes the second half in the graph, or, in frames mode on the bf16 engine,
+ct_pack_stem_frames_flip stores every packed pixel at its mirrored position too.  One ct_flip_merge_heads launch
+averages the flipped heads into [B] buffers; decode and tracking then run at B on those and on the first half of the
+other heads.  Records, tracks, uploads and downloads are the same size as without the flip.
 """
 import ctypes as C
 
@@ -47,7 +55,7 @@ import torch
 from . import _lib as L
 from .dataset_info import get_dataset
 from .decode import generic_decode
-from .detector import default_calib, frame_geometry
+from .detector import default_calib, flip_output, flip_plan, frame_geometry
 from .device_tracker import DeviceTracker, plan_starts
 
 
@@ -63,7 +71,8 @@ class StreamRunner(object):
     camera matrix per stream (DeviceTracker's default otherwise; in frames mode Detector._get_default_calib of the
     stream's source size).  frame_sizes: B (height, width) source sizes, fixed for the runner's lifetime, to feed raw
     uint8 frames with step_frames; each must map to the network input (H, W) under opt's resolution policy
-    (ValueError otherwise)."""
+    (ValueError otherwise).  opt.flip_test: every stream's frame runs with its mirror (2B images per step) and the
+    averaged heads are merged before decode, as Detector.process does; inputs and outputs keep their B shapes."""
     self.B, self.H, self.W, self.K = B, H, W, K
     self.device = torch.device(device)
     self.model = model
@@ -71,11 +80,18 @@ class StreamRunner(object):
     self.frames_mode = frame_sizes is not None
     if self.frames_mode:
       calibs = self._frame_geometry(frame_sizes, calibs)
-    self.eng = model.engine_for(B, H, W, self.device, precision)
+    self.flip = bool(getattr(self.opt, 'flip_test', False))
+    NB = 2 * B if self.flip else B                           # --flip_test: frames [0, B), their mirrors [B, 2B)
+    self.eng = model.engine_for(NB, H, W, self.device, precision)
     self.eng.set_fused_activations(True)
     f32 = torch.float32
-    self.img = [torch.zeros((B, 3, H, W), dtype=f32, device=self.device) for _ in range(NS)]
-    self.hm = [torch.zeros((B, 1, H, W), dtype=f32, device=self.device) for _ in range(NS)]
+    self.img = [torch.zeros((NB, 3, H, W), dtype=f32, device=self.device) for _ in range(NS)]
+    self.hm = [torch.zeros((NB, 1, H, W), dtype=f32, device=self.device) for _ in range(NS)]
+    if self.flip:                                            # the averaged heads, merged per stream
+      self.flip_plan = flip_plan(self.eng.outputs, get_dataset(self.opt.dataset).flip_idx, self.device)
+      self.merged = {h: torch.zeros((B,) + tuple(self.eng.outputs[h].shape[1:]), dtype=f32, device=self.device)
+                     for h in self.flip_plan}
+    self._pack_mirror = self.flip and self.frames_mode and self.eng.use_halo   # the flip pack writes the mirrors
     self.h_img = [torch.zeros((B, 3, H, W), dtype=f32).pin_memory() for _ in range(NS)]
     self.h_hm = [torch.zeros((B, 1, H, W), dtype=f32).pin_memory() for _ in range(NS)]
     if self.frames_mode:      # frame slots: B uint8 frames at 16-byte aligned offsets, pinned staging + device
@@ -117,10 +133,13 @@ class StreamRunner(object):
       if self.tracker.payload is not None:
         self.h_pay = [torch.zeros_like(self.tracker.payload, device='cpu').pin_memory() for _ in range(2)]
     # launches of one step: the network plan + decode (+ memset-free: render + track step); frames mode: the pack op
-    # becomes ct_pack_stem_frames (one launch per CT_FRAMES_PER_LAUNCH streams), or B warps come before the plan
+    # becomes ct_pack_stem_frames (one launch per CT_FRAMES_PER_LAUNCH streams), or B warps come before the plan.
+    # --flip_test: + the merge, + the mirrors of the images and pre_hm unless the flip pack writes them
     self.launches_per_step = self.eng.n_launches + 1 + (2 if device_tracking else 0)
     if self.frames_mode:
       self.launches_per_step += (-(-B // L.CT_FRAMES_PER_LAUNCH) - 1) if self.eng.use_halo else B
+    if self.flip:
+      self.launches_per_step += 1 + (0 if self._pack_mirror else 1 + int(self.eng.has_pre_hm))
 
   def _frame_geometry(self, frame_sizes, calibs):
     """Per-stream geometry of frames mode (Detector.pre_process_device's, through detector.frame_geometry): the
@@ -169,11 +188,12 @@ class StreamRunner(object):
   # one step, eager launches on the current stream
   def _eager(self, slot, first=False):
     if self.tracker is not None:
-      self.tracker.render(self.hm[slot])                     # pre_hm(t) from tracks(t-1)
+      self.tracker.render(self.hm[slot][:self.B])            # pre_hm(t) from tracks(t-1)
     prev = slot if first else (slot - 1) % NS
     if self.frames_mode and self.eng.use_halo:
       eng = self.eng
-      L.check(L.lib().ct_pack_stem_frames(
+      pack = L.lib().ct_pack_stem_frames_flip if self.flip else L.lib().ct_pack_stem_frames
+      L.check(pack(
           L.ptr(self.u8[slot]), L.ptr(self.u8[prev] if eng.has_pre_img else None), self.frames, self.B,
           C.c_void_p(self.mean.ctypes.data), C.c_void_p(self.std.ctypes.data),
           L.ptr(self.hm[slot] if eng.has_pre_hm else None), L.ptr(eng.stem_input), self.H, self.W, L.stream_ptr()),
@@ -182,7 +202,13 @@ class StreamRunner(object):
     else:
       if self.frames_mode:
         self._warp_frames(slot)
+      if self.flip:                  # the mirrored half; pre_images (img[prev]) was mirrored by its own step
+        self._mirror(self.img[slot], 0, self.B)
+        if self.eng.has_pre_hm:
+          self._mirror(self.hm[slot], 0, self.B)
       out = dict(self.eng.forward(self.img[slot], self.img[prev], self.hm[slot]))
+    if self.flip:
+      out = flip_output(out, self.flip_plan, self.merged)
     if self.ws is None:
       cat = out['hm'].shape[1]
       J = out['hm_hp'].shape[1] if ('hm_hp' in out and 'hps' in out) else 0
@@ -194,6 +220,11 @@ class StreamRunner(object):
     if self.tracker is not None:
       self.tracker.step(self.rec, *(self.pub[slot] if self.public else ()))    # tracks(t)
     return res
+
+  def _mirror(self, x, b, n):
+    """--flip_test: x[B+b : B+b+n] <- x[b : b+n] mirrored along W (ct_mirror_x), on the current stream."""
+    _, c, h, w = x.shape
+    L.check(L.lib().ct_mirror_x(L.ptr(x[b]), L.ptr(x[self.B + b]), n, c, h, w, L.stream_ptr()), 'ct_mirror_x')
 
   def _warp_frames(self, slot):
     """fp32 and bf16x3 engines: the slot's frames -> its fp32 image, one ct_warp_affine_normalize per stream."""
@@ -325,9 +356,9 @@ class StreamRunner(object):
     """Copies step_device's inputs into `slot` on the current stream; starts / pre_dets as in step_host."""
     pub = self._check_public(public_dets)
     plan = self._check_starts(starts, pre_dets)
-    self.img[slot].copy_(images)
+    self.img[slot][:self.B].copy_(images)
     if pre_hms is not None:
-      self.hm[slot].copy_(pre_hms)
+      self.hm[slot][:self.B].copy_(pre_hms)
     if pub is not None:
       self._fill_public(self.h_pub[slot], pub)
       self.pub[slot][0].copy_(self.h_pub[slot][0])
@@ -343,11 +374,12 @@ class StreamRunner(object):
       # it is next written by the upload of step t+2, which waits for ev_done[prev], recorded after this step.
       prev = (slot - 1) % NS
       for b in streams:
-        if self.frames_mode and self.eng.use_halo:          # the pack kernel warps u8[prev] again
+        if self.frames_mode and self.eng.use_halo:          # the pack kernel warps (and mirrors) u8[prev] again
           f = self.frames[b]
           o, n = f.offset, f.h * f.w * 3
           self.u8[prev][o:o + n].copy_(self.u8[slot][o:o + n])
-        elif self.frames_mode:                               # the plan reads img[prev]: warp this frame into it
+          continue
+        if self.frames_mode:                                 # the plan reads img[prev]: warp this frame into it
           f = self.frames[b]
           L.check(L.lib().ct_warp_affine_normalize(
               C.c_void_p(self.u8[slot].data_ptr() + f.offset), 1, f.h, f.w, f.step, L.ptr(self.minv[b]),
@@ -355,6 +387,8 @@ class StreamRunner(object):
               self.W, L.stream_ptr()), 'ct_warp_affine_normalize')
         else:
           self.img[prev][b].copy_(self.img[slot][b])
+        if self.flip:                                        # --flip_test: pre_images is the (frame, mirror) pair
+          self._mirror(self.img[prev], b, 1)
     if self.tracker is not None:                             # reset + seeds + boxes: the step's render splats them
       self.tracker.start_device(self.d_start[slot], len(streams), self.d_seed[slot])
 
@@ -399,9 +433,9 @@ class StreamRunner(object):
         src_hm = self.h_hm[slot]
     with torch.cuda.stream(self.copy):
       self.copy.wait_event(self.ev_done[slot])       # slot's old contents were last read as pre_images of step t-2
-      self.img[slot].copy_(src_img, non_blocking=True)
+      self.img[slot][:self.B].copy_(src_img, non_blocking=True)
       if use_hm:
-        self.hm[slot].copy_(src_hm, non_blocking=True)
+        self.hm[slot][:self.B].copy_(src_hm, non_blocking=True)
       if pub is not None:
         self.pub[slot][0].copy_(self.h_pub[slot][0], non_blocking=True)
         self.pub[slot][1].copy_(self.h_pub[slot][1], non_blocking=True)
@@ -470,7 +504,7 @@ class StreamRunner(object):
       self.copy.wait_event(self.ev_done[slot])       # slot's old contents were last read as pre_images of step t-2
       self.u8[slot].copy_(self.h_u8[slot], non_blocking=True)
       if use_hm:
-        self.hm[slot].copy_(src_hm, non_blocking=True)
+        self.hm[slot][:self.B].copy_(src_hm, non_blocking=True)
       if pub is not None:
         self.pub[slot][0].copy_(self.h_pub[slot][0], non_blocking=True)
         self.pub[slot][1].copy_(self.h_pub[slot][1], non_blocking=True)

@@ -25,10 +25,13 @@
  *                     ct_track_step_payload adds the pose / 3D / velocity / attribute fields (post_process.py:55-89).
  *                     ct_track_start: reset_tracking + Tracker.init_track(pre_dets) on some streams alone
  *                     (detector.py:97-103, utils/tracker.py:11-22).
- *   ct_flip_merge     Detector._flip_output, detector.py:311-332 (flip_tensor / flip_lr / flip_lr_off, model/utils.py:28-50).
+ *   ct_flip_merge     Detector._flip_output, detector.py:311-332 (flip_tensor / flip_lr / flip_lr_off, model/utils.py:28-50);
+ *                     ct_flip_merge_heads merges every head of B pairs at once, ct_mirror_x mirrors the --flip_test
+ *                     batch's second half (detector.py:225-226,285-286).
  *   ct_warp_affine_normalize   Detector.pre_process's cv2.warpAffine + normalise + HWC->CHW, detector.py:207-226.
  *   ct_pack_stem_frames        the same for B ragged uint8 frames and their previous frames, written as the packed
- *                     input of the tensor-core stem (no fp32 image in between).
+ *                     input of the tensor-core stem (no fp32 image in between); ct_pack_stem_frames_flip also writes
+ *                     each stream's mirror image for --flip_test.
  */
 #ifndef CTB200_H_
 #define CTB200_H_
@@ -351,6 +354,29 @@ int ct_render_tracks(const float* boxes, int32_t n, float* pre_hm, int32_t B, in
 int ct_flip_merge(const float* in2, float* out, int32_t C, int32_t H, int32_t W, const int32_t* perm,
                   const float* sign, void* stream);
 
+/* One averaged head of a --flip_test batch of B (frame, mirrored frame) pairs: frames [0, B), mirrors [B, 2B). */
+typedef struct {
+  const float* in;            /* fp32 [2B,C,H,W] (device) */
+  float* out;                 /* fp32 [B,C,H,W] (device) */
+  int32_t C;
+  int32_t reserved;
+  const int32_t* perm;        /* int32 [C] (device) or NULL = identity */
+  const float* sign;          /* fp32 [C] (device) or NULL = +1 */
+} ct_flip_head;
+
+/* Heads per ct_flip_merge_heads launch (the descriptors travel in the kernel parameters). */
+#define CT_FLIP_MAX_HEADS 12
+
+/* ct_flip_merge of every head in `heads` (HOST array [n_heads], read during the call and passed to the kernel by
+ * value, so a captured CUDA graph keeps it) and of all B pairs, in one launch:
+ *   out[b,c,y,x] = (in[b,c,y,x] + sign[c] * in[B+b,perm[c],y,W-1-x]) / 2, with ct_flip_merge's rounding.
+ * ct_flip_merge is the case n_heads = 1, B = 1. */
+int ct_flip_merge_heads(const ct_flip_head* heads, int32_t n_heads, int32_t B, int32_t H, int32_t W, void* stream);
+
+/* dst[i,c,y,x] = src[i,c,y,W-1-x] for fp32 [n,C,H,W] (device, non-overlapping): the mirrored half of a --flip_test
+ * batch. */
+int ct_mirror_x(const float* src, float* dst, int32_t n, int32_t C, int32_t H, int32_t W, void* stream);
+
 /* dst fp32 [B,3,out_h,out_w] = ((warpAffine(src) / 255 - mean) / std), src uint8 [B,src_h,src_w,3] (row pitch src_step
  * bytes), minv fp64 [B,6] = the INVERTED 2x3 map (dst -> src) exactly as cv::warpAffine inverts it; mean/std host fp32[3].
  * Bilinear in cv2's fixed point (1/32 px, 15-bit weights), zero border. */
@@ -376,6 +402,12 @@ typedef struct {
  * by value (a captured CUDA graph keeps them); one launch per CT_FRAMES_PER_LAUNCH streams.  mean / std host fp32[3]. */
 int ct_pack_stem_frames(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames, int32_t B, const float* mean,
                         const float* std, const float* pre_hm, void* out, int32_t H, int32_t W, void* stream);
+/* --flip_test: ct_pack_stem_frames into out [2B,H,W,8] whose image B+b is image b mirrored along W (out[B+b][y][W-1-x]
+ * = out[b][y][x]), as if frame, previous frame and pre_hm had all been mirrored.  Same arguments; pre_hm stays [B,1,H,W]
+ * (un-mirrored). */
+int ct_pack_stem_frames_flip(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames, int32_t B,
+                             const float* mean, const float* std, const float* pre_hm, void* out, int32_t H, int32_t W,
+                             void* stream);
 
 /* ---- misc --------------------------------------------------------------------------- */
 const char* ct_last_error(void);

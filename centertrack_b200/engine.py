@@ -565,7 +565,10 @@ class DLA34Engine(object):
     fused = [h for h, n in first if n >= 2]
     mid_c = {h: sd[h + '.0.weight'].shape[0] for h in fused}
     ks = {sd[h + '.0.weight'].shape[2] for h in fused}
-    assert len(ks) <= 1, 'heads with different first-conv kernel sizes are not supported'
+    if len(ks) > 1:
+      raise ValueError('heads: first convs of different kernel sizes %s are not supported' % sorted(ks))
+    if any(k % 2 == 0 for k in ks):        # padding k // 2 would make the head maps one row / column larger
+      raise ValueError('heads: --head_kernel must be odd (got %d)' % ks.pop())
     if (self.head_fuse and self.use_halo and fused and all(n == 2 for _, n in first) and ks == {3} and feat.C == 64 and
         len(set(mid_c.values())) == 1 and set(mid_c.values()) <= {64, 256} and
         len(fused) <= L.CT_MAX_FUSED_HEADS and max(self.heads[h] for h in fused) <= 80):

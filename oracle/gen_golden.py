@@ -76,6 +76,36 @@ def gen_net():
     print('net', cfg, node, {k: v.shape for k, v in data.items() if k != 'keys'})
 
 
+def gen_head_layouts():
+  """The output-head layouts of tests/helpers.py::HEAD_LAYOUTS (--num_classes, --head_conv, --num_head_conv,
+  --head_kernel, the optional heads) through the reference model on the synthetic checkpoint: head outputs and
+  state-dict keys per layout: the heads' own keys, and once the trunk's, which every layout shares.  The fused and the
+  two-pass layouts go to two files so that each stays under 1 MB; tests/helpers.py::load_head_layout_golden merges
+  them."""
+  sys.path.insert(0, os.path.join(HERE, '..', 'tests'))
+  from helpers import HEAD_LAYOUTS
+  img, pre, hm = wt.synthetic_inputs(1, *SMALL_HW)
+  data = {}
+  for tag, cfg, extra, _ in HEAD_LAYOUTS:
+    opt, model = rh.build_reference_model(cfg, input_hw=SMALL_HW, extra=extra)
+    sd = wt.make_state_dict(model.state_dict(), 317)
+    model.load_state_dict(sd)
+    with torch.no_grad():
+      out = model(img, pre, hm)[-1]
+    data.update({'%s.head.%s' % (tag, k): v.numpy() for k, v in out.items()})
+    is_head = lambda k: k.split('.')[0] in opt.heads
+    data[tag + '.keys'] = np.array(sorted(k for k in sd if is_head(k)))
+    trunk = np.array(sorted(k for k in sd if not is_head(k)))
+    assert 'trunk.keys' not in data or np.array_equal(data['trunk.keys'], trunk), tag
+    data['trunk.keys'] = trunk
+  fused = {tag for tag, _, _, plan in HEAD_LAYOUTS if plan[0] == 'fused'}
+  np.savez_compressed(os.path.join(OUT, 'net_head_layouts_64x96.npz'),
+                      **{k: v for k, v in data.items() if k.split('.')[0] in fused | {'trunk'}})
+  np.savez_compressed(os.path.join(OUT, 'net_head_layouts_two_pass_64x96.npz'),
+                      **{k: v for k, v in data.items() if k.split('.')[0] not in fused | {'trunk'}})
+  print('head layouts', {k: v.shape for k, v in data.items() if '.head.' in k})
+
+
 GENERIC_RENAME = (('backbone.', 'base.'), ('neck.dla_up.', 'dla_up.'), ('neck.ida_up.', 'ida_up.'))
 
 
@@ -430,10 +460,12 @@ def gen_host():
 if __name__ == '__main__':
   os.makedirs(OUT, exist_ok=True)
   torch.manual_seed(0)
-  which = sys.argv[1:] or ['net', 'generic', 'e2e', 'decode', 'post', 'track', 'host', 'opts', 'flip']
+  which = sys.argv[1:] or ['net', 'heads', 'generic', 'e2e', 'decode', 'post', 'track', 'host', 'opts', 'flip']
   rh.install()
   if 'net' in which:
     gen_net()
+  if 'heads' in which:
+    gen_head_layouts()
   if 'generic' in which:
     gen_generic()
   if 'decode' in which:

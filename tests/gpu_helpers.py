@@ -68,6 +68,58 @@ def conv_desc(engine, dtype, x_nchw, w, bias, stride, relu=True, residual=None, 
   return d, out, (xb, wp, sh, rb if residual is not None else None)
 
 
+def packed_weights(engine, w, n_tile):
+  """ct_pack_weights of w [O, I, kh, kw] (fp32, then bf16 RNE on the tensor-core engines) -> device blob."""
+  lib = L.lib()
+  w32 = w.detach().float().cpu().contiguous()
+  O, I, kh, kw = w32.shape
+  wp = torch.empty(lib.ct_packed_weight_bytes(engine, O, I, kh, kw, n_tile), dtype=torch.uint8)
+  L.check(lib.ct_pack_weights(engine, C.c_void_p(w32.data_ptr()), O, I, kh, kw, n_tile, C.c_void_p(wp.data_ptr())))
+  return wp.to(dev)
+
+
+def heads_desc(x_nchw, w1, b1, heads, n2, ld_pad=0, ch_off=0, depth_scale=1.0):
+  """The fused head launch as engine._fused_heads builds it: heads.0 = 3x3 64 -> n_heads x mid (+ b1, ReLU) on the
+  halo engine at n_tile NH = 128 (mid 256) or 64 (mid 64), then per head a 1x1 mid -> C_out (+ bias, activation) at
+  the common 1x1 n_tile n2, its weights zero-padded to n2 by the packer.  heads: [(w2 [C_out, mid, 1, 1], b2, act)].
+
+  Every head's fp32 NCHW planes lie in one NaN-filled buffer, each followed by a guard band of n2 planes plus one
+  tile row (16 image rows): any store from a ragged tile's out-of-image rows or columns C_out .. n2 - 1 lands in one.
+  -> (descriptor, [head output views], buffer, [guard band slices of it], device buffers the descriptor points to)."""
+  B, Cin, H, W = x_nchw.shape
+  nh = 128 if w1.shape[0] // len(heads) == 256 else 64
+  xb = torch.zeros((B, H, W, Cin + ld_pad), dtype=torch.bfloat16, device=dev)
+  xb[..., ch_off:ch_off + Cin] = x_nchw.permute(0, 2, 3, 1).to(dev, torch.bfloat16)
+  w1p = packed_weights(L.CT_ENGINE_TCGEN05_HALO, w1, nh)
+  sh = b1.float().contiguous().to(dev)
+  guard = (n2 * H * W + 16 * W + 3) // 4 * 4
+  sizes = [B * w2.shape[0] * H * W for w2, _, _ in heads]
+  offs, pos = [], guard
+  for s in sizes:                                       # 16-byte aligned planes
+    offs.append(pos)
+    pos += (s + 3) // 4 * 4 + guard
+  buf = torch.full((pos,), float('nan'), dtype=torch.float32, device=dev)
+  table = (L.Head * len(heads))()
+  keep, outs = [xb, w1p, sh, buf, table], []
+  for t, (w2, b2, act), off, s in zip(table, heads, offs, sizes):
+    wp, bb = packed_weights(L.CT_ENGINE_TCGEN05_HALO, w2, n2), b2.float().contiguous().to(dev)
+    keep += [wp, bb]
+    outs.append(buf[off:off + s].view(B, w2.shape[0], H, W))
+    t.w, t.bias, t.out = wp.data_ptr(), bb.data_ptr(), outs[-1].data_ptr()
+    t.C_out, t.n_tile, t.head_act = w2.shape[0], n2, act
+  guards = [slice(0, offs[0])] + [slice(off + s, nxt) for off, s, nxt in zip(offs, sizes, offs[1:] + [pos])]
+  d = L.ConvDesc()
+  d.engine, d.dtype, d.a_mode = L.CT_ENGINE_TCGEN05_HALO, L.CT_BF16, L.CT_A_CONV
+  d.B, d.H, d.W, d.C_in, d.ld_in, d.C_out = B, H, W, Cin, Cin + ld_pad, w1.shape[0]
+  d.KH = d.KW = 3
+  d.stride, d.pad, d.OH, d.OW = 1, 1, H, W
+  d.out_mode, d.relu, d.sig_from, d.depth_scale, d.n_tile = L.CT_OUT_NCHW_F32, 1, 1 << 30, depth_scale, nh
+  d.x = xb.data_ptr() + ch_off * xb.element_size()
+  d.w, d.shift = w1p.data_ptr(), sh.data_ptr()
+  d.n_heads, d.heads = len(heads), C.cast(table, C.POINTER(L.Head))
+  return d, outs, buf, guards, keep
+
+
 def run_conv(*args, **kwargs):
   d, out, _buffers = conv_desc(*args, **kwargs)
   L.check(L.lib().ct_conv_forward(C.byref(d), L.stream_ptr()), 'conv')

@@ -32,11 +32,43 @@ def make_model(cfg, seed=317, extra=()):
   return opt, m, sd
 
 
+# Output-head layouts beyond the shipped tables, one option each (opts.py --num_classes / --head_conv /
+# --num_head_conv / --head_kernel and the optional heads), with the head plan DLA34Engine builds for each on the bf16
+# tensor-core path:
+#   ('fused', NH, N2, n_heads): one launch of csrc/conv_heads.cu, NH mid channels per pass, a common 1x1 n_tile N2;
+#   ('two_pass', k, hidden): heads.0 (k x k, every head's first conv), `hidden` extra 1x1 convs for each head but reg
+#   (opts.py: reg keeps one hidden conv), then one 1x1 per head.
+# oracle/gen_golden.py::gen_head_layouts runs the reference on the same rows (tests/golden/net_head_layouts_64x96.npz).
+HEAD_LAYOUTS = [
+    ('classes20', 'coco_tracking', ['--num_classes', '20'], ('fused', 128, 32, 4)),
+    ('classes60', 'coco_tracking', ['--num_classes', '60'], ('fused', 128, 64, 4)),
+    ('hc64', 'coco_tracking', ['--head_conv', '64'], ('fused', 64, 80, 4)),
+    ('classes1_hc64', 'coco_tracking', ['--num_classes', '1', '--head_conv', '64'], ('fused', 64, 16, 4)),
+    ('pose_hc64', 'coco_pose', ['--head_conv', '64'], ('fused', 64, 48, 7)),
+    ('ddd_12_heads', 'nuscenes_ddd', ['--ltrb', '--ltrb_amodal', '--velocity', '--nuscenes_att'], ('fused', 128, 16, 12)),
+    ('classes90', 'coco_tracking', ['--num_classes', '90'], ('two_pass', 3, 0)),
+    ('hc128', 'coco_tracking', ['--head_conv', '128'], ('two_pass', 3, 0)),
+    ('num_head_conv2', 'coco_tracking', ['--num_head_conv', '2'], ('two_pass', 3, 1)),
+    ('head_kernel1', 'coco_tracking', ['--head_kernel', '1'], ('two_pass', 1, 0)),
+    ('head_kernel5', 'coco_tracking', ['--head_kernel', '5'], ('two_pass', 5, 0)),
+]
+
+
 def load_generic_golden(golden_dir):
   """The --arch generic goldens (oracle/gen_golden.py::gen_generic): the hc256 and hc64 tags are stored in two files
   so that each stays under 1 MB."""
   g = _NpzDict()
   for f in ('net_generic_coco_tracking_64x96.npz', 'net_generic_coco_tracking_64x96_hc64.npz'):
+    z = np.load(os.path.join(golden_dir, f))
+    g.update({k: z[k] for k in z.files})
+  return g
+
+
+def load_head_layout_golden(golden_dir):
+  """The HEAD_LAYOUTS goldens (oracle/gen_golden.py::gen_head_layouts), stored as two files (fused and two-pass
+  layouts) so that each stays under 1 MB."""
+  g = _NpzDict()
+  for f in ('net_head_layouts_64x96.npz', 'net_head_layouts_two_pass_64x96.npz'):
     z = np.load(os.path.join(golden_dir, f))
     g.update({k: z[k] for k in z.files})
   return g

@@ -112,3 +112,116 @@ def test_halo_overlap_rule(built_lib, case):
   C_in, n, ctas, overlap = case
   c = L.conv_config(_desc(C_in=C_in, C_out=n, n_tile=n))
   assert (c.ctas_per_sm, c.overlap) == (ctas, overlap)
+
+
+# ---- the fused head launch (csrc/conv_heads.cu): a halo descriptor with a head table ----------------------------------
+def _heads_desc(mid=256, n_heads=4, nh=None, n2=80, c_outs=None):
+  """heads.0 (3x3 64 -> n_heads x mid at n_tile nh) with a table of n_heads heads at the common 1x1 n_tile n2, no
+  pointers but the table (which the descriptor keeps alive)."""
+  d = _desc(C_in=64, C_out=n_heads * mid, n_tile=nh or (128 if mid == 256 else 64))
+  d.out_mode, d.ld_out, d.relu = L.CT_OUT_NCHW_F32, 0, 1
+  c_outs = c_outs or [n2] * n_heads
+  table = (L.Head * max(1, len(c_outs)))()
+  for t, c in zip(table, c_outs):
+    t.C_out, t.n_tile = c, n2
+  d.n_heads, d.heads = n_heads, C.cast(table, C.POINTER(L.Head))
+  d._table = table
+  return d
+
+
+@pytest.mark.parametrize('n2', [16, 32, 48, 64, 80])
+@pytest.mark.parametrize('mid', [64, 256])
+def test_fused_heads_configuration_on_every_instantiation(built_lib, mid, n2):
+  for n_heads in (1, 12):
+    c = L.conv_config(_heads_desc(mid, n_heads, n2=n2, c_outs=[1, n2, n2 - 7, 2][:n_heads] + [n2] * (n_heads - 4)))
+    assert c is not None and c.smem_bytes <= SMEM_PER_CTA and c.stages >= 3, (mid, n2, n_heads)
+    assert (c.tile_w, c.tile_h, c.ctas_per_sm, c.overlap) == (8, 16, 1, 0), (mid, n2, n_heads)
+
+
+def _set(**kw):
+  def f(d):
+    for k, v in kw.items():
+      setattr(d, k, v)
+  return f
+
+
+def _head(i, **kw):
+  def f(d):
+    for k, v in kw.items():
+      setattr(d.heads[i], k, v)
+  return f
+
+
+HEADS_BAD = [
+    ('n_heads -1', _set(n_heads=-1), b'1 .. 12 heads'),
+    ('n_heads 13', lambda d: setattr(d, 'n_heads', 13) or setattr(d, 'C_out', 13 * 256), b'1 .. 12 heads'),
+    ('null table', _set(heads=C.POINTER(L.Head)()), b'1 .. 12 heads'),
+    ('mid 128', _set(C_out=4 * 128), b'64 or 256 mid channels'),
+    ('C_out not a multiple of n_heads', _set(C_out=4 * 256 + 2), b'64 or 256 mid channels'),
+    ('n_tile 64 for mid 256', _set(n_tile=64), b'n_tile must be 128'),
+    ('n_tile 128 for mid 64', lambda d: setattr(d, 'C_out', 4 * 64), b'n_tile must be 128'),
+    ('different 1x1 n_tiles', _head(2, n_tile=64), b'one n_tile for every head'),
+    ('C_out > n_tile', _head(1, C_out=81), b'one n_tile for every head'),
+    ('C_out 0', _head(3, C_out=0), b'one n_tile for every head'),
+    ('n_tile 96', lambda d: [setattr(d.heads[i], 'n_tile', 96) for i in range(4)], b'one n_tile for every head'),
+    ('n_tile 40', lambda d: [setattr(d.heads[i], 'n_tile', 40) or setattr(d.heads[i], 'C_out', 40) for i in range(4)],
+     b'one n_tile for every head'),
+    ('NHWC output', _set(out_mode=L.CT_OUT_NHWC, ld_out=1024), b'fp32 NCHW outputs'),
+    ('no ReLU', _set(relu=0), b'fp32 NCHW outputs'),
+    ('residual', _set(residual=1 << 20, ld_res=1024), b'fp32 NCHW outputs'),
+    ('epilogue_sum3', _set(epilogue_sum3=1), b'fp32 NCHW outputs'),
+    ('C_in 32', _set(C_in=32, ld_in=32), b'C_in must be 64'),
+    ('1x1 kernel', _set(KH=1, KW=1, pad=0), b"3x3 stride-1 'same'"),
+    ('stride 2', _set(stride=2, OH=32, OW=32), b"3x3 stride-1 'same'"),
+]
+
+
+@pytest.mark.parametrize('case', HEADS_BAD, ids=[b[0] for b in HEADS_BAD])
+def test_fused_heads_refusals_get_the_status_and_message_of_ct_conv_forward(built_lib, case):
+  _, edit, what = case
+  d = _heads_desc()
+  edit(d)
+  rc, msg, _ = _config(d)
+  assert rc == L.CT_ERR_INVALID and what in msg, msg
+  assert _forward(d) == (rc, msg)
+
+
+def _forward_heads(d, **ptrs):
+  """ct_conv_forward of a valid head descriptor on stand-in pointers (16-byte aligned unless given): it must refuse
+  before any CUDA call."""
+  lib = L.lib()
+  d.x = d.w = d.shift = 1 << 20
+  for i in range(d.n_heads):
+    d.heads[i].w = d.heads[i].bias = d.heads[i].out = 1 << 20
+  for k, v in ptrs.items():
+    if k.startswith('head_'):
+      setattr(d.heads[1], k[5:], v)
+    else:
+      setattr(d, k, v)
+  return lib.ct_conv_forward(C.byref(d), None), lib.ct_last_error()
+
+
+@pytest.mark.parametrize('ptrs,what', [
+    (dict(head_w=(1 << 20) + 8), b'every head needs 16-byte aligned w'),
+    (dict(head_w=0), b'every head needs 16-byte aligned w'),
+    (dict(head_bias=0), b'every head needs 16-byte aligned w'),
+    (dict(head_out=0), b'every head needs 16-byte aligned w'),
+    (dict(x=(1 << 20) + 2), b'x / w must be 16-byte aligned'),
+    (dict(w=(1 << 20) + 4), b'x / w must be 16-byte aligned'),
+    (dict(shift=0), b'x / w must be 16-byte aligned'),
+], ids=['misaligned_head_w', 'null_head_w', 'null_head_bias', 'null_head_out', 'misaligned_x', 'misaligned_w',
+        'null_shift'])
+def test_fused_heads_pointer_checks_refuse_before_any_cuda_call(built_lib, ptrs, what):
+  rc, msg = _forward_heads(_heads_desc(), **ptrs)
+  assert rc == L.CT_ERR_INVALID and what in msg, msg
+  if next(iter(ptrs)).startswith('head_'):
+    assert b'(head 1)' in msg, msg
+
+
+def test_fused_heads_need_n_heads_to_route_to_the_head_launch(built_lib):
+  """n_heads = 0 is a plain halo convolution: with the head table but no output it is refused as a null pointer."""
+  d = _heads_desc()
+  d.n_heads = 0
+  lib = L.lib()
+  d.x = d.w = d.shift = 1 << 20
+  assert lib.ct_conv_forward(C.byref(d), None) == L.CT_ERR_INVALID and b'null pointer' in lib.ct_last_error()

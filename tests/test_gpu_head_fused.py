@@ -1,11 +1,12 @@
 """The fused head launch (csrc/conv_heads.cu): all heads' 3x3 + ReLU + 1x1 in one launch whose 3x3 result never leaves
 the chip.  Its K order and MMA shapes are those of the two-pass plan (CTB_HEAD_FUSE=0: heads.0, then one 1x1 per head),
-so the head maps must be bit-identical to it; and the kernel alone against a torch reference of one head."""
+so the head maps must be bit-identical to it; and every head against an fp64 reference with the per-element bounds of
+tests/bounds.py.  tests/test_gpu_head_launch.py runs the launch itself on every instantiation."""
 import pytest
 import torch
-import torch.nn.functional as F
 
 from centertrack_b200 import _lib as L
+from helpers import HEAD_LAYOUTS
 
 SMEM_PER_CTA = 227 << 10
 
@@ -46,7 +47,8 @@ CASES = [
     ('coco_pose', [], (64, 96)),
     ('generic_hc64', ['--arch', 'generic'], (64, 96)),
     ('coco_tracking_partial_tiles', [], (96, 128)),       # 24 x 32 output: the last tile row is half outside
-]
+] + [('layout_' + tag, extra, (64, 96)) for tag, _, extra, plan in HEAD_LAYOUTS if plan[0] == 'fused']
+LAYOUT_CFG = {'layout_' + tag: cfg for tag, cfg, _, _ in HEAD_LAYOUTS}
 
 
 @pytest.mark.gpu
@@ -54,7 +56,7 @@ CASES = [
 def test_fused_heads_bit_identical_to_two_pass_plan(case, monkeypatch):
   from centertrack_b200 import synthetic as syn
   name, extra, hw = case
-  cfg = 'coco_tracking' if name.startswith(('generic', 'coco_tracking')) else name
+  cfg = LAYOUT_CFG.get(name) or ('coco_tracking' if name.startswith(('generic', 'coco_tracking')) else name)
   dev = torch.device('cuda')
   fused = _engine(cfg, extra, hw, 2, True, monkeypatch, dev)
   two_pass = _engine(cfg, extra, hw, 2, False, monkeypatch, dev)
@@ -77,21 +79,22 @@ def test_fused_heads_bit_identical_to_two_pass_plan(case, monkeypatch):
 
 @pytest.mark.gpu
 def test_fused_head_against_torch_reference(monkeypatch):
-  """One head (hm, 80 classes) of the fused launch against relu(conv3x3) -> conv1x1 in fp64 on the bf16-rounded
-  operands the kernel reads, with the intermediate rounded to bf16 as the kernel rounds it."""
+  """Every head of the fused launch (coco_tracking) against the fp64 1x1 over its intermediate, within ALPHA_BF16 x mag
+  (tests/bounds.py), and that intermediate -- heads.0's launch on the same operands, which the fused maps equal bit
+  for bit -- within the bf16 bound of the fp64 3x3 of the bf16-rounded operands."""
+  import bounds as bd
   from centertrack_b200 import synthetic as syn
   dev = torch.device('cuda')
   eng = _engine('coco_tracking', [], (64, 96), 2, True, monkeypatch, dev)
   img, pre, hm = (t.to(dev) for t in syn.synthetic_inputs(2, 64, 96, seed=3))
-  out = eng.forward(img, pre, hm)['hm'].double()
+  out = eng.forward(img, pre, hm)
   torch.cuda.synchronize()
   feat = eng.named['feat'].tensor().permute(0, 3, 1, 2).double()
-  bf = lambda t: t.to(dev).float().bfloat16().double()
-  w1, b1 = bf(eng.sd['hm.0.weight']), eng.sd['hm.0.bias'].float().double().to(dev)
-  w2, b2 = bf(eng.sd['hm.2.weight']), eng.sd['hm.2.bias'].float().double().to(dev)
-  mid = F.relu(F.conv2d(feat, w1, b1, padding=1)).float().bfloat16().double()
-  ref = F.conv2d(mid, w2, b2)
-  mag = F.conv2d(mid.abs(), w2.abs(), b2.abs())
-  err = (out - ref).abs()
-  # fp32 accumulation of the 1x1, plus one bf16 step of mid where the fp32 and fp64 3x3 sums round differently
-  assert bool((err <= 1e-2 * mag + 1e-4).all()), float((err / (mag + 1e-6)).max())
+  bf = lambda t: t.float().bfloat16().double()
+  spec = {sp['name']: sp for sp in eng.specs}
+  for h in eng.heads:
+    mid = spec[h]['x'].tensor().permute(0, 3, 1, 2).double()     # fills heads.0's output on first read
+    ref, mag = bd.conv_ref(feat, bf(eng.sd[h + '.0.weight']), eng.sd[h + '.0.bias'].float(), pad=(1, 1, 1, 1))
+    bd.assert_bound(mid, ref, mag, bd.ALPHA_BF16, True, h + ' intermediate', 'relu')
+    ref, mag = bd.conv_ref(mid, bf(eng.sd[h + '.2.weight']), eng.sd[h + '.2.bias'].float())
+    bd.assert_bound(out[h].double(), ref, mag, bd.ALPHA_BF16, False, h)

@@ -24,7 +24,7 @@ import torch
 
 import ct_oracle as co
 from centertrack_b200 import synthetic as wt
-from helpers import make_model
+from helpers import HEAD_LAYOUTS, load_head_layout_golden, make_model
 
 pytestmark = pytest.mark.gpu
 TOL = {'fp32': (1e-3, 2e-4), 'bf16x3': (1e-3, 2e-4)}
@@ -94,6 +94,33 @@ def test_network_matches_reference_golden(cfg, precision, golden_dir):
   rep = eng.replay()
   torch.cuda.synchronize()
   assert all(torch.equal(eager[h], rep[h]) for h in eager)
+
+
+@pytest.mark.parametrize('layout', HEAD_LAYOUTS, ids=[r[0] for r in HEAD_LAYOUTS])
+def test_head_layouts_match_oracle(layout, golden_dir):
+  """Every output-head layout (tests/helpers.py::HEAD_LAYOUTS: fused launches at other (NH, N2) and head counts,
+  two-pass plans with hidden 1x1 layers, 1x1 / 5x5 first convs, 128-wide or over-80-class heads) end to end: the fp32
+  engine against the fp32 oracle (itself pinned to the reference by net_head_layouts_*.npz) at the fp32 bar, and the
+  bf16 engine against the bf16-emulating oracle and the reference's outputs with the bounds of the shipped configs.
+  This ties each plan to the model's layers and head order."""
+  tag, cfg, extra, _ = layout
+  g = load_head_layout_golden(golden_dir)
+  opt, model, sd = make_model(cfg, extra=extra)
+  model = model.cuda()
+  img, pre, hm = wt.synthetic_inputs(1, 64, 96)
+  ref = co.DLA34Oracle(sd, opt.heads).forward(img, pre, hm)
+  emu = co.DLA34Oracle(sd, opt.heads, emulate_bf16=True).forward(img, pre, hm)
+  for precision in ('fp32', 'bf16'):
+    eng = model.engine_for(1, 64, 96, torch.device('cuda'), precision)
+    out = eng.forward(img.cuda(), pre.cuda(), hm.cuda())
+    torch.cuda.synchronize()
+    assert list(out) == list(opt.heads)
+    for h in opt.heads:
+      if precision == 'fp32':
+        _check(out[h], ref[h].numpy(), 'fp32', '%s %s' % (tag, h))
+      else:
+        _check_stat(out[h], emu[h].numpy(), '%s %s' % (tag, h), EMU_TOL)
+        _check_stat(out[h], g['%s.head.%s' % (tag, h)], '%s %s vs fp32 reference' % (tag, h), 0.4, corr_min=0.9)
 
 
 @pytest.mark.parametrize('precision', ['fp32', 'bf16'])

@@ -13,6 +13,7 @@ import torch.nn.functional as F
 import bounds as bd
 import ct_oracle as co
 from centertrack_b200 import _lib as L
+from helpers import HEAD_LAYOUTS
 
 pytestmark = pytest.mark.gpu
 
@@ -39,7 +40,10 @@ CASES = [
     ('dla_node_gcn_64x96_b2_bf16', 'coco_tracking', (64, 96), 2, 'bf16', ['--dla_node', 'gcn'], {}, {}),
     ('coco_tracking_256_b2_bf16_no_halo', 'coco_tracking', (256, 256), 2, 'bf16', [], {'use_halo': False}, {}),
     ('coco_tracking_256_b2_bf16_dcn_global', 'coco_tracking', (256, 256), 2, 'bf16', [], {}, {'CTB_DCN_WINDOW': '0'}),
-]
+] + [  # the other output-head layouts (tests/helpers.py::HEAD_LAYOUTS); bf16x3 plans them all in two passes
+    ('heads_%s_64x96_b2_%s' % (tag, precision), cfg, (64, 96), 2, precision, extra, {}, {})
+    for tag, cfg, extra, plan in HEAD_LAYOUTS for precision in ('bf16', 'bf16x3')
+    if precision == 'bf16' or plan[0] == 'two_pass']
 
 CHUNK = 4      # images per fp64 reference pass (bounds the memory of the fp64 DCN columns)
 

@@ -12,7 +12,8 @@ import torch
 
 import ct_oracle as co
 from centertrack_b200 import synthetic as wt
-from helpers import DECODE_CASES, HOST_CASES, decode_inputs, host_case_inputs, load_generic_golden, make_opt, make_model
+from helpers import (DECODE_CASES, HEAD_LAYOUTS, HOST_CASES, decode_inputs, host_case_inputs, load_generic_golden,
+                     load_head_layout_golden, make_opt, make_model)
 
 
 @pytest.mark.parametrize('cfg', ['coco_tracking', 'mot', 'nuscenes_ddd', 'coco_pose', 'coco_tracking_conv',
@@ -372,6 +373,23 @@ def test_generic_arch_oracle_and_product_keys_match_reference_golden(tag, extra,
     name = k[len(tag + '.stage.'):]
     key = 'feat' if name == 'ida_up.node_2' else name
     assert np.abs(trace[key].numpy() - g[k]).max() < 1e-3 * max(1.0, np.abs(g[k]).max()), name
+
+
+@pytest.mark.parametrize('layout', HEAD_LAYOUTS, ids=[r[0] for r in HEAD_LAYOUTS])
+def test_oracle_head_layouts_match_reference_golden(layout, golden_dir):
+  """The head layouts of --num_classes, --head_conv, --num_head_conv, --head_kernel and the optional heads
+  (tests/helpers.py::HEAD_LAYOUTS): the product module's state-dict keys are the reference's, and the oracle's head()
+  reproduces the reference's head outputs."""
+  g = load_head_layout_golden(golden_dir)
+  tag, cfg, extra, _ = layout
+  opt, model, sd = make_model(cfg, extra=extra)
+  assert sorted(sd.keys()) == sorted(list(g['trunk.keys']) + list(g[tag + '.keys']))
+  img, pre, hm = wt.synthetic_inputs(1, 64, 96)
+  out = co.DLA34Oracle(sd, opt.heads).forward(img, pre, hm)
+  assert sorted(out) == sorted(k.split('.', 2)[2] for k in g.files if k.startswith(tag + '.head.'))
+  for k in out:
+    ref = g['%s.head.%s' % (tag, k)]
+    assert out[k].shape == ref.shape and np.abs(out[k].numpy() - ref).max() < 1e-3, k
 
 
 def test_generic_arch_is_the_dla34_graph_under_other_names(golden_dir):

@@ -644,6 +644,17 @@ __device__ __forceinline__ float normalize_u8(int v, float mean, float stdv) {
   return (float)(((double)v / 255.0 - (double)mean) / (double)stdv);
 }
 
+// One fp32 CHW output pixel (x, y) of ct_warp_affine_normalize: o points at channel 0, planes `plane` floats apart.
+__device__ __forceinline__ void warp_norm_pixel(const unsigned char* __restrict__ img, int sh, int sw, int sstep,
+                                                const double* M, int x, int y, float* o, size_t plane, float3 mean,
+                                                float3 stdv) {
+  int p8[3];
+  warp_bilinear_u8(img, sh, sw, sstep, M, x, y, p8);
+  o[0] = normalize_u8(p8[0], mean.x, stdv.x);
+  o[plane] = normalize_u8(p8[1], mean.y, stdv.y);
+  o[2 * plane] = normalize_u8(p8[2], mean.z, stdv.z);
+}
+
 __global__ void warp_affine_norm_kernel(const unsigned char* __restrict__ src, int sh, int sw, int sstep,
                                         float* __restrict__ dst, int B, int oh, int ow,
                                         const double* __restrict__ minv /*[B][6] dst->src*/, float3 mean, float3 stdv) {
@@ -652,44 +663,93 @@ __global__ void warp_affine_norm_kernel(const unsigned char* __restrict__ src, i
     const int b = (int)(i / ((size_t)oh * ow));
     const size_t r = i - (size_t)b * oh * ow;
     const int y = (int)(r / ow), x = (int)(r - (size_t)y * ow);
-    int p8[3];
-    warp_bilinear_u8(src + (size_t)b * sh * sstep, sh, sw, sstep, minv + b * 6, x, y, p8);
     const size_t plane = (size_t)oh * ow;
-    float* o = dst + (size_t)b * 3 * plane + (size_t)y * ow + x;
-    o[0] = normalize_u8(p8[0], mean.x, stdv.x);
-    o[plane] = normalize_u8(p8[1], mean.y, stdv.y);
-    o[2 * plane] = normalize_u8(p8[2], mean.z, stdv.z);
+    warp_norm_pixel(src + (size_t)b * sh * sstep, sh, sw, sstep, minv + b * 6, x, y,
+                    dst + (size_t)b * 3 * plane + (size_t)y * ow + x, plane, mean, stdv);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Where a frames kernel finds stream b's ct_frame.  ParamFrames: in the kernel parameters, CT_FRAMES_PER_LAUNCH per
+// launch (a captured graph keeps them by value).  DeviceFrames: a device array [B] that may change between graph
+// replays; each CTA copies its stream's descriptor to shared memory once and checks it against the buffer size, since
+// the host cannot: an invalid one yields zeros and no read of the frame buffers.
+// ------------------------------------------------------------------------------------------------------------------
+struct ParamFrames {
+  ct_frame f[CT_FRAMES_PER_LAUNCH];
+};
+
+struct DeviceFrames {
+  const ct_frame* f;
+  long long buf_bytes;
+};
+
+__device__ __forceinline__ bool frame_in_buffer(const ct_frame& f, long long buf_bytes) {
+  return f.h > 0 && f.w > 0 && f.offset >= 0 && (long long)f.step >= 3LL * f.w &&
+         f.offset <= buf_bytes && (long long)(f.h - 1) * f.step + 3LL * f.w <= buf_bytes - f.offset;
+}
+
+// -> this CTA's descriptor (stream b0 + blockIdx.y) and whether it may be read; ends with __syncthreads()
+__device__ __forceinline__ const ct_frame& cta_frame(const ParamFrames& fs, int b0, ct_frame*, bool& ok) {
+  ok = true;
+  __syncthreads();
+  return fs.f[blockIdx.y];
+}
+
+__device__ __forceinline__ const ct_frame& cta_frame(const DeviceFrames& fs, int b0, ct_frame* s_f, bool& ok) {
+  __shared__ int s_ok;
+  if (threadIdx.x == 0) {
+    *s_f = fs.f[b0 + blockIdx.y];
+    s_ok = frame_in_buffer(*s_f, fs.buf_bytes);
+  }
+  __syncthreads();
+  ok = s_ok != 0;
+  return *s_f;
+}
+
+// ct_warp_frames_normalize: blockIdx.y = stream, its image by a grid-stride loop over blockIdx.x
+__global__ void warp_frames_norm_kernel(const unsigned char* __restrict__ src, const __grid_constant__ DeviceFrames fs,
+                                        float* __restrict__ dst, int oh, int ow, float3 mean, float3 stdv) {
+  __shared__ ct_frame s_f;
+  bool ok;
+  const ct_frame& f = cta_frame(fs, 0, &s_f, ok);
+  const size_t plane = (size_t)oh * ow;
+  float* o = dst + (size_t)blockIdx.y * 3 * plane;
+  for (size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x; r < plane; r += (size_t)gridDim.x * blockDim.x) {
+    const int y = (int)(r / ow), x = (int)(r - (size_t)y * ow);
+    if (ok)
+      warp_norm_pixel(src + f.offset, f.h, f.w, f.step, f.minv, x, y, o + r, plane, mean, stdv);
+    else
+      o[r] = o[r + plane] = o[r + 2 * plane] = 0.f;
   }
 }
 
 // ------------------------------------------------------------------------------------------------------------------
 // ct_pack_stem_frames: the tensor-core stem's input [B,H,W,8] bf16 = (norm(warp(cur_b)) x3, norm(warp(prev_b)) x3,
 // pre_hm, 0) straight from each stream's uint8 frame.  blockIdx.y = stream (its descriptor read once, from the kernel
-// parameters), one 16-byte output pixel per thread and iteration.  The normalisation depends on the 8-bit value only:
-// a 3 x 256 table built per CTA with normalize_u8 gives the same floats without a per-pixel fp64 divide.
+// parameters or, in the _dev forms, from device memory: Frames), one 16-byte output pixel per thread and iteration.
+// The normalisation depends on the 8-bit value only: a 3 x 256 table built per CTA with normalize_u8 gives the same
+// floats without a per-pixel fp64 divide.
 // FLIP (ct_pack_stem_frames_flip): out is [2B,H,W,8] and image B+b is image b mirrored.  The mirrored packed pixel
 // (y, W-1-x) equals the original's (y, x) in all 8 channels (frame, previous frame and pre_hm are all mirrored), so each
 // pixel is warped once and its 16-byte vector stored twice.
 // ------------------------------------------------------------------------------------------------------------------
-struct FramesArgs {
-  ct_frame f[CT_FRAMES_PER_LAUNCH];
-};
-
 constexpr int PACK_THREADS = 256;
 constexpr int PACK_PIX_PER_THREAD = 4;      // pixels per thread: amortises the table build over 1024 pixels per CTA
 
-template <bool FLIP>
+template <bool FLIP, class Frames>
 __global__ void __launch_bounds__(PACK_THREADS)
 pack_stem_frames_kernel(const unsigned char* __restrict__ cur, const unsigned char* __restrict__ prev,
-                        const __grid_constant__ FramesArgs fa, int b0, int B, float3 mean, float3 stdv,
+                        const __grid_constant__ Frames fs, int b0, int B, float3 mean, float3 stdv,
                         const float* __restrict__ hm, uint4* __restrict__ out, int H, int W) {
   __shared__ float tab[3][256];
+  __shared__ ct_frame s_f;
   for (int i = threadIdx.x; i < 3 * 256; i += PACK_THREADS) {
     const int c = i >> 8, v = i & 255;
     tab[c][v] = normalize_u8(v, c == 0 ? mean.x : (c == 1 ? mean.y : mean.z), c == 0 ? stdv.x : (c == 1 ? stdv.y : stdv.z));
   }
-  __syncthreads();
-  const ct_frame& f = fa.f[blockIdx.y];
+  bool ok;
+  const ct_frame& f = cta_frame(fs, b0, &s_f, ok);
   const int b = b0 + blockIdx.y;
   const size_t plane = (size_t)H * W;
   const unsigned char* src = cur + f.offset;
@@ -700,24 +760,26 @@ pack_stem_frames_kernel(const unsigned char* __restrict__ cur, const unsigned ch
     const size_t r = base + (size_t)k * PACK_THREADS;
     if (r >= plane) break;
     const int y = (int)(r / W), x = (int)(r - (size_t)y * W);
-    float v[8];
-    int p8[3];
-    warp_bilinear_u8(src, f.h, f.w, f.step, f.minv, x, y, p8);
+    uint4 o = make_uint4(0u, 0u, 0u, 0u);
+    if (ok) {
+      float v[8];
+      int p8[3];
+      warp_bilinear_u8(src, f.h, f.w, f.step, f.minv, x, y, p8);
 #pragma unroll
-    for (int c = 0; c < 3; ++c) v[c] = tab[c][p8[c]];
-    if (psrc) {
-      warp_bilinear_u8(psrc, f.h, f.w, f.step, f.minv, x, y, p8);
+      for (int c = 0; c < 3; ++c) v[c] = tab[c][p8[c]];
+      if (psrc) {
+        warp_bilinear_u8(psrc, f.h, f.w, f.step, f.minv, x, y, p8);
 #pragma unroll
-      for (int c = 0; c < 3; ++c) v[3 + c] = tab[c][p8[c]];
-    } else {
-      v[3] = v[4] = v[5] = 0.f;
+        for (int c = 0; c < 3; ++c) v[3 + c] = tab[c][p8[c]];
+      } else {
+        v[3] = v[4] = v[5] = 0.f;
+      }
+      v[6] = hm ? __ldg(hm + (size_t)b * plane + r) : 0.f;
+      v[7] = 0.f;
+      __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&o);
+#pragma unroll
+      for (int q = 0; q < 4; ++q) h[q] = __floats2bfloat162_rn(v[2 * q], v[2 * q + 1]);
     }
-    v[6] = hm ? __ldg(hm + (size_t)b * plane + r) : 0.f;
-    v[7] = 0.f;
-    uint4 o;
-    __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&o);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) h[q] = __floats2bfloat162_rn(v[2 * q], v[2 * q + 1]);
     out[(size_t)b * plane + r] = o;
     if constexpr (FLIP) out[(size_t)(B + b) * plane + (size_t)y * W + (W - 1 - x)] = o;
   }
@@ -884,11 +946,11 @@ static int pack_stem_frames(const uint8_t* cur, const uint8_t* prev, const ct_fr
   // descriptors travel in the kernel parameters (captured by value in a CUDA graph): CT_FRAMES_PER_LAUNCH per launch
   for (int32_t b0 = 0; b0 < B; b0 += CT_FRAMES_PER_LAUNCH) {
     const int n = B - b0 < CT_FRAMES_PER_LAUNCH ? B - b0 : CT_FRAMES_PER_LAUNCH;
-    FramesArgs fa = {};
+    ParamFrames fa = {};
     memcpy(fa.f, frames + b0, sizeof(ct_frame) * n);
     dim3 grid((unsigned)((plane + per_cta - 1) / per_cta), (unsigned)n);
-    pack_stem_frames_kernel<FLIP><<<grid, PACK_THREADS, 0, (cudaStream_t)stream>>>(cur, prev, fa, b0, B, m, s, pre_hm,
-                                                                                   (uint4*)out, H, W);
+    pack_stem_frames_kernel<FLIP, ParamFrames><<<grid, PACK_THREADS, 0, (cudaStream_t)stream>>>(
+        cur, prev, fa, b0, B, m, s, pre_hm, (uint4*)out, H, W);
     const int rc = after_launch();
     if (rc != CT_OK) return rc;
   }
@@ -905,4 +967,50 @@ extern "C" int ct_pack_stem_frames_flip(const uint8_t* cur, const uint8_t* prev,
                                         const float* mean, const float* std, const float* pre_hm, void* out, int32_t H,
                                         int32_t W, void* stream) {
   return pack_stem_frames<true>(cur, prev, frames, B, mean, std, pre_hm, out, H, W, stream);
+}
+
+template <bool FLIP>
+static int pack_stem_frames_dev(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames_dev, int32_t B,
+                                int64_t buf_bytes, const float* mean, const float* std, const float* pre_hm, void* out,
+                                int32_t H, int32_t W, void* stream) {
+  CT_REQUIRE(cur && frames_dev && mean && std && out, "null pointer");
+  CT_REQUIRE(B > 0 && B <= 65535 && H > 0 && W > 0, "bad shape");
+  CT_REQUIRE(buf_bytes >= 0, "buf_bytes < 0");
+  const size_t plane = (size_t)H * W;
+  const size_t per_cta = (size_t)PACK_THREADS * PACK_PIX_PER_THREAD;
+  CT_REQUIRE((plane + per_cta - 1) / per_cta <= 0x7fffffffu, "output too large");
+  const DeviceFrames fs = {frames_dev, (long long)buf_bytes};
+  dim3 grid((unsigned)((plane + per_cta - 1) / per_cta), (unsigned)B);
+  pack_stem_frames_kernel<FLIP, DeviceFrames><<<grid, PACK_THREADS, 0, (cudaStream_t)stream>>>(
+      cur, prev, fs, 0, B, make_float3(mean[0], mean[1], mean[2]), make_float3(std[0], std[1], std[2]), pre_hm,
+      (uint4*)out, H, W);
+  return after_launch();
+}
+
+extern "C" int ct_pack_stem_frames_dev(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames_dev, int32_t B,
+                                       int64_t buf_bytes, const float* mean, const float* std, const float* pre_hm,
+                                       void* out, int32_t H, int32_t W, void* stream) {
+  return pack_stem_frames_dev<false>(cur, prev, frames_dev, B, buf_bytes, mean, std, pre_hm, out, H, W, stream);
+}
+
+extern "C" int ct_pack_stem_frames_flip_dev(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames_dev,
+                                            int32_t B, int64_t buf_bytes, const float* mean, const float* std,
+                                            const float* pre_hm, void* out, int32_t H, int32_t W, void* stream) {
+  return pack_stem_frames_dev<true>(cur, prev, frames_dev, B, buf_bytes, mean, std, pre_hm, out, H, W, stream);
+}
+
+extern "C" int ct_warp_frames_normalize(const uint8_t* src, const ct_frame* frames_dev, int32_t B, int64_t buf_bytes,
+                                        const float* mean, const float* std, float* dst, int32_t out_h, int32_t out_w,
+                                        void* stream) {
+  CT_REQUIRE(src && frames_dev && mean && std && dst, "null pointer");
+  CT_REQUIRE(B > 0 && B <= 65535 && out_h > 0 && out_w > 0, "bad shape");
+  CT_REQUIRE(buf_bytes >= 0, "buf_bytes < 0");
+  // the same total as ct_warp_affine_normalize's grid-stride launch, split over the B streams
+  const size_t plane = (size_t)out_h * out_w;
+  const size_t cap = ((size_t)device_sm_count() * 16 + B - 1) / B;
+  const size_t nx = (plane + 255) / 256 < cap ? (plane + 255) / 256 : cap;
+  const DeviceFrames fs = {frames_dev, (long long)buf_bytes};
+  warp_frames_norm_kernel<<<dim3((unsigned)nx, (unsigned)B), 256, 0, (cudaStream_t)stream>>>(
+      src, fs, dst, out_h, out_w, make_float3(mean[0], mean[1], mean[2]), make_float3(std[0], std[1], std[2]));
+  return after_launch();
 }

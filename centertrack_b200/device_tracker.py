@@ -102,6 +102,11 @@ def plan_starts(B, T, new_thresh, has_payload, starts, pre_dets):
   return streams, seeds
 
 
+def default_geometry(inp_h, inp_w):
+  """(c, s) of a source image of exactly the network input size: DeviceTracker's default camera geometry."""
+  return np.array([inp_w / 2., inp_h / 2.], np.float32), max(inp_h, inp_w) * 1.0
+
+
 class DeviceTracker(object):
 
   def __init__(self, opt, B, K, rec_floats, layout, inp_h, inp_w, device, centers=None, scales=None, max_tracks=None,
@@ -121,15 +126,9 @@ class DeviceTracker(object):
     self.device = torch.device(device)
     self.T = int(max_tracks or (K * (1 + max(0, int(opt.max_age)))))
     self.T = max(self.T, K)
-    down = getattr(opt, 'down_ratio', 4)
-    out_w, out_h = inp_w // down, inp_h // down
-    t_out = np.zeros((B, 6), np.float32)
-    t_in = np.zeros((B, 6), np.float64)
-    for b in range(B):
-      c = np.array([inp_w / 2., inp_h / 2.], np.float32) if centers is None else np.asarray(centers[b], np.float32)
-      s = max(inp_h, inp_w) * 1.0 if scales is None else scales[b]
-      t_out[b] = get_affine_transform(c, s, 0, (out_w, out_h), inv=1).astype(np.float32).reshape(6)
-      t_in[b] = get_affine_transform(c, s, 0, [inp_w, inp_h]).reshape(6)
+    c0, s0 = default_geometry(inp_h, inp_w)
+    t_in, t_out = self._trans_rows([c0 if centers is None else centers[b] for b in range(B)],
+                                   [s0 if scales is None else scales[b] for b in range(B)])
     self.trans_out_inv = torch.from_numpy(t_out).to(self.device)
     self.trans_input = torch.from_numpy(t_in).to(self.device)
     self.tracks = torch.zeros((B, self.T, L.CT_TRK_FLOATS), dtype=torch.float32, device=self.device)
@@ -182,6 +181,36 @@ class DeviceTracker(object):
       cx, cy = (inp_w / 2., inp_h / 2.) if centers is None else (float(centers[b][0]), float(centers[b][1]))
       out[b] = [[f, 0, cx, 0], [0, f, cy, 0], [0, 0, 1, 0]]      # Detector._get_default_calib(2 cx, 2 cy)
     return out
+
+  def _trans_rows(self, centers, scales):
+    """(c, s) per stream -> (trans_input float64 [n, 6], trans_out_inv float32 [n, 6]) rows."""
+    down = getattr(self.opt, 'down_ratio', 4)
+    out_w, out_h = self.inp_w // down, self.inp_h // down
+    t_out = np.zeros((len(centers), 6), np.float32)
+    t_in = np.zeros((len(centers), 6), np.float64)
+    for i, (c, s) in enumerate(zip(centers, scales)):
+      c = np.asarray(c, np.float32)
+      t_out[i] = get_affine_transform(c, s, 0, (out_w, out_h), inv=1).astype(np.float32).reshape(6)
+      t_in[i] = get_affine_transform(c, s, 0, [self.inp_w, self.inp_h]).reshape(6)
+    return t_in, t_out
+
+  def geometry_rows(self, centers, scales, calibs):
+    """The camera geometry of n streams ((c, s) of their source rectangle and [3,4] camera matrices) -> the rows
+    set_geometry writes: (float64 [n, 6] trans_input, float32 [n, 18] = trans_out_inv (6) then calib (12)), computed
+    exactly as the constructor computes them."""
+    t_in, t_out = self._trans_rows(centers, scales)
+    cal = np.asarray(calibs, np.float32).reshape(len(t_out), 12)
+    return t_in, np.concatenate([t_out, cal], axis=1)
+
+  def set_geometry(self, streams, rows_in, rows_out):
+    """trans_input, trans_out_inv (and calib on 3D head sets) of `streams` <- rows (geometry_rows, device tensors), on
+    the current stream.  The descriptors keep pointing at the same tensors, so captured graphs read the new rows: call
+    it between two steps, before start_device renders the streams' seeds."""
+    for i, b in enumerate(streams):
+      self.trans_input[b].copy_(rows_in[i])
+      self.trans_out_inv[b].copy_(rows_out[i, :6])
+      if self.calib is not None:
+        self.calib[b].view(12).copy_(rows_out[i, 6:])
 
   def reset(self):
     """Detector.reset_tracking / Tracker.reset for every stream."""

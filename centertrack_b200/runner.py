@@ -31,7 +31,9 @@ normalises them on the device exactly as Detector.pre_process_device does (cv2's
 engine ct_pack_stem_frames writes the stem's packed bf16 input straight from slot t (images) and slot t-1 (pre_images,
 warped again: no fp32 copy is kept); the fp32 and bf16x3 engines warp each stream into the fp32 image slot with
 ct_warp_affine_normalize and run their plan unchanged.  The tracker gets each stream's (c, s) and default calib, so
-tracks, public detections and 3D boxes are in that camera's pixels.
+tracks, public detections and 3D boxes are in that camera's pixels.  With max_frame_size, stream b's frame lives at
+b * cap in every slot and each slot's descriptors are a device array (ct_pack_stem_frames_dev, ct_warp_frames_normalize),
+so a stream may take a frame of another size, and a new camera, when it starts a video, without recapturing a graph.
 
 Video starts (`starts=`, `pre_dets=` of step_host / step_frames / load_device_inputs): a stream may begin a new video at
 any step, as Detector.reset_tracking + Tracker.init_track(pre_dets) on that stream alone.  A start is rare (once per
@@ -56,7 +58,7 @@ from . import _lib as L
 from .dataset_info import get_dataset
 from .decode import generic_decode
 from .detector import default_calib, flip_output, flip_plan, frame_geometry
-from .device_tracker import DeviceTracker, plan_starts
+from .device_tracker import DeviceTracker, default_geometry, plan_starts
 
 
 NS = 3          # input slots
@@ -65,21 +67,27 @@ NS = 3          # input slots
 class StreamRunner(object):
 
   def __init__(self, model, B, H, W, K=100, precision='bf16', device='cuda', use_graph=True, opt=None,
-               device_tracking=False, max_public_dets=512, calibs=None, frame_sizes=None):
+               device_tracking=False, max_public_dets=512, calibs=None, frame_sizes=None, max_frame_size=None):
     """max_public_dets: with device_tracking and --public_det, the most public detections a stream may bring per
     frame (more raise ValueError; none is ever dropped).  calibs: with device_tracking on a 3D head set, one [3,4]
     camera matrix per stream (DeviceTracker's default otherwise; in frames mode Detector._get_default_calib of the
-    stream's source size).  frame_sizes: B (height, width) source sizes, fixed for the runner's lifetime, to feed raw
-    uint8 frames with step_frames; each must map to the network input (H, W) under opt's resolution policy
-    (ValueError otherwise).  opt.flip_test: every stream's frame runs with its mirror (2B images per step) and the
-    averaged heads are merged before decode, as Detector.process does; inputs and outputs keep their B shapes."""
+    stream's source size).  frame_sizes: B (height, width) source sizes to feed raw uint8 frames with step_frames; each
+    must map to the network input (H, W) under opt's resolution policy (ValueError otherwise).  Without
+    max_frame_size they are fixed for the runner's lifetime.  max_frame_size (h, w): every stream gets a frame region
+    of h * w * 3 bytes in each slot, and may bring a frame of any size that fits it and maps to (H, W) when it starts
+    a video (frame_sizes are then the first sizes); the descriptors of the frames live on the device.
+    opt.flip_test: every stream's frame runs with its mirror (2B images per step) and the averaged heads are merged
+    before decode, as Detector.process does; inputs and outputs keep their B shapes."""
     self.B, self.H, self.W, self.K = B, H, W, K
     self.device = torch.device(device)
     self.model = model
     self.opt = opt if opt is not None else getattr(model, 'opt', None)
     self.frames_mode = frame_sizes is not None
+    if max_frame_size is not None and not self.frames_mode:
+      raise ValueError('max_frame_size needs frame_sizes (frames mode)')
+    self.cap = self.max_frame_bytes = None
     if self.frames_mode:
-      calibs = self._frame_geometry(frame_sizes, calibs)
+      calibs = self._frame_geometry(frame_sizes, calibs, max_frame_size)
     self.flip = bool(getattr(self.opt, 'flip_test', False))
     NB = 2 * B if self.flip else B                           # --flip_test: frames [0, B), their mirrors [B, 2B)
     self.eng = model.engine_for(NB, H, W, self.device, precision)
@@ -97,7 +105,13 @@ class StreamRunner(object):
     if self.frames_mode:      # frame slots: B uint8 frames at 16-byte aligned offsets, pinned staging + device
       self.u8 = [torch.zeros(self.slot_bytes, dtype=torch.uint8, device=self.device) for _ in range(NS)]
       self.h_u8 = [torch.zeros(self.slot_bytes, dtype=torch.uint8).pin_memory() for _ in range(NS)]
-      self.minv = torch.from_numpy(np.stack([f.minv[:] for f in self.frames])).to(self.device)
+      if self.cap is None:
+        self.minv = torch.from_numpy(np.stack([f.minv[:] for f in self.frames])).to(self.device)
+      else:                  # per slot: the device descriptors of its frames, their pinned staging and a host mirror
+        desc = torch.from_numpy(np.frombuffer(bytes(self.frames), np.uint8).copy())
+        self.h_frames = [desc.clone().pin_memory() for _ in range(NS)]
+        self.d_frames = [desc.to(self.device) for _ in range(NS)]
+        self._desc_mirror = [bytes(self.frames)] * NS
     self.rec = None
     self.layout = None
     self.ws = None                                           # private decode workspace (captured by the graphs)
@@ -113,6 +127,11 @@ class StreamRunner(object):
     self._starts = [None] * NS                               # per slot: the streams whose frame starts a video
     self._start_bytes = 0                                    # start list + seed rows uploaded by the last step
     self.h_start = None                                      # per slot start list / seed staging, made on first use
+    self.h_geo = None                                        # per slot camera geometry rows staging, made on first use
+    self._geo = [None] * NS                                  # per slot: the streams whose geometry rows it carries
+    self._frame_bytes = 0                                    # frame (+ descriptor) bytes of the last upload
+    if self.frames_mode:
+      self._frame_bytes = self.slot_bytes if self.cap is None else sum(e - a for a, e in self._upload_runs())
     self._eager(0, first=True)                               # sizes the record buffer
     if device_tracking:
       assert self.opt is not None, 'device tracking needs opt (thresholds, max_age)'
@@ -136,12 +155,14 @@ class StreamRunner(object):
     # becomes ct_pack_stem_frames (one launch per CT_FRAMES_PER_LAUNCH streams), or B warps come before the plan.
     # --flip_test: + the merge, + the mirrors of the images and pre_hm unless the flip pack writes them
     self.launches_per_step = self.eng.n_launches + 1 + (2 if device_tracking else 0)
-    if self.frames_mode:
+    if self.frames_mode and self.cap is not None:           # device descriptors: one pack or one warp for all B
+      self.launches_per_step += 0 if self.eng.use_halo else 1
+    elif self.frames_mode:
       self.launches_per_step += (-(-B // L.CT_FRAMES_PER_LAUNCH) - 1) if self.eng.use_halo else B
     if self.flip:
       self.launches_per_step += 1 + (0 if self._pack_mirror else 1 + int(self.eng.has_pre_hm))
 
-  def _frame_geometry(self, frame_sizes, calibs):
+  def _frame_geometry(self, frame_sizes, calibs, max_frame_size=None):
     """Per-stream geometry of frames mode (Detector.pre_process_device's, through detector.frame_geometry): the
     ct_frame descriptors, the metas, the slot size.  -> the tracker's calibs."""
     opt, B = self.opt, self.B
@@ -153,8 +174,15 @@ class StreamRunner(object):
       calibs = np.asarray(calibs, np.float32)
       if calibs.shape != (B, 3, 4):
         raise ValueError('calibs: expected %d camera matrices [3, 4], got shape %s' % (B, calibs.shape))
+    self.cap = self.max_frame_bytes = None
+    if max_frame_size is not None:
+      mh, mw = (int(v) for v in max_frame_size)
+      if mh <= 0 or mw <= 0:
+        raise ValueError('max_frame_size: bad size %s' % ((mh, mw),))
+      self.max_frame_bytes = mh * mw * 3
+      self.cap = (self.max_frame_bytes + 15) // 16 * 16        # stream b's frame lives at b * cap in every slot
     ds = get_dataset(opt.dataset)
-    focal = opt.test_focal_length if getattr(opt, 'test_focal_length', -1) >= 0 else ds.rest_focal_length
+    self.focal = opt.test_focal_length if getattr(opt, 'test_focal_length', -1) >= 0 else ds.rest_focal_length
     self.mean = np.ascontiguousarray(ds.mean, dtype=np.float32).reshape(3)
     self.std = np.ascontiguousarray(ds.std, dtype=np.float32).reshape(3)
     self.frames = (L.Frame * B)()
@@ -162,28 +190,129 @@ class StreamRunner(object):
     off = 0
     for b, (h, w) in enumerate(frame_sizes):
       h, w = int(h), int(w)
-      if h <= 0 or w <= 0:
-        raise ValueError('frame_sizes[%d]: bad size %s' % (b, (h, w)))
-      meta, minv = frame_geometry(opt, h, w)
-      if (meta['inp_height'], meta['inp_width']) != (self.H, self.W):
-        raise ValueError('frame_sizes[%d] = %s maps to a %dx%d network input under this resolution policy, not the '
-                         "runner's %dx%d" % (b, (h, w), meta['inp_height'], meta['inp_width'], self.H, self.W))
-      meta['calib'] = calibs[b] if calibs is not None else default_calib(focal, w, h)
+      meta, minv = self._size_geometry('frame_sizes[%d]' % b, h, w)
+      meta['calib'] = calibs[b] if calibs is not None else default_calib(self.focal, w, h)
       self._meta.append(meta)
       f = self.frames[b]
-      f.offset, f.h, f.w, f.step = off, h, w, 3 * w
+      f.offset, f.h, f.w, f.step = (off if self.cap is None else b * self.cap), h, w, 3 * w
       f.minv[:] = minv.tolist()
       off += (h * w * 3 + 15) // 16 * 16
+    self._prev_meta = self._meta
     self.frame_sizes = [(int(h), int(w)) for h, w in frame_sizes]
-    self.slot_bytes = off
+    self.slot_bytes = off if self.cap is None else B * self.cap
     return calibs if calibs is not None else np.stack([m['calib'] for m in self._meta]).astype(np.float32)
 
+  def _size_geometry(self, what, h, w):
+    """(meta without calib, minv) of an h x w source frame; ValueError when it is empty, does not fit a capacity
+    runner's frame region, or maps to another network input than (H, W)."""
+    if h <= 0 or w <= 0:
+      raise ValueError('%s: bad size %s' % (what, (h, w)))
+    if self.cap is not None and h * w * 3 > self.max_frame_bytes:
+      raise ValueError('%s = %s: %d bytes, more than the %d of max_frame_size' % (what, (h, w), h * w * 3,
+                                                                                 self.max_frame_bytes))
+    meta, minv = frame_geometry(self.opt, h, w)
+    if (meta['inp_height'], meta['inp_width']) != (self.H, self.W):
+      raise ValueError('%s = %s maps to a %dx%d network input under this resolution policy, not the '
+                       "runner's %dx%d" % (what, (h, w), meta['inp_height'], meta['inp_width'], self.H, self.W))
+    return meta, minv
+
+  def check_frame_size(self, size):
+    """ValueError unless a stream of this runner can take frames of size (height, width) at a video start."""
+    h, w = (int(v) for v in size)
+    if self.cap is None:
+      if (h, w) not in self.frame_sizes:
+        raise ValueError('frame size %s: the streams take %s' % ((h, w), sorted(set(self.frame_sizes))))
+      return
+    self._size_geometry('frame size', h, w)
+
   def meta(self, b):
-    """Frames mode: the meta dict Detector.pre_process returns for stream b's frames (c, s, sizes, trans_input,
-    trans_output, calib) -- what generic_post_process needs when the records are post-processed on the host."""
+    """Frames mode: the meta dict Detector.pre_process returns for stream b's frame in the last submitted step (c, s,
+    sizes, trans_input, trans_output, calib) -- what generic_post_process needs when the records are post-processed on
+    the host."""
     if not self.frames_mode:
       raise ValueError('meta(): the runner was not built with frame_sizes')
     return {k: (v.copy() if isinstance(v, np.ndarray) else v) for k, v in self._meta[b].items()}
+
+  def previous_meta(self, b):
+    """Frames mode: meta(b) of the step whose records the last step_frames call returned (the step before the last
+    submitted one), for generic_post_process of those records; as previous_results() is to fetch_results()."""
+    if not self.frames_mode:
+      raise ValueError('previous_meta(): the runner was not built with frame_sizes')
+    return {k: (v.copy() if isinstance(v, np.ndarray) else v) for k, v in self._prev_meta[b].items()}
+
+  def _check_calibs(self, calibs, streams):
+    """calibs ({stream: [3, 4]} of started streams) -> {stream: float32 [3, 4]}; ValueError before anything is
+    enqueued."""
+    out = {}
+    for s, k in (calibs or {}).items():
+      if s not in streams:
+        raise ValueError('calibs: stream %r does not start a video in this step' % (s,))
+      k = np.asarray(k, np.float32)
+      if k.shape != (3, 4):
+        raise ValueError('calibs[%d]: expected a [3, 4] camera matrix, got shape %s' % (s, k.shape))
+      out[s] = k
+    return out
+
+  def _check_sizes(self, sizes, streams):
+    """This step's (h, w) per stream -> {stream: (meta without calib, minv)} of the streams whose size changes.
+    ValueError (before anything is enqueued) for a change on a fixed-size runner or on a stream that does not start a
+    video (its pre_hm boxes were rendered with its old trans_input), or a size _size_geometry refuses."""
+    changed = {}
+    for b, (hw, now) in enumerate(zip(sizes, self.frame_sizes)):
+      if tuple(hw) == tuple(now):
+        continue
+      if self.cap is None:
+        raise ValueError('frames[%d]: expected shape %s, got %s' % (b, tuple(now) + (3,), tuple(hw) + (3,)))
+      if b not in streams:
+        raise ValueError('frames[%d]: size %s differs from the stream\'s %s; a stream changes its frame size only when '
+                         'it starts a video (starts=)' % (b, tuple(hw), tuple(now)))
+      changed[b] = self._size_geometry('frames[%d]' % b, int(hw[0]), int(hw[1]))
+    return changed
+
+  def _plan_geometry(self, slot, changed, calibs):
+    """Host state of one step's geometry changes (changed: _check_sizes, calibs: _check_calibs): the descriptors and
+    metas of the changed streams, the slot's descriptor staging when its device copy differs, and the tracker rows of
+    the streams whose camera changes.  -> (descriptor bytes to upload or None, [(stream, c, s, calib)])."""
+    rows = []
+    if self.frames_mode:
+      self._prev_meta = self._meta
+      if changed or calibs:
+        self._meta = list(self._meta)
+      for b, (meta, minv) in changed.items():
+        h, w = meta['height'], meta['width']
+        f = self.frames[b]
+        f.h, f.w, f.step = h, w, 3 * w
+        f.minv[:] = minv.tolist()
+        meta['calib'] = calibs[b] if b in calibs else default_calib(self.focal, w, h)
+        self._meta[b] = meta
+        self.frame_sizes[b] = (h, w)
+      for b, k in calibs.items():
+        if b not in changed:
+          self._meta[b] = dict(self._meta[b], calib=k)
+      for b in sorted(set(changed) | set(calibs)):
+        m = self._meta[b]
+        rows.append((b, m['c'], m['s'], np.asarray(m['calib'], np.float32)))
+    elif self.tracker is not None:           # fp32 images of the input size: the tracker's default (c, s) throughout
+      c, s = default_geometry(self.H, self.W)
+      rows = [(b, c, s, k) for b, k in sorted(calibs.items())]
+    desc = None
+    if self.cap is not None:
+      now = bytes(self.frames)
+      if now != self._desc_mirror[slot]:
+        desc = self._desc_mirror[slot] = now
+    return desc, rows
+
+  def _upload_runs(self):
+    """Maximal runs [start, end) of the slot bytes this step's frames use: stream b's frame, padded to 16 bytes, at
+    b * cap.  One run of slot_bytes when every stream is at capacity."""
+    runs = []
+    for b, f in enumerate(self.frames):
+      a, e = b * self.cap, b * self.cap + (f.h * f.w * 3 + 15) // 16 * 16
+      if runs and runs[-1][1] == a:
+        runs[-1][1] = e
+      else:
+        runs.append([a, e])
+    return [tuple(r) for r in runs]
 
   # one step, eager launches on the current stream
   def _eager(self, slot, first=False):
@@ -192,12 +321,15 @@ class StreamRunner(object):
     prev = slot if first else (slot - 1) % NS
     if self.frames_mode and self.eng.use_halo:
       eng = self.eng
-      pack = L.lib().ct_pack_stem_frames_flip if self.flip else L.lib().ct_pack_stem_frames
-      L.check(pack(
-          L.ptr(self.u8[slot]), L.ptr(self.u8[prev] if eng.has_pre_img else None), self.frames, self.B,
-          C.c_void_p(self.mean.ctypes.data), C.c_void_p(self.std.ctypes.data),
-          L.ptr(self.hm[slot] if eng.has_pre_hm else None), L.ptr(eng.stem_input), self.H, self.W, L.stream_ptr()),
-          'ct_pack_stem_frames')
+      cur, pre = L.ptr(self.u8[slot]), L.ptr(self.u8[prev] if eng.has_pre_img else None)
+      ms = (C.c_void_p(self.mean.ctypes.data), C.c_void_p(self.std.ctypes.data),
+            L.ptr(self.hm[slot] if eng.has_pre_hm else None), L.ptr(eng.stem_input), self.H, self.W, L.stream_ptr())
+      if self.cap is None:
+        pack = L.lib().ct_pack_stem_frames_flip if self.flip else L.lib().ct_pack_stem_frames
+        L.check(pack(cur, pre, self.frames, self.B, *ms), 'ct_pack_stem_frames')
+      else:                  # the slot's device descriptors: a replayed graph reads the geometry the slot holds
+        pack = L.lib().ct_pack_stem_frames_flip_dev if self.flip else L.lib().ct_pack_stem_frames_dev
+        L.check(pack(cur, pre, L.ptr(self.d_frames[slot]), self.B, self.slot_bytes, *ms), 'ct_pack_stem_frames_dev')
       out = dict(eng.forward_packed(eng.has_pre_img, eng.has_pre_hm))
     else:
       if self.frames_mode:
@@ -227,9 +359,15 @@ class StreamRunner(object):
     L.check(L.lib().ct_mirror_x(L.ptr(x[b]), L.ptr(x[self.B + b]), n, c, h, w, L.stream_ptr()), 'ct_mirror_x')
 
   def _warp_frames(self, slot):
-    """fp32 and bf16x3 engines: the slot's frames -> its fp32 image, one ct_warp_affine_normalize per stream."""
+    """fp32 and bf16x3 engines: the slot's frames -> its fp32 image, one ct_warp_affine_normalize per stream (one
+    ct_warp_frames_normalize for all of them from the device descriptors on a capacity runner)."""
     lib, st = L.lib(), L.stream_ptr()
     src, dst = self.u8[slot].data_ptr(), self.img[slot]
+    if self.cap is not None:
+      L.check(lib.ct_warp_frames_normalize(C.c_void_p(src), L.ptr(self.d_frames[slot]), self.B, self.slot_bytes,
+                                           C.c_void_p(self.mean.ctypes.data), C.c_void_p(self.std.ctypes.data),
+                                           L.ptr(dst), self.H, self.W, st), 'ct_warp_frames_normalize')
+      return
     for b, f in enumerate(self.frames):
       L.check(lib.ct_warp_affine_normalize(C.c_void_p(src + f.offset), 1, f.h, f.w, f.step, L.ptr(self.minv[b]),
                                            C.c_void_p(self.mean.ctypes.data), C.c_void_p(self.std.ctypes.data),
@@ -352,10 +490,32 @@ class StreamRunner(object):
       self.d_seed[slot][:n].copy_(self.h_seed[slot][:n], non_blocking=non_blocking)
     return e * 8 + n * L.CT_TRK_FLOATS * 4
 
-  def load_device_inputs(self, images, pre_hms, slot, public_dets=None, starts=None, pre_dets=None):
-    """Copies step_device's inputs into `slot` on the current stream; starts / pre_dets as in step_host."""
+  def _upload_geometry(self, slot, rows, non_blocking):
+    """Stages and uploads the tracker geometry rows of the streams whose camera changes in this step (_plan_geometry)
+    for slot's start prologue (the current stream is the upload's); -> the bytes uploaded."""
+    self._geo[slot] = None
+    if not rows or self.tracker is None:
+      return 0
+    if self.h_geo is None:
+      self.h_geo = [(torch.zeros((self.B, 6), dtype=torch.float64).pin_memory(),
+                     torch.zeros((self.B, 18), dtype=torch.float32).pin_memory()) for _ in range(NS)]
+      self.d_geo_in = [torch.zeros((self.B, 6), dtype=torch.float64, device=self.device) for _ in range(NS)]
+      self.d_geo_out = [torch.zeros((self.B, 18), dtype=torch.float32, device=self.device) for _ in range(NS)]
+    streams, cs, ss, ks = zip(*rows)
+    t_in, t_out = self.tracker.geometry_rows(cs, ss, ks)
+    n = len(streams)
+    h_in, h_out = self.h_geo[slot]
+    h_in[:n], h_out[:n] = torch.from_numpy(t_in), torch.from_numpy(t_out)
+    self.d_geo_in[slot][:n].copy_(h_in[:n], non_blocking=non_blocking)
+    self.d_geo_out[slot][:n].copy_(h_out[:n], non_blocking=non_blocking)
+    self._geo[slot] = list(streams)
+    return n * (6 * 8 + 18 * 4)
+
+  def load_device_inputs(self, images, pre_hms, slot, public_dets=None, starts=None, pre_dets=None, calibs=None):
+    """Copies step_device's inputs into `slot` on the current stream; starts / pre_dets / calibs as in step_host."""
     pub = self._check_public(public_dets)
     plan = self._check_starts(starts, pre_dets)
+    cal = self._check_calibs(calibs, plan[0] if plan else ())
     self.img[slot][:self.B].copy_(images)
     if pre_hms is not None:
       self.hm[slot][:self.B].copy_(pre_hms)
@@ -363,7 +523,9 @@ class StreamRunner(object):
       self._fill_public(self.h_pub[slot], pub)
       self.pub[slot][0].copy_(self.h_pub[slot][0])
       self.pub[slot][1].copy_(self.h_pub[slot][1])
-    self._start_bytes = self._upload_starts(slot, plan, non_blocking=False)
+    _, rows = self._plan_geometry(slot, {}, cal)
+    self._start_bytes = self._upload_starts(slot, plan, non_blocking=False) + \
+        self._upload_geometry(slot, rows, non_blocking=False)
 
   def _start_prologue(self, slot, streams):
     """A step whose frames start new videos on `streams`, before the step itself (graph replay or eager), on the same
@@ -381,14 +543,20 @@ class StreamRunner(object):
           continue
         if self.frames_mode:                                 # the plan reads img[prev]: warp this frame into it
           f = self.frames[b]
+          # a capacity runner's minv: the slot's device descriptor of this frame (its new geometry after a size change)
+          minv = L.ptr(self.minv[b]) if self.cap is None else \
+              C.c_void_p(self.d_frames[slot].data_ptr() + b * C.sizeof(L.Frame) + L.Frame.minv.offset)
           L.check(L.lib().ct_warp_affine_normalize(
-              C.c_void_p(self.u8[slot].data_ptr() + f.offset), 1, f.h, f.w, f.step, L.ptr(self.minv[b]),
+              C.c_void_p(self.u8[slot].data_ptr() + f.offset), 1, f.h, f.w, f.step, minv,
               C.c_void_p(self.mean.ctypes.data), C.c_void_p(self.std.ctypes.data), L.ptr(self.img[prev][b]), self.H,
               self.W, L.stream_ptr()), 'ct_warp_affine_normalize')
         else:
           self.img[prev][b].copy_(self.img[slot][b])
         if self.flip:                                        # --flip_test: pre_images is the (frame, mirror) pair
           self._mirror(self.img[prev], b, 1)
+    geo, self._geo[slot] = self._geo[slot], None
+    if self.tracker is not None and geo:                     # new cameras: before the seeds' boxes are rendered
+      self.tracker.set_geometry(geo, self.d_geo_in[slot], self.d_geo_out[slot])
     if self.tracker is not None:                             # reset + seeds + boxes: the step's render splats them
       self.tracker.start_device(self.d_start[slot], len(streams), self.d_seed[slot])
 
@@ -410,17 +578,21 @@ class StreamRunner(object):
     self.t += 1
     return self.rec
 
-  def step_host(self, images, pre_hms=None, public_dets=None, starts=None, pre_dets=None):
+  def step_host(self, images, pre_hms=None, public_dets=None, starts=None, pre_dets=None, calibs=None):
     """images [B,3,H,W] (and pre_hms [B,1,H,W] unless device_tracking): float32 HOST tensors (what
     Detector.pre_process / _get_additional_inputs produce); with --public_det, public_dets = B arrays [P_b, 2] (the
     `ct`s of each frame's public detections).  starts: the streams whose frame in this step is a new video's first
     (Detector.reset_tracking on those streams alone: the frame is its own pre_images and the stream's tracker restarts
     empty, or from pre_dets = {stream: list of result dicts} as Tracker.init_track; the other streams are unaffected).
+    calibs: {stream: [3, 4] camera matrix} of some started streams, their camera from this frame on (3D head sets:
+    loc, rot_y); a started stream without one keeps its camera.
     Returns the records of the PREVIOUS call (None the first time) -- a one-step software pipeline: this step's H2D
     overlaps the previous step's compute."""
     pub = self._check_public(public_dets)
     plan = self._check_starts(starts, pre_dets)
+    cal = self._check_calibs(calibs, plan[0] if plan else ())
     slot = self.t % NS
+    _, rows = self._plan_geometry(slot, {}, cal)
     if pub is not None:        # the slot's staging was last read by step t-3's upload, which the last fetch() waited for
       self._fill_public(self.h_pub[slot], pub)
     use_hm = self.tracker is None and pre_hms is not None
@@ -439,7 +611,8 @@ class StreamRunner(object):
       if pub is not None:
         self.pub[slot][0].copy_(self.h_pub[slot][0], non_blocking=True)
         self.pub[slot][1].copy_(self.h_pub[slot][1], non_blocking=True)
-      self._start_bytes = self._upload_starts(slot, plan, non_blocking=True)
+      self._start_bytes = self._upload_starts(slot, plan, non_blocking=True) + \
+          self._upload_geometry(slot, rows, non_blocking=True)
       self.ev_in[slot].record(self.copy)
     return self._submit(slot)
 
@@ -461,38 +634,75 @@ class StreamRunner(object):
     self.t += 1
     return prev
 
-  def frame_buffers(self):
+  def frame_buffers(self, sizes=None):
     """Frames mode: numpy views [h_b, w_b, 3] uint8 of the pinned staging the NEXT step_frames uploads, one per stream,
     for a decoder to write its frames in place; then call step_frames(None).  They may be written once the previous
     step_frames call has returned (its upload of three steps ago, which last read this staging, has completed by
-    then) and until the next step_frames call."""
+    then) and until the next step_frames call.  sizes ({stream: (h, w)}, capacity runners): the views of those streams
+    at a new size, for frames that start a video; the next step_frames(None, starts=...) must start them."""
     if not self.frames_mode:
       raise ValueError('frame_buffers(): the runner was not built with frame_sizes')
-    buf = self.h_u8[self.t % NS].numpy()
-    return [buf[f.offset:f.offset + f.h * f.w * 3].reshape(f.h, f.w, 3) for f in self.frames]
+    now = list(self.frame_sizes)
+    for b, hw in (sizes or {}).items():
+      if not 0 <= b < self.B:
+        raise ValueError('sizes: stream %r out of range [0, %d)' % (b, self.B))
+      hw = (int(hw[0]), int(hw[1]))
+      if hw != now[b]:
+        if self.cap is None:
+          raise ValueError('sizes[%d]: the frame sizes of a runner built without max_frame_size are fixed' % b)
+        self._size_geometry('sizes[%d]' % b, *hw)
+      now[b] = hw
+    self._pending_sizes = now
+    return self._views(self.t % NS, now)
 
-  def step_frames(self, frames, pre_hms=None, public_dets=None, starts=None, pre_dets=None):
+  def _views(self, slot, sizes):
+    buf = self.h_u8[slot].numpy()
+    return [buf[f.offset:f.offset + h * w * 3].reshape(h, w, 3) for f, (h, w) in zip(self.frames, sizes)]
+
+  def _frame_sizes_of(self, frames):
+    """This step's (h, w) per stream: the shapes of `frames`, or the sizes of the last frame_buffers() call when None.
+    ValueError on a wrong count or dtype, or a shape that is not [h, w, 3]."""
+    if frames is None:
+      return list(getattr(self, '_pending_sizes', None) or self.frame_sizes)
+    if len(frames) != self.B:
+      raise ValueError('frames: expected %d arrays (one per stream), got %d' % (self.B, len(frames)))
+    sizes = []
+    for b, (a, (h, w)) in enumerate(zip(frames, self.frame_sizes)):
+      if not isinstance(a, np.ndarray) or a.dtype != np.uint8:
+        raise ValueError('frames[%d]: expected a uint8 numpy array, got %s' %
+                         (b, getattr(a, 'dtype', type(a).__name__)))
+      if self.cap is None and a.shape != (h, w, 3):
+        raise ValueError('frames[%d]: expected shape %s, got %s' % (b, (h, w, 3), a.shape))
+      if a.ndim != 3 or a.shape[2] != 3:
+        raise ValueError('frames[%d]: expected shape [h, w, 3], got %s' % (b, a.shape))
+      sizes.append(a.shape[:2])
+    return sizes
+
+  def step_frames(self, frames, pre_hms=None, public_dets=None, starts=None, pre_dets=None, calibs=None):
     """frames: B uint8 [h_b, w_b, 3] BGR arrays of the sizes given as frame_sizes, or None when they were written
-    through frame_buffers().  pre_hms, public_dets, starts, pre_dets and the return value as in step_host; public
-    detections and pre_dets are in each stream's source pixels, and so are the tracks.  ValueError on a wrong count,
-    dtype or shape, or when the runner was not built with frame_sizes."""
+    through frame_buffers().  pre_hms, public_dets, starts, pre_dets, calibs and the return value as in step_host;
+    public detections and pre_dets are in each stream's source pixels, and so are the tracks.  On a runner built with
+    max_frame_size, a stream in `starts` may bring a frame of another size (that fits the region and maps to (H, W));
+    without a calibs entry it then gets Detector._get_default_calib of that size.  ValueError (before anything is
+    enqueued) on a wrong count, dtype or shape, a size change that is not allowed, or when the runner was not built
+    with frame_sizes."""
     if not self.frames_mode:
       raise ValueError('step_frames: the runner was not built with frame_sizes (use step_host)')
     pub = self._check_public(public_dets)
     plan = self._check_starts(starts, pre_dets)
+    started = plan[0] if plan else ()
+    cal = self._check_calibs(calibs, started)
+    sizes = self._frame_sizes_of(frames)
+    changed = self._check_sizes(sizes, started)
     slot = self.t % NS
+    self._pending_sizes = None
+    desc, rows = self._plan_geometry(slot, changed, cal)
     if frames is not None:
-      if len(frames) != self.B:
-        raise ValueError('frames: expected %d arrays (one per stream), got %d' % (self.B, len(frames)))
-      for b, (a, (h, w)) in enumerate(zip(frames, self.frame_sizes)):
-        if not isinstance(a, np.ndarray) or a.dtype != np.uint8:
-          raise ValueError('frames[%d]: expected a uint8 numpy array, got %s' %
-                           (b, getattr(a, 'dtype', type(a).__name__)))
-        if a.shape != (h, w, 3):
-          raise ValueError('frames[%d]: expected shape %s, got %s' % (b, (h, w, 3), a.shape))
       # the slot's staging was last read by step t-3's upload, which the last fetch() waited for
-      for a, v in zip(frames, self.frame_buffers()):
+      for a, v in zip(frames, self._views(slot, self.frame_sizes)):
         np.copyto(v, a)
+    if desc is not None:
+      self.h_frames[slot].numpy()[:] = np.frombuffer(desc, np.uint8)
     if pub is not None:
       self._fill_public(self.h_pub[slot], pub)
     use_hm = self.tracker is None and pre_hms is not None
@@ -502,13 +712,23 @@ class StreamRunner(object):
       src_hm = self.h_hm[slot]
     with torch.cuda.stream(self.copy):
       self.copy.wait_event(self.ev_done[slot])       # slot's old contents were last read as pre_images of step t-2
-      self.u8[slot].copy_(self.h_u8[slot], non_blocking=True)
+      if self.cap is None:
+        self.u8[slot].copy_(self.h_u8[slot], non_blocking=True)
+      else:                                          # the used bytes only, and the descriptors when they changed
+        self._frame_bytes = 0
+        for a, e in self._upload_runs():
+          self.u8[slot][a:e].copy_(self.h_u8[slot][a:e], non_blocking=True)
+          self._frame_bytes += e - a
+        if desc is not None:
+          self.d_frames[slot].copy_(self.h_frames[slot], non_blocking=True)
+          self._frame_bytes += len(desc)
       if use_hm:
         self.hm[slot][:self.B].copy_(src_hm, non_blocking=True)
       if pub is not None:
         self.pub[slot][0].copy_(self.h_pub[slot][0], non_blocking=True)
         self.pub[slot][1].copy_(self.h_pub[slot][1], non_blocking=True)
-      self._start_bytes = self._upload_starts(slot, plan, non_blocking=True)
+      self._start_bytes = self._upload_starts(slot, plan, non_blocking=True) + \
+          self._upload_geometry(slot, rows, non_blocking=True)
       self.ev_in[slot].record(self.copy)
     return self._submit(slot)
 
@@ -547,11 +767,13 @@ class StreamRunner(object):
   @property
   def h2d_bytes_per_step(self):
     """Bytes uploaded per step: the frames (and pre_hm / public detections); a step that starts videos with device
-    tracking also uploads its start list and seed rows, counted here after that step is submitted."""
+    tracking also uploads its start list and seed rows (and the tracker geometry rows of streams whose camera
+    changes), counted here after that step is submitted.  A capacity runner uploads the bytes its streams' frames use,
+    plus the slot's descriptors in a step where they changed."""
     pub = self.B * (self.tracker.max_public * 2 + 1) * 4 if self.public else 0
     hm = self.B * self.H * self.W * 4 if self.tracker is None else 0
     if self.frames_mode:
-      return self.slot_bytes + hm + pub + self._start_bytes
+      return self._frame_bytes + hm + pub + self._start_bytes
     return self.B * 3 * self.H * self.W * 4 + hm + pub + self._start_bytes
 
   @property

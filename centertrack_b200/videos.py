@@ -3,9 +3,10 @@ frame to its last -- the batched form of the reference's evaluation loop (src/te
 init_track(pre_dets) at each video's first frame, then Detector.run on every frame).
 
 A video goes to the first free stream (in frames mode, a free stream whose frame_sizes entry is the video's frame
-size) and starts there with StreamRunner's `starts=` / `pre_dets=`; when it ends, the stream takes the next video in the
-same step.  A stream with no video re-feeds its last frame and its results are dropped.  The runner's one-step pipeline
-is kept: the upload of step t+1 overlaps step t, and step t's tracks are yielded after step t+1 is submitted.
+size; on a runner built with max_frame_size, any free stream, whose frame size changes at the start) and starts there
+with StreamRunner's `starts=` / `pre_dets=` / `calibs=`; when it ends, the stream takes the next video in the same step.
+A stream with no video re-feeds its last frame and its results are dropped.  The runner's one-step pipeline is kept:
+the upload of step t+1 overlaps step t, and step t's tracks are yielded after step t+1 is submitted.
 """
 import numpy as np
 import torch
@@ -14,10 +15,16 @@ import torch
 class Video(object):
   """One video: `id`, `frames` (an iterable: uint8 [h, w, 3] BGR arrays in frames mode, pre-processed fp32 [3, H, W]
   images otherwise), optional `pre_dets` (result dicts seeding the tracker at the first frame, as the reference's
-  --load_results does) and `public_dets` (per frame, the [P, 2] centres of its public detections, for --public_det)."""
+  --load_results does), `public_dets` (per frame, the [P, 2] centres of its public detections, for --public_det) and
+  `calib` (the [3, 4] camera matrix of its frames).  Without `calib` the video runs in whatever camera its stream
+  has: Detector._get_default_calib of its frame size when that size differs from the stream's last one, otherwise the
+  stream's current camera -- which may be the `calib` of the previous video on that stream.  When some videos of a
+  dataset carry a calib, give every video one (e.g. detector.default_calib of its size) so that its camera does not
+  depend on the stream it lands on."""
 
-  def __init__(self, id, frames, pre_dets=None, public_dets=None):
+  def __init__(self, id, frames, pre_dets=None, public_dets=None, calib=None):
     self.id, self.frames, self.pre_dets, self.public_dets = id, frames, pre_dets, public_dets
+    self.calib = calib
 
 
 class _Playing(object):
@@ -35,10 +42,11 @@ def track_videos(runner, videos):
   """runner: a StreamRunner with device tracking; videos: an iterable of Video (or dicts of its fields).  Yields
   (video id, frame index, results) for every frame of every video exactly once, as its tracks come back; results is the
   list of dicts fetch_results() gives for that stream (in source pixels in frames mode).  ValueError for a video whose
-  frame size no stream has, or a runner without device tracking."""
+  frame size no stream can take, or a runner without device tracking."""
   if runner.tracker is None:
     raise ValueError('track_videos: the runner needs device_tracking=True')
   B = runner.B
+  capacity = runner.frames_mode and getattr(runner, 'max_frame_bytes', None) is not None
   if runner.frames_mode:
     sizes = [tuple(s) for s in runner.frame_sizes]
   else:
@@ -60,21 +68,27 @@ def track_videos(runner, videos):
       first = next(it, None)
       if first is None:               # no frames: nothing to yield
         continue
-      if size_of(first) not in sizes:
+      if capacity:
+        try:
+          runner.check_frame_size(size_of(first))
+        except ValueError as e:
+          raise ValueError('track_videos: video %r: %s' % (v.id, e))
+      elif size_of(first) not in sizes:
         raise ValueError('track_videos: video %r has frames of size %s; the streams take %s' %
                          (v.id, size_of(first), sorted(set(sizes))))
       return _Playing(v, it, first)
     return None
 
   def place():
-    """Pending videos in order, each to the first free stream of its size; then new videos while a stream is free
-    (looking at most B videos ahead).  -> the streams that start a video."""
+    """Pending videos in order, each to the first free stream of its size (any free stream on a capacity runner);
+    then new videos while a stream is free (looking at most B videos ahead).  -> the streams that start a video."""
     started = []
 
     def put(p):
       for b in range(B):
-        if playing[b] is None and sizes[b] == size_of(p.frame):
+        if playing[b] is None and (capacity or sizes[b] == size_of(p.frame)):
           playing[b] = p
+          sizes[b] = size_of(p.frame)
           started.append(b)
           return True
       return False
@@ -109,6 +123,9 @@ def track_videos(runner, videos):
         pd = p.video.public_dets if p is not None else None
         public.append(np.zeros((0, 2), np.float32) if pd is None else pd[p.index])
     kw = dict(public_dets=public, starts=started, pre_dets=pre_dets or None)
+    calibs = {b: playing[b].video.calib for b in started if playing[b].video.calib is not None}
+    if calibs:
+      kw['calibs'] = calibs
     if runner.frames_mode:
       runner.step_frames(frames, **kw)
     else:

@@ -31,7 +31,8 @@
  *   ct_warp_affine_normalize   Detector.pre_process's cv2.warpAffine + normalise + HWC->CHW, detector.py:207-226.
  *   ct_pack_stem_frames        the same for B ragged uint8 frames and their previous frames, written as the packed
  *                     input of the tensor-core stem (no fp32 image in between); ct_pack_stem_frames_flip also writes
- *                     each stream's mirror image for --flip_test.
+ *                     each stream's mirror image for --flip_test.  The _dev forms and ct_warp_frames_normalize read
+ *                     the descriptors from device memory (frame sizes that change between graph replays).
  */
 #ifndef CTB200_H_
 #define CTB200_H_
@@ -407,6 +408,24 @@ int ct_pack_stem_frames(const uint8_t* cur, const uint8_t* prev, const ct_frame*
  * (un-mirrored). */
 int ct_pack_stem_frames_flip(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames, int32_t B,
                              const float* mean, const float* std, const float* pre_hm, void* out, int32_t H, int32_t W,
+                             void* stream);
+
+/* Device-resident descriptors: the output of ct_pack_stem_frames(_flip), byte for byte, with frames_dev a DEVICE array
+ * ct_frame[B] read by the kernel (a replayed CUDA graph reads whatever geometry it holds then) in one launch.  cur and
+ * prev are buf_bytes long each.  A descriptor with h <= 0, w <= 0, step < 3 w, offset < 0 or a frame extending past
+ * buf_bytes gives zeros for its stream (in both images under _flip) and reads nothing of cur / prev. */
+int ct_pack_stem_frames_dev(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames_dev, int32_t B,
+                            int64_t buf_bytes, const float* mean, const float* std, const float* pre_hm, void* out,
+                            int32_t H, int32_t W, void* stream);
+int ct_pack_stem_frames_flip_dev(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames_dev, int32_t B,
+                                 int64_t buf_bytes, const float* mean, const float* std, const float* pre_hm, void* out,
+                                 int32_t H, int32_t W, void* stream);
+
+/* dst fp32 [B,3,out_h,out_w]: image b = ct_warp_affine_normalize of the frame frames_dev[b] describes in src (buf_bytes
+ * long), bit for bit, all B streams in one launch.  frames_dev: DEVICE array ct_frame[B]; an invalid descriptor (as for
+ * ct_pack_stem_frames_dev) gives a zero image. */
+int ct_warp_frames_normalize(const uint8_t* src, const ct_frame* frames_dev, int32_t B, int64_t buf_bytes,
+                             const float* mean, const float* std, float* dst, int32_t out_h, int32_t out_w,
                              void* stream);
 
 /* ---- misc --------------------------------------------------------------------------- */

@@ -616,9 +616,11 @@ __device__ __forceinline__ void warp_bilinear_u8(const unsigned char* __restrict
                                                  const double* M, int x, int y, int p8[3]) {
   const int AB_BITS = 10, AB_SCALE = 1 << AB_BITS, INTER_BITS = 5, INTER_TAB = 1 << INTER_BITS;
   const int round_delta = AB_SCALE / INTER_TAB / 2;
-  const int adelta = sat_int(M[0] * x * AB_SCALE), bdelta = sat_int(M[3] * x * AB_SCALE);
-  const int X0 = sat_int((M[1] * y + M[2]) * AB_SCALE) + round_delta;
-  const int Y0 = sat_int((M[4] * y + M[5]) * AB_SCALE) + round_delta;
+  // cv2 rounds M[1]*y and the sum + M[2] separately: the _rn intrinsics keep nvcc from fusing them into one DFMA, whose
+  // single rounding moves a row term that lands on a 1/2048 px tie to the other 1/32 px step
+  const int adelta = sat_int(__dmul_rn(__dmul_rn(M[0], x), AB_SCALE)), bdelta = sat_int(__dmul_rn(__dmul_rn(M[3], x), AB_SCALE));
+  const int X0 = sat_int(__dmul_rn(__dadd_rn(__dmul_rn(M[1], y), M[2]), AB_SCALE)) + round_delta;
+  const int Y0 = sat_int(__dmul_rn(__dadd_rn(__dmul_rn(M[4], y), M[5]), AB_SCALE)) + round_delta;
   const int X = (X0 + adelta) >> (AB_BITS - INTER_BITS), Y = (Y0 + bdelta) >> (AB_BITS - INTER_BITS);
   const int sx = X >> INTER_BITS, sy = Y >> INTER_BITS;          // arithmetic shifts: floor
   // BilinearTab_i: (1-fy|fy) x (1-fx|fx) in 1/32 steps, scaled by 2^15: exact integers (the table's one saturated

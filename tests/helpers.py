@@ -129,6 +129,86 @@ def host_case_inputs(i, hw):
   return image, tracks, calib
 
 
+# pre_process's warp (cv2.warpAffine, INTER_LINEAR) on every resolution policy of detector.py:175-204 -- fixed input
+# size, --keep_res with the DLA's pad 31 and the hourglass's 127, --fix_short in both orientations -- over camera
+# frame sizes (1080p, KITTI, nuScenes, VGA, 4K), tiny upscales and 1 x 1, 1 x N, N x 1 frames:
+# (name, cfg, extra argv, pad or None = the option's, source (h, w)).
+WARP_GEOMETRIES = [
+    ('coco_vga', 'coco_tracking', [], None, (480, 640)),
+    ('mot_1080p', 'mot', [], None, (1080, 1920)),
+    ('mot_portrait', 'mot', [], None, (1920, 1080)),
+    ('kitti', 'coco_tracking', ['--input_h', '384', '--input_w', '1280'], None, (375, 1242)),
+    ('nuscenes', 'coco_tracking', ['--input_h', '448', '--input_w', '800'], None, (900, 1600)),
+    ('down_4k', 'coco_tracking', [], None, (2160, 3840)),
+    ('up_100x60', 'coco_tracking', [], None, (60, 100)),
+    ('up_7x5', 'coco_tracking', ['--input_h', '64', '--input_w', '96'], None, (5, 7)),
+    ('odd_203x121', 'coco_tracking', ['--input_h', '128', '--input_w', '160'], None, (121, 203)),
+    ('px_1x1', 'coco_tracking', ['--input_h', '64', '--input_w', '96'], None, (1, 1)),
+    ('row_1x37', 'coco_tracking', ['--input_h', '64', '--input_w', '96'], None, (1, 37)),
+    ('col_29x1', 'coco_tracking', ['--input_h', '64', '--input_w', '96'], None, (29, 1)),
+    ('keep_res_kitti', 'coco_tracking', ['--keep_res'], None, (375, 1242)),
+    ('keep_res_odd', 'coco_tracking', ['--keep_res'], None, (97, 131)),
+    ('keep_res_1x1', 'coco_tracking', ['--keep_res'], None, (1, 1)),
+    ('keep_res127_vga', 'coco_tracking', ['--keep_res'], 127, (480, 640)),
+    ('keep_res127_nuscenes', 'coco_tracking', ['--keep_res'], 127, (900, 1600)),
+    ('fix_short_wide', 'coco_tracking', ['--fix_short', '384'], None, (1080, 1920)),
+    ('fix_short_tall', 'coco_tracking', ['--fix_short', '256'], None, (1920, 1080)),
+    ('fix_short_kitti', 'coco_tracking', ['--fix_short', '128'], None, (375, 1242)),
+]
+
+
+def warp_geometry(i):
+  """WARP_GEOMETRIES[i] -> (source (h, w), network input (oh, ow), minv fp64 [6], forward map fp64 [2, 3])."""
+  from centertrack_b200.detector import frame_geometry
+  _, cfg, extra, pad, hw = WARP_GEOMETRIES[i]
+  opt = make_opt(cfg, extra)
+  if pad is not None:
+    opt.pad = pad
+  meta, minv = frame_geometry(opt, *hw)
+  return hw, (meta['inp_height'], meta['inp_width']), minv, np.asarray(meta['trans_input'], np.float64)
+
+
+def _tie_maps(rng, n, term):
+  """n inverse maps on which a fused multiply-add changes a whole output row: for one row y0 the row term M[1] y0 + M[2]
+  (term 'x') or M[4] y0 + M[5] (term 'y'), rounded after the product and after the sum as cv2 rounds it, lands exactly on
+  (32 m + 15 + 1/2) / 1024 px.  cvRound takes that tie to the even 32 m + 16, the next 1/32 px step, while the exact
+  value -- what one rounding of a fused multiply-add keeps -- lies on one side of it and rounds to the other step."""
+  from fractions import Fraction
+  maps = []
+  while len(maps) < n:
+    a, c = float(rng.uniform(0.3, 1.5)), float(rng.uniform(0.05, 0.4))
+    y0 = int(rng.randint(1, 300))
+    tie = (32 * int(rng.randint(0, 100 * 1024 // 32)) + 15.5) / 1024
+    slope = c if term == 'x' else a
+    off = tie - slope * y0
+    if slope * y0 + off != tie or np.rint((slope * y0 + off) * 1024) == \
+        np.rint(float(Fraction(slope) * y0 + Fraction(off)) * 1024):
+      continue
+    m = [a, c, off, 0., 1.0, 0.5] if term == 'x' else [a, 0., 0.25, 0., a, off]
+    maps.append(('tie_%s_row%d' % (term, y0), np.array(m, np.float64), (400, 500), (320, 200)))
+  return maps
+
+
+def warp_maps():
+  """Inverse (dst -> src) maps beyond the resolution policies: (name, minv fp64 [6], source (h, w), output (oh, ow)).
+  The fused-multiply-add tie maps, rotation and shear (M[1], M[3] != 0), a mirror, negative and fractional
+  translations, and maps that land partly or wholly outside the frame.  Source coordinates stay within +-32767."""
+  rng = np.random.RandomState(2024)
+  maps = _tie_maps(rng, 3, 'y') + _tie_maps(rng, 3, 'x')
+  ang, sc = np.deg2rad(17.0), 1.3
+  maps += [
+      ('rotate', np.array([sc * np.cos(ang), -sc * np.sin(ang), 120.25, sc * np.sin(ang), sc * np.cos(ang), -40.5]),
+       (400, 500), (320, 200)),
+      ('shear', np.array([1.0, 0.37, -20.5, 0.21, 0.9, 3.25]), (400, 500), (320, 200)),
+      ('mirror', np.array([-1.0, 0.0, 499.0, 0.0, 1.0, 0.0]), (400, 500), (320, 200)),
+      ('negative_fractional', np.array([0.75, 0.0, -13.37, 0.0, 1.25, -7.0625]), (400, 500), (320, 200)),
+      ('partly_outside', np.array([2.5, 0.0, -100.3, 0.0, 2.5, -50.7]), (400, 500), (320, 200)),
+      ('wholly_outside', np.array([1.0, 0.0, 5000.0, 0.0, 1.0, -3000.0]), (400, 500), (320, 200)),
+      ('down_3_7x', np.array([3.7, 0.0, 0.4, 0.0, 3.7, 0.9]), (1080, 1920), (288, 512)),
+  ]
+  return maps
+
+
 def flip_inputs(hw=(64, 96)):
   """Must stay identical to oracle/gen_golden.py::flip_inputs (--flip_test goldens)."""
   img, pre, hm = wt.synthetic_inputs(1, hw[0], hw[1], seed=77)

@@ -1,7 +1,7 @@
 """-m gpu: StreamRunner's frames mode -- raw uint8 camera frames of per-stream sizes warped, normalised and packed on the
 device (ct_pack_stem_frames on the bf16 engine, ct_warp_affine_normalize per stream on the others), tracks in each
-stream's source pixels.  Against the unfused kernels byte for byte, against a runner fed the fp32 images of
-pre_process_device bit for bit, and closed-loop against the host pipeline."""
+stream's source pixels.  Against the unfused kernels byte for byte, against a runner fed the fp32 images of the host
+pre_process (cv2) bit for bit, and closed-loop against the host pipeline."""
 import ctypes as C
 
 import numpy as np
@@ -113,8 +113,8 @@ def _coco(extra=()):
 @pytest.mark.parametrize('precision', ['bf16', 'bf16x3'])
 @pytest.mark.parametrize('graph', [True, False], ids=['graph', 'eager'])
 def test_frames_mode_records_equal_the_fp32_image_runner(precision, graph):
-  """device_tracking=False, 5 steps: step_frames on uint8 frames of three sizes vs step_host on the stacked
-  pre_process_device images of the same frames -- the same records, bit for bit."""
+  """device_tracking=False, 5 steps: step_frames on uint8 frames of three sizes vs step_host on the stacked images
+  Detector.pre_process (cv2.warpAffine on the host) makes of the same frames -- the same records, bit for bit."""
   from centertrack_b200.runner import StreamRunner
   opt, model, _ = _coco()
   model = model.cuda()
@@ -133,7 +133,7 @@ def test_frames_mode_records_equal_the_fp32_image_runner(precision, graph):
     frames = [_frame(h, w, 100 * t + b) for b, (h, w) in enumerate(SIZES)]
     fr.step_frames(frames)
     a = fr.fetch()                      # one runner at a time: the two share the engine's activation buffers
-    imgs = torch.cat([det.pre_process_device(f, 1.0)[0] for f in frames], 0).cpu()
+    imgs = torch.cat([det.pre_process(f, 1.0)[0] for f in frames], 0)
     ref.step_host(imgs)
     b = ref.fetch()
     assert np.array_equal(a, b), (precision, graph, t)

@@ -223,8 +223,7 @@ def test_flip_test_process_matches_reference_golden(cfg, golden_dir):
 @pytest.mark.parametrize('i', range(len(HOST_CASES)), ids=[c[0] for c in HOST_CASES])
 def test_device_pre_process_matches_cv2_pre_process(i):
   """ct_warp_affine_normalize (cv2's fixed-point bilinear restated) vs Detector.pre_process (cv2.warpAffine on the
-  host, itself pinned to the reference by host_pre.npz): same meta, image equal up to one grey level (1/255/std) on a
-  vanishing fraction of pixels -- the interpolation rounding the host test allows between cv2 builds."""
+  host, itself pinned to the reference by host_pre.npz): same meta, the same fp32 image bit for bit."""
   name, extra, hw, with_calib = HOST_CASES[i]
   opt = make_opt('coco_tracking', ['--pre_thresh', '0.3'] + extra)
   opt.device = DEV
@@ -235,10 +234,8 @@ def test_device_pre_process_matches_cv2_pre_process(i):
   assert img.is_cuda and img.dtype == torch.float32 and tuple(img.shape) == tuple(ref_img.shape)
   for k in ref_meta:
     assert np.array_equal(np.asarray(meta[k]), np.asarray(ref_meta[k])), k
-  err = np.abs(img.cpu().numpy() - ref_img.numpy())
-  one_level = 1.0 / 255.0 / float(det.std.min())
-  assert err.max() <= 1.01 * one_level, (name, float(err.max()), one_level)
-  assert (err > 1e-5).mean() < 2e-3, (name, float((err > 1e-5).mean()))
+  bad = img.cpu().numpy().view(np.int32) != ref_img.numpy().view(np.int32)
+  assert not bad.any(), (name, int(bad.sum()), np.argwhere(bad)[:4].tolist())
 
 
 def test_detector_process_graph_replay_equals_eager(monkeypatch):

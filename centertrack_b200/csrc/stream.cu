@@ -7,6 +7,8 @@
 //                    the pose / 3D / velocity / attribute fields of generic_post_process (post_process.py:55-89) in a
 //                    payload table beside the track table, and the amodal centre on 3D head sets
 //   ct_render_tracks the gaussian max-splat of those boxes into pre_hm (image.py:128-154)
+//   ct_track_step_mapped / ct_render_tracks_mapped   the same two on a compacted batch of live streams (image i =
+//                    stream streams[i]), for StreamRunner's idle streams
 //   ct_flip_merge    Detector._flip_output (detector.py:311-332; model/utils.py:28-50) for --flip_test;
 //                    ct_flip_merge_heads: every averaged head of B (frame, mirror) pairs in one launch
 //   ct_mirror_x      the mirrored half of a --flip_test batch (detector.py:225-226,285-286)
@@ -75,6 +77,8 @@ struct TrackArgs {
   ct_track_assoc as;       // all zero: greedy association, private births (ct_track_step)
   ct_track_payload p;      // read by the payload instantiation only
   int pay_smem;            // byte offset of the staged payload rows in dynamic shared memory
+  const int* streams;      // ct_track_step_mapped: CTA i runs stream streams[i] on records[i]; NULL = identity
+  int n_streams;           // rows of every per-stream array when streams != NULL
 };
 
 // bytes of the greedy layout before the association scratch (a multiple of 8: the scratch starts with fp64 arrays)
@@ -328,12 +332,16 @@ __device__ __forceinline__ void track_boxes(const ct_track_desc& d, int b, const
 }
 
 // PAY: also write the payload table (ct_track_step_payload); the 2-D head sets run the <false> instantiation.
-template <bool PAY>
+// MAP: ct_track_step_mapped (a.streams); a template parameter so that the identity instantiations stay as they were.
+template <bool PAY, bool MAP = false>
 __global__ void __launch_bounds__(TRK_THREADS)
 track_step_kernel(const TrackArgs a) {
   extern __shared__ __align__(16) unsigned char tsm[];
   const ct_track_desc& d = a.d;
-  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  // b indexes every per-stream array; the CTA's records are always records[blockIdx.x]
+  const int b = MAP ? a.streams[blockIdx.x] : blockIdx.x;
+  if (MAP && (b < 0 || b >= a.n_streams)) return;           // a padding image, or no stream: nothing is written
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int T = d.max_tracks, K = d.K;
   float* s_old = reinterpret_cast<float*>(tsm);                 // [T][TF]   previous tracks
   float* s_det = s_old + (size_t)T * TF;                        // [K][TF]   this frame's detections (image coords)
@@ -374,7 +382,7 @@ track_step_kernel(const TrackArgs a) {
   __syncthreads();
 
   // ---- detections of this frame: generic_post_process (post_process.py:21-91), merge_outputs (detector.py:371-377)
-  const float* rec = d.records + (size_t)b * K * d.F;
+  const float* rec = d.records + (size_t)(MAP ? (int)blockIdx.x : b) * K * d.F;
   const float* to = d.trans_out_inv + b * 6;
   int cnt = 0;
   for (int i = tid; i < K; i += TRK_THREADS) cnt += rec[(size_t)i * d.F + CT_REC_SCORE] > d.out_thresh ? 1 : 0;
@@ -581,12 +589,20 @@ track_start_kernel(const ct_track_desc d, float* __restrict__ payload, int Wp, c
 }
 
 // splat of the boxes written by track_step_kernel; rows with radius < 0 are skipped.  grid = B*T (fixed: graph-capturable)
-__global__ void render_tracks_kernel(const float* __restrict__ boxes, int n, float* __restrict__ hm, int B, int H, int W) {
+// image_of (ct_render_tracks_mapped): a row of stream s splats into image image_of[s] (< 0: skipped); NULL = identity.
+template <bool MAP = false>
+__global__ void render_tracks_kernel(const float* __restrict__ boxes, int n, float* __restrict__ hm, int B, int H, int W,
+                                     const int* __restrict__ image_of, int n_streams) {
   const int i = blockIdx.x;
   if (i >= n) return;
   const float rf = boxes[i * 5 + 3];
   if (rf < 0.f) return;
-  const int b = (int)boxes[i * 5 + 0], cx = (int)boxes[i * 5 + 1], cy = (int)boxes[i * 5 + 2], r = (int)rf;
+  int b = (int)boxes[i * 5 + 0];
+  const int cx = (int)boxes[i * 5 + 1], cy = (int)boxes[i * 5 + 2], r = (int)rf;
+  if constexpr (MAP) {
+    if (b < 0 || b >= n_streams) return;
+    b = image_of[b];
+  }
   if (b < 0 || b >= B) return;
   const double sigma = (double)(2 * r + 1) / 6.0;
   const int left = min(cx, r), right = min(W - cx, r + 1), top = min(cy, r), bottom = min(H - cy, r + 1);
@@ -850,8 +866,9 @@ static inline bool rec_field_ok(int32_t off, int32_t w, int32_t F) {
   return off < 0 || (w > 0 && off >= CT_REC_HEADS && off + w <= F);
 }
 
-extern "C" int ct_track_step_payload(const ct_track_desc* d, const ct_track_assoc* as, const ct_track_payload* p,
-                                     void* stream) {
+// One track step launch: CTA i on records[i] and stream streams[i] (streams == NULL: stream i of d->B).
+static int track_step_launch(const ct_track_desc* d, const ct_track_assoc* as, const ct_track_payload* p,
+                             const int32_t* streams, int32_t n_streams, void* stream) {
   CT_REQUIRE(d && as && d->records && d->trans_out_inv && d->tracks && d->counts, "null pointer");
   CT_REQUIRE(d->B > 0 && d->K > 0 && d->F >= CT_REC_HEADS && d->max_tracks >= d->K, "bad shape");
   CT_REQUIRE(d->rec_tracking < 0 || d->rec_tracking + 2 <= d->F, "tracking offset outside the record");
@@ -875,7 +892,8 @@ extern "C" int ct_track_step_payload(const ct_track_desc* d, const ct_track_asso
   const bool scratch = as->hungarian || as->public_det;
   const size_t smem = (size_t)ct_track_payload_smem_bytes(d->K, d->max_tracks, p ? p->width : 0, scratch);
   CT_REQUIRE(smem <= 200 * 1024, "track table does not fit in shared memory (lower max_tracks)");
-  auto kernel = p ? track_step_kernel<true> : track_step_kernel<false>;
+  auto kernel = streams ? (p ? track_step_kernel<true, true> : track_step_kernel<false, true>)
+                        : (p ? track_step_kernel<true> : track_step_kernel<false>);
   if (smem > 48 * 1024)
     CT_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   TrackArgs a = {};
@@ -885,8 +903,23 @@ extern "C" int ct_track_step_payload(const ct_track_desc* d, const ct_track_asso
   a.pay_smem = (int)(trk_base_bytes(d->K, d->max_tracks) +
                      (scratch ? ct_track_assoc_smem_bytes(d->K, d->max_tracks) - ct_track_smem_bytes(d->K, d->max_tracks)
                               : 0));
+  a.streams = streams;
+  a.n_streams = n_streams;
   kernel<<<d->B, TRK_THREADS, smem, (cudaStream_t)stream>>>(a);
   return after_launch();
+}
+
+extern "C" int ct_track_step_payload(const ct_track_desc* d, const ct_track_assoc* as, const ct_track_payload* p,
+                                     void* stream) {
+  return track_step_launch(d, as, p, nullptr, 0, stream);
+}
+
+extern "C" int ct_track_step_mapped(const ct_track_desc* d, const ct_track_assoc* as, const ct_track_payload* p,
+                                    const int32_t* streams, int32_t n_streams, void* stream) {
+  CT_REQUIRE(streams, "null stream map");
+  CT_REQUIRE(n_streams > 0, "n_streams <= 0");
+  const ct_track_assoc greedy = {};
+  return track_step_launch(d, as ? as : &greedy, p, streams, n_streams, stream);
 }
 
 extern "C" int ct_track_step_assoc(const ct_track_desc* d, const ct_track_assoc* as, void* stream) {
@@ -917,7 +950,17 @@ extern "C" int ct_render_tracks(const float* boxes, int32_t n, float* pre_hm, in
   CT_REQUIRE(pre_hm && boxes && n > 0, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
   CT_CUDA_OK(cudaMemsetAsync(pre_hm, 0, (size_t)B * H * W * sizeof(float), st));
-  render_tracks_kernel<<<n, 128, 0, st>>>(boxes, n, pre_hm, B, H, W);
+  render_tracks_kernel<<<n, 128, 0, st>>>(boxes, n, pre_hm, B, H, W, nullptr, 0);
+  return after_launch();
+}
+
+extern "C" int ct_render_tracks_mapped(const float* boxes, int32_t n, const int32_t* image_of, int32_t n_streams,
+                                       float* pre_hm, int32_t n_images, int32_t H, int32_t W, void* stream) {
+  CT_REQUIRE(pre_hm && boxes && image_of && n > 0, "null pointer");
+  CT_REQUIRE(n_streams > 0 && n_images > 0 && H > 0 && W > 0, "bad shape");
+  cudaStream_t st = (cudaStream_t)stream;
+  CT_CUDA_OK(cudaMemsetAsync(pre_hm, 0, (size_t)n_images * H * W * sizeof(float), st));
+  render_tracks_kernel<true><<<n, 128, 0, st>>>(boxes, n, pre_hm, n_images, H, W, image_of, n_streams);
   return after_launch();
 }
 

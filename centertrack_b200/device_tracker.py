@@ -281,19 +281,51 @@ class DeviceTracker(object):
     L.check(L.lib().ct_render_tracks(L.ptr(self.boxes), self.B * self.T, L.ptr(pre_hm), self.B, self.inp_h,
                                      self.inp_w, L.stream_ptr()), 'ct_render_tracks')
 
+  def step_mapped(self, records, streams, public_ct=None, public_n=None):
+    """step() on a compacted batch: records [n,K,F], streams int32 [>= n] device map (image i is stream streams[i];
+    < 0: a padding image, nothing is written).  Streams that are not listed keep their tables byte for byte.
+    public_ct / public_n stay indexed by the stream, as in step()."""
+    if self.public_det and (public_ct is None or public_n is None):
+      raise ValueError('--public_det: step_mapped() needs the public detections (public_ct, public_n)')
+    n = records.shape[0]
+    assert records.is_cuda and records.dtype == torch.float32 and records.is_contiguous() and \
+        tuple(records.shape) == (n, self.K, self.F) and 0 < n <= self.B
+    assert streams.is_cuda and streams.dtype == torch.int32 and streams.numel() >= n
+    d = L.TrackDesc.from_buffer_copy(self.desc)
+    d.B, d.records = n, records.data_ptr()
+    a = L.TrackAssoc.from_buffer_copy(self.assoc)
+    a.public_ct = a.public_n = a.steps = None
+    if self.public_det:
+      a.public_ct, a.public_n = public_ct.data_ptr(), public_n.data_ptr()
+    L.check(L.lib().ct_track_step_mapped(C.byref(d), C.byref(a), C.byref(self.pay) if self.pay is not None else None,
+                                         L.ptr(streams), self.B, L.stream_ptr()), 'ct_track_step_mapped')
+
+  def render_mapped(self, pre_hm, image_of):
+    """render() on a compacted batch: pre_hm [n,1,H,W] fp32 <- the tracks of stream s splatted into image
+    image_of[s] (int32 [B] device map; < 0 or >= n: not rendered); every image of pre_hm is zeroed first."""
+    n = pre_hm.shape[0]
+    assert pre_hm.is_cuda and pre_hm.dtype == torch.float32 and tuple(pre_hm.shape) == (n, 1, self.inp_h, self.inp_w)
+    assert image_of.is_cuda and image_of.dtype == torch.int32 and image_of.numel() == self.B
+    L.check(L.lib().ct_render_tracks_mapped(L.ptr(self.boxes), self.B * self.T, L.ptr(image_of), self.B, L.ptr(pre_hm),
+                                            n, self.inp_h, self.inp_w, L.stream_ptr()), 'ct_render_tracks_mapped')
+
   @property
   def d2h_bytes(self):
     return self.tracks.numel() * 4 + self.counts.numel() * 4 + (self.payload.numel() * 4 if self.Wp else 0)
 
-  def results(self, tracks_np, counts_np, payload_np=None):
+  def results(self, tracks_np, counts_np, payload_np=None, idle=()):
     """Host copies -> [[{score, class, ct, tracking, bbox, tracking_id, age, active}, ...] per stream], plus the payload
     fields of the head set (payload_np [B,T,Wp], needed when it has any) with the host path's shapes: hps [2J],
-    dep [1], dim [3], alpha, loc [3], rot_y, velocity, nuscenes_att."""
+    dep [1], dim [3], alpha, loc [3], rot_y, velocity, nuscenes_att.  idle: streams that had no frame in that step;
+    their entry is None."""
     if self.Wp and payload_np is None:
       raise ValueError('results(): this head set has payload fields (%s): pass payload_np' %
                        ', '.join(self.payload_layout))
     out = []
     for b in range(tracks_np.shape[0]):
+      if b in idle:
+        out.append(None)
+        continue
       n = int(counts_np[b, 0])
       rows = tracks_np[b, :n]
       res = [{'score': float(r[L.CT_TRK_SCORE]), 'class': int(r[L.CT_TRK_CLASS]),

@@ -660,8 +660,10 @@ class DLA34Engine(object):
     self.fused_act = on
     self.graph = None
 
-  def _run_one(self, kind, pl, name, img_ptr, pre_ptr, hm_ptr, st, mask=None):
+  def _run_one(self, kind, pl, name, img_ptr, pre_ptr, hm_ptr, st, mask=None, n=None):
+    """n: the batch of this launch, the first n images of every buffer (default B)."""
     lib = self.lib
+    n = self.B if n is None else n
     if mask is None:               # which of (img, pre_img, pre_hm) exist this call (dla.py:308-311)
       mask = 1 | (2 if pre_ptr.value else 0) | (4 if hm_ptr.value else 0)
     if kind == 'conv':
@@ -669,25 +671,30 @@ class DLA34Engine(object):
         pl.epilogue_sum3 = mask
       elif name == 'stem48':
         pl.shift = self.stem48_shift[mask].data_ptr()
-      rc = lib.ct_conv_forward(C.byref(pl), st)
+      if n == self.B:
+        rc = lib.ct_conv_forward(C.byref(pl), st)
+      else:                         # the descriptor at batch n: same buffers, weights, N tile and configuration
+        d = L.ConvDesc.from_buffer_copy(pl)
+        d.B = n
+        rc = lib.ct_conv_forward(C.byref(d), st)
     elif kind == 'stem':
       rc = lib.ct_stem_forward(img_ptr, pre_ptr, hm_ptr, L.ptr(self.stem_w), L.ptr(self.stem_shift),
-                               C.c_void_p(pl.ptr), self.ct_dtype, self.B, self.H, self.W, pl.ld, st)
+                               C.c_void_p(pl.ptr), self.ct_dtype, n, self.H, self.W, pl.ld, st)
     elif kind == 'pack':
-      rc = lib.ct_pack_stem_input(img_ptr, pre_ptr, hm_ptr, C.c_void_p(pl.ptr), self.B, self.H, self.W, st)
+      rc = lib.ct_pack_stem_input(img_ptr, pre_ptr, hm_ptr, C.c_void_p(pl.ptr), n, self.H, self.W, st)
     elif kind == 'pack32':
-      rc = lib.ct_pack_stem_input_f32(img_ptr, pre_ptr, hm_ptr, C.c_void_p(pl.ptr), self.B, self.H, self.W, st)
+      rc = lib.ct_pack_stem_input_f32(img_ptr, pre_ptr, hm_ptr, C.c_void_p(pl.ptr), n, self.H, self.W, st)
     elif kind == 'pool_s2d':
       x, o = pl
-      rc = lib.ct_maxpool2_s2d(C.c_void_p(x.ptr), C.c_void_p(o.ptr), self.ct_dtype, self.B, x.H, x.W, o.C, x.ld, o.ld, st)
+      rc = lib.ct_maxpool2_s2d(C.c_void_p(x.ptr), C.c_void_p(o.ptr), self.ct_dtype, n, x.H, x.W, o.C, x.ld, o.ld, st)
     elif kind == 'pool':
       x, o = pl
-      rc = lib.ct_maxpool2(C.c_void_p(x.ptr), C.c_void_p(o.ptr), self.ct_dtype, self.B, x.H, x.W, x.C,
+      rc = lib.ct_maxpool2(C.c_void_p(x.ptr), C.c_void_p(o.ptr), self.ct_dtype, n, x.H, x.W, x.C,
                            x.ld, o.ld, st)
     else:
       x, skip, w, o, f = pl
       rc = lib.ct_upsample_add(C.c_void_p(x.ptr), C.c_void_p(skip.ptr), L.ptr(w), C.c_void_p(o.ptr),
-                               self.ct_dtype, self.B, x.H, x.W, x.C, f, x.ld, skip.ld, o.ld, st)
+                               self.ct_dtype, n, x.H, x.W, x.C, f, x.ld, skip.ld, o.ld, st)
     if rc != 0:
       L.check(rc, '%s (%s)' % (kind, name))
     if self.debug_sync:                  # CTB_DEBUG_SYNC=1: attribute an asynchronous kernel fault to its layer
@@ -696,40 +703,55 @@ class DLA34Engine(object):
       except Exception as e:
         raise RuntimeError('kernel fault in op %s (%s): %s' % (kind, name, e))
 
-  def _run_ops(self, img_ptr, pre_ptr, hm_ptr, mask=None, packed=False):
+  def _run_ops(self, img_ptr, pre_ptr, hm_ptr, mask=None, packed=False, n=None):
     """mask: which stem inputs (bit 0 img, 1 pre_img, 2 pre_hm) are present, by default those whose pointer is set.
-    packed: the stem input is already in stem_input; the pack op is skipped."""
+    packed: the stem input is already in stem_input; the pack op is skipped.  n: the batch (default B)."""
     st = L.stream_ptr()
     for kind, pl, name in self.ops:
       if not (packed and kind == 'pack'):
-        self._run_one(kind, pl, name, img_ptr, pre_ptr, hm_ptr, st, mask)
+        self._run_one(kind, pl, name, img_ptr, pre_ptr, hm_ptr, st, mask, n)
+
+  def _batch(self, n):
+    if n is None:
+      return self.B
+    n = int(n)
+    if not 0 < n <= self.B:
+      raise ValueError('batch %d outside [1, %d]' % (n, self.B))
+    return n
+
+  def _outputs(self, n):
+    return self.outputs if n == self.B else {h: t[:n] for h, t in self.outputs.items()}
 
   @property
   def n_launches(self):
     return len(self.ops)
 
-  def forward(self, images, pre_images=None, pre_hms=None):
-    """images/pre_images [B,3,H,W], pre_hms [B,1,H,W]: fp32 CUDA NCHW contiguous.
-    Returns {head: fp32 [B,c,H/4,W/4]} (buffers owned by the engine, overwritten by the next call)."""
+  def forward(self, images, pre_images=None, pre_hms=None, n=None):
+    """images/pre_images [n,3,H,W], pre_hms [n,1,H,W]: fp32 CUDA NCHW contiguous; n <= B (default B) runs every
+    launch at batch n on the first n images of the engine's buffers, with the results the B-image run gives on them.
+    Returns {head: fp32 [n,c,H/4,W/4]} (views of buffers owned by the engine, overwritten by the next call)."""
+    n = self._batch(n)
     for t in (images, pre_images, pre_hms):
       if t is not None:
         assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous(), 'fp32 contiguous CUDA input'
-    assert tuple(images.shape) == (self.B, 3, self.H, self.W), (images.shape, self.B, self.H, self.W)
+    assert tuple(images.shape) == (n, 3, self.H, self.W), (images.shape, n, self.H, self.W)
     pre = pre_images if self.has_pre_img else None
     hm = pre_hms if self.has_pre_hm else None
-    self._run_ops(L.ptr(images), L.ptr(pre), L.ptr(hm))
-    return self.outputs
+    self._run_ops(L.ptr(images), L.ptr(pre), L.ptr(hm), n=n)
+    return self._outputs(n)
 
-  def forward_packed(self, has_pre, has_hm):
+  def forward_packed(self, has_pre, has_hm, n=None):
     """The plan without its pack op, on a stem input the caller wrote into `stem_input` (bf16 NHWC [B,H,W,8],
     ct_pack_stem_input's layout, e.g. by ct_pack_stem_frames): has_pre / has_hm say whether its pre_img / pre_hm
-    channels are present, as forward's pre_images / pre_hms being given does.  bf16 tensor-core plan only."""
+    channels are present, as forward's pre_images / pre_hms being given does.  n: the batch, as in forward.  bf16
+    tensor-core plan only."""
     if not self.use_halo:
       raise ValueError('forward_packed: only the bf16 tensor-core plan reads a packed stem input')
+    n = self._batch(n)
     mask = 1 | (2 if has_pre and self.has_pre_img else 0) | (4 if has_hm and self.has_pre_hm else 0)
     none = C.c_void_p(0)
-    self._run_ops(none, none, none, mask, packed=True)
-    return self.outputs
+    self._run_ops(none, none, none, mask, packed=True, n=n)
+    return self._outputs(n)
 
   # CUDA-graph replay: inputs are first copied into the engine's static buffers
   def capture(self):

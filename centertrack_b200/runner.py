@@ -48,6 +48,15 @@ B images; ct_mirror_x writes the second half in the graph, or, in frames mode on
 ct_pack_stem_frames_flip stores every packed pixel at its mirrored position too.  One ct_flip_merge_heads launch
 averages the flipped heads into [B] buffers; decode and tracking then run at B on those and on the first half of the
 other heads.  Records, tracks, uploads and downloads are the same size as without the flip.
+
+Idle streams (`idle_streams=g`, `step_frames(..., idle=)`, capacity frames runners): a step computes only the streams
+that have a frame.  The live streams s_0 < ... < s_{n-1} are compacted into the first n images (image i = stream s_i),
+the batch rounded up to a multiple of g (capped at B) with padding images whose invalid descriptors give zero input.
+Every launch runs at that batch; the track step and the prior heat-map render map images to streams through per-slot
+device maps (ct_track_step_mapped, ct_render_tracks_mapped), uploaded with the slot's descriptors when they change.
+One CUDA graph per (slot, batch).  pre_images must not depend on an image index, so the fp32 and bf16x3 engines warp
+the previous slot's frames again (the bf16 engine's pack already does).  An idle stream's tables, frame region and
+camera rows are left as they are; it comes back with a video start.
 """
 import ctypes as C
 
@@ -62,12 +71,16 @@ from .device_tracker import DeviceTracker, default_geometry, plan_starts
 
 
 NS = 3          # input slots
+# idle_streams=True: the batch granule.  On an H100 (DESIGN §5) g = 4 was never faster than g = 1 and slower where it
+# pads (n = 1, 2); a larger g only saves graphs.
+IDLE_GRANULE = 1
 
 
 class StreamRunner(object):
 
   def __init__(self, model, B, H, W, K=100, precision='bf16', device='cuda', use_graph=True, opt=None,
-               device_tracking=False, max_public_dets=512, calibs=None, frame_sizes=None, max_frame_size=None):
+               device_tracking=False, max_public_dets=512, calibs=None, frame_sizes=None, max_frame_size=None,
+               idle_streams=None):
     """max_public_dets: with device_tracking and --public_det, the most public detections a stream may bring per
     frame (more raise ValueError; none is ever dropped).  calibs: with device_tracking on a 3D head set, one [3,4]
     camera matrix per stream (DeviceTracker's default otherwise; in frames mode Detector._get_default_calib of the
@@ -77,7 +90,10 @@ class StreamRunner(object):
     of h * w * 3 bytes in each slot, and may bring a frame of any size that fits it and maps to (H, W) when it starts
     a video (frame_sizes are then the first sizes); the descriptors of the frames live on the device.
     opt.flip_test: every stream's frame runs with its mirror (2B images per step) and the averaged heads are merged
-    before decode, as Detector.process does; inputs and outputs keep their B shapes."""
+    before decode, as Detector.process does; inputs and outputs keep their B shapes.
+    idle_streams g >= 1, or True for g = IDLE_GRANULE (capacity frames runners only): step_frames(idle=) may leave
+    streams without a frame, and a step computes only the live ones, in a batch rounded up to a multiple of g (see the
+    module docstring).  None or False: off."""
     self.B, self.H, self.W, self.K = B, H, W, K
     self.device = torch.device(device)
     self.model = model
@@ -85,6 +101,16 @@ class StreamRunner(object):
     self.frames_mode = frame_sizes is not None
     if max_frame_size is not None and not self.frames_mode:
       raise ValueError('max_frame_size needs frame_sizes (frames mode)')
+    self.idle_g = None
+    if idle_streams is True:                                 # on, with the default granule
+      idle_streams = IDLE_GRANULE
+    if idle_streams is not None and idle_streams is not False:
+      if isinstance(idle_streams, np.bool_) or not isinstance(idle_streams, (int, np.integer)) or idle_streams < 1:
+        raise ValueError('idle_streams: expected True or an integer batch granule >= 1, got %r' % (idle_streams,))
+      if max_frame_size is None:
+        raise ValueError('idle_streams needs a capacity frames runner (frame_sizes and max_frame_size)')
+      self.idle_g = int(idle_streams)
+    self._n = B                                              # the (padded) batch of the step being launched
     self.cap = self.max_frame_bytes = None
     if self.frames_mode:
       calibs = self._frame_geometry(frame_sizes, calibs, max_frame_size)
@@ -112,6 +138,16 @@ class StreamRunner(object):
         self.h_frames = [desc.clone().pin_memory() for _ in range(NS)]
         self.d_frames = [desc.to(self.device) for _ in range(NS)]
         self._desc_mirror = [bytes(self.frames)] * NS
+    if self.idle_g is not None:  # per slot: streams [B] (image -> stream) then image_of [B] (stream -> image), int32
+      ident = torch.arange(B, dtype=torch.int32).repeat(2)
+      self.h_map = [ident.clone().pin_memory() for _ in range(NS)]
+      self.d_map = [ident.to(self.device) for _ in range(NS)]
+      self._map_mirror = [ident.numpy().tobytes()] * NS
+      self._live = [None, None]                              # per D2H buffer: the live streams of its step
+      self._was_idle = set()                                 # the streams idle in the last submitted step
+      self.idle_graphs = {}                                  # (slot, batch) -> graph
+      if not self.eng.use_halo and self.eng.has_pre_img:     # pre_images, warped again from the previous slot
+        self.pre_img = torch.zeros((NB, 3, H, W), dtype=f32, device=self.device)
     self.rec = None
     self.layout = None
     self.ws = None                                           # private decode workspace (captured by the graphs)
@@ -161,6 +197,8 @@ class StreamRunner(object):
       self.launches_per_step += (-(-B // L.CT_FRAMES_PER_LAUNCH) - 1) if self.eng.use_halo else B
     if self.flip:
       self.launches_per_step += 1 + (0 if self._pack_mirror else 1 + int(self.eng.has_pre_hm))
+    if self.idle_g is not None and not self.eng.use_halo and self.eng.has_pre_img:   # + the pre_images warp (+ mirror)
+      self.launches_per_step += 1 + int(self.flip)
 
   def _frame_geometry(self, frame_sizes, calibs, max_frame_size=None):
     """Per-stream geometry of frames mode (Detector.pre_process_device's, through detector.frame_geometry): the
@@ -269,10 +307,11 @@ class StreamRunner(object):
       changed[b] = self._size_geometry('frames[%d]' % b, int(hw[0]), int(hw[1]))
     return changed
 
-  def _plan_geometry(self, slot, changed, calibs):
+  def _plan_geometry(self, slot, changed, calibs, live=None):
     """Host state of one step's geometry changes (changed: _check_sizes, calibs: _check_calibs): the descriptors and
     metas of the changed streams, the slot's descriptor staging when its device copy differs, and the tracker rows of
-    the streams whose camera changes.  -> (descriptor bytes to upload or None, [(stream, c, s, calib)])."""
+    the streams whose camera changes.  live (idle-streams runners): the step's live streams, whose descriptors the
+    slot holds in image order.  -> (descriptor bytes to upload or None, [(stream, c, s, calib)])."""
     rows = []
     if self.frames_mode:
       self._prev_meta = self._meta
@@ -297,16 +336,18 @@ class StreamRunner(object):
       rows = [(b, c, s, k) for b, k in sorted(calibs.items())]
     desc = None
     if self.cap is not None:
-      now = bytes(self.frames)
+      now = bytes(self.frames) if live is None else bytes(self._image_frames(live))
       if now != self._desc_mirror[slot]:
         desc = self._desc_mirror[slot] = now
     return desc, rows
 
-  def _upload_runs(self):
+  def _upload_runs(self, live=None):
     """Maximal runs [start, end) of the slot bytes this step's frames use: stream b's frame, padded to 16 bytes, at
-    b * cap.  One run of slot_bytes when every stream is at capacity."""
+    b * cap, for every stream or the `live` ones.  One run of slot_bytes when every stream is at capacity."""
     runs = []
     for b, f in enumerate(self.frames):
+      if live is not None and b not in live:
+        continue
       a, e = b * self.cap, b * self.cap + (f.h * f.w * 3 + 15) // 16 * 16
       if runs and runs[-1][1] == a:
         runs[-1][1] = e
@@ -314,10 +355,35 @@ class StreamRunner(object):
         runs.append([a, e])
     return [tuple(r) for r in runs]
 
-  # one step, eager launches on the current stream
+  def _image_frames(self, live):
+    """Idle-streams runners: the slot's descriptors in image order (image i = stream live[i]); the padding images'
+    are zero, which the frames kernels read as invalid (a zero input)."""
+    arr = (L.Frame * self.B)()
+    for i, b in enumerate(live):
+      arr[i] = self.frames[b]
+    return arr
+
+  def _maps(self, live):
+    """int32 [2B]: streams (image -> stream, -1 for padding) then image_of (stream -> image, -1 when idle)."""
+    m = np.full(2 * self.B, -1, np.int32)
+    m[:len(live)] = live
+    m[self.B + np.asarray(live, np.int64)] = np.arange(len(live), dtype=np.int32)
+    return m
+
+  def padded_batch(self, n):
+    """The network batch of a step with n live streams: n rounded up to a multiple of idle_streams, at most B."""
+    g = self.idle_g or self.B
+    return min(-(-n // g) * g, self.B)
+
+  # one step, eager launches on the current stream, at the batch self._n (B but on an idle-streams runner)
   def _eager(self, slot, first=False):
-    if self.tracker is not None:
-      self.tracker.render(self.hm[slot][:self.B])            # pre_hm(t) from tracks(t-1)
+    n = self._n
+    NBn = 2 * n if self.flip else n
+    if self.tracker is not None:                             # pre_hm(t) from tracks(t-1)
+      if self.idle_g is None:
+        self.tracker.render(self.hm[slot][:self.B])
+      else:
+        self.tracker.render_mapped(self.hm[slot][:n], self.d_map[slot][self.B:])
     prev = slot if first else (slot - 1) % NS
     if self.frames_mode and self.eng.use_halo:
       eng = self.eng
@@ -329,42 +395,68 @@ class StreamRunner(object):
         L.check(pack(cur, pre, self.frames, self.B, *ms), 'ct_pack_stem_frames')
       else:                  # the slot's device descriptors: a replayed graph reads the geometry the slot holds
         pack = L.lib().ct_pack_stem_frames_flip_dev if self.flip else L.lib().ct_pack_stem_frames_dev
-        L.check(pack(cur, pre, L.ptr(self.d_frames[slot]), self.B, self.slot_bytes, *ms), 'ct_pack_stem_frames_dev')
-      out = dict(eng.forward_packed(eng.has_pre_img, eng.has_pre_hm))
+        L.check(pack(cur, pre, L.ptr(self.d_frames[slot]), n, self.slot_bytes, *ms), 'ct_pack_stem_frames_dev')
+      out = dict(eng.forward_packed(eng.has_pre_img, eng.has_pre_hm, n=NBn))
     else:
       if self.frames_mode:
         self._warp_frames(slot)
+      pre = self.img[prev]
+      if self.idle_g is not None and self.eng.has_pre_img:   # the previous frames through this step's descriptors
+        pre = self.pre_img
+        self._warp_frames(slot, src=self.u8[prev], dst=pre)
       if self.flip:                  # the mirrored half; pre_images (img[prev]) was mirrored by its own step
-        self._mirror(self.img[slot], 0, self.B)
+        self._mirror(self.img[slot], 0, n, n)
         if self.eng.has_pre_hm:
-          self._mirror(self.hm[slot], 0, self.B)
-      out = dict(self.eng.forward(self.img[slot], self.img[prev], self.hm[slot]))
+          self._mirror(self.hm[slot], 0, n, n)
+        if pre is not self.img[prev]:
+          self._mirror(pre, 0, n, n)
+      out = dict(self.eng.forward(self.img[slot][:NBn], pre[:NBn], self.hm[slot][:NBn], n=NBn))
     if self.flip:
-      out = flip_output(out, self.flip_plan, self.merged)
+      merged = self.merged if n == self.B else {h: m[:n] for h, m in self.merged.items()}
+      out = flip_output(out, self.flip_plan, merged)
     if self.ws is None:
       cat = out['hm'].shape[1]
       J = out['hm_hp'].shape[1] if ('hm_hp' in out and 'hps' in out) else 0
       self.ws = torch.zeros(L.lib().ct_decode_workspace_bytes(self.B, cat, J, self.K), dtype=torch.uint8,
                             device=self.device)
-    res = generic_decode(out, K=self.K, records_out=self.rec, workspace=self.ws)
+    rec = self.rec if (self.rec is None or n == self.B) else self.rec[:n]
+    res = generic_decode(out, K=self.K, records_out=rec, workspace=self._decode_ws(n))
     if self.rec is None:
       self.rec, self.layout = res.records, res.layout
-    if self.tracker is not None:
-      self.tracker.step(self.rec, *(self.pub[slot] if self.public else ()))    # tracks(t)
+    if self.tracker is not None:                             # tracks(t)
+      pub = self.pub[slot] if self.public else ()
+      if self.idle_g is None:
+        self.tracker.step(self.rec, *pub)
+      else:
+        self.tracker.step_mapped(self.rec[:n], self.d_map[slot][:self.B], *pub)
     return res
 
-  def _mirror(self, x, b, n):
-    """--flip_test: x[B+b : B+b+n] <- x[b : b+n] mirrored along W (ct_mirror_x), on the current stream."""
-    _, c, h, w = x.shape
-    L.check(L.lib().ct_mirror_x(L.ptr(x[b]), L.ptr(x[self.B + b]), n, c, h, w, L.stream_ptr()), 'ct_mirror_x')
+  def _decode_ws(self, n):
+    """The decode workspace of a batch n <= B.  ct_decode keeps n per-image counters at its start, which must be zero
+    on entry (each image's last CTA resets its own), and its candidates from align256(4 n) on.  At n < B the view starts
+    align256(4 B) - align256(4 n) bytes in, so that the candidates of every batch begin where the B-image layout's do
+    and never overwrite a counter of another batch."""
+    if n == self.B:
+      return self.ws
+    a = lambda x: (x + 255) // 256 * 256
+    return self.ws[a(4 * self.B) - a(4 * n):]
 
-  def _warp_frames(self, slot):
+  def _mirror(self, x, b, n, half=None):
+    """--flip_test: x[half+b : half+b+n] <- x[b : b+n] mirrored along W (ct_mirror_x), on the current stream; half =
+    the step's batch (B by default)."""
+    _, c, h, w = x.shape
+    half = self.B if half is None else half
+    L.check(L.lib().ct_mirror_x(L.ptr(x[b]), L.ptr(x[half + b]), n, c, h, w, L.stream_ptr()), 'ct_mirror_x')
+
+  def _warp_frames(self, slot, src=None, dst=None):
     """fp32 and bf16x3 engines: the slot's frames -> its fp32 image, one ct_warp_affine_normalize per stream (one
-    ct_warp_frames_normalize for all of them from the device descriptors on a capacity runner)."""
+    ct_warp_frames_normalize for all of them from the device descriptors on a capacity runner, at the step's batch).
+    src / dst (capacity runners): another frame slot through this slot's descriptors, into another image buffer."""
     lib, st = L.lib(), L.stream_ptr()
-    src, dst = self.u8[slot].data_ptr(), self.img[slot]
+    src = (self.u8[slot] if src is None else src).data_ptr()
+    dst = self.img[slot] if dst is None else dst
     if self.cap is not None:
-      L.check(lib.ct_warp_frames_normalize(C.c_void_p(src), L.ptr(self.d_frames[slot]), self.B, self.slot_bytes,
+      L.check(lib.ct_warp_frames_normalize(C.c_void_p(src), L.ptr(self.d_frames[slot]), self._n, self.slot_bytes,
                                            C.c_void_p(self.mean.ctypes.data), C.c_void_p(self.std.ctypes.data),
                                            L.ptr(dst), self.H, self.W, st), 'ct_warp_frames_normalize')
       return
@@ -374,46 +466,64 @@ class StreamRunner(object):
                                            L.ptr(dst[b]), self.H, self.W, st), 'ct_warp_affine_normalize')
 
   def _graph(self, slot):
+    if self.idle_g is not None:                              # one graph per (slot, batch), captured on first use
+      key = (slot, self._n)
+      if key not in self.idle_graphs:
+        self.idle_graphs[key] = self._capture(slot)
+      return self.idle_graphs[key]
     if self.graphs[slot] is None:
-      saved = None
-      if self.tracker is not None:                           # capture must not disturb live stream state
-        saved = [t.clone() for t in self._tracker_state()]
-      s = torch.cuda.Stream(device=self.device)
-      s.wait_stream(torch.cuda.current_stream())
-      with torch.cuda.stream(s):
-        self._eager(slot)
-      torch.cuda.current_stream().wait_stream(s)
-      g = torch.cuda.CUDAGraph()
-      with torch.cuda.graph(g):
-        self._eager(slot)
-      self.graphs[slot] = g
-      if saved is not None:
-        for t, v in zip(self._tracker_state(), saved):
-          t.copy_(v)
+      self.graphs[slot] = self._capture(slot)
     return self.graphs[slot]
+
+  def _capture(self, slot):
+    saved = None
+    if self.tracker is not None:                             # capture must not disturb live stream state
+      saved = [t.clone() for t in self._tracker_state()]
+    s = torch.cuda.Stream(device=self.device)
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+      self._eager(slot)
+    torch.cuda.current_stream().wait_stream(s)
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+      self._eager(slot)
+    if saved is not None:
+      for t, v in zip(self._tracker_state(), saved):
+        t.copy_(v)
+    return g
 
   def _tracker_state(self):
     trk = self.tracker
     return [trk.tracks, trk.counts, trk.boxes] + ([trk.payload] if trk.payload is not None else [])
 
+  def batches(self):
+    """The network batches a step may run at: B, or on an idle-streams runner every padded batch."""
+    return [self.B] if self.idle_g is None else sorted({self.padded_batch(n) for n in range(1, self.B + 1)})
+
   def warm(self):
-    for s in range(NS):
-      if self.use_graph:
-        self._graph(s)
-      else:
-        self._eager(s)
+    for n in self.batches():
+      self._n = n
+      for s in range(NS):
+        if self.use_graph:
+          self._graph(s)
+        else:
+          self._eager(s)
+    self._n = self.B
     if self.tracker is not None:
       self.tracker.reset()
     torch.cuda.synchronize(self.device)
 
   def reset_tracking(self):
     self.t = 0
+    if self.idle_g is not None:
+      self._was_idle = set()
     if self.tracker is not None:
       self.tracker.reset()
 
-  def _check_public(self, public_dets):
+  def _check_public(self, public_dets, idle=()):
     """public_dets: list of B arrays [P_b, 2] (the `ct` of each of the frame's public detections, image coordinates)
-    -> list of B float32 arrays; ValueError when they are missing, unexpected, or more than max_public_dets."""
+    -> list of B float32 arrays; ValueError when they are missing, unexpected, or more than max_public_dets.  The
+    entries of `idle` streams are ignored (and may be None)."""
     if not self.public:
       if public_dets is not None:
         raise ValueError('public detections are only read by device tracking with --public_det')
@@ -424,6 +534,9 @@ class StreamRunner(object):
       raise ValueError('public_dets: expected %d arrays (one per stream), got %d' % (self.B, len(public_dets)))
     out = []
     for b, p in enumerate(public_dets):
+      if b in idle:
+        out.append(np.zeros((0, 2), np.float32))
+        continue
       a = np.asarray(p, np.float32)
       if a.size == 0:
         a = a.reshape(0, 2)
@@ -536,7 +649,8 @@ class StreamRunner(object):
       # it is next written by the upload of step t+2, which waits for ev_done[prev], recorded after this step.
       prev = (slot - 1) % NS
       for b in streams:
-        if self.frames_mode and self.eng.use_halo:          # the pack kernel warps (and mirrors) u8[prev] again
+        # the pack kernel (or, on an idle-streams runner, the pre_images warp) reads u8[prev] again
+        if self.frames_mode and (self.eng.use_halo or self.idle_g is not None):
           f = self.frames[b]
           o, n = f.offset, f.h * f.w * 3
           self.u8[prev][o:o + n].copy_(self.u8[slot][o:o + n])
@@ -588,6 +702,8 @@ class StreamRunner(object):
     loc, rot_y); a started stream without one keeps its camera.
     Returns the records of the PREVIOUS call (None the first time) -- a one-step software pipeline: this step's H2D
     overlaps the previous step's compute."""
+    if self.idle_g is not None:
+      raise ValueError('step_host: a runner built with idle_streams takes raw frames (step_frames)')
     pub = self._check_public(public_dets)
     plan = self._check_starts(starts, pre_dets)
     cal = self._check_calibs(calibs, plan[0] if plan else ())
@@ -623,7 +739,10 @@ class StreamRunner(object):
     with torch.cuda.stream(self.compute):
       self.compute.wait_event(self.ev_in[slot])
       self._launch(slot)
-      self.h_rec[self.t & 1].copy_(self.rec, non_blocking=True)
+      if self._n == self.B:
+        self.h_rec[self.t & 1].copy_(self.rec, non_blocking=True)
+      else:                                          # the step's [n, K, F]; fetch() expands them to the streams
+        self.h_rec[self.t & 1][:self._n].copy_(self.rec[:self._n], non_blocking=True)
       if self.tracker is not None:
         self.h_trk[self.t & 1].copy_(self.tracker.tracks, non_blocking=True)
         self.h_cnt[self.t & 1].copy_(self.tracker.counts, non_blocking=True)
@@ -659,15 +778,20 @@ class StreamRunner(object):
     buf = self.h_u8[slot].numpy()
     return [buf[f.offset:f.offset + h * w * 3].reshape(h, w, 3) for f, (h, w) in zip(self.frames, sizes)]
 
-  def _frame_sizes_of(self, frames):
+  def _frame_sizes_of(self, frames, idle=()):
     """This step's (h, w) per stream: the shapes of `frames`, or the sizes of the last frame_buffers() call when None.
-    ValueError on a wrong count or dtype, or a shape that is not [h, w, 3]."""
+    ValueError on a wrong count or dtype, or a shape that is not [h, w, 3].  `idle` streams keep their size and their
+    entries are not looked at."""
     if frames is None:
-      return list(getattr(self, '_pending_sizes', None) or self.frame_sizes)
+      sizes = list(getattr(self, '_pending_sizes', None) or self.frame_sizes)
+      return [self.frame_sizes[b] if b in idle else hw for b, hw in enumerate(sizes)]
     if len(frames) != self.B:
       raise ValueError('frames: expected %d arrays (one per stream), got %d' % (self.B, len(frames)))
     sizes = []
     for b, (a, (h, w)) in enumerate(zip(frames, self.frame_sizes)):
+      if b in idle:
+        sizes.append((h, w))
+        continue
       if not isinstance(a, np.ndarray) or a.dtype != np.uint8:
         raise ValueError('frames[%d]: expected a uint8 numpy array, got %s' %
                          (b, getattr(a, 'dtype', type(a).__name__)))
@@ -678,29 +802,79 @@ class StreamRunner(object):
       sizes.append(a.shape[:2])
     return sizes
 
-  def step_frames(self, frames, pre_hms=None, public_dets=None, starts=None, pre_dets=None, calibs=None):
+  def _check_idle(self, idle, started, pre_hms):
+    """idle (the streams without a frame in this step) -> the live streams, ascending, or None on a runner built
+    without idle_streams.  ValueError before anything is enqueued: idle on such a runner, pre_hms on an idle-streams
+    runner, a stream out of range or repeated, every stream idle, a stream both idle and started, or a stream that was
+    idle in the last step and comes back without a video start."""
+    if self.idle_g is None:
+      if idle is not None:
+        raise ValueError('idle: this runner was built without idle_streams')
+      return None
+    if pre_hms is not None:
+      raise ValueError('pre_hms: a runner built with idle_streams renders its prior heat-maps itself (device_tracking) '
+                       'or runs without them')
+    gone = set()
+    for s in idle or ():
+      if isinstance(s, (bool, np.bool_)) or not isinstance(s, (int, np.integer)):
+        raise ValueError('idle: stream indices must be integers, got %r' % (s,))
+      s = int(s)
+      if not 0 <= s < self.B:
+        raise ValueError('idle: stream %d out of range [0, %d)' % (s, self.B))
+      if s in gone:
+        raise ValueError('idle: stream %d given twice' % s)
+      gone.add(s)
+    if len(gone) == self.B:
+      raise ValueError('idle: every stream is idle; a step needs at least one frame')
+    both = sorted(gone & set(started))
+    if both:
+      raise ValueError('idle: stream(s) %s also start a video in this step' % both)
+    live = [b for b in range(self.B) if b not in gone]
+    back = [b for b in live if b in self._was_idle and b not in started]
+    if back:
+      raise ValueError('stream(s) %s were idle in the last step: an idle stream comes back only with a video start '
+                       '(starts=)' % back)
+    return live
+
+  def step_frames(self, frames, pre_hms=None, public_dets=None, starts=None, pre_dets=None, calibs=None, idle=None):
     """frames: B uint8 [h_b, w_b, 3] BGR arrays of the sizes given as frame_sizes, or None when they were written
     through frame_buffers().  pre_hms, public_dets, starts, pre_dets, calibs and the return value as in step_host;
     public detections and pre_dets are in each stream's source pixels, and so are the tracks.  On a runner built with
     max_frame_size, a stream in `starts` may bring a frame of another size (that fits the region and maps to (H, W));
     without a calibs entry it then gets Detector._get_default_calib of that size.  ValueError (before anything is
     enqueued) on a wrong count, dtype or shape, a size change that is not allowed, or when the runner was not built
-    with frame_sizes."""
+    with frame_sizes.
+    idle (runners built with idle_streams): the streams without a frame in this step; their frames and public_dets
+    entries are ignored (and may be None), their tables, camera and frame region are left as they are, and their
+    records come back zero and their fetch_results() entries None.  A stream idle in one step comes back only with a
+    video start."""
     if not self.frames_mode:
       raise ValueError('step_frames: the runner was not built with frame_sizes (use step_host)')
-    pub = self._check_public(public_dets)
     plan = self._check_starts(starts, pre_dets)
     started = plan[0] if plan else ()
+    live = self._check_idle(idle, started, pre_hms)
+    gone = () if live is None else set(range(self.B)) - set(live)
+    pub = self._check_public(public_dets, gone)
     cal = self._check_calibs(calibs, started)
-    sizes = self._frame_sizes_of(frames)
+    sizes = self._frame_sizes_of(frames, gone)
     changed = self._check_sizes(sizes, started)
     slot = self.t % NS
     self._pending_sizes = None
-    desc, rows = self._plan_geometry(slot, changed, cal)
+    desc, rows = self._plan_geometry(slot, changed, cal, live)
+    maps = None
+    if live is not None:
+      self._was_idle = set(gone)
+      self._n = self.padded_batch(len(live))
+      self._live[self.t & 1] = live
+      now = self._maps(live).tobytes()
+      if now != self._map_mirror[slot]:
+        maps = self._map_mirror[slot] = now
+        self.h_map[slot].numpy()[:] = np.frombuffer(maps, np.int32)
     if frames is not None:
       # the slot's staging was last read by step t-3's upload, which the last fetch() waited for
-      for a, v in zip(frames, self._views(slot, self.frame_sizes)):
-        np.copyto(v, a)
+      for b, (a, v) in enumerate(zip(frames, self._views(slot, self.frame_sizes))):
+        if b not in gone:
+          np.copyto(v, a)
     if desc is not None:
       self.h_frames[slot].numpy()[:] = np.frombuffer(desc, np.uint8)
     if pub is not None:
@@ -716,12 +890,15 @@ class StreamRunner(object):
         self.u8[slot].copy_(self.h_u8[slot], non_blocking=True)
       else:                                          # the used bytes only, and the descriptors when they changed
         self._frame_bytes = 0
-        for a, e in self._upload_runs():
+        for a, e in self._upload_runs(live):
           self.u8[slot][a:e].copy_(self.h_u8[slot][a:e], non_blocking=True)
           self._frame_bytes += e - a
         if desc is not None:
           self.d_frames[slot].copy_(self.h_frames[slot], non_blocking=True)
           self._frame_bytes += len(desc)
+        if maps is not None:
+          self.d_map[slot].copy_(self.h_map[slot], non_blocking=True)
+          self._frame_bytes += len(maps)
       if use_hm:
         self.hm[slot][:self.B].copy_(src_hm, non_blocking=True)
       if pub is not None:
@@ -738,7 +915,26 @@ class StreamRunner(object):
     until the step after next is submitted)."""
     self.compute.synchronize()
     rec = self.h_rec[(self.t - 1) & 1].numpy()
+    live = self._live_of(self.t - 1)
+    if live is not None:                             # idle streams: zero rows
+      out = np.zeros_like(rec)
+      out[live] = rec[:len(live)]
+      return out
     return rec.copy() if copy else rec
+
+  def _live_of(self, t):
+    """The live streams of step t (one of the last two), or None when every stream had a frame."""
+    if self.idle_g is None:
+      return None
+    live = self._live[t & 1]
+    return None if live is None or len(live) == self.B else live
+
+  def _results(self, t):
+    i = t & 1
+    pay = self.h_pay[i].numpy() if self.tracker.payload is not None else None
+    live = self._live_of(t)
+    idle = () if live is None else set(range(self.B)) - set(live)
+    return self.tracker.results(self.h_trk[i].numpy(), self.h_cnt[i].numpy(), pay, idle)
 
   def fetch_tracks(self):
     """(tracks [B,T,CT_TRK_FLOATS], counts [B,2]) of the last submitted step (device_tracking), as numpy copies."""
@@ -748,11 +944,9 @@ class StreamRunner(object):
 
   def fetch_results(self):
     """The last submitted step's tracks (device_tracking) as the host path's per-stream lists of dicts
-    (DeviceTracker.results), payload fields included."""
+    (DeviceTracker.results), payload fields included; None for a stream that was idle in that step."""
     self.compute.synchronize()
-    i = (self.t - 1) & 1
-    pay = self.h_pay[i].numpy() if self.tracker.payload is not None else None
-    return self.tracker.results(self.h_trk[i].numpy(), self.h_cnt[i].numpy(), pay)
+    return self._results(self.t - 1)
 
   def previous_results(self):
     """After a step_host / step_frames call: the tracks of the step before it, as fetch_results() gives them.  No wait:
@@ -760,16 +954,15 @@ class StreamRunner(object):
     overwritten before the next call."""
     if self.t < 2:
       raise ValueError('previous_results(): fewer than two steps submitted')
-    i = (self.t - 2) & 1
-    pay = self.h_pay[i].numpy() if self.tracker.payload is not None else None
-    return self.tracker.results(self.h_trk[i].numpy(), self.h_cnt[i].numpy(), pay)
+    return self._results(self.t - 2)
 
   @property
   def h2d_bytes_per_step(self):
     """Bytes uploaded per step: the frames (and pre_hm / public detections); a step that starts videos with device
     tracking also uploads its start list and seed rows (and the tracker geometry rows of streams whose camera
     changes), counted here after that step is submitted.  A capacity runner uploads the bytes its streams' frames use,
-    plus the slot's descriptors in a step where they changed."""
+    plus the slot's descriptors in a step where they changed; an idle-streams runner the live streams' frames, plus the
+    descriptors and stream maps when they changed."""
     pub = self.B * (self.tracker.max_public * 2 + 1) * 4 if self.public else 0
     hm = self.B * self.H * self.W * 4 if self.tracker is None else 0
     if self.frames_mode:

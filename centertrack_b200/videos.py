@@ -5,7 +5,8 @@ init_track(pre_dets) at each video's first frame, then Detector.run on every fra
 A video goes to the first free stream (in frames mode, a free stream whose frame_sizes entry is the video's frame
 size; on a runner built with max_frame_size, any free stream, whose frame size changes at the start) and starts there
 with StreamRunner's `starts=` / `pre_dets=` / `calibs=`; when it ends, the stream takes the next video in the same step.
-A stream with no video re-feeds its last frame and its results are dropped.  The runner's one-step pipeline is kept:
+A stream with no video re-feeds its last frame and its results are dropped; on a runner built with idle_streams it is
+marked idle instead, and the step computes only the streams that play a video.  The runner's one-step pipeline is kept:
 the upload of step t+1 overlaps step t, and step t's tracks are yielded after step t+1 is submitted.
 """
 import numpy as np
@@ -47,6 +48,7 @@ def track_videos(runner, videos):
     raise ValueError('track_videos: the runner needs device_tracking=True')
   B = runner.B
   capacity = runner.frames_mode and getattr(runner, 'max_frame_bytes', None) is not None
+  idle_runner = getattr(runner, 'idle_g', None) is not None
   if runner.frames_mode:
     sizes = [tuple(s) for s in runner.frame_sizes]
   else:
@@ -112,6 +114,9 @@ def track_videos(runner, videos):
       if p is not None:
         last[b] = p.frame
         now[b] = (p.video.id, p.index)
+      elif idle_runner:               # no frame: the stream is idle in this step
+        frames.append(None)
+        continue
       elif last[b] is None:           # a stream that never had a video: any frame of its size
         last[b] = np.zeros(sizes[b] + (3,), np.uint8) if runner.frames_mode else torch.zeros(sizes[b])
       frames.append(last[b])
@@ -123,6 +128,8 @@ def track_videos(runner, videos):
         pd = p.video.public_dets if p is not None else None
         public.append(np.zeros((0, 2), np.float32) if pd is None else pd[p.index])
     kw = dict(public_dets=public, starts=started, pre_dets=pre_dets or None)
+    if idle_runner:
+      kw['idle'] = [b for b, p in enumerate(playing) if p is None]
     calibs = {b: playing[b].video.calib for b in started if playing[b].video.calib is not None}
     if calibs:
       kw['calibs'] = calibs

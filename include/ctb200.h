@@ -349,6 +349,19 @@ int ct_track_start(const ct_track_desc* d, const ct_track_payload* p, const int3
 /* pre_hm (fp32 [B,1,H,W], zeroed here) <- max-splat of boxes [n,5] (rows with radius < 0 skipped); n is the grid size,
  * so the launch shape does not depend on the data (CUDA-graph capturable). */
 int ct_render_tracks(const float* boxes, int32_t n, float* pre_hm, int32_t B, int32_t H, int32_t W, void* stream);
+/* Idle streams: the track step on a compacted batch.  CTA i (of d->B) runs stream streams[i] (device int32 [d->B]) on
+ * records[i], in every mode of ct_track_step_payload (a == NULL: greedy, private births; p == NULL: no payload).
+ * Every per-stream array (tracks, counts, boxes, trans_out_inv, trans_input, public_ct / public_n, steps, payload,
+ * calib) is indexed by the stream and has n_streams rows.  An entry < 0 or >= n_streams writes nothing; streams that
+ * are not listed are untouched.  A stream may appear at most once in `streams`: two CTAs on one stream would race on
+ * its tracks, counts, boxes and payload (not checked: the map is device memory). */
+int ct_track_step_mapped(const ct_track_desc* d, const ct_track_assoc* a, const ct_track_payload* p,
+                         const int32_t* streams, int32_t n_streams, void* stream);
+/* ct_render_tracks on a compacted batch: pre_hm (fp32 [n_images,1,H,W], zeroed here) <- the box rows of stream s
+ * (boxes [n,5], column 0 = s in [0, n_streams)) splatted into image image_of[s] (device int32 [n_streams]); rows whose
+ * stream maps outside [0, n_images) are skipped.  The launch shape depends on n alone (CUDA-graph capturable). */
+int ct_render_tracks_mapped(const float* boxes, int32_t n, const int32_t* image_of, int32_t n_streams, float* pre_hm,
+                            int32_t n_images, int32_t H, int32_t W, void* stream);
 
 /* out[c,y,x] = (in2[0,c,y,x] + sign[c] * in2[1,perm[c],y,W-1-x]) / 2;  in2 fp32 [2,C,H,W], out [1,C,H,W];
  * perm (int32 [C], device) / sign (fp32 [C], device) may be NULL (identity / +1). */

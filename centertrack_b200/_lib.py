@@ -100,10 +100,11 @@ class TrackPayload(C.Structure):
 
 
 CT_FRAMES_PER_LAUNCH = 48
+CT_FRAME_BGR, CT_FRAME_NV12, CT_FRAME_I420 = 0, 1, 2
 
 
 class Frame(C.Structure):
-  _fields_ = [('offset', C.c_int64), ('h', C.c_int32), ('w', C.c_int32), ('step', C.c_int32), ('reserved', C.c_int32),
+  _fields_ = [('offset', C.c_int64), ('h', C.c_int32), ('w', C.c_int32), ('step', C.c_int32), ('format', C.c_int32),
               ('minv', C.c_double * 6)]
 
 

@@ -16,7 +16,8 @@
 //                    (detector.py:207-226), cv2's fixed-point bilinear restated
 //   ct_pack_stem_frames        the same warp + normalise of B ragged uint8 frames (and of their previous frames),
 //                    written straight as the tensor-core stem's packed bf16 input; ct_pack_stem_frames_flip also
-//                    writes each stream's mirror image (--flip_test)
+//                    writes each stream's mirror image (--flip_test); the device-descriptor forms also take NV12 /
+//                    I420 frames, cv2.cvtColor(COLOR_YUV2BGR_NV12 / _I420) applied to each bilinear tap
 // All HBM-bound byte/index work: one pass over the data, coalesced, no tensor cores.
 #include <math_constants.h>
 
@@ -625,9 +626,23 @@ __device__ __forceinline__ int sat_int(double v) {        // cv::saturate_cast<i
   return __double2int_rn(v);
 }
 
+__device__ __forceinline__ int sat_u8(int v) { return v < 0 ? 0 : (v > 255 ? 255 : v); }
+
+// cv2.cvtColor's YUV 4:2:0 -> BGR of one pixel (COLOR_YUV2BGR_NV12 / _I420): BT.601 limited range in 20-bit fixed
+// point, y = max(Y - 16, 0) * 1.164, rounded by + 2^19 before the shift.  Every sum stays below 2^30 in magnitude.
+__device__ __forceinline__ void yuv_to_bgr(int Y, int U, int V, int bgr[3]) {
+  const int y = max(Y - 16, 0) * 1220542 + (1 << 19), u = U - 128, v = V - 128;
+  bgr[0] = sat_u8((y + 2116026 * u) >> 20);
+  bgr[1] = sat_u8((y - 852492 * v - 409993 * u) >> 20);
+  bgr[2] = sat_u8((y + 1673527 * v) >> 20);
+}
+
 // The warped uint8 BGR value of output pixel (x, y): src uint8 [sh, sw, 3] with row pitch sstep bytes, M the inverted
 // (dst -> src) map.  The one copy of the per-pixel warp arithmetic: ct_warp_affine_normalize and ct_pack_stem_frames
 // both call it, so that the fused stem input is byte-identical to the fp32 image packed afterwards.
+// FMT = CT_FRAME_NV12 / CT_FRAME_I420: src is the [3sh/2, sw] 4:2:0 frame (luma pitch sstep) and each tap inside the
+// frame is converted to BGR first, so the result is the warp of cv2.cvtColor's BGR image; taps outside read BGR 0.
+template <int FMT = CT_FRAME_BGR>
 __device__ __forceinline__ void warp_bilinear_u8(const unsigned char* __restrict__ img, int sh, int sw, int sstep,
                                                  const double* M, int x, int y, int p8[3]) {
   const int AB_BITS = 10, AB_SCALE = 1 << AB_BITS, INTER_BITS = 5, INTER_TAB = 1 << INTER_BITS;
@@ -643,17 +658,43 @@ __device__ __forceinline__ void warp_bilinear_u8(const unsigned char* __restrict
   // entry, fx = fy = 0, yields the same pixel as the exact weight 32768)
   const int fx = X & (INTER_TAB - 1), fy = Y & (INTER_TAB - 1);
   const int w[4] = {(32 - fy) * (32 - fx) * 32, (32 - fy) * fx * 32, fy * (32 - fx) * 32, fy * fx * 32};
+  if constexpr (FMT == CT_FRAME_BGR) {
 #pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    int acc = 0;
+    for (int c = 0; c < 3; ++c) {
+      int acc = 0;
+#pragma unroll
+      for (int t = 0; t < 4; ++t) {
+        const int yy = sy + (t >> 1), xx = sx + (t & 1);
+        const int v = ((unsigned)yy < (unsigned)sh && (unsigned)xx < (unsigned)sw) ? img[(size_t)yy * sstep + xx * 3 + c] : 0;
+        acc += v * w[t];
+      }
+      p8[c] = sat_u8((acc + (1 << 14)) >> 15);
+    }
+  } else {
+    const unsigned char* chroma = img + (size_t)sh * sstep;
+    int acc[3] = {0, 0, 0};
 #pragma unroll
     for (int t = 0; t < 4; ++t) {
       const int yy = sy + (t >> 1), xx = sx + (t & 1);
-      const int v = ((unsigned)yy < (unsigned)sh && (unsigned)xx < (unsigned)sw) ? img[(size_t)yy * sstep + xx * 3 + c] : 0;
-      acc += v * w[t];
+      if ((unsigned)yy < (unsigned)sh && (unsigned)xx < (unsigned)sw) {
+        int U, V;
+        if constexpr (FMT == CT_FRAME_NV12) {       // row yy/2 of interleaved U V, the pair of column xx/2
+          const unsigned char* uv = chroma + (size_t)(yy >> 1) * sstep + (xx & ~1);
+          U = uv[0];
+          V = uv[1];
+        } else {       // I420: half-row k of the chroma planes lies at (k/2) pitch + (k%2) sw/2; U = 0..sh/2-1, V after
+          const int ku = yy >> 1, kv = (sh >> 1) + ku, cx = xx >> 1;
+          U = chroma[(size_t)(ku >> 1) * sstep + (ku & 1) * (sw >> 1) + cx];
+          V = chroma[(size_t)(kv >> 1) * sstep + (kv & 1) * (sw >> 1) + cx];
+        }
+        int bgr[3];
+        yuv_to_bgr(img[(size_t)yy * sstep + xx], U, V, bgr);
+#pragma unroll
+        for (int c = 0; c < 3; ++c) acc[c] += bgr[c] * w[t];
+      }
     }
-    const int pix = (acc + (1 << 14)) >> 15;
-    p8[c] = pix < 0 ? 0 : (pix > 255 ? 255 : pix);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) p8[c] = sat_u8((acc[c] + (1 << 14)) >> 15);
   }
 }
 
@@ -662,15 +703,20 @@ __device__ __forceinline__ float normalize_u8(int v, float mean, float stdv) {
   return (float)(((double)v / 255.0 - (double)mean) / (double)stdv);
 }
 
-// One fp32 CHW output pixel (x, y) of ct_warp_affine_normalize: o points at channel 0, planes `plane` floats apart.
+// ((v / 255 - mean) / std) of a warped pixel into an fp32 CHW image: o points at channel 0, planes `plane` floats apart.
+__device__ __forceinline__ void store_norm_pixel(const int p8[3], float* o, size_t plane, float3 mean, float3 stdv) {
+  o[0] = normalize_u8(p8[0], mean.x, stdv.x);
+  o[plane] = normalize_u8(p8[1], mean.y, stdv.y);
+  o[2 * plane] = normalize_u8(p8[2], mean.z, stdv.z);
+}
+
+// One fp32 CHW output pixel (x, y) of ct_warp_affine_normalize.
 __device__ __forceinline__ void warp_norm_pixel(const unsigned char* __restrict__ img, int sh, int sw, int sstep,
                                                 const double* M, int x, int y, float* o, size_t plane, float3 mean,
                                                 float3 stdv) {
   int p8[3];
   warp_bilinear_u8(img, sh, sw, sstep, M, x, y, p8);
-  o[0] = normalize_u8(p8[0], mean.x, stdv.x);
-  o[plane] = normalize_u8(p8[1], mean.y, stdv.y);
-  o[2 * plane] = normalize_u8(p8[2], mean.z, stdv.z);
+  store_norm_pixel(p8, o, plane, mean, stdv);
 }
 
 __global__ void warp_affine_norm_kernel(const unsigned char* __restrict__ src, int sh, int sw, int sstep,
@@ -693,18 +739,42 @@ __global__ void warp_affine_norm_kernel(const unsigned char* __restrict__ src, i
 // replays; each CTA copies its stream's descriptor to shared memory once and checks it against the buffer size, since
 // the host cannot: an invalid one yields zeros and no read of the frame buffers.
 // ------------------------------------------------------------------------------------------------------------------
+// kFormats: the descriptors may name any CT_FRAME_* format (the host checks the by-value ones to be BGR).
 struct ParamFrames {
+  static constexpr bool kFormats = false;
   ct_frame f[CT_FRAMES_PER_LAUNCH];
 };
 
 struct DeviceFrames {
+  static constexpr bool kFormats = true;
   const ct_frame* f;
   long long buf_bytes;
 };
 
+// a known format, even sizes for 4:2:0, a row pitch that holds a row, and every row read inside the buffer
 __device__ __forceinline__ bool frame_in_buffer(const ct_frame& f, long long buf_bytes) {
-  return f.h > 0 && f.w > 0 && f.offset >= 0 && (long long)f.step >= 3LL * f.w &&
-         f.offset <= buf_bytes && (long long)(f.h - 1) * f.step + 3LL * f.w <= buf_bytes - f.offset;
+  if (f.h <= 0 || f.w <= 0 || f.offset < 0 || f.offset > buf_bytes) return false;
+  long long rows = f.h, row_bytes = 3LL * f.w;
+  if (f.format == CT_FRAME_NV12 || f.format == CT_FRAME_I420) {
+    if ((f.h | f.w) & 1) return false;
+    rows = 3LL * (f.h / 2);
+    row_bytes = f.w;
+  } else if (f.format != CT_FRAME_BGR) {
+    return false;
+  }
+  return (long long)f.step >= row_bytes && (rows - 1) * f.step + row_bytes <= buf_bytes - f.offset;
+}
+
+// The warped BGR pixel (x, y) of the frame f describes at src (its first byte), in f's format `fmt`.  Frames without
+// formats compile the BGR sampler alone.
+template <class Frames>
+__device__ __forceinline__ void warp_frame_u8(const unsigned char* __restrict__ src, const ct_frame& f, int fmt, int x,
+                                              int y, int p8[3]) {
+  if constexpr (Frames::kFormats) {
+    if (fmt == CT_FRAME_NV12) return warp_bilinear_u8<CT_FRAME_NV12>(src, f.h, f.w, f.step, f.minv, x, y, p8);
+    if (fmt == CT_FRAME_I420) return warp_bilinear_u8<CT_FRAME_I420>(src, f.h, f.w, f.step, f.minv, x, y, p8);
+  }
+  warp_bilinear_u8(src, f.h, f.w, f.step, f.minv, x, y, p8);
 }
 
 // -> this CTA's descriptor (stream b0 + blockIdx.y) and whether it may be read; ends with __syncthreads()
@@ -731,14 +801,18 @@ __global__ void warp_frames_norm_kernel(const unsigned char* __restrict__ src, c
   __shared__ ct_frame s_f;
   bool ok;
   const ct_frame& f = cta_frame(fs, 0, &s_f, ok);
+  const int fmt = f.format;
   const size_t plane = (size_t)oh * ow;
   float* o = dst + (size_t)blockIdx.y * 3 * plane;
   for (size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x; r < plane; r += (size_t)gridDim.x * blockDim.x) {
     const int y = (int)(r / ow), x = (int)(r - (size_t)y * ow);
-    if (ok)
-      warp_norm_pixel(src + f.offset, f.h, f.w, f.step, f.minv, x, y, o + r, plane, mean, stdv);
-    else
+    if (ok) {
+      int p8[3];
+      warp_frame_u8<DeviceFrames>(src + f.offset, f, fmt, x, y, p8);
+      store_norm_pixel(p8, o + r, plane, mean, stdv);
+    } else {
       o[r] = o[r + plane] = o[r + 2 * plane] = 0.f;
+    }
   }
 }
 
@@ -755,24 +829,14 @@ __global__ void warp_frames_norm_kernel(const unsigned char* __restrict__ src, c
 constexpr int PACK_THREADS = 256;
 constexpr int PACK_PIX_PER_THREAD = 4;      // pixels per thread: amortises the table build over 1024 pixels per CTA
 
-template <bool FLIP, class Frames>
-__global__ void __launch_bounds__(PACK_THREADS)
-pack_stem_frames_kernel(const unsigned char* __restrict__ cur, const unsigned char* __restrict__ prev,
-                        const __grid_constant__ Frames fs, int b0, int B, float3 mean, float3 stdv,
-                        const float* __restrict__ hm, uint4* __restrict__ out, int H, int W) {
-  __shared__ float tab[3][256];
-  __shared__ ct_frame s_f;
-  for (int i = threadIdx.x; i < 3 * 256; i += PACK_THREADS) {
-    const int c = i >> 8, v = i & 255;
-    tab[c][v] = normalize_u8(v, c == 0 ? mean.x : (c == 1 ? mean.y : mean.z), c == 0 ? stdv.x : (c == 1 ? stdv.y : stdv.z));
-  }
-  bool ok;
-  const ct_frame& f = cta_frame(fs, b0, &s_f, ok);
-  const int b = b0 + blockIdx.y;
+// The PACK_PIX_PER_THREAD output pixels of one thread, frame format FMT (uniform over the CTA, so each format's loop
+// is a code region of its own and a BGR stream runs the BGR-only loop)
+template <bool FLIP, int FMT>
+__device__ __forceinline__ void pack_pixels(const unsigned char* __restrict__ src, const unsigned char* __restrict__ psrc,
+                                            const ct_frame& f, bool ok, const float (*tab)[256], int b, int B,
+                                            size_t base, const float* __restrict__ hm, uint4* __restrict__ out, int H,
+                                            int W) {
   const size_t plane = (size_t)H * W;
-  const unsigned char* src = cur + f.offset;
-  const unsigned char* psrc = prev ? prev + f.offset : nullptr;
-  const size_t base = (size_t)blockIdx.x * PACK_THREADS * PACK_PIX_PER_THREAD + threadIdx.x;
 #pragma unroll
   for (int k = 0; k < PACK_PIX_PER_THREAD; ++k) {
     const size_t r = base + (size_t)k * PACK_THREADS;
@@ -782,11 +846,11 @@ pack_stem_frames_kernel(const unsigned char* __restrict__ cur, const unsigned ch
     if (ok) {
       float v[8];
       int p8[3];
-      warp_bilinear_u8(src, f.h, f.w, f.step, f.minv, x, y, p8);
+      warp_bilinear_u8<FMT>(src, f.h, f.w, f.step, f.minv, x, y, p8);
 #pragma unroll
       for (int c = 0; c < 3; ++c) v[c] = tab[c][p8[c]];
       if (psrc) {
-        warp_bilinear_u8(psrc, f.h, f.w, f.step, f.minv, x, y, p8);
+        warp_bilinear_u8<FMT>(psrc, f.h, f.w, f.step, f.minv, x, y, p8);
 #pragma unroll
         for (int c = 0; c < 3; ++c) v[3 + c] = tab[c][p8[c]];
       } else {
@@ -801,6 +865,53 @@ pack_stem_frames_kernel(const unsigned char* __restrict__ cur, const unsigned ch
     out[(size_t)b * plane + r] = o;
     if constexpr (FLIP) out[(size_t)(B + b) * plane + (size_t)y * W + (W - 1 - x)] = o;
   }
+}
+
+template <bool FLIP, class Frames>
+__device__ __forceinline__ void pack_stem_frames_body(const unsigned char* __restrict__ cur,
+                                                      const unsigned char* __restrict__ prev, const Frames& fs, int b0,
+                                                      int B, float3 mean, float3 stdv, const float* __restrict__ hm,
+                                                      uint4* __restrict__ out, int H, int W) {
+  __shared__ float tab[3][256];
+  __shared__ ct_frame s_f;
+  for (int i = threadIdx.x; i < 3 * 256; i += PACK_THREADS) {
+    const int c = i >> 8, v = i & 255;
+    tab[c][v] = normalize_u8(v, c == 0 ? mean.x : (c == 1 ? mean.y : mean.z), c == 0 ? stdv.x : (c == 1 ? stdv.y : stdv.z));
+  }
+  bool ok;
+  const ct_frame& f = cta_frame(fs, b0, &s_f, ok);
+  const int b = b0 + blockIdx.y;
+  const unsigned char* src = cur + f.offset;
+  const unsigned char* psrc = prev ? prev + f.offset : nullptr;
+  const size_t base = (size_t)blockIdx.x * PACK_THREADS * PACK_PIX_PER_THREAD + threadIdx.x;
+  if constexpr (Frames::kFormats) {
+    const int fmt = f.format;
+    if (fmt == CT_FRAME_NV12)
+      return pack_pixels<FLIP, CT_FRAME_NV12>(src, psrc, f, ok, tab, b, B, base, hm, out, H, W);
+    if (fmt == CT_FRAME_I420)
+      return pack_pixels<FLIP, CT_FRAME_I420>(src, psrc, f, ok, tab, b, B, base, hm, out, H, W);
+  }
+  pack_pixels<FLIP, CT_FRAME_BGR>(src, psrc, f, ok, tab, b, B, base, hm, out, H, W);
+}
+
+template <bool FLIP>
+__global__ void __launch_bounds__(PACK_THREADS)
+pack_stem_frames_kernel(const unsigned char* __restrict__ cur, const unsigned char* __restrict__ prev,
+                        const __grid_constant__ ParamFrames fs, int b0, int B, float3 mean, float3 stdv,
+                        const float* __restrict__ hm, uint4* __restrict__ out, int H, int W) {
+  pack_stem_frames_body<FLIP>(cur, prev, fs, b0, B, mean, stdv, hm, out, H, W);
+}
+
+// The device-descriptor forms: 6 CTAs per SM, at most 40 registers -- the occupancy of the BGR-only sampler's 36
+// (allocated in steps of 8); without the bound the YUV samplers take the flip form to 48 registers and 5 CTAs.
+constexpr int PACK_DEV_MIN_CTAS = 6;
+
+template <bool FLIP>
+__global__ void __launch_bounds__(PACK_THREADS, PACK_DEV_MIN_CTAS)
+pack_stem_frames_dev_kernel(const unsigned char* __restrict__ cur, const unsigned char* __restrict__ prev,
+                            const __grid_constant__ DeviceFrames fs, float3 mean, float3 stdv,
+                            const float* __restrict__ hm, uint4* __restrict__ out, int H, int W) {
+  pack_stem_frames_body<FLIP>(cur, prev, fs, 0, gridDim.y, mean, stdv, hm, out, H, W);
 }
 
 }  // namespace ctb
@@ -981,9 +1092,12 @@ static int pack_stem_frames(const uint8_t* cur, const uint8_t* prev, const ct_fr
                             void* stream) {
   CT_REQUIRE(cur && frames && mean && std && out, "null pointer");
   CT_REQUIRE(B > 0 && H > 0 && W > 0, "bad shape");
-  for (int32_t b = 0; b < B; ++b)
+  for (int32_t b = 0; b < B; ++b) {
+    CT_REQUIRE(frames[b].format == CT_FRAME_BGR,
+               "by-value frame descriptors take CT_FRAME_BGR only (YUV frames: the _dev entry points)");
     CT_REQUIRE(frames[b].offset >= 0 && frames[b].h > 0 && frames[b].w > 0 && frames[b].step >= 3 * frames[b].w,
                "bad frame descriptor (offset >= 0, h > 0, w > 0, step >= 3 w)");
+  }
   const size_t plane = (size_t)H * W;
   const size_t per_cta = (size_t)PACK_THREADS * PACK_PIX_PER_THREAD;
   CT_REQUIRE((plane + per_cta - 1) / per_cta <= 0x7fffffffu, "output too large");
@@ -994,7 +1108,7 @@ static int pack_stem_frames(const uint8_t* cur, const uint8_t* prev, const ct_fr
     ParamFrames fa = {};
     memcpy(fa.f, frames + b0, sizeof(ct_frame) * n);
     dim3 grid((unsigned)((plane + per_cta - 1) / per_cta), (unsigned)n);
-    pack_stem_frames_kernel<FLIP, ParamFrames><<<grid, PACK_THREADS, 0, (cudaStream_t)stream>>>(
+    pack_stem_frames_kernel<FLIP><<<grid, PACK_THREADS, 0, (cudaStream_t)stream>>>(
         cur, prev, fa, b0, B, m, s, pre_hm, (uint4*)out, H, W);
     const int rc = after_launch();
     if (rc != CT_OK) return rc;
@@ -1026,8 +1140,8 @@ static int pack_stem_frames_dev(const uint8_t* cur, const uint8_t* prev, const c
   CT_REQUIRE((plane + per_cta - 1) / per_cta <= 0x7fffffffu, "output too large");
   const DeviceFrames fs = {frames_dev, (long long)buf_bytes};
   dim3 grid((unsigned)((plane + per_cta - 1) / per_cta), (unsigned)B);
-  pack_stem_frames_kernel<FLIP, DeviceFrames><<<grid, PACK_THREADS, 0, (cudaStream_t)stream>>>(
-      cur, prev, fs, 0, B, make_float3(mean[0], mean[1], mean[2]), make_float3(std[0], std[1], std[2]), pre_hm,
+  pack_stem_frames_dev_kernel<FLIP><<<grid, PACK_THREADS, 0, (cudaStream_t)stream>>>(
+      cur, prev, fs, make_float3(mean[0], mean[1], mean[2]), make_float3(std[0], std[1], std[2]), pre_hm,
       (uint4*)out, H, W);
   return after_launch();
 }

@@ -34,6 +34,9 @@ ct_warp_affine_normalize and run their plan unchanged.  The tracker gets each st
 tracks, public detections and 3D boxes are in that camera's pixels.  With max_frame_size, stream b's frame lives at
 b * cap in every slot and each slot's descriptors are a device array (ct_pack_stem_frames_dev, ct_warp_frames_normalize),
 so a stream may take a frame of another size, and a new camera, when it starts a video, without recapturing a graph.
+A capacity runner may take NV12 or I420 frames instead (`frame_format`, what video decoders emit): each [3h/2, w] frame
+is uploaded as it is, half the bytes of BGR, and the device-descriptor kernels convert each bilinear tap to BGR with
+cv2.cvtColor's fixed-point arithmetic, so the stream computes what it computes on the cv2-converted BGR frame.
 
 Video starts (`starts=`, `pre_dets=` of step_host / step_frames / load_device_inputs): a stream may begin a new video at
 any step, as Detector.reset_tracking + Tracker.init_track(pre_dets) on that stream alone.  A start is rare (once per
@@ -75,12 +78,36 @@ NS = 3          # input slots
 # pads (n = 1, 2); a larger g only saves graphs.
 IDLE_GRANULE = 1
 
+# frame_format -> ct_frame.format
+FRAME_FORMATS = {'bgr': L.CT_FRAME_BGR, 'nv12': L.CT_FRAME_NV12, 'i420': L.CT_FRAME_I420}
+
+
+def frame_layout(fmt, h, w):
+  """(array shape, bytes, row pitch) of an h x w source frame in format fmt: BGR is [h, w, 3]; NV12 and I420 are one
+  [3h/2, w] uint8 array each (cv2's 4:2:0 layouts), half the bytes."""
+  if fmt == 'bgr':
+    return (h, w, 3), h * w * 3, 3 * w
+  return (h * 3 // 2, w), h * w * 3 // 2, w
+
+
+def frame_size_of(fmt, shape):
+  """The (h, w) of a frame array of this shape in format fmt, or None when the shape is not one of fmt's: BGR
+  [h, w, 3]; NV12 / I420 [R, w] with R a multiple of 3 (h = 2R/3) and w even."""
+  shape = tuple(shape)
+  if fmt == 'bgr':
+    return shape[:2] if len(shape) == 3 and shape[2] == 3 else None
+  if len(shape) != 2 or shape[0] % 3 or shape[1] % 2:
+    return None
+  return shape[0] // 3 * 2, shape[1]
+
 
 class StreamRunner(object):
 
+  frame_format = 'bgr'
+
   def __init__(self, model, B, H, W, K=100, precision='bf16', device='cuda', use_graph=True, opt=None,
                device_tracking=False, max_public_dets=512, calibs=None, frame_sizes=None, max_frame_size=None,
-               idle_streams=None):
+               idle_streams=None, frame_format='bgr'):
     """max_public_dets: with device_tracking and --public_det, the most public detections a stream may bring per
     frame (more raise ValueError; none is ever dropped).  calibs: with device_tracking on a 3D head set, one [3,4]
     camera matrix per stream (DeviceTracker's default otherwise; in frames mode Detector._get_default_calib of the
@@ -93,7 +120,11 @@ class StreamRunner(object):
     before decode, as Detector.process does; inputs and outputs keep their B shapes.
     idle_streams g >= 1, or True for g = IDLE_GRANULE (capacity frames runners only): step_frames(idle=) may leave
     streams without a frame, and a step computes only the live ones, in a batch rounded up to a multiple of g (see the
-    module docstring).  None or False: off."""
+    module docstring).  None or False: off.
+    frame_format: what step_frames and frame_buffers take -- 'bgr' (uint8 [h, w, 3]), or 'nv12' / 'i420' (one uint8
+    [3h/2, w] array per frame in cv2's 4:2:0 layout, h and w even; needs max_frame_size, whose region is then
+    h * w * 3 / 2 bytes).  A 4:2:0 frame is converted on the device, inside the warp, exactly as
+    cv2.cvtColor(COLOR_YUV2BGR_NV12 / _I420) converts it: a stream gives what it gives on that BGR image."""
     self.B, self.H, self.W, self.K = B, H, W, K
     self.device = torch.device(device)
     self.model = model
@@ -101,6 +132,12 @@ class StreamRunner(object):
     self.frames_mode = frame_sizes is not None
     if max_frame_size is not None and not self.frames_mode:
       raise ValueError('max_frame_size needs frame_sizes (frames mode)')
+    if frame_format not in FRAME_FORMATS:
+      raise ValueError('frame_format: expected one of %s, got %r' % (sorted(FRAME_FORMATS), frame_format))
+    if frame_format != 'bgr' and max_frame_size is None:
+      raise ValueError("frame_format=%r needs frame_sizes and max_frame_size (the device-descriptor frames path)" %
+                       (frame_format,))
+    self.frame_format = frame_format
     self.idle_g = None
     if idle_streams is True:                                 # on, with the default granule
       idle_streams = IDLE_GRANULE
@@ -217,7 +254,7 @@ class StreamRunner(object):
       mh, mw = (int(v) for v in max_frame_size)
       if mh <= 0 or mw <= 0:
         raise ValueError('max_frame_size: bad size %s' % ((mh, mw),))
-      self.max_frame_bytes = mh * mw * 3
+      self.max_frame_bytes = frame_layout(self.frame_format, mh, mw)[1]
       self.cap = (self.max_frame_bytes + 15) // 16 * 16        # stream b's frame lives at b * cap in every slot
     ds = get_dataset(opt.dataset)
     self.focal = opt.test_focal_length if getattr(opt, 'test_focal_length', -1) >= 0 else ds.rest_focal_length
@@ -232,9 +269,10 @@ class StreamRunner(object):
       meta['calib'] = calibs[b] if calibs is not None else default_calib(self.focal, w, h)
       self._meta.append(meta)
       f = self.frames[b]
-      f.offset, f.h, f.w, f.step = (off if self.cap is None else b * self.cap), h, w, 3 * w
+      _, nbytes, f.step = frame_layout(self.frame_format, h, w)
+      f.offset, f.h, f.w, f.format = (off if self.cap is None else b * self.cap), h, w, FRAME_FORMATS[self.frame_format]
       f.minv[:] = minv.tolist()
-      off += (h * w * 3 + 15) // 16 * 16
+      off += (nbytes + 15) // 16 * 16
     self._prev_meta = self._meta
     self.frame_sizes = [(int(h), int(w)) for h, w in frame_sizes]
     self.slot_bytes = off if self.cap is None else B * self.cap
@@ -242,11 +280,14 @@ class StreamRunner(object):
 
   def _size_geometry(self, what, h, w):
     """(meta without calib, minv) of an h x w source frame; ValueError when it is empty, does not fit a capacity
-    runner's frame region, or maps to another network input than (H, W)."""
+    runner's frame region, is odd in a 4:2:0 format, or maps to another network input than (H, W)."""
     if h <= 0 or w <= 0:
       raise ValueError('%s: bad size %s' % (what, (h, w)))
-    if self.cap is not None and h * w * 3 > self.max_frame_bytes:
-      raise ValueError('%s = %s: %d bytes, more than the %d of max_frame_size' % (what, (h, w), h * w * 3,
+    if self.frame_format != 'bgr' and (h % 2 or w % 2):
+      raise ValueError('%s = %s: %s frames have an even height and width' % (what, (h, w), self.frame_format.upper()))
+    nbytes = frame_layout(self.frame_format, h, w)[1]
+    if self.cap is not None and nbytes > self.max_frame_bytes:
+      raise ValueError('%s = %s: %d bytes, more than the %d of max_frame_size' % (what, (h, w), nbytes,
                                                                                  self.max_frame_bytes))
     meta, minv = frame_geometry(self.opt, h, w)
     if (meta['inp_height'], meta['inp_width']) != (self.H, self.W):
@@ -320,7 +361,7 @@ class StreamRunner(object):
       for b, (meta, minv) in changed.items():
         h, w = meta['height'], meta['width']
         f = self.frames[b]
-        f.h, f.w, f.step = h, w, 3 * w
+        f.h, f.w, f.step = h, w, frame_layout(self.frame_format, h, w)[2]
         f.minv[:] = minv.tolist()
         meta['calib'] = calibs[b] if b in calibs else default_calib(self.focal, w, h)
         self._meta[b] = meta
@@ -348,7 +389,7 @@ class StreamRunner(object):
     for b, f in enumerate(self.frames):
       if live is not None and b not in live:
         continue
-      a, e = b * self.cap, b * self.cap + (f.h * f.w * 3 + 15) // 16 * 16
+      a, e = b * self.cap, b * self.cap + (frame_layout(self.frame_format, f.h, f.w)[1] + 15) // 16 * 16
       if runs and runs[-1][1] == a:
         runs[-1][1] = e
       else:
@@ -652,10 +693,15 @@ class StreamRunner(object):
         # the pack kernel (or, on an idle-streams runner, the pre_images warp) reads u8[prev] again
         if self.frames_mode and (self.eng.use_halo or self.idle_g is not None):
           f = self.frames[b]
-          o, n = f.offset, f.h * f.w * 3
+          o, n = f.offset, frame_layout(self.frame_format, f.h, f.w)[1]
           self.u8[prev][o:o + n].copy_(self.u8[slot][o:o + n])
           continue
-        if self.frames_mode:                                 # the plan reads img[prev]: warp this frame into it
+        if self.frames_mode and self.frame_format != 'bgr':  # through the slot's device descriptor, which has the format
+          L.check(L.lib().ct_warp_frames_normalize(
+              L.ptr(self.u8[slot]), C.c_void_p(self.d_frames[slot].data_ptr() + b * C.sizeof(L.Frame)), 1,
+              self.slot_bytes, C.c_void_p(self.mean.ctypes.data), C.c_void_p(self.std.ctypes.data),
+              L.ptr(self.img[prev][b]), self.H, self.W, L.stream_ptr()), 'ct_warp_frames_normalize')
+        elif self.frames_mode:                               # the plan reads img[prev]: warp this frame into it
           f = self.frames[b]
           # a capacity runner's minv: the slot's device descriptor of this frame (its new geometry after a size change)
           minv = L.ptr(self.minv[b]) if self.cap is None else \
@@ -754,7 +800,8 @@ class StreamRunner(object):
     return prev
 
   def frame_buffers(self, sizes=None):
-    """Frames mode: numpy views [h_b, w_b, 3] uint8 of the pinned staging the NEXT step_frames uploads, one per stream,
+    """Frames mode: numpy views [h_b, w_b, 3] uint8 ([3h_b/2, w_b] with frame_format 'nv12' or 'i420') of the pinned
+    staging the NEXT step_frames uploads, one per stream,
     for a decoder to write its frames in place; then call step_frames(None).  They may be written once the previous
     step_frames call has returned (its upload of three steps ago, which last read this staging, has completed by
     then) and until the next step_frames call.  sizes ({stream: (h, w)}, capacity runners): the views of those streams
@@ -776,12 +823,16 @@ class StreamRunner(object):
 
   def _views(self, slot, sizes):
     buf = self.h_u8[slot].numpy()
-    return [buf[f.offset:f.offset + h * w * 3].reshape(h, w, 3) for f, (h, w) in zip(self.frames, sizes)]
+    views = []
+    for f, (h, w) in zip(self.frames, sizes):
+      shape, n, _ = frame_layout(self.frame_format, h, w)
+      views.append(buf[f.offset:f.offset + n].reshape(shape))
+    return views
 
   def _frame_sizes_of(self, frames, idle=()):
     """This step's (h, w) per stream: the shapes of `frames`, or the sizes of the last frame_buffers() call when None.
-    ValueError on a wrong count or dtype, or a shape that is not [h, w, 3].  `idle` streams keep their size and their
-    entries are not looked at."""
+    ValueError on a wrong count or dtype, or a shape that is not [h, w, 3] ([3h/2, w] with R = 3h/2 a multiple of 3 and
+    w even, in a 4:2:0 frame_format).  `idle` streams keep their size and their entries are not looked at."""
     if frames is None:
       sizes = list(getattr(self, '_pending_sizes', None) or self.frame_sizes)
       return [self.frame_sizes[b] if b in idle else hw for b, hw in enumerate(sizes)]
@@ -797,9 +848,13 @@ class StreamRunner(object):
                          (b, getattr(a, 'dtype', type(a).__name__)))
       if self.cap is None and a.shape != (h, w, 3):
         raise ValueError('frames[%d]: expected shape %s, got %s' % (b, (h, w, 3), a.shape))
-      if a.ndim != 3 or a.shape[2] != 3:
+      hw = frame_size_of(self.frame_format, a.shape)
+      if hw is None and self.frame_format == 'bgr':
         raise ValueError('frames[%d]: expected shape [h, w, 3], got %s' % (b, a.shape))
-      sizes.append(a.shape[:2])
+      if hw is None:
+        raise ValueError('frames[%d]: expected a %s frame of shape [3h/2, w] (rows a multiple of 3, w even), got %s' %
+                         (b, self.frame_format.upper(), a.shape))
+      sizes.append(hw)
     return sizes
 
   def _check_idle(self, idle, started, pre_hms):
@@ -837,8 +892,8 @@ class StreamRunner(object):
     return live
 
   def step_frames(self, frames, pre_hms=None, public_dets=None, starts=None, pre_dets=None, calibs=None, idle=None):
-    """frames: B uint8 [h_b, w_b, 3] BGR arrays of the sizes given as frame_sizes, or None when they were written
-    through frame_buffers().  pre_hms, public_dets, starts, pre_dets, calibs and the return value as in step_host;
+    """frames: B uint8 [h_b, w_b, 3] BGR arrays of the sizes given as frame_sizes (with frame_format 'nv12' / 'i420':
+    [3h_b/2, w_b] arrays in that layout), or None when they were written through frame_buffers().  pre_hms, public_dets, starts, pre_dets, calibs and the return value as in step_host;
     public detections and pre_dets are in each stream's source pixels, and so are the tracks.  On a runner built with
     max_frame_size, a stream in `starts` may bring a frame of another size (that fits the region and maps to (H, W));
     without a calibs entry it then gets Detector._get_default_calib of that size.  ValueError (before anything is
@@ -962,7 +1017,8 @@ class StreamRunner(object):
     tracking also uploads its start list and seed rows (and the tracker geometry rows of streams whose camera
     changes), counted here after that step is submitted.  A capacity runner uploads the bytes its streams' frames use,
     plus the slot's descriptors in a step where they changed; an idle-streams runner the live streams' frames, plus the
-    descriptors and stream maps when they changed."""
+    descriptors and stream maps when they changed.  A frame's bytes are those of its frame_format: h * w * 3 / 2 in
+    NV12 / I420."""
     pub = self.B * (self.tracker.max_public * 2 + 1) * 4 if self.public else 0
     hm = self.B * self.H * self.W * 4 if self.tracker is None else 0
     if self.frames_mode:

@@ -12,10 +12,12 @@ the upload of step t+1 overlaps step t, and step t's tracks are yielded after st
 import numpy as np
 import torch
 
+from .runner import frame_layout, frame_size_of
+
 
 class Video(object):
-  """One video: `id`, `frames` (an iterable: uint8 [h, w, 3] BGR arrays in frames mode, pre-processed fp32 [3, H, W]
-  images otherwise), optional `pre_dets` (result dicts seeding the tracker at the first frame, as the reference's
+  """One video: `id`, `frames` (an iterable: uint8 [h, w, 3] BGR arrays in frames mode -- [3h/2, w] NV12 / I420 arrays
+  on a runner of that frame_format --, pre-processed fp32 [3, H, W] images otherwise), optional `pre_dets` (result dicts seeding the tracker at the first frame, as the reference's
   --load_results does), `public_dets` (per frame, the [P, 2] centres of its public detections, for --public_det) and
   `calib` (the [3, 4] camera matrix of its frames).  Without `calib` the video runs in whatever camera its stream
   has: Detector._get_default_calib of its frame size when that size differs from the stream's last one, otherwise the
@@ -49,6 +51,7 @@ def track_videos(runner, videos):
   B = runner.B
   capacity = runner.frames_mode and getattr(runner, 'max_frame_bytes', None) is not None
   idle_runner = getattr(runner, 'idle_g', None) is not None
+  fmt = getattr(runner, 'frame_format', 'bgr')
   if runner.frames_mode:
     sizes = [tuple(s) for s in runner.frame_sizes]
   else:
@@ -56,7 +59,9 @@ def track_videos(runner, videos):
 
   def size_of(frame):
     shape = tuple(np.shape(frame))
-    return shape[:2] if runner.frames_mode else shape[-3:]
+    if not runner.frames_mode:
+      return shape[-3:]
+    return shape[:2] if fmt == 'bgr' else frame_size_of(fmt, shape)     # None: not a frame of that format
 
   source = iter(videos)
   pending = []                        # pulled, not yet placed: _Playing with index 0
@@ -70,6 +75,9 @@ def track_videos(runner, videos):
       first = next(it, None)
       if first is None:               # no frames: nothing to yield
         continue
+      if size_of(first) is None:
+        raise ValueError('track_videos: video %r: a frame of shape %s is not a %s frame [3h/2, w]' %
+                         (v.id, np.shape(first), fmt.upper()))
       if capacity:
         try:
           runner.check_frame_size(size_of(first))
@@ -118,7 +126,7 @@ def track_videos(runner, videos):
         frames.append(None)
         continue
       elif last[b] is None:           # a stream that never had a video: any frame of its size
-        last[b] = np.zeros(sizes[b] + (3,), np.uint8) if runner.frames_mode else torch.zeros(sizes[b])
+        last[b] = np.zeros(frame_layout(fmt, *sizes[b])[0], np.uint8) if runner.frames_mode else torch.zeros(sizes[b])
       frames.append(last[b])
     pre_dets = {b: playing[b].video.pre_dets for b in started if playing[b].video.pre_dets is not None}
     public = None

@@ -32,7 +32,8 @@
  *   ct_pack_stem_frames        the same for B ragged uint8 frames and their previous frames, written as the packed
  *                     input of the tensor-core stem (no fp32 image in between); ct_pack_stem_frames_flip also writes
  *                     each stream's mirror image for --flip_test.  The _dev forms and ct_warp_frames_normalize read
- *                     the descriptors from device memory (frame sizes that change between graph replays).
+ *                     the descriptors from device memory (frame sizes that change between graph replays), and take
+ *                     NV12 / I420 frames too: cv2.cvtColor(COLOR_YUV2BGR_NV12 / _I420) fused into the warp's taps.
  */
 #ifndef CTB200_H_
 #define CTB200_H_
@@ -398,11 +399,20 @@ int ct_warp_affine_normalize(const uint8_t* src, int32_t B, int32_t src_h, int32
                              const double* minv, const float* mean, const float* std, float* dst, int32_t out_h,
                              int32_t out_w, void* stream);
 
-/* One stream's frame inside a buffer of B ragged uint8 BGR frames (StreamRunner's frame slots). */
+/* Pixel formats of a ct_frame.  The YUV 4:2:0 ones are cv2's layouts of one [3h/2, w] uint8 image (h and w even):
+ * NV12 = the h luma rows, then h/2 rows of interleaved U V; I420 = the luma plane, then the U plane (h/2 x w/2), then
+ * the V plane, the chroma planes' half-width rows packed two to a luma-pitch row as cv2 reads them.  Each source pixel
+ * is converted to BGR with cv2.cvtColor's fixed-point BT.601 (COLOR_YUV2BGR_NV12 / _I420) before the bilinear warp. */
+#define CT_FRAME_BGR  0
+#define CT_FRAME_NV12 1
+#define CT_FRAME_I420 2
+
+/* One stream's frame inside a buffer of B ragged uint8 frames (StreamRunner's frame slots). */
 typedef struct {
   int64_t offset;             /* byte offset of the frame in the buffer (StreamRunner aligns it to 16 bytes) */
-  int32_t h, w, step;         /* source rows, columns, row pitch in bytes (>= 3 w) */
-  int32_t reserved;
+  int32_t h, w, step;         /* source rows, columns, row pitch in bytes (BGR: >= 3 w; YUV: the luma pitch, >= w,
+                                 the chroma rows start at offset + h step) */
+  int32_t format;             /* CT_FRAME_*; the by-value entry points take CT_FRAME_BGR only */
   double  minv[6];            /* dst -> src map, inverted exactly as cv::warpAffine inverts it (see above) */
 } ct_frame;
 
@@ -412,8 +422,9 @@ typedef struct {
 /* out bf16 NHWC [B,H,W,8] = (norm(warp(cur_b)) x3, norm(warp(prev_b)) x3, pre_hm_b, 0): the tensor-core stem's input,
  * byte-identical to ct_warp_affine_normalize of each stream followed by ct_pack_stem_input.  cur / prev: device buffers
  * holding each stream's frame at frames[b].offset (the same descriptor is used for both); prev == NULL or
- * pre_hm == NULL (fp32 [B,1,H,W]) give zeros.  frames: HOST array [B], read during the call and passed to the kernels
- * by value (a captured CUDA graph keeps them); one launch per CT_FRAMES_PER_LAUNCH streams.  mean / std host fp32[3]. */
+ * pre_hm == NULL (fp32 [B,1,H,W]) give zeros.  frames: HOST array [B] of CT_FRAME_BGR frames (another format is
+ * CT_ERR_INVALID), read during the call and passed to the kernels by value (a captured CUDA graph keeps them); one
+ * launch per CT_FRAMES_PER_LAUNCH streams.  mean / std host fp32[3]. */
 int ct_pack_stem_frames(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames, int32_t B, const float* mean,
                         const float* std, const float* pre_hm, void* out, int32_t H, int32_t W, void* stream);
 /* --flip_test: ct_pack_stem_frames into out [2B,H,W,8] whose image B+b is image b mirrored along W (out[B+b][y][W-1-x]
@@ -425,7 +436,9 @@ int ct_pack_stem_frames_flip(const uint8_t* cur, const uint8_t* prev, const ct_f
 
 /* Device-resident descriptors: the output of ct_pack_stem_frames(_flip), byte for byte, with frames_dev a DEVICE array
  * ct_frame[B] read by the kernel (a replayed CUDA graph reads whatever geometry it holds then) in one launch.  cur and
- * prev are buf_bytes long each.  A descriptor with h <= 0, w <= 0, step < 3 w, offset < 0 or a frame extending past
+ * prev are buf_bytes long each.  Each descriptor may have any CT_FRAME_* format (one launch may mix them); a YUV frame
+ * gives exactly what its cv2.cvtColor BGR image gives, zero border included.  A descriptor with h <= 0, w <= 0,
+ * offset < 0, an unknown format, step < 3 w (BGR) or < w (YUV), an odd h or w (YUV), or a frame extending past
  * buf_bytes gives zeros for its stream (in both images under _flip) and reads nothing of cur / prev. */
 int ct_pack_stem_frames_dev(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames_dev, int32_t B,
                             int64_t buf_bytes, const float* mean, const float* std, const float* pre_hm, void* out,

@@ -108,6 +108,13 @@ class Frame(C.Structure):
               ('minv', C.c_double * 6)]
 
 
+CT_SRC_BGR, CT_SRC_RGB, CT_SRC_RGB_PLANAR, CT_SRC_NV12, CT_SRC_I420 = 0, 1, 2, 3, 4
+
+
+class FrameSrc(C.Structure):
+  _fields_ = [('plane', C.c_void_p * 3), ('pitch', C.c_int64 * 3), ('layout', C.c_int32), ('reserved', C.c_int32)]
+
+
 CT_FLIP_MAX_HEADS = 12
 
 
@@ -122,7 +129,7 @@ EXPORTS = ['ct_packed_weight_bytes', 'ct_pack_weights', 'ct_conv_forward', 'ct_c
            'ct_track_step_assoc', 'ct_track_payload_smem_bytes', 'ct_track_step_payload', 'ct_track_start',
            'ct_render_tracks', 'ct_track_step_mapped', 'ct_render_tracks_mapped', 'ct_flip_merge', 'ct_flip_merge_heads', 'ct_mirror_x',
            'ct_warp_affine_normalize', 'ct_pack_stem_frames', 'ct_pack_stem_frames_flip', 'ct_pack_stem_frames_dev',
-           'ct_pack_stem_frames_flip_dev', 'ct_warp_frames_normalize', 'ct_last_error',
+           'ct_pack_stem_frames_flip_dev', 'ct_warp_frames_normalize', 'ct_stage_frames', 'ct_last_error',
            'ct_abi_version', 'ct_launch_count', 'ct_reset_launch_count', 'ct_debug_trace', 'ct_debug_watch']
 
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17', '-Xcompiler', '-fPIC']
@@ -216,6 +223,7 @@ def lib():
   L.ct_pack_stem_frames_flip_dev.argtypes = L.ct_pack_stem_frames_dev.argtypes
   L.ct_warp_frames_normalize.argtypes = [C.c_void_p] * 2 + [C.c_int32, C.c_int64] + [C.c_void_p] * 3 + \
       [C.c_int32] * 2 + [C.c_void_p]
+  L.ct_stage_frames.argtypes = [C.POINTER(FrameSrc), C.POINTER(Frame), C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]
   L.ct_launch_count.restype = C.c_int64
   L.ct_reset_launch_count.restype = None
   L.ct_debug_trace.argtypes = [C.c_void_p]

@@ -18,6 +18,7 @@
 //                    written straight as the tensor-core stem's packed bf16 input; ct_pack_stem_frames_flip also
 //                    writes each stream's mirror image (--flip_test); the device-descriptor forms also take NV12 /
 //                    I420 frames, cv2.cvtColor(COLOR_YUV2BGR_NV12 / _I420) applied to each bilinear tap
+//   ct_stage_frames  B frames already in device memory (a GPU decoder's) copied into a frame slot in its layout
 // All HBM-bound byte/index work: one pass over the data, coalesced, no tensor cores.
 #include <math_constants.h>
 
@@ -914,6 +915,121 @@ pack_stem_frames_dev_kernel(const unsigned char* __restrict__ cur, const unsigne
   pack_stem_frames_body<FLIP>(cur, prev, fs, 0, gridDim.y, mean, stdv, hm, out, H, W);
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// ct_stage_frames: each stream's device frame copied into its region of a frame slot, in the slot's layout.
+// blockIdx.y = stream, one warp per destination row, the frame's rows spread over blockIdx.x.  A row whose source and
+// destination rows are 16-byte aligned moves 16 bytes per lane and access (the RGB -> BGR swap and the planar ->
+// interleaved transpose work on 16 pixels = 48 bytes in registers); unaligned rows and the end of a row go byte by byte.
+// A pure copy: HBM-bound.
+// ------------------------------------------------------------------------------------------------------------------
+constexpr int STAGE_THREADS = 256;
+constexpr int STAGE_WARPS = STAGE_THREADS / 32;
+
+struct StageFrame {
+  const unsigned char* src[3];
+  long long pitch[3];
+  long long offset;           // destination
+  int h, w, step, layout;
+};
+
+struct StageArgs {
+  StageFrame f[CT_FRAMES_PER_LAUNCH];
+};
+
+__device__ __forceinline__ bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
+// byte j of the little-endian words v
+__device__ __forceinline__ uint32_t byte_at(const uint32_t* v, int j) { return (v[j >> 2] >> (8 * (j & 3))) & 0xffu; }
+
+// d[0, n) <- s[0, n) by one warp: 16-byte accesses when s and d share their alignment
+__device__ __forceinline__ void stage_copy(const unsigned char* __restrict__ s, unsigned char* __restrict__ d, int n,
+                                           int lane) {
+  int head = n, body = 0;
+  if ((((uintptr_t)s ^ (uintptr_t)d) & 15) == 0) {
+    head = min((int)((16 - ((uintptr_t)d & 15)) & 15), n);
+    body = (n - head) >> 4;
+    const uint4* sv = reinterpret_cast<const uint4*>(s + head);
+    uint4* dv = reinterpret_cast<uint4*>(d + head);
+    for (int i = lane; i < body; i += 32) dv[i] = __ldg(sv + i);
+  }
+  for (int i = lane; i < head; i += 32) d[i] = s[i];
+  for (int i = head + (body << 4) + lane; i < n; i += 32) d[i] = s[i];
+}
+
+// One BGR row of w pixels from interleaved RGB (PLANAR = false: s0) or from the R, G, B rows s0, s1, s2.  Output byte
+// j = 3x + c takes source byte 3x + 2 - c, or byte x of plane 2 - c.
+template <bool PLANAR>
+__device__ __forceinline__ void stage_bgr_row(const unsigned char* __restrict__ s0, const unsigned char* __restrict__ s1,
+                                              const unsigned char* __restrict__ s2, unsigned char* __restrict__ d, int w,
+                                              int lane) {
+  int done = 0;
+  if (aligned16(s0) && aligned16(d) && (!PLANAR || (aligned16(s1) && aligned16(s2)))) {
+    done = w >> 4;                                          // chunks of 16 pixels
+    for (int c = lane; c < done; c += 32) {
+      uint32_t in[12], out[12];
+#pragma unroll
+      for (int q = 0; q < 3; ++q) {
+        const unsigned char* sq = !PLANAR ? s0 : (q == 0 ? s0 : (q == 1 ? s1 : s2));
+        const uint4 t = __ldg(reinterpret_cast<const uint4*>(sq) + (PLANAR ? c : 3 * c + q));
+        in[4 * q] = t.x, in[4 * q + 1] = t.y, in[4 * q + 2] = t.z, in[4 * q + 3] = t.w;
+      }
+#pragma unroll
+      for (int k = 0; k < 12; ++k) {
+        uint32_t o = 0;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int j = 4 * k + i, x = j / 3, ch = j % 3;
+          o |= byte_at(in, PLANAR ? (2 - ch) * 16 + x : 3 * x + 2 - ch) << (8 * i);
+        }
+        out[k] = o;
+      }
+      uint4* dv = reinterpret_cast<uint4*>(d) + 3 * c;
+#pragma unroll
+      for (int q = 0; q < 3; ++q) dv[q] = make_uint4(out[4 * q], out[4 * q + 1], out[4 * q + 2], out[4 * q + 3]);
+    }
+    done <<= 4;
+  }
+  for (int j = 3 * done + lane; j < 3 * w; j += 32) {
+    const int x = j / 3, ch = j - 3 * x;
+    d[j] = !PLANAR ? s0[3 * x + 2 - ch] : (ch == 0 ? s2[x] : (ch == 1 ? s1[x] : s0[x]));
+  }
+}
+
+__global__ void __launch_bounds__(STAGE_THREADS)
+stage_frames_kernel(const __grid_constant__ StageArgs a, unsigned char* __restrict__ buf) {
+  const StageFrame& f = a.f[blockIdx.y];
+  const int h = f.h, w = f.w, step = f.step, layout = f.layout, lane = threadIdx.x & 31;
+  const unsigned char *src0 = f.src[0], *src1 = f.src[1], *src2 = f.src[2];
+  const long long p0 = f.pitch[0], p1 = f.pitch[1], p2 = f.pitch[2];
+  const int rows = layout == CT_SRC_NV12 ? h + h / 2 : (layout == CT_SRC_I420 ? 2 * h : h);
+  unsigned char* dst = buf + f.offset;
+  for (int r = blockIdx.x * STAGE_WARPS + (threadIdx.x >> 5); r < rows; r += gridDim.x * STAGE_WARPS) {
+    unsigned char* d = dst + (size_t)r * step;
+    if (layout == CT_SRC_RGB) {
+      stage_bgr_row<false>(src0 + r * p0, nullptr, nullptr, d, w, lane);
+      continue;
+    }
+    if (layout == CT_SRC_RGB_PLANAR) {
+      stage_bgr_row<true>(src0 + r * p0, src1 + r * p1, src2 + r * p2, d, w, lane);
+      continue;
+    }
+    // a plain copy: a BGR row, a luma row, an NV12 UV row or an I420 chroma half-row
+    const unsigned char* s = src0 + r * p0;
+    int n = layout == CT_SRC_BGR ? 3 * w : w;
+    if (layout != CT_SRC_BGR && r >= h) {
+      const int k = r - h, hh = h >> 1;
+      if (layout == CT_SRC_NV12) {
+        s = src1 + k * p1;
+      } else {   // I420 half-row k: U rows 0..h/2-1, then V; two half-rows to a destination row, as cv2 lays them out
+        s = k < hh ? src1 + k * p1 : src2 + (k - hh) * p2;
+        d = dst + (size_t)(h + (k >> 1)) * step + (k & 1) * (w >> 1);
+        n = w >> 1;
+      }
+    }
+    stage_copy(s, d, n, lane);
+  }
+}
+
 }  // namespace ctb
 
 using namespace ctb;
@@ -1172,4 +1288,58 @@ extern "C" int ct_warp_frames_normalize(const uint8_t* src, const ct_frame* fram
   warp_frames_norm_kernel<<<dim3((unsigned)nx, (unsigned)B), 256, 0, (cudaStream_t)stream>>>(
       src, fs, dst, out_h, out_w, make_float3(mean[0], mean[1], mean[2]), make_float3(std[0], std[1], std[2]));
   return after_launch();
+}
+
+extern "C" int ct_stage_frames(const ct_frame_src* srcs, const ct_frame* dst, int32_t n, uint8_t* buf,
+                               int64_t buf_bytes, void* stream) {
+  CT_REQUIRE(srcs && dst && buf, "null pointer");
+  CT_REQUIRE(n > 0, "n <= 0");
+  CT_REQUIRE(buf_bytes >= 0, "buf_bytes < 0");
+  // everything is on the host: check every stream before the first launch
+  for (int32_t i = 0; i < n; ++i) {
+    const ct_frame_src& s = srcs[i];
+    const ct_frame& f = dst[i];
+    CT_REQUIRE(s.layout >= CT_SRC_BGR && s.layout <= CT_SRC_I420, "unknown source layout");
+    const bool yuv = s.layout == CT_SRC_NV12 || s.layout == CT_SRC_I420;
+    const int32_t fmt = s.layout == CT_SRC_NV12 ? CT_FRAME_NV12 : (s.layout == CT_SRC_I420 ? CT_FRAME_I420 : CT_FRAME_BGR);
+    CT_REQUIRE(f.format == fmt, "source layout and destination format differ (BGR / RGB / RGB_PLANAR -> BGR, NV12 -> "
+                                "NV12, I420 -> I420)");
+    CT_REQUIRE(f.h > 0 && f.w > 0 && f.offset >= 0, "bad destination frame (h > 0, w > 0, offset >= 0)");
+    CT_REQUIRE(f.h < (1 << 29) && f.w < (1 << 28), "frame too large");
+    CT_REQUIRE(!yuv || ((f.h | f.w) & 1) == 0, "4:2:0 frames have an even height and width");
+    const int planes = s.layout == CT_SRC_NV12 ? 2 : ((s.layout == CT_SRC_I420 || s.layout == CT_SRC_RGB_PLANAR) ? 3 : 1);
+    const int64_t row[3] = {yuv || s.layout == CT_SRC_RGB_PLANAR ? f.w : 3LL * f.w,
+                            s.layout == CT_SRC_I420 ? f.w / 2 : f.w, s.layout == CT_SRC_I420 ? f.w / 2 : f.w};
+    for (int p = 0; p < planes; ++p) {
+      CT_REQUIRE(s.plane[p] != nullptr, "null source plane");
+      CT_REQUIRE(s.pitch[p] >= row[p], "source pitch shorter than a row");
+    }
+    const int64_t rows = yuv ? 3LL * (f.h / 2) : f.h, row_bytes = yuv ? f.w : 3LL * f.w;
+    CT_REQUIRE(f.step >= row_bytes, "destination step shorter than a row");
+    CT_REQUIRE(f.offset <= buf_bytes && (rows - 1) * f.step + row_bytes <= buf_bytes - f.offset,
+               "destination extends past buf_bytes");
+  }
+  for (int32_t i0 = 0; i0 < n; i0 += CT_FRAMES_PER_LAUNCH) {
+    const int m = n - i0 < CT_FRAMES_PER_LAUNCH ? n - i0 : CT_FRAMES_PER_LAUNCH;
+    StageArgs a = {};
+    int64_t most = 0;
+    for (int i = 0; i < m; ++i) {
+      const ct_frame_src& s = srcs[i0 + i];
+      const ct_frame& f = dst[i0 + i];
+      StageFrame& g = a.f[i];
+      for (int p = 0; p < 3; ++p) {
+        g.src[p] = (const unsigned char*)s.plane[p];
+        g.pitch[p] = s.pitch[p];
+      }
+      g.offset = f.offset;
+      g.h = f.h, g.w = f.w, g.step = f.step, g.layout = s.layout;
+      const int64_t rows = s.layout == CT_SRC_NV12 ? f.h + f.h / 2 : (s.layout == CT_SRC_I420 ? 2LL * f.h : f.h);
+      most = rows > most ? rows : most;
+    }
+    const dim3 grid((unsigned)((most + STAGE_WARPS - 1) / STAGE_WARPS), (unsigned)m);
+    stage_frames_kernel<<<grid, STAGE_THREADS, 0, (cudaStream_t)stream>>>(a, buf);
+    const int rc = after_launch();
+    if (rc != CT_OK) return rc;
+  }
+  return CT_OK;
 }

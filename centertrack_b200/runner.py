@@ -37,6 +37,10 @@ so a stream may take a frame of another size, and a new camera, when it starts a
 A capacity runner may take NV12 or I420 frames instead (`frame_format`, what video decoders emit): each [3h/2, w] frame
 is uploaded as it is, half the bytes of BGR, and the device-descriptor kernels convert each bilinear tap to BGR with
 cv2.cvtColor's fixed-point arithmetic, so the stream computes what it computes on the cv2-converted BGR frame.
+Device frames (step_frames with CUDA tensors, what GPU decoders hand out): instead of the host staging and upload, one
+ct_stage_frames on the copy stream copies every live stream's frame from the caller's tensors (any row pitch; RGB and
+planar RGB written as BGR, NV12 / I420 planes written in cv2's layout) into its region of the slot.  Everything after
+that -- packs, warps, graphs, start prologue, tracker -- reads the slot as it reads an uploaded one.
 
 Video starts (`starts=`, `pre_dets=` of step_host / step_frames / load_device_inputs): a stream may begin a new video at
 any step, as Detector.reset_tracking + Tracker.init_track(pre_dets) on that stream alone.  A start is rare (once per
@@ -99,6 +103,116 @@ def frame_size_of(fmt, shape):
   if len(shape) != 2 or shape[0] % 3 or shape[1] % 2:
     return None
   return shape[0] // 3 * 2, shape[1]
+
+
+# step_frames(layout=) of a device frame on a BGR runner -> ct_frame_src.layout
+DEVICE_LAYOUTS = {'bgr': L.CT_SRC_BGR, 'rgb': L.CT_SRC_RGB, 'rgb_planar': L.CT_SRC_RGB_PLANAR}
+
+
+def is_device_frame(x):
+  """Whether a step_frames entry is a device frame (a torch tensor, or a tuple of plane tensors) rather than an array."""
+  return isinstance(x, torch.Tensor) or (isinstance(x, tuple) and len(x) > 0 and
+                                         all(isinstance(t, torch.Tensor) for t in x))
+
+
+def device_frame_source(x, fmt, layout, device, what='frame'):
+  """A device frame -> ((h, w), L.FrameSrc) for ct_stage_frames, reading only each tensor's dtype, device, shape,
+  stride() and data_ptr().  fmt: the runner's frame_format; layout: 'bgr', 'rgb' ([h, w, 3]) or 'rgb_planar' ([3, h, w])
+  on a BGR runner, 'bgr' on a 4:2:0 one.  NV12 / I420: one uint8 [3h/2, w] tensor in cv2's layout (I420 with rows of
+  exactly w bytes, since its chroma half-rows are packed two to a row), or the planes (Y [h, w], UV [h/2, w]) /
+  (Y [h, w], U [h/2, w/2], V [h/2, w/2]).  Rows may have any pitch; the innermost stride must be 1 (and 3 for the pixels
+  of an interleaved frame).  ValueError naming `what` on a wrong dtype or device, strides, a pitch shorter than a row,
+  plane shapes that disagree, or odd 4:2:0 sizes."""
+  if fmt not in FRAME_FORMATS:
+    raise ValueError('frame_format: expected one of %s, got %r' % (sorted(FRAME_FORMATS), fmt))
+  if fmt == 'bgr' and layout not in DEVICE_LAYOUTS:
+    raise ValueError('layout: expected one of %s, got %r' % (sorted(DEVICE_LAYOUTS), layout))
+  if fmt != 'bgr' and layout != 'bgr':
+    raise ValueError("layout=%r: a %s runner takes its own format only (layout='bgr')" % (layout, fmt.upper()))
+  planes = x if isinstance(x, tuple) else (x,)
+  device = torch.device(device)
+  for i, t in enumerate(planes):
+    name = what if len(planes) == 1 else '%s[%d]' % (what, i)
+    if not isinstance(t, torch.Tensor):
+      raise ValueError('%s: expected a torch tensor, got %s' % (name, type(t).__name__))
+    if t.dtype != torch.uint8:
+      raise ValueError('%s: expected a uint8 tensor, got %s' % (name, t.dtype))
+    if t.device.type != device.type or (device.index is not None and t.device.index != device.index):
+      raise ValueError("%s: on %s, not on the runner's device %s" % (name, t.device, device))
+
+  def pitch(shape, stride, name, row):
+    """The row pitch of a [rows, row] plane of these (shape, strides) (its innermost stride 1); a single row's pitch is
+    its length."""
+    if shape[1] > 1 and stride[1] != 1:
+      raise ValueError('%s: the innermost stride must be 1, got strides %s' % (name, tuple(stride)))
+    p = stride[0] if shape[0] > 1 else row
+    if p < row:
+      raise ValueError('%s: row pitch of %d bytes is shorter than a row of %d' % (name, p, row))
+    return p
+
+  src = L.FrameSrc()
+  if fmt == 'bgr':
+    if len(planes) != 1:
+      raise ValueError('%s: a BGR runner takes one tensor per frame, got %d' % (what, len(planes)))
+    if layout == 'rgb_planar':
+      if x.dim() != 3 or x.shape[0] != 3:
+        raise ValueError("%s: layout 'rgb_planar' expects shape [3, h, w], got %s" % (what, tuple(x.shape)))
+      h, w = int(x.shape[1]), int(x.shape[2])
+      if h <= 0 or w <= 0:
+        raise ValueError('%s: empty frame of shape %s' % (what, tuple(x.shape)))
+      p = pitch(x.shape[1:], x.stride()[1:], what, w)
+      src.layout = L.CT_SRC_RGB_PLANAR
+      for c in range(3):
+        src.plane[c], src.pitch[c] = x.data_ptr() + c * x.stride(0), p
+      return (h, w), src
+    if x.dim() != 3 or x.shape[2] != 3:
+      raise ValueError("%s: layout %r expects shape [h, w, 3], got %s" % (what, layout, tuple(x.shape)))
+    h, w = int(x.shape[0]), int(x.shape[1])
+    if h <= 0 or w <= 0:
+      raise ValueError('%s: empty frame of shape %s' % (what, tuple(x.shape)))
+    if x.stride(2) != 1 or (w > 1 and x.stride(1) != 3):
+      raise ValueError('%s: the innermost stride must be 1 and the pixel stride 3, got strides %s' % (what, x.stride()))
+    src.layout = DEVICE_LAYOUTS[layout]
+    src.plane[0], src.pitch[0] = x.data_ptr(), (x.stride(0) if h > 1 else 3 * w)
+    if src.pitch[0] < 3 * w:
+      raise ValueError('%s: row pitch of %d bytes is shorter than a row of %d' % (what, src.pitch[0], 3 * w))
+    return (h, w), src
+  n_planes = 2 if fmt == 'nv12' else 3
+  src.layout = L.CT_SRC_NV12 if fmt == 'nv12' else L.CT_SRC_I420
+  if len(planes) == 1:                      # cv2's [3h/2, w] layout
+    if x.dim() != 2 or x.shape[0] % 3 or x.shape[1] % 2 or x.shape[0] == 0 or x.shape[1] == 0:
+      raise ValueError('%s: expected a %s frame of shape [3h/2, w] (rows a multiple of 3, w even), got %s' %
+                       (what, fmt.upper(), tuple(x.shape)))
+    h, w = int(x.shape[0]) // 3 * 2, int(x.shape[1])
+    p = pitch(x.shape, x.stride(), what, w)
+    if fmt == 'i420' and p != w:
+      raise ValueError('%s: an I420 frame given as one tensor needs rows of exactly w = %d bytes (its chroma half-rows '
+                       'are packed two to a row), got a pitch of %d; give a pitched surface as (Y, U, V) planes' %
+                       (what, w, p))
+    y = x.data_ptr()
+    src.plane[0], src.pitch[0] = y, p
+    if fmt == 'nv12':
+      src.plane[1], src.pitch[1] = y + h * p, p
+    else:
+      src.plane[1], src.plane[2] = y + h * w, y + h * w + (h // 2) * (w // 2)
+      src.pitch[1] = src.pitch[2] = w // 2
+    return (h, w), src
+  if len(planes) != n_planes:
+    raise ValueError('%s: expected %s planes %s, got %d tensors' %
+                     (what, fmt.upper(), '(Y, UV)' if fmt == 'nv12' else '(Y, U, V)', len(planes)))
+  Y = planes[0]
+  if Y.dim() != 2:
+    raise ValueError('%s[0]: expected a 2-D plane, got shape %s' % (what, tuple(Y.shape)))
+  h, w = int(Y.shape[0]), int(Y.shape[1])
+  if h <= 0 or w <= 0 or h % 2 or w % 2:
+    raise ValueError('%s[0]: Y plane of shape %s; %s frames have an even, non-zero height and width' %
+                     (what, (h, w), fmt.upper()))
+  want = [(h, w), (h // 2, w)] if fmt == 'nv12' else [(h, w), (h // 2, w // 2), (h // 2, w // 2)]
+  for i, (t, s) in enumerate(zip(planes, want)):
+    if tuple(t.shape) != s:
+      raise ValueError('%s[%d]: expected shape %s for a Y plane of %s, got %s' % (what, i, s, (h, w), tuple(t.shape)))
+    src.plane[i], src.pitch[i] = t.data_ptr(), pitch(t.shape, t.stride(), '%s[%d]' % (what, i), s[1])
+  return (h, w), src
 
 
 class StreamRunner(object):
@@ -203,6 +317,7 @@ class StreamRunner(object):
     self.h_geo = None                                        # per slot camera geometry rows staging, made on first use
     self._geo = [None] * NS                                  # per slot: the streams whose geometry rows it carries
     self._frame_bytes = 0                                    # frame (+ descriptor) bytes of the last upload
+    self._ev_read = None                                     # recorded after the last staging of device frames
     if self.frames_mode:
       self._frame_bytes = self.slot_bytes if self.cap is None else sum(e - a for a, e in self._upload_runs())
     self._eager(0, first=True)                               # sizes the record buffer
@@ -891,9 +1006,11 @@ class StreamRunner(object):
                        '(starts=)' % back)
     return live
 
-  def step_frames(self, frames, pre_hms=None, public_dets=None, starts=None, pre_dets=None, calibs=None, idle=None):
+  def step_frames(self, frames, pre_hms=None, public_dets=None, starts=None, pre_dets=None, calibs=None, idle=None,
+                  layout='bgr'):
     """frames: B uint8 [h_b, w_b, 3] BGR arrays of the sizes given as frame_sizes (with frame_format 'nv12' / 'i420':
-    [3h_b/2, w_b] arrays in that layout), or None when they were written through frame_buffers().  pre_hms, public_dets, starts, pre_dets, calibs and the return value as in step_host;
+    [3h_b/2, w_b] arrays in that layout), or None when they were written through frame_buffers(), or B device frames
+    (below).  pre_hms, public_dets, starts, pre_dets, calibs and the return value as in step_host;
     public detections and pre_dets are in each stream's source pixels, and so are the tracks.  On a runner built with
     max_frame_size, a stream in `starts` may bring a frame of another size (that fits the region and maps to (H, W));
     without a calibs entry it then gets Detector._get_default_calib of that size.  ValueError (before anything is
@@ -902,7 +1019,18 @@ class StreamRunner(object):
     idle (runners built with idle_streams): the streams without a frame in this step; their frames and public_dets
     entries are ignored (and may be None), their tables, camera and frame region are left as they are, and their
     records come back zero and their fetch_results() entries None.  A stream idle in one step comes back only with a
-    video start."""
+    video start.
+    Device frames (what GPU decoders hand out): uint8 CUDA tensors on the runner's device instead of arrays, for every
+    stream with a frame in this step (a step never mixes the two).  A BGR runner takes [h, w, 3] with layout 'bgr' or
+    'rgb', or [3, h, w] with layout 'rgb_planar'; an NV12 runner one [3h/2, w] tensor in cv2's layout or the planes
+    (Y [h, w], UV [h/2, w]); an I420 runner one [3h/2, w] tensor of rows of exactly w bytes or the planes
+    (Y [h, w], U [h/2, w/2], V [h/2, w/2]).  Rows may have any pitch (views of wider or taller surfaces); the innermost
+    stride must be 1 (device_frame_source).  One ct_stage_frames copies them into the slot on the runner's copy stream,
+    after the work queued on the caller's current stream at this call (which writes the frames); nothing of them is
+    uploaded, and the step computes bit for bit what it computes on the same frames given as arrays (RGB swapped to
+    BGR).  The tensors may be freed after the call (the caching allocator keeps their memory until the copy has run), but
+    memory the caller reuses itself, such as a decoder's surface pool, must not be written again before frames_read()
+    has completed: make the decoder's stream wait on it."""
     if not self.frames_mode:
       raise ValueError('step_frames: the runner was not built with frame_sizes (use step_host)')
     plan = self._check_starts(starts, pre_dets)
@@ -911,7 +1039,13 @@ class StreamRunner(object):
     gone = () if live is None else set(range(self.B)) - set(live)
     pub = self._check_public(public_dets, gone)
     cal = self._check_calibs(calibs, started)
-    sizes = self._frame_sizes_of(frames, gone)
+    dev = None                                       # device frames: [(stream, ct_frame_src, tensors)]
+    if frames is not None and self._device_step(frames, gone):
+      sizes, dev = self._device_sources(frames, gone, layout)
+    else:
+      if layout != 'bgr':
+        raise ValueError("layout=%r: applies to device frames; arrays are in the runner's frame_format" % (layout,))
+      sizes = self._frame_sizes_of(frames, gone)
     changed = self._check_sizes(sizes, started)
     slot = self.t % NS
     self._pending_sizes = None
@@ -925,7 +1059,7 @@ class StreamRunner(object):
       if now != self._map_mirror[slot]:
         maps = self._map_mirror[slot] = now
         self.h_map[slot].numpy()[:] = np.frombuffer(maps, np.int32)
-    if frames is not None:
+    if frames is not None and dev is None:
       # the slot's staging was last read by step t-3's upload, which the last fetch() waited for
       for b, (a, v) in enumerate(zip(frames, self._views(slot, self.frame_sizes))):
         if b not in gone:
@@ -939,13 +1073,19 @@ class StreamRunner(object):
     if use_hm and not pre_hms.is_pinned():
       self.h_hm[slot].copy_(pre_hms)
       src_hm = self.h_hm[slot]
+    caller = torch.cuda.current_stream(self.device)
     with torch.cuda.stream(self.copy):
       self.copy.wait_event(self.ev_done[slot])       # slot's old contents were last read as pre_images of step t-2
+      if dev is not None:                            # staged from the caller's tensors once its stream has written them
+        self.copy.wait_stream(caller)
+        self._stage_frames(slot, dev)
       if self.cap is None:
-        self.u8[slot].copy_(self.h_u8[slot], non_blocking=True)
+        if dev is None:
+          self.u8[slot].copy_(self.h_u8[slot], non_blocking=True)
+        self._frame_bytes = 0 if dev is not None else self.slot_bytes
       else:                                          # the used bytes only, and the descriptors when they changed
         self._frame_bytes = 0
-        for a, e in self._upload_runs(live):
+        for a, e in (self._upload_runs(live) if dev is None else ()):
           self.u8[slot][a:e].copy_(self.h_u8[slot][a:e], non_blocking=True)
           self._frame_bytes += e - a
         if desc is not None:
@@ -963,6 +1103,52 @@ class StreamRunner(object):
           self._upload_geometry(slot, rows, non_blocking=True)
       self.ev_in[slot].record(self.copy)
     return self._submit(slot)
+
+  def _device_step(self, frames, idle):
+    """Whether this step's frames are device frames; ValueError on a wrong count or when the live streams' entries mix
+    device tensors and arrays."""
+    if len(frames) != self.B:
+      raise ValueError('frames: expected %d arrays (one per stream), got %d' % (self.B, len(frames)))
+    kinds = [(b, is_device_frame(a)) for b, a in enumerate(frames) if b not in idle]
+    dev, host = [b for b, k in kinds if k], [b for b, k in kinds if not k]
+    if dev and host:
+      raise ValueError('frames: stream(s) %s bring device tensors and stream(s) %s host arrays; a step takes uint8 '
+                       "tensors on the runner's device for all its streams or uint8 numpy arrays for all" % (dev, host))
+    return bool(dev)
+
+  def _device_sources(self, frames, idle, layout):
+    """Device frames -> (this step's (h, w) per stream, [(stream, ct_frame_src, tensors)] of the live streams);
+    ValueError (device_frame_source) before anything is enqueued.  `idle` streams keep their size."""
+    sizes, out = [], []
+    for b, (x, hw) in enumerate(zip(frames, self.frame_sizes)):
+      if b in idle:
+        sizes.append(hw)
+        continue
+      size, src = device_frame_source(x, self.frame_format, layout, self.u8[0].device, 'frames[%d]' % b)
+      sizes.append(size)
+      out.append((b, src, x if isinstance(x, tuple) else (x,)))
+    return sizes, out
+
+  def _stage_frames(self, slot, dev):
+    """ct_stage_frames of the device frames `dev` (_device_sources) into u8[slot], each at its stream's region in the
+    descriptor this step gives it, on the current (copy) stream; the source tensors are marked used by that stream."""
+    n = len(dev)
+    srcs = (L.FrameSrc * n)(*[s for _, s, _ in dev])
+    dst = (L.Frame * n)(*[self.frames[b] for b, _, _ in dev])
+    L.check(L.lib().ct_stage_frames(srcs, dst, n, L.ptr(self.u8[slot]), self.slot_bytes, L.stream_ptr()),
+            'ct_stage_frames')
+    for _, _, ts in dev:
+      for t in ts:
+        t.record_stream(self.copy)
+    if self._ev_read is None:
+      self._ev_read = torch.cuda.Event()
+    self._ev_read.record(self.copy)
+
+  def frames_read(self):
+    """The torch.cuda.Event recorded on the copy stream after the last step_frames call that took device frames (None
+    before the first): once it has completed, that call's source tensors have been read and their memory may be
+    written again.  A decoder that recycles its surfaces makes its stream wait on it (stream.wait_event)."""
+    return self._ev_read
 
   def fetch(self, copy=True):
     """Blocks until the last submitted step finished; returns its records as numpy [B,K,F].  A copy by default: the
@@ -1018,7 +1204,7 @@ class StreamRunner(object):
     changes), counted here after that step is submitted.  A capacity runner uploads the bytes its streams' frames use,
     plus the slot's descriptors in a step where they changed; an idle-streams runner the live streams' frames, plus the
     descriptors and stream maps when they changed.  A frame's bytes are those of its frame_format: h * w * 3 / 2 in
-    NV12 / I420."""
+    NV12 / I420.  A step fed device frames uploads none of its frames' bytes."""
     pub = self.B * (self.tracker.max_public * 2 + 1) * 4 if self.public else 0
     hm = self.B * self.H * self.W * 4 if self.tracker is None else 0
     if self.frames_mode:

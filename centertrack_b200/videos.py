@@ -6,18 +6,19 @@ A video goes to the first free stream (in frames mode, a free stream whose frame
 size; on a runner built with max_frame_size, any free stream, whose frame size changes at the start) and starts there
 with StreamRunner's `starts=` / `pre_dets=` / `calibs=`; when it ends, the stream takes the next video in the same step.
 A stream with no video re-feeds its last frame and its results are dropped; on a runner built with idle_streams it is
-marked idle instead, and the step computes only the streams that play a video.  The runner's one-step pipeline is kept:
+marked idle instead, and the step computes only the streams that play a video.  In frames mode the videos' frames may
+instead be device frames (CUDA tensors, StreamRunner.step_frames), all videos of one call being of one kind.  The runner's one-step pipeline is kept:
 the upload of step t+1 overlaps step t, and step t's tracks are yielded after step t+1 is submitted.
 """
 import numpy as np
 import torch
 
-from .runner import frame_layout, frame_size_of
+from .runner import device_frame_source, frame_layout, frame_size_of, is_device_frame
 
 
 class Video(object):
   """One video: `id`, `frames` (an iterable: uint8 [h, w, 3] BGR arrays in frames mode -- [3h/2, w] NV12 / I420 arrays
-  on a runner of that frame_format --, pre-processed fp32 [3, H, W] images otherwise), optional `pre_dets` (result dicts seeding the tracker at the first frame, as the reference's
+  on a runner of that frame_format, or device frames as step_frames takes them --, pre-processed fp32 [3, H, W] images otherwise), optional `pre_dets` (result dicts seeding the tracker at the first frame, as the reference's
   --load_results does), `public_dets` (per frame, the [P, 2] centres of its public detections, for --public_det) and
   `calib` (the [3, 4] camera matrix of its frames).  Without `calib` the video runs in whatever camera its stream
   has: Detector._get_default_calib of its frame size when that size differs from the stream's last one, otherwise the
@@ -41,13 +42,16 @@ def _as_video(v):
   return v if isinstance(v, Video) else Video(**v)
 
 
-def track_videos(runner, videos):
+def track_videos(runner, videos, layout='bgr'):
   """runner: a StreamRunner with device tracking; videos: an iterable of Video (or dicts of its fields).  Yields
   (video id, frame index, results) for every frame of every video exactly once, as its tracks come back; results is the
-  list of dicts fetch_results() gives for that stream (in source pixels in frames mode).  ValueError for a video whose
-  frame size no stream can take, or a runner without device tracking."""
+  list of dicts fetch_results() gives for that stream (in source pixels in frames mode).  layout: step_frames' layout of
+  device frames.  ValueError for a video whose frame size no stream can take, a video whose frames are of another kind
+  (device tensors or arrays) than the first video's, or a runner without device tracking."""
   if runner.tracker is None:
     raise ValueError('track_videos: the runner needs device_tracking=True')
+  if layout != 'bgr' and not runner.frames_mode:
+    raise ValueError('track_videos: layout=%r needs a frames-mode runner' % (layout,))
   B = runner.B
   capacity = runner.frames_mode and getattr(runner, 'max_frame_bytes', None) is not None
   idle_runner = getattr(runner, 'idle_g', None) is not None
@@ -57,11 +61,24 @@ def track_videos(runner, videos):
   else:
     sizes = [(3, runner.H, runner.W)] * B
 
+  kind = []                           # frames mode: [whether the videos bring device frames], set by the first video
+
   def size_of(frame):
+    if runner.frames_mode and is_device_frame(frame):
+      return device_frame_source(frame, fmt, layout, runner.u8[0].device)[0]
     shape = tuple(np.shape(frame))
     if not runner.frames_mode:
       return shape[-3:]
     return shape[:2] if fmt == 'bgr' else frame_size_of(fmt, shape)     # None: not a frame of that format
+
+  def filler(size):
+    """A frame of this size for a stream that never had a video, of the videos' kind."""
+    if not runner.frames_mode:
+      return torch.zeros(size)
+    if not kind[0]:
+      return np.zeros(frame_layout(fmt, *size)[0], np.uint8)
+    shape = (3,) + tuple(size) if layout == 'rgb_planar' else frame_layout(fmt, *size)[0]
+    return torch.zeros(shape, dtype=torch.uint8, device=runner.u8[0].device)
 
   source = iter(videos)
   pending = []                        # pulled, not yet placed: _Playing with index 0
@@ -75,6 +92,18 @@ def track_videos(runner, videos):
       first = next(it, None)
       if first is None:               # no frames: nothing to yield
         continue
+      if runner.frames_mode:
+        dev = is_device_frame(first)
+        if not kind:
+          kind.append(dev)
+        elif kind[0] != dev:
+          raise ValueError('track_videos: video %r brings %s; the videos before it bring %s' %
+                           (v.id, *(('device frames', 'arrays') if dev else ('arrays', 'device frames'))))
+        if dev:
+          try:
+            size_of(first)
+          except ValueError as e:
+            raise ValueError('track_videos: video %r: %s' % (v.id, e))
       if size_of(first) is None:
         raise ValueError('track_videos: video %r: a frame of shape %s is not a %s frame [3h/2, w]' %
                          (v.id, np.shape(first), fmt.upper()))
@@ -126,7 +155,7 @@ def track_videos(runner, videos):
         frames.append(None)
         continue
       elif last[b] is None:           # a stream that never had a video: any frame of its size
-        last[b] = np.zeros(frame_layout(fmt, *sizes[b])[0], np.uint8) if runner.frames_mode else torch.zeros(sizes[b])
+        last[b] = filler(sizes[b])
       frames.append(last[b])
     pre_dets = {b: playing[b].video.pre_dets for b in started if playing[b].video.pre_dets is not None}
     public = None
@@ -142,6 +171,8 @@ def track_videos(runner, videos):
     if calibs:
       kw['calibs'] = calibs
     if runner.frames_mode:
+      if layout != 'bgr' or kind[0]:
+        kw['layout'] = layout
       runner.step_frames(frames, **kw)
     else:
       runner.step_host(torch.stack([torch.as_tensor(f, dtype=torch.float32).reshape(sizes[0]) for f in frames]), **kw)

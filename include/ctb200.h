@@ -34,6 +34,9 @@
  *                     each stream's mirror image for --flip_test.  The _dev forms and ct_warp_frames_normalize read
  *                     the descriptors from device memory (frame sizes that change between graph replays), and take
  *                     NV12 / I420 frames too: cv2.cvtColor(COLOR_YUV2BGR_NV12 / _I420) fused into the warp's taps.
+ *   ct_stage_frames            copies B decoder frames already in device memory (BGR / RGB / planar RGB, NV12, I420
+ *                     planes at any pitch) into a frame slot in that slot's layout, so the kernels above read them as
+ *                     uploaded frames.
  */
 #ifndef CTB200_H_
 #define CTB200_H_
@@ -453,6 +456,35 @@ int ct_pack_stem_frames_flip_dev(const uint8_t* cur, const uint8_t* prev, const 
 int ct_warp_frames_normalize(const uint8_t* src, const ct_frame* frames_dev, int32_t B, int64_t buf_bytes,
                              const float* mean, const float* std, float* dst, int32_t out_h, int32_t out_w,
                              void* stream);
+
+/* Layouts of a frame already in device memory (what GPU decoders hand out), for ct_stage_frames.  Every row is
+ * `pitch` bytes after the previous one in its plane; pixels within a row are packed (innermost stride 1). */
+#define CT_SRC_BGR        0   /* plane[0]: interleaved [h, w, 3] BGR */
+#define CT_SRC_RGB        1   /* plane[0]: interleaved [h, w, 3] RGB, staged as BGR */
+#define CT_SRC_RGB_PLANAR 2   /* plane[0..2]: the R, G and B planes [h, w] (CHW), staged as interleaved BGR */
+#define CT_SRC_NV12       3   /* plane[0]: Y [h, w]; plane[1]: interleaved U V [h/2, w] */
+#define CT_SRC_I420       4   /* plane[0]: Y [h, w]; plane[1]: U [h/2, w/2]; plane[2]: V [h/2, w/2] */
+
+/* One stream's source frame for ct_stage_frames; its size is the destination ct_frame's h, w.  Unused planes may be
+ * NULL. */
+typedef struct {
+  const void* plane[3];       /* device pointers to each plane's first byte */
+  int64_t pitch[3];           /* row pitch in bytes of each plane, >= the plane's row bytes */
+  int32_t layout;             /* CT_SRC_* */
+  int32_t reserved;
+} ct_frame_src;
+
+/* Stages n device frames into a frame slot: stream i's source srcs[i] is copied to buf + dst[i].offset in dst[i]'s
+ * format at its row pitch dst[i].step -- interleaved BGR rows of 3 w bytes (CT_SRC_RGB swapped, CT_SRC_RGB_PLANAR
+ * interleaved), or cv2's [3h/2, w] NV12 / I420 layout that the frames kernels read.  Allowed pairs: CT_SRC_BGR, _RGB and
+ * _RGB_PLANAR into CT_FRAME_BGR, CT_SRC_NV12 into CT_FRAME_NV12, CT_SRC_I420 into CT_FRAME_I420.  srcs and dst are HOST
+ * arrays [n], read during the call and passed to the kernels by value; one launch per CT_FRAMES_PER_LAUNCH streams, on
+ * `stream`.  CT_ERR_INVALID before any launch for n <= 0, a null pointer, an unknown layout or a pair not listed, h or
+ * w <= 0, an odd h or w in 4:2:0, a source pitch or destination step shorter than a row, or a destination that extends
+ * past buf_bytes.  The sources' extents (h rows at their pitch in each plane) are the caller's to guarantee; the
+ * destination regions must not overlap each other or the sources. */
+int ct_stage_frames(const ct_frame_src* srcs, const ct_frame* dst, int32_t n, uint8_t* buf, int64_t buf_bytes,
+                    void* stream);
 
 /* ---- misc --------------------------------------------------------------------------- */
 const char* ct_last_error(void);

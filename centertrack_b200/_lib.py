@@ -99,6 +99,16 @@ class TrackPayload(C.Structure):
   ]
 
 
+CT_DET_FLOATS = 10
+
+
+class DetDesc(C.Structure):
+  _fields_ = [
+      ('n', C.c_int32), ('K', C.c_int32), ('F', C.c_int32), ('rec_tracking', C.c_int32), ('out_thresh', C.c_float),
+      ('records', C.c_void_p), ('trans_out_inv', C.c_void_p), ('dets', C.c_void_p), ('counts', C.c_void_p),
+  ]
+
+
 CT_FRAMES_PER_LAUNCH = 48
 CT_FRAME_BGR, CT_FRAME_NV12, CT_FRAME_I420 = 0, 1, 2
 
@@ -127,7 +137,7 @@ EXPORTS = ['ct_packed_weight_bytes', 'ct_pack_weights', 'ct_conv_forward', 'ct_c
            'ct_pack_stem_input', 'ct_pack_stem_input_f32', 'ct_maxpool2', 'ct_maxpool2_s2d', 'ct_upsample_add', 'ct_decode_workspace_bytes', 'ct_decode',
            'ct_render_pre_hm', 'ct_track_smem_bytes', 'ct_track_step', 'ct_track_assoc_smem_bytes',
            'ct_track_step_assoc', 'ct_track_payload_smem_bytes', 'ct_track_step_payload', 'ct_track_start',
-           'ct_render_tracks', 'ct_track_step_mapped', 'ct_render_tracks_mapped', 'ct_flip_merge', 'ct_flip_merge_heads', 'ct_mirror_x',
+           'ct_render_tracks', 'ct_track_step_mapped', 'ct_render_tracks_mapped', 'ct_post_process', 'ct_flip_merge', 'ct_flip_merge_heads', 'ct_mirror_x',
            'ct_warp_affine_normalize', 'ct_pack_stem_frames', 'ct_pack_stem_frames_flip', 'ct_pack_stem_frames_dev',
            'ct_pack_stem_frames_flip_dev', 'ct_warp_frames_normalize', 'ct_stage_frames', 'ct_last_error',
            'ct_abi_version', 'ct_launch_count', 'ct_reset_launch_count', 'ct_debug_trace', 'ct_debug_watch']
@@ -211,6 +221,7 @@ def lib():
                                      C.c_int32, C.c_void_p]
   L.ct_render_tracks_mapped.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p] + [C.c_int32] * 3 + \
       [C.c_void_p]
+  L.ct_post_process.argtypes = [C.POINTER(DetDesc), C.POINTER(TrackPayload), C.c_void_p, C.c_int32, C.c_void_p]
   L.ct_flip_merge.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p, C.c_void_p, C.c_void_p]
   L.ct_warp_affine_normalize.argtypes = [C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 4 + [C.c_int32] * 2 + [C.c_void_p]
   L.ct_flip_merge_heads.argtypes = [C.POINTER(FlipHead)] + [C.c_int32] * 4 + [C.c_void_p]

@@ -9,6 +9,8 @@
 //   ct_render_tracks the gaussian max-splat of those boxes into pre_hm (image.py:128-154)
 //   ct_track_step_mapped / ct_render_tracks_mapped   the same two on a compacted batch of live streams (image i =
 //                    stream streams[i]), for StreamRunner's idle streams
+//   ct_post_process  Detector.post_process + merge_outputs (detector.py:356-377) for runners without a tracker: the
+//                    track step's per-detection affine and payload fields, each stream's kept records in parallel
 //   ct_flip_merge    Detector._flip_output (detector.py:311-332; model/utils.py:28-50) for --flip_test;
 //                    ct_flip_merge_heads: every averaged head of B (frame, mirror) pairs in one launch
 //   ct_mirror_x      the mirrored half of a --flip_test batch (detector.py:225-226,285-286)
@@ -257,6 +259,43 @@ __device__ int public_claims(const float* pc, int P, const float* s_px, const fl
   return n;
 }
 
+// generic_post_process (post_process.py:21-91) of one record r: the first CT_DET_FLOATS columns of its result row --
+// score, class + 1, ct, tracking, bbox -- in image coordinates through the output affine `to`.  amodal (3D head sets,
+// post_process.py:76-84): ct becomes the amodal centre after `tracking` was taken from the heat-map peak; the output-grid
+// box centre + amodel_offset (rec_amodel_offset >= 0) or the image box centre.  (acx, acy) = the written ct, (tx, ty) =
+// the written tracking, for the track step's association.  The one copy of this arithmetic: the track step and
+// ct_post_process both call it.
+__device__ __forceinline__ void det_row(const float* r, const float* to, int rec_tracking, bool amodal,
+                                        int rec_amodel_offset, float* o, float& acx, float& acy, float& tx, float& ty) {
+  const float cx = r[CT_REC_XS], cy = r[CT_REC_YS];
+  const float ctx = aff_f32(to, cx, cy), cty = aff_f32(to + 3, cx, cy);
+  tx = 0.f, ty = 0.f;
+  if (rec_tracking >= 0) {
+    const float px = __fadd_rn(r[rec_tracking], cx), py = __fadd_rn(r[rec_tracking + 1], cy);
+    tx = __fsub_rn(aff_f32(to, px, py), ctx);
+    ty = __fsub_rn(aff_f32(to + 3, px, py), cty);
+  }
+  const float bl = r[CT_REC_BBOX], bt = r[CT_REC_BBOX + 1], br = r[CT_REC_BBOX + 2], bb = r[CT_REC_BBOX + 3];
+  o[CT_TRK_SCORE] = r[CT_REC_SCORE];
+  o[CT_TRK_CLASS] = r[CT_REC_CLS] + 1.f;
+  o[CT_TRK_CT] = ctx; o[CT_TRK_CT + 1] = cty;
+  o[CT_TRK_TRACKING] = tx; o[CT_TRK_TRACKING + 1] = ty;
+  o[CT_TRK_BBOX] = aff_f32(to, bl, bt); o[CT_TRK_BBOX + 1] = aff_f32(to + 3, bl, bt);
+  o[CT_TRK_BBOX + 2] = aff_f32(to, br, bb); o[CT_TRK_BBOX + 3] = aff_f32(to + 3, br, bb);
+  acx = ctx, acy = cty;
+  if (amodal) {
+    if (rec_amodel_offset >= 0) {         // numpy's fp32 mean of the two output-grid corners + amodel_offset
+      const float mx = __fadd_rn(__fmul_rn(__fadd_rn(bl, br), 0.5f), r[rec_amodel_offset]);
+      const float my = __fadd_rn(__fmul_rn(__fadd_rn(bt, bb), 0.5f), r[rec_amodel_offset + 1]);
+      acx = aff_f32(to, mx, my); acy = aff_f32(to + 3, mx, my);
+    } else {                              // the image box centre
+      acx = __fmul_rn(__fadd_rn(o[CT_TRK_BBOX], o[CT_TRK_BBOX + 2]), 0.5f);
+      acy = __fmul_rn(__fadd_rn(o[CT_TRK_BBOX + 1], o[CT_TRK_BBOX + 3]), 0.5f);
+    }
+    o[CT_TRK_CT] = acx; o[CT_TRK_CT + 1] = acy;
+  }
+}
+
 // The payload row of one detection (ct_track_payload's field order), generic_post_process's fp32 arithmetic
 // (post_process.py:55-89, ddd_utils.py:91-136): r = its record, ct = its (amodal) image centre, P = the stream's calib.
 __device__ __forceinline__ void det_payload(const ct_track_payload& p, const float* r, const float* to,
@@ -393,36 +432,10 @@ track_step_kernel(const TrackArgs a) {
   const int N = s_n;                     // records are sorted by score: the kept detections are a prefix
   const bool amodal = PAY && a.p.rec_rot >= 0 && a.p.rec_dep >= 0 && a.p.rec_dim >= 0;
   for (int i = tid; i < N; i += TRK_THREADS) {
-    const float* r = rec + (size_t)i * d.F;
     float* o = s_det + (size_t)i * TF;
-    const float cx = r[CT_REC_XS], cy = r[CT_REC_YS];
-    const float ctx = aff_f32(to, cx, cy), cty = aff_f32(to + 3, cx, cy);
-    float tx = 0.f, ty = 0.f;
-    if (d.rec_tracking >= 0) {
-      const float px = __fadd_rn(r[d.rec_tracking], cx), py = __fadd_rn(r[d.rec_tracking + 1], cy);
-      tx = __fsub_rn(aff_f32(to, px, py), ctx);
-      ty = __fsub_rn(aff_f32(to + 3, px, py), cty);
-    }
-    const float bl = r[CT_REC_BBOX], bt = r[CT_REC_BBOX + 1], br = r[CT_REC_BBOX + 2], bb = r[CT_REC_BBOX + 3];
-    o[CT_TRK_SCORE] = r[CT_REC_SCORE];
-    o[CT_TRK_CLASS] = r[CT_REC_CLS] + 1.f;
-    o[CT_TRK_CT] = ctx; o[CT_TRK_CT + 1] = cty;
-    o[CT_TRK_TRACKING] = tx; o[CT_TRK_TRACKING + 1] = ty;
-    o[CT_TRK_BBOX] = aff_f32(to, bl, bt); o[CT_TRK_BBOX + 1] = aff_f32(to + 3, bl, bt);
-    o[CT_TRK_BBOX + 2] = aff_f32(to, br, bb); o[CT_TRK_BBOX + 3] = aff_f32(to + 3, br, bb);
+    float acx, acy, tx, ty;
+    det_row(rec + (size_t)i * d.F, to, d.rec_tracking, amodal, a.p.rec_amodel_offset, o, acx, acy, tx, ty);
     o[CT_TRK_ID] = 0.f; o[CT_TRK_AGE] = 1.f; o[CT_TRK_ACTIVE] = 0.f;
-    float acx = ctx, acy = cty;
-    if (amodal) {      // post_process.py:76-84: ct becomes the amodal centre after `tracking` was taken from the peak
-      if (a.p.rec_amodel_offset >= 0) {   // numpy's fp32 mean of the two output-grid corners + amodel_offset
-        const float mx = __fadd_rn(__fmul_rn(__fadd_rn(bl, br), 0.5f), r[a.p.rec_amodel_offset]);
-        const float my = __fadd_rn(__fmul_rn(__fadd_rn(bt, bb), 0.5f), r[a.p.rec_amodel_offset + 1]);
-        acx = aff_f32(to, mx, my); acy = aff_f32(to + 3, mx, my);
-      } else {                            // the image box centre
-        acx = __fmul_rn(__fadd_rn(o[CT_TRK_BBOX], o[CT_TRK_BBOX + 2]), 0.5f);
-        acy = __fmul_rn(__fadd_rn(o[CT_TRK_BBOX + 1], o[CT_TRK_BBOX + 3]), 0.5f);
-      }
-      o[CT_TRK_CT] = acx; o[CT_TRK_CT + 1] = acy;
-    }
     s_px[i] = __fadd_rn(acx, tx);
     s_py[i] = __fadd_rn(acy, ty);
     s_isz[i] = __fmul_rn(__fsub_rn(o[CT_TRK_BBOX + 2], o[CT_TRK_BBOX]), __fsub_rn(o[CT_TRK_BBOX + 3], o[CT_TRK_BBOX + 1]));
@@ -616,6 +629,49 @@ __global__ void render_tracks_kernel(const float* __restrict__ boxes, int n, flo
     if (v < 2.220446049250313e-16) v = 0.0;
     atomicMax(reinterpret_cast<int*>(hm + ((size_t)b * H + cy + yy) * W + cx + xx), __float_as_int((float)v));
   }
+}
+
+// ct_post_process: Detector.post_process + merge_outputs of runners without a tracker.  CTA i on records[i] writes
+// stream b = streams[i]'s (identity without a map) kept detections: the score-sorted records with score > out_thresh
+// are a prefix, each of its rows computed by det_row (+ det_payload) independently of the others.
+constexpr int DET_THREADS = 128;
+constexpr int DF = CT_DET_FLOATS;
+
+struct DetArgs {
+  ct_det_desc d;
+  ct_track_payload p;      // read by the payload instantiation only
+  const int* streams;      // NULL = identity
+  int n_streams;
+};
+
+template <bool PAY>
+__global__ void __launch_bounds__(DET_THREADS) post_process_kernel(const DetArgs a) {
+  const ct_det_desc& d = a.d;
+  const int b = a.streams ? a.streams[blockIdx.x] : (int)blockIdx.x;
+  if (b < 0 || b >= a.n_streams) return;                    // a padding image, or no stream: nothing is written
+  __shared__ int s_n;
+  if (threadIdx.x == 0) s_n = 0;
+  __syncthreads();
+  const int K = d.K, F = d.F;
+  const float* rec = d.records + (size_t)blockIdx.x * K * F;
+  int cnt = 0;
+  for (int i = threadIdx.x; i < K; i += DET_THREADS) cnt += rec[(size_t)i * F + CT_REC_SCORE] > d.out_thresh ? 1 : 0;
+  atomicAdd(&s_n, cnt);
+  __syncthreads();
+  const int N = s_n;
+  const float* to = d.trans_out_inv + b * 6;
+  const bool amodal = PAY && a.p.rec_rot >= 0 && a.p.rec_dep >= 0 && a.p.rec_dim >= 0;
+  const float* P = PAY && a.p.calib ? a.p.calib + b * 12 : nullptr;
+  float* out = d.dets + (size_t)b * K * DF;
+  for (int i = threadIdx.x; i < N; i += DET_THREADS) {
+    const float* r = rec + (size_t)i * F;
+    float o[DF], acx, acy, tx, ty;
+    det_row(r, to, d.rec_tracking, amodal, PAY ? a.p.rec_amodel_offset : -1, o, acx, acy, tx, ty);
+#pragma unroll
+    for (int f = 0; f < DF; ++f) out[(size_t)i * DF + f] = o[f];
+    if constexpr (PAY) det_payload(a.p, r, to, o + CT_TRK_CT, P, a.p.payload + ((size_t)b * K + i) * a.p.width);
+  }
+  if (threadIdx.x == 0) d.counts[b] = N;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1093,6 +1149,23 @@ static inline bool rec_field_ok(int32_t off, int32_t w, int32_t F) {
   return off < 0 || (w > 0 && off >= CT_REC_HEADS && off + w <= F);
 }
 
+// The payload descriptor of an F-float record: its fields inside the record, its width their sum, calib for 3D sets.
+static int payload_check(const ct_track_payload* p, int32_t F) {
+  CT_REQUIRE(p->payload, "null payload table");
+  CT_REQUIRE(rec_field_ok(p->rec_hps, p->hps_floats, F) && (p->rec_hps < 0 || p->hps_floats % 2 == 0) &&
+             rec_field_ok(p->rec_dep, 1, F) && rec_field_ok(p->rec_dim, 3, F) &&
+             rec_field_ok(p->rec_rot, 8, F) && rec_field_ok(p->rec_amodel_offset, 2, F) &&
+             rec_field_ok(p->rec_velocity, p->velocity_floats, F) &&
+             rec_field_ok(p->rec_nuscenes_att, p->att_floats, F), "payload field outside the record");
+  const bool ddd = p->rec_rot >= 0 && p->rec_dep >= 0 && p->rec_dim >= 0;
+  const int64_t w = (p->rec_hps >= 0 ? p->hps_floats : 0) + (p->rec_dep >= 0 ? 1 : 0) + (p->rec_dim >= 0 ? 3 : 0) +
+                    (p->rec_rot >= 0 ? 1 : 0) + (ddd ? 4 : 0) + (p->rec_velocity >= 0 ? p->velocity_floats : 0) +
+                    (p->rec_nuscenes_att >= 0 ? p->att_floats : 0);
+  CT_REQUIRE(w > 0 && p->width == w, "payload width does not match its fields");
+  CT_REQUIRE(!ddd || p->calib, "rot, dep and dim need calib");
+  return CT_OK;
+}
+
 // One track step launch: CTA i on records[i] and stream streams[i] (streams == NULL: stream i of d->B).
 static int track_step_launch(const ct_track_desc* d, const ct_track_assoc* as, const ct_track_payload* p,
                              const int32_t* streams, int32_t n_streams, void* stream) {
@@ -1103,18 +1176,8 @@ static int track_step_launch(const ct_track_desc* d, const ct_track_assoc* as, c
   CT_REQUIRE(!as->public_det || (as->public_ct && as->public_n), "public_det needs public_ct and public_n");
   CT_REQUIRE(!as->public_det || as->max_public > 0, "public_det needs max_public > 0");
   if (p) {
-    CT_REQUIRE(p->payload, "null payload table");
-    CT_REQUIRE(rec_field_ok(p->rec_hps, p->hps_floats, d->F) && (p->rec_hps < 0 || p->hps_floats % 2 == 0) &&
-               rec_field_ok(p->rec_dep, 1, d->F) && rec_field_ok(p->rec_dim, 3, d->F) &&
-               rec_field_ok(p->rec_rot, 8, d->F) && rec_field_ok(p->rec_amodel_offset, 2, d->F) &&
-               rec_field_ok(p->rec_velocity, p->velocity_floats, d->F) &&
-               rec_field_ok(p->rec_nuscenes_att, p->att_floats, d->F), "payload field outside the record");
-    const bool ddd = p->rec_rot >= 0 && p->rec_dep >= 0 && p->rec_dim >= 0;
-    const int64_t w = (p->rec_hps >= 0 ? p->hps_floats : 0) + (p->rec_dep >= 0 ? 1 : 0) + (p->rec_dim >= 0 ? 3 : 0) +
-                      (p->rec_rot >= 0 ? 1 : 0) + (ddd ? 4 : 0) + (p->rec_velocity >= 0 ? p->velocity_floats : 0) +
-                      (p->rec_nuscenes_att >= 0 ? p->att_floats : 0);
-    CT_REQUIRE(w > 0 && p->width == w, "payload width does not match its fields");
-    CT_REQUIRE(!ddd || p->calib, "rot, dep and dim need calib");
+    const int rc = payload_check(p, d->F);
+    if (rc != CT_OK) return rc;
   }
   const bool scratch = as->hungarian || as->public_det;
   const size_t smem = (size_t)ct_track_payload_smem_bytes(d->K, d->max_tracks, p ? p->width : 0, scratch);
@@ -1169,6 +1232,28 @@ extern "C" int ct_track_start(const ct_track_desc* d, const ct_track_payload* p,
   if (n_starts == 0) return CT_OK;
   track_start_kernel<<<n_starts, TRK_THREADS, 0, (cudaStream_t)stream>>>(*d, p ? p->payload : nullptr, p ? p->width : 0,
                                                                           starts, seeds);
+  return after_launch();
+}
+
+extern "C" int ct_post_process(const ct_det_desc* d, const ct_track_payload* p, const int32_t* streams,
+                               int32_t n_streams, void* stream) {
+  CT_REQUIRE(d && d->records && d->trans_out_inv && d->dets && d->counts, "null pointer");
+  CT_REQUIRE(d->n > 0 && d->K > 0 && d->F >= CT_REC_HEADS, "bad shape (n > 0, K > 0, F >= CT_REC_HEADS)");
+  CT_REQUIRE(d->rec_tracking < 0 || (d->rec_tracking >= CT_REC_HEADS && d->rec_tracking + 2 <= d->F),
+             "tracking offset outside the record");
+  CT_REQUIRE(n_streams > 0, "n_streams <= 0");
+  CT_REQUIRE(streams || d->n <= n_streams, "without a stream map every image needs a stream (n <= n_streams)");
+  if (p) {
+    const int rc = payload_check(p, d->F);
+    if (rc != CT_OK) return rc;
+  }
+  DetArgs a = {};
+  a.d = *d;
+  if (p) a.p = *p;
+  a.streams = streams;
+  a.n_streams = n_streams;
+  auto kernel = p ? post_process_kernel<true> : post_process_kernel<false>;
+  kernel<<<d->n, DET_THREADS, 0, (cudaStream_t)stream>>>(a);
   return after_launch();
 }
 

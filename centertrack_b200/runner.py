@@ -21,6 +21,9 @@ Two ways to feed the prior heat-map (`--pre_hm`):
     the payload table beside it (hps, dep, dim, alpha, loc, rot_y, velocity, nuscenes_att).  Every association mode
     of the host Tracker runs there: greedy, `--hungarian`, and `--public_det`, whose public detections (the `ct`s of
     each frame's provided detections) are staged per input slot like the frames and uploaded with them.
+  Without a tracker, device_post_process=True post-processes the records inside the same graph (`DeviceDetections`:
+  ct_post_process, Detector.post_process + merge_outputs) and downloads each stream's detections with them, so a
+  detection model (ctdet, ddd, multi_pose) needs no host generic_post_process either.
 
 The end-to-end form (`step_host`) takes HOST frames: pinned staging, H2D on a copy stream overlapped
 with the previous step's compute, graph replay, D2H of the records (and tracks).
@@ -74,6 +77,7 @@ from . import _lib as L
 from .dataset_info import get_dataset
 from .decode import generic_decode
 from .detector import default_calib, flip_output, flip_plan, frame_geometry
+from .device_detections import DeviceDetections
 from .device_tracker import DeviceTracker, default_geometry, plan_starts
 
 
@@ -218,10 +222,11 @@ def device_frame_source(x, fmt, layout, device, what='frame'):
 class StreamRunner(object):
 
   frame_format = 'bgr'
+  post = None                                                # device_post_process: DeviceDetections
 
   def __init__(self, model, B, H, W, K=100, precision='bf16', device='cuda', use_graph=True, opt=None,
                device_tracking=False, max_public_dets=512, calibs=None, frame_sizes=None, max_frame_size=None,
-               idle_streams=None, frame_format='bgr'):
+               idle_streams=None, frame_format='bgr', device_post_process=False):
     """max_public_dets: with device_tracking and --public_det, the most public detections a stream may bring per
     frame (more raise ValueError; none is ever dropped).  calibs: with device_tracking on a 3D head set, one [3,4]
     camera matrix per stream (DeviceTracker's default otherwise; in frames mode Detector._get_default_calib of the
@@ -238,7 +243,14 @@ class StreamRunner(object):
     frame_format: what step_frames and frame_buffers take -- 'bgr' (uint8 [h, w, 3]), or 'nv12' / 'i420' (one uint8
     [3h/2, w] array per frame in cv2's 4:2:0 layout, h and w even; needs max_frame_size, whose region is then
     h * w * 3 / 2 bytes).  A 4:2:0 frame is converted on the device, inside the warp, exactly as
-    cv2.cvtColor(COLOR_YUV2BGR_NV12 / _I420) converts it: a stream gives what it gives on that BGR image."""
+    cv2.cvtColor(COLOR_YUV2BGR_NV12 / _I420) converts it: a stream gives what it gives on that BGR image.
+    device_post_process (runners without device_tracking): each step also post-processes its records on the device
+    (ct_post_process, inside the graph) into each stream's detections in its source pixels -- Detector.post_process +
+    merge_outputs -- and downloads them with the records: fetch_results() / previous_results() give the host path's
+    dicts, fetch_detections() the tables.  calibs then give the 3D head sets' cameras, as with device_tracking."""
+    if device_post_process and device_tracking:
+      raise ValueError('device_post_process is for runners without a tracker: device_tracking already post-processes '
+                       'the detections (fetch_results() gives its tracks)')
     self.B, self.H, self.W, self.K = B, H, W, K
     self.device = torch.device(device)
     self.model = model
@@ -328,6 +340,13 @@ class StreamRunner(object):
         geo = dict(centers=[m['c'] for m in self._meta], scales=[m['s'] for m in self._meta])
       self.tracker = DeviceTracker(self.opt, B, K, self.rec.shape[2], self.layout, H, W, self.device,
                                    max_public_dets=max_public_dets, calibs=calibs, **geo)
+    elif device_post_process:
+      assert self.opt is not None, 'device post-processing needs opt (out_thresh)'
+      geo = {}
+      if self.frames_mode:
+        geo = dict(centers=[m['c'] for m in self._meta], scales=[m['s'] for m in self._meta])
+      self.post = DeviceDetections(self.opt, B, K, self.rec.shape[2], self.layout, H, W, self.device, calibs=calibs,
+                                   **geo)
     self.public = self.tracker is not None and self.tracker.public_det
     if self.public:                                          # per slot: device (public_ct, public_n) + pinned staging
       self.pub = [self.tracker.public_buffers() for _ in range(NS)]
@@ -339,10 +358,16 @@ class StreamRunner(object):
       self.h_cnt = [torch.zeros_like(self.tracker.counts, device='cpu').pin_memory() for _ in range(2)]
       if self.tracker.payload is not None:
         self.h_pay = [torch.zeros_like(self.tracker.payload, device='cpu').pin_memory() for _ in range(2)]
+    if self.post is not None:
+      self.h_det = [torch.zeros_like(self.post.dets, device='cpu').pin_memory() for _ in range(2)]
+      self.h_det_cnt = [torch.zeros_like(self.post.counts, device='cpu').pin_memory() for _ in range(2)]
+      if self.post.payload is not None:
+        self.h_det_pay = [torch.zeros_like(self.post.payload, device='cpu').pin_memory() for _ in range(2)]
     # launches of one step: the network plan + decode (+ memset-free: render + track step); frames mode: the pack op
     # becomes ct_pack_stem_frames (one launch per CT_FRAMES_PER_LAUNCH streams), or B warps come before the plan.
-    # --flip_test: + the merge, + the mirrors of the images and pre_hm unless the flip pack writes them
-    self.launches_per_step = self.eng.n_launches + 1 + (2 if device_tracking else 0)
+    # --flip_test: + the merge, + the mirrors of the images and pre_hm unless the flip pack writes them;
+    # device_post_process: + ct_post_process
+    self.launches_per_step = self.eng.n_launches + 1 + (2 if device_tracking else 0) + (1 if self.post else 0)
     if self.frames_mode and self.cap is not None:           # device descriptors: one pack or one warp for all B
       self.launches_per_step += 0 if self.eng.use_halo else 1
     elif self.frames_mode:
@@ -487,7 +512,7 @@ class StreamRunner(object):
       for b in sorted(set(changed) | set(calibs)):
         m = self._meta[b]
         rows.append((b, m['c'], m['s'], np.asarray(m['calib'], np.float32)))
-    elif self.tracker is not None:           # fp32 images of the input size: the tracker's default (c, s) throughout
+    elif self._geo_tables() is not None:     # fp32 images of the input size: the default (c, s) throughout
       c, s = default_geometry(self.H, self.W)
       rows = [(b, c, s, k) for b, k in sorted(calibs.items())]
     desc = None
@@ -585,6 +610,11 @@ class StreamRunner(object):
         self.tracker.step(self.rec, *pub)
       else:
         self.tracker.step_mapped(self.rec[:n], self.d_map[slot][:self.B], *pub)
+    if self.post is not None:                                # each stream's detections in its source pixels
+      if self.idle_g is None:
+        self.post.step(self.rec)
+      else:
+        self.post.step_mapped(self.rec[:n], self.d_map[slot][:self.B])
     return res
 
   def _decode_ws(self, n):
@@ -647,6 +677,10 @@ class StreamRunner(object):
       for t, v in zip(self._tracker_state(), saved):
         t.copy_(v)
     return g
+
+  def _geo_tables(self):
+    """The device tables that hold per-stream camera rows (the tracker, or the post-processed detections), or None."""
+    return self.tracker if self.tracker is not None else self.post
 
   def _tracker_state(self):
     trk = self.tracker
@@ -763,7 +797,7 @@ class StreamRunner(object):
     """Stages and uploads the tracker geometry rows of the streams whose camera changes in this step (_plan_geometry)
     for slot's start prologue (the current stream is the upload's); -> the bytes uploaded."""
     self._geo[slot] = None
-    if not rows or self.tracker is None:
+    if not rows or self._geo_tables() is None:
       return 0
     if self.h_geo is None:
       self.h_geo = [(torch.zeros((self.B, 6), dtype=torch.float64).pin_memory(),
@@ -771,7 +805,7 @@ class StreamRunner(object):
       self.d_geo_in = [torch.zeros((self.B, 6), dtype=torch.float64, device=self.device) for _ in range(NS)]
       self.d_geo_out = [torch.zeros((self.B, 18), dtype=torch.float32, device=self.device) for _ in range(NS)]
     streams, cs, ss, ks = zip(*rows)
-    t_in, t_out = self.tracker.geometry_rows(cs, ss, ks)
+    t_in, t_out = self._geo_tables().geometry_rows(cs, ss, ks)
     n = len(streams)
     h_in, h_out = self.h_geo[slot]
     h_in[:n], h_out[:n] = torch.from_numpy(t_in), torch.from_numpy(t_out)
@@ -830,8 +864,8 @@ class StreamRunner(object):
         if self.flip:                                        # --flip_test: pre_images is the (frame, mirror) pair
           self._mirror(self.img[prev], b, 1)
     geo, self._geo[slot] = self._geo[slot], None
-    if self.tracker is not None and geo:                     # new cameras: before the seeds' boxes are rendered
-      self.tracker.set_geometry(geo, self.d_geo_in[slot], self.d_geo_out[slot])
+    if geo:                                                  # new cameras: before the seeds' boxes are rendered
+      self._geo_tables().set_geometry(geo, self.d_geo_in[slot], self.d_geo_out[slot])
     if self.tracker is not None:                             # reset + seeds + boxes: the step's render splats them
       self.tracker.start_device(self.d_start[slot], len(streams), self.d_seed[slot])
 
@@ -909,6 +943,11 @@ class StreamRunner(object):
         self.h_cnt[self.t & 1].copy_(self.tracker.counts, non_blocking=True)
         if self.tracker.payload is not None:
           self.h_pay[self.t & 1].copy_(self.tracker.payload, non_blocking=True)
+      if self.post is not None:
+        self.h_det[self.t & 1].copy_(self.post.dets, non_blocking=True)
+        self.h_det_cnt[self.t & 1].copy_(self.post.counts, non_blocking=True)
+        if self.post.payload is not None:
+          self.h_det_pay[self.t & 1].copy_(self.post.payload, non_blocking=True)
       # this step's pre_images slot may be overwritten once this step is done
       self.ev_done[(slot - 1) % NS].record(self.compute)
     self.t += 1
@@ -1170,12 +1209,19 @@ class StreamRunner(object):
     live = self._live[t & 1]
     return None if live is None or len(live) == self.B else live
 
+  def _idle_of(self, t):
+    live = self._live_of(t)
+    return () if live is None else set(range(self.B)) - set(live)
+
   def _results(self, t):
     i = t & 1
+    if self.post is not None:
+      pay = self.h_det_pay[i].numpy() if self.post.payload is not None else None
+      return self.post.results(self.h_det[i].numpy(), self.h_det_cnt[i].numpy(), pay, self._idle_of(t))
+    if self.tracker is None:
+      raise ValueError('results: the runner was built without device_tracking or device_post_process')
     pay = self.h_pay[i].numpy() if self.tracker.payload is not None else None
-    live = self._live_of(t)
-    idle = () if live is None else set(range(self.B)) - set(live)
-    return self.tracker.results(self.h_trk[i].numpy(), self.h_cnt[i].numpy(), pay, idle)
+    return self.tracker.results(self.h_trk[i].numpy(), self.h_cnt[i].numpy(), pay, self._idle_of(t))
 
   def fetch_tracks(self):
     """(tracks [B,T,CT_TRK_FLOATS], counts [B,2]) of the last submitted step (device_tracking), as numpy copies."""
@@ -1183,16 +1229,42 @@ class StreamRunner(object):
     i = (self.t - 1) & 1
     return self.h_trk[i].numpy().copy(), self.h_cnt[i].numpy().copy()
 
+  def fetch_detections(self):
+    """(dets [B,K,CT_DET_FLOATS], counts [B], payload [B,K,Wp] or None) of the last submitted step
+    (device_post_process), as numpy copies: stream b's detections are its first counts[b] rows.  A stream that was idle
+    in that step has count 0."""
+    if self.post is None:
+      raise ValueError('fetch_detections(): the runner was built without device_post_process')
+    self.compute.synchronize()
+    return self._detections(self.t - 1)
+
+  def previous_detections(self):
+    """After a step_host / step_frames call: fetch_detections() of the step before it, without a wait (as
+    previous_results())."""
+    if self.post is None:
+      raise ValueError('previous_detections(): the runner was built without device_post_process')
+    if self.t < 2:
+      raise ValueError('previous_detections(): fewer than two steps submitted')
+    return self._detections(self.t - 2)
+
+  def _detections(self, t):
+    i = t & 1
+    cnt = self.h_det_cnt[i].numpy().copy()
+    cnt[sorted(self._idle_of(t))] = 0
+    pay = self.h_det_pay[i].numpy().copy() if self.post.payload is not None else None
+    return self.h_det[i].numpy().copy(), cnt, pay
+
   def fetch_results(self):
-    """The last submitted step's tracks (device_tracking) as the host path's per-stream lists of dicts
-    (DeviceTracker.results), payload fields included; None for a stream that was idle in that step."""
+    """The last submitted step's tracks (device_tracking), or detections (device_post_process), as the host path's
+    per-stream lists of dicts (DeviceTracker.results, DeviceDetections.results), payload fields included; None for a
+    stream that was idle in that step."""
     self.compute.synchronize()
     return self._results(self.t - 1)
 
   def previous_results(self):
-    """After a step_host / step_frames call: the tracks of the step before it, as fetch_results() gives them.  No wait:
-    the call returned once that step had finished (its records are what the call returned), and its tables are not
-    overwritten before the next call."""
+    """After a step_host / step_frames call: the tracks (or detections) of the step before it, as fetch_results()
+    gives them.  No wait: the call returned once that step had finished (its records are what the call returned), and
+    its tables are not overwritten before the next call."""
     if self.t < 2:
       raise ValueError('previous_results(): fewer than two steps submitted')
     return self._results(self.t - 2)
@@ -1213,7 +1285,8 @@ class StreamRunner(object):
 
   @property
   def d2h_bytes_per_step(self):
-    return self.rec.numel() * 4 + (self.tracker.d2h_bytes if self.tracker is not None else 0)
+    tables = self._geo_tables()
+    return self.rec.numel() * 4 + (tables.d2h_bytes if tables is not None else 0)
 
   def views(self, rec_np):
     from .decode import views_from_records

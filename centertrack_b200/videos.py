@@ -43,13 +43,15 @@ def _as_video(v):
 
 
 def track_videos(runner, videos, layout='bgr'):
-  """runner: a StreamRunner with device tracking; videos: an iterable of Video (or dicts of its fields).  Yields
+  """runner: a StreamRunner with device tracking, or with device_post_process (detection models: each frame's
+  detections, and no video may bring pre_dets); videos: an iterable of Video (or dicts of its fields).  Yields
   (video id, frame index, results) for every frame of every video exactly once, as its tracks come back; results is the
   list of dicts fetch_results() gives for that stream (in source pixels in frames mode).  layout: step_frames' layout of
   device frames.  ValueError for a video whose frame size no stream can take, a video whose frames are of another kind
-  (device tensors or arrays) than the first video's, or a runner without device tracking."""
-  if runner.tracker is None:
-    raise ValueError('track_videos: the runner needs device_tracking=True')
+  (device tensors or arrays) than the first video's, or a runner with neither device tracking nor device
+  post-processing."""
+  if runner.tracker is None and getattr(runner, 'post', None) is None:
+    raise ValueError('track_videos: the runner needs device_tracking=True or device_post_process=True')
   if layout != 'bgr' and not runner.frames_mode:
     raise ValueError('track_videos: layout=%r needs a frames-mode runner' % (layout,))
   B = runner.B

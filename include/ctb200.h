@@ -25,6 +25,8 @@
  *                     ct_track_step_payload adds the pose / 3D / velocity / attribute fields (post_process.py:55-89).
  *                     ct_track_start: reset_tracking + Tracker.init_track(pre_dets) on some streams alone
  *                     (detector.py:97-103, utils/tracker.py:11-22).
+ *   ct_post_process   Detector.post_process + merge_outputs (detector.py:356-377) on the device for runners without a
+ *                     tracker: each stream's kept detections in its source pixels, with ct_track_step's arithmetic.
  *   ct_flip_merge     Detector._flip_output, detector.py:311-332 (flip_tensor / flip_lr / flip_lr_off, model/utils.py:28-50);
  *                     ct_flip_merge_heads merges every head of B pairs at once, ct_mirror_x mirrors the --flip_test
  *                     batch's second half (detector.py:225-226,285-286).
@@ -366,6 +368,32 @@ int ct_track_step_mapped(const ct_track_desc* d, const ct_track_assoc* a, const 
  * stream maps outside [0, n_images) are skipped.  The launch shape depends on n alone (CUDA-graph capturable). */
 int ct_render_tracks_mapped(const float* boxes, int32_t n, const int32_t* image_of, int32_t n_streams, float* pre_hm,
                             int32_t n_images, int32_t H, int32_t W, void* stream);
+
+/* Detections of runners without a tracker (Detector.post_process + merge_outputs, detector.py:356-377): each image's
+ * records with score > out_thresh -- a prefix, the records being sorted by score -- as rows of the first CT_DET_FLOATS
+ * columns of a track row (CT_TRK_SCORE .. CT_TRK_BBOX: score, class + 1, ct, tracking, bbox) in the stream's source
+ * pixels, computed as ct_track_step computes them (tracking 0 without rec_tracking; on 3D head sets ct is the amodal
+ * centre). */
+#define CT_DET_FLOATS 10
+typedef struct {
+  int32_t n, K, F;            /* decode records [n,K,F] (ct_decode), sorted by score */
+  int32_t rec_tracking;       /* float offset of the `tracking` head inside a record, -1 if absent */
+  float out_thresh;           /* records with score > out_thresh are kept */
+  const float* records;
+  const float* trans_out_inv; /* [n_streams,6] fp32: output grid -> image (as ct_track_desc's) */
+  float* dets;                /* out [n_streams,K,CT_DET_FLOATS] */
+  int32_t* counts;            /* out [n_streams]: the rows written for each stream */
+} ct_det_desc;
+
+/* Writes image i's kept detections as stream b's rows dets[b][0 .. counts[b]) and counts[b], where b = i, or
+ * streams[i] when streams (device int32 [n]) is not NULL; an entry outside [0, n_streams) writes nothing.  Rows at or
+ * beyond counts[b], and streams no image maps to, are left untouched.  p (NULL on 2-D head sets): the task fields of
+ * ct_track_payload's row for each detection, written to p->payload [n_streams,K,p->width] row for row beside dets, with
+ * p->calib [n_streams,3,4].  One CTA per image (the launch shape depends on n alone: CUDA-graph capturable).
+ * CT_ERR_INVALID before any launch for a null pointer, n, K or n_streams <= 0, F < CT_REC_HEADS, n > n_streams without
+ * a map, or a field outside the record / payload width / missing calib as ct_track_step_payload checks them. */
+int ct_post_process(const ct_det_desc* d, const ct_track_payload* p, const int32_t* streams, int32_t n_streams,
+                    void* stream);
 
 /* out[c,y,x] = (in2[0,c,y,x] + sign[c] * in2[1,perm[c],y,W-1-x]) / 2;  in2 fp32 [2,C,H,W], out [1,C,H,W];
  * perm (int32 [C], device) / sign (fp32 [C], device) may be NULL (identity / +1). */

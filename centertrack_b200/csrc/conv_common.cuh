@@ -63,10 +63,11 @@ __device__ __forceinline__ float head_transform(float v, int head_act, float dep
 
 // ---- host side of the tensor-core engines ----
 // TMA descriptor of a bf16 tensor: `rank` dims and box sizes innermost first, rank - 1 byte strides of the outer
-// dims; elements outside the tensor read as zero.  cuTensorMapEncodeTiled is reached through the runtime's driver
-// entry point (no -lcuda at link time).
+// dims; elements outside the tensor read as zero.  estr: element strides of the box (nullptr: 1 in every dim).
+// cuTensorMapEncodeTiled is reached through the runtime's driver entry point (no -lcuda at link time).
 inline int encode_tmap_bf16(CUtensorMap* map, const void* ptr, int rank, const cuuint64_t* dims,
-                            const cuuint64_t* strides, const cuuint32_t* box, CUtensorMapSwizzle swizzle) {
+                            const cuuint64_t* strides, const cuuint32_t* box, CUtensorMapSwizzle swizzle,
+                            const cuuint32_t* estr = nullptr) {
   static const PFN_cuTensorMapEncodeTiled encode = [] {
     void* p = nullptr;
     cudaDriverEntryPointQueryResult q;
@@ -75,9 +76,9 @@ inline int encode_tmap_bf16(CUtensorMap* map, const void* ptr, int rank, const c
     return ok ? reinterpret_cast<PFN_cuTensorMapEncodeTiled>(p) : nullptr;
   }();
   if (!encode) return fail(CT_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable%s", "");
-  const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+  const cuuint32_t ones[5] = {1, 1, 1, 1, 1};
   const CUresult cr = encode(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(ptr), dims,
-                             strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
+                             strides, box, estr ? estr : ones, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
                              CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return cr == CUDA_SUCCESS ? CT_OK : fail(CT_ERR_CUDA, "cuTensorMapEncodeTiled failed%s (%ld)", "", (long)cr);
 }

@@ -363,6 +363,44 @@ __device__ __forceinline__ void gather_window(const TcArgs& a, const Gather& t, 
   }
 }
 
+// Output columns o0 .. o0 + 15 of pixel p (accumulator values v): + folded-BN shift, then residual / ReLU and the store
+// of the output mode.  X3: fp32 NHWC activations.
+template <bool X3>
+__device__ __forceinline__ void tc_store16(const TcArgs& a, int p, int o0, float (&v)[16]) {
+  const ConvGeom& g = a.g;
+  if (a.shift) {
+    if (o0 + 16 <= g.C_out && (reinterpret_cast<size_t>(a.shift + o0) & 15) == 0) {   // four 16-byte loads
+      const float4* sh4 = reinterpret_cast<const float4*>(a.shift + o0);
+#pragma unroll
+      for (int j4 = 0; j4 < 4; ++j4) {
+        const float4 sh = __ldg(sh4 + j4);
+        v[4 * j4] += sh.x; v[4 * j4 + 1] += sh.y; v[4 * j4 + 2] += sh.z; v[4 * j4 + 3] += sh.w;
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < 16; ++j) if (o0 + j < g.C_out) v[j] += __ldg(a.shift + o0 + j);
+    }
+  }
+  if (X3 && g.out_mode == CT_OUT_NHWC) {            // fp32 activations in, fp32 activations out
+    const float* res = a.residual ? reinterpret_cast<const float*>(a.residual) + (size_t)p * g.ld_res + o0 : nullptr;
+    store_f32_act16(reinterpret_cast<float*>(a.out) + (size_t)p * g.ld_out + o0, v, res, g.relu);
+  } else if (g.out_mode == CT_OUT_NHWC) {
+    if (a.residual) {
+      const uint4* rp = reinterpret_cast<const uint4*>(a.residual + (size_t)p * g.ld_res + o0);
+      const uint4 ra = ldg_nc16(rp), rb2 = ldg_nc16(rp + 1);
+      add_residual_bf16(v, ra, rb2);
+    }
+    relu16(v, g.relu);
+    store_bf16x16(reinterpret_cast<__nv_bfloat16*>(a.out) + (size_t)p * g.ld_out + o0, v);
+  } else if (g.out_mode == CT_OUT_NHWC_F32) {
+    store_f32_nhwc16(reinterpret_cast<float*>(a.out) + (size_t)p * g.ld_out + o0, v, o0, g);
+  } else {
+    const int HWo = g.OH * g.OW;
+    const int b = p / HWo, rr = p - b * HWo;
+    store_head16(reinterpret_cast<float*>(a.out) + ((size_t)b * g.C_out + o0) * HWo + rr, HWo, v, o0, g);
+  }
+}
+
 template <bool X3, int N>
 __global__ void __launch_bounds__(TC_THREADS, (!X3 && N <= 64) ? 2 : 1)
 conv_tc_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
@@ -581,40 +619,132 @@ conv_tc_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
     if (col < N && p_ok && o0 < g.C_out) {
       float v[16];
       lds_f(stg + ((uint32_t)row * EPI_PITCH + (uint32_t)chalf * 16u) * 4u, v);
-      if (a.shift) {
-        if (o0 + 16 <= g.C_out && (reinterpret_cast<size_t>(a.shift + o0) & 15) == 0) {   // four 16-byte loads
-          const float4* sh4 = reinterpret_cast<const float4*>(a.shift + o0);
-#pragma unroll
-          for (int j4 = 0; j4 < 4; ++j4) {
-            const float4 sh = __ldg(sh4 + j4);
-            v[4 * j4] += sh.x; v[4 * j4 + 1] += sh.y; v[4 * j4 + 2] += sh.z; v[4 * j4 + 3] += sh.w;
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) if (o0 + j < g.C_out) v[j] += __ldg(a.shift + o0 + j);
-        }
-      }
-      if (X3 && g.out_mode == CT_OUT_NHWC) {            // fp32 activations in, fp32 activations out
-        const float* res = a.residual ? reinterpret_cast<const float*>(a.residual) + (size_t)p * g.ld_res + o0 : nullptr;
-        store_f32_act16(reinterpret_cast<float*>(a.out) + (size_t)p * g.ld_out + o0, v, res, g.relu);
-      } else if (g.out_mode == CT_OUT_NHWC) {
-        if (a.residual) {
-          const uint4* rp = reinterpret_cast<const uint4*>(a.residual + (size_t)p * g.ld_res + o0);
-          const uint4 ra = ldg_nc16(rp), rb2 = ldg_nc16(rp + 1);
-          add_residual_bf16(v, ra, rb2);
-        }
-        relu16(v, g.relu);
-        store_bf16x16(reinterpret_cast<__nv_bfloat16*>(a.out) + (size_t)p * g.ld_out + o0, v);
-      } else if (g.out_mode == CT_OUT_NHWC_F32) {
-        store_f32_nhwc16(reinterpret_cast<float*>(a.out) + (size_t)p * g.ld_out + o0, v, o0, g);
-      } else {
-        const int b = p / HWo, rr = p - b * HWo;
-        store_head16(reinterpret_cast<float*>(a.out) + ((size_t)b * g.C_out + o0) * HWo + rr, HWo, v, o0, g);
-      }
+      tc_store16<X3>(a, p, o0, v);
     }
     __syncthreads();
   }
   if (tid == 0) tc_stamp(trace, 6);
+}
+
+// ---- plain convolutions of the bf16 engine with C_in % 64 == 0: TMA-fed, persistent, warp-specialised ----
+// K order as above (k = tap * C_in + c): K slice s is one tap of one 64-channel chunk, so the A operand of a slice is ONE
+// tensor-map box {64 channels, 16 x, 8 y, 1 image} at (c0, ox0 * stride - pad_w + kx, oy0 * stride - pad + ky, b): its 128
+// rows of 128 bytes land in tc_pixel's 8 x 16 patch order, 128B-swizzled, i.e. exactly the K-major layout make_sdesc
+// describes.  The map's zero fill is the padding, its element strides (= stride in x and y) the strided convolutions,
+// and its channel stride ld_in reads channel slices of wider (concat) buffers in place.
+//
+// Two warpgroups issue the MMAs of GEMM rows 64 w .. 64 w + 63 and then store them (tc_store16); one arrival per warp on
+// the empty barrier releases a stage.  Thread 0 issues the A box and the weight tile of each slice into one stage, both
+// completing the stage's full barrier: S slices up front, then one per released stage, S - 1 slices ahead of the MMAs.
+// CTAs are persistent (static stride over the (m, n) tiles), so these loads run into the next tile's slices while the
+// warpgroups finish the current one; at N <= 128 two CTAs share an SM and one CTA's epilogue runs under the other's MMAs.
+// (A separate producer warp would make 9 warps per CTA: the register file of an SM sub-partition then holds two such
+// CTAs only at 96 registers, where N = 128 spills.)
+constexpr int TMA_THREADS = 256;
+constexpr int TMA_STAGING_BYTES = 2 * 64 * EPI_PITCH * 4;     // per warpgroup: 64 rows x 32 columns of fp32
+
+template <int N>
+__global__ void __launch_bounds__(TMA_THREADS, N <= 128 ? 2 : 1)
+conv_tma_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
+  extern __shared__ __align__(1024) unsigned char smem_dyn[];
+  unsigned char* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
+  const ConvGeom& g = a.g;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int S = a.stages;
+  constexpr uint32_t b_bytes = (uint32_t)N * 128u;
+  // smem: [A stages][B stages][staging 2 x 64 x EPI_PITCH fp32][full[S], empty[S]]
+  const uint32_t sA = smem_u32(smem);
+  const uint32_t sB = sA + S * A_STAGE_BYTES;
+  const uint32_t sStg = sB + S * b_bytes;
+  const uint32_t bars = sStg + TMA_STAGING_BYTES;
+  auto full_bar = [&](int s) { return bars + 8u * s; };
+  auto empty_bar = [&](int s) { return bars + 8u * (S + s); };
+  const int m_tiles = g.B * a.tiles_x * a.tiles_y;
+  const int items = m_tiles * ((g.C_out + N - 1) / N);
+  const int KS = a.k_slices;
+
+  pdl_trigger();
+  if (tid == 0) {
+    for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 8); }
+    mbar_init_fence();
+  }
+  __syncthreads();
+  pdl_wait();
+
+  // ---- loads (thread 0): the next slice (l_item, l_s) of this CTA's items, into stage l_it % S once it is empty
+  int l_item = blockIdx.x, l_s = 0, l_it = 0;
+  auto load_next = [&]() {
+    if (l_item >= items) return;
+    const int stage = l_it % S;
+    mbar_wait(empty_bar(stage), ((uint32_t)(l_it / S) & 1u) ^ 1u, 1, l_it);
+    const int nt = l_item / m_tiles, mt = l_item - nt * m_tiles;
+    const int tpi = a.tiles_x * a.tiles_y;
+    const int b = mt / tpi, t = mt - b * tpi;
+    const int ty = t / a.tiles_x, tx = t - ty * a.tiles_x;
+    const int nch = g.C_in >> 6;
+    const int tap = l_s / nch, ch = l_s - tap * nch;
+    const int ky = tap / g.KW, kx = tap - ky * g.KW;
+    mbar_arrive_expect_tx(full_bar(stage), (uint32_t)A_STAGE_BYTES + b_bytes);
+    tma_4d(sA + stage * A_STAGE_BYTES, &tmap, ch << 6, tx * 16 * g.stride - g.pad_w + kx,
+           ty * 8 * g.stride - g.pad + ky, b, full_bar(stage));
+    bulk_g2s(sB + stage * b_bytes, a.w + ((size_t)nt * KS + l_s) * (N * TC_BK), b_bytes, full_bar(stage));
+    ++l_it;
+    if (++l_s == KS) { l_s = 0; l_item += gridDim.x; }
+  };
+  if (tid == 0)
+    for (int i = 0; i < S; ++i) load_next();
+
+  // ===================== MMA + epilogue warpgroups =====================
+  const int wg = warp >> 2, w4 = warp & 3;
+  const int lrow = 32 * (w4 & 1) + lane;           // epilogue: row of this warpgroup's 64, 16-column half chalf
+  const int chalf = w4 >> 1;
+  const uint32_t stg = sStg + (uint32_t)wg * (64u * EPI_PITCH * 4u);
+  float acc[N / 2];
+  int it = 0;
+  for (int item = blockIdx.x; item < items; item += gridDim.x) {
+    const int nt = item / m_tiles, mt = item - nt * m_tiles;
+    for (int s = 0; s < KS; ++s, ++it) {
+      const int stage = it % S;
+      mbar_wait(full_bar(stage), (uint32_t)(it / S) & 1u, 2, it);
+      const uint64_t ad = make_sdesc(sA + stage * A_STAGE_BYTES + (uint32_t)wg * (64u * 128u));
+      const uint64_t bd = make_sdesc(sB + stage * b_bytes);
+      wg_fence();
+#pragma unroll
+      for (int k = 0; k < TC_BK / 16; ++k)
+        Wgmma<N>::mma(acc, ad + 2ull * k, bd + 2ull * k, (s > 0 || k > 0) ? 1u : 0u);
+      wg_commit();
+      wg_wait<1>();
+      wg_fence_operand(acc);
+      if (s > 0) {                                   // the previous slice's MMAs are done with its stage
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty_bar((it - 1) % S));
+        if (tid == 0) load_next();
+      }
+    }
+    wg_wait<0>();
+    wg_fence_operand(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(empty_bar((it - 1) % S));
+    if (tid == 0) load_next();
+
+    // ---- epilogue of this warpgroup's 64 rows, 32 accumulator columns at a time through its staging tile
+    const int p = tc_pixel(a, mt, 64 * wg + lrow);
+    const bool p_ok = p < g.P_out;
+    const int n0 = nt * N;
+#pragma unroll
+    for (int c0 = 0; c0 < N; c0 += 32) {
+      named_sync(1 + wg, 128);                     // the previous chunk's readers are done with the staging tile
+      stage_acc_chunk(acc, c0, stg, 0);
+      named_sync(1 + wg, 128);
+      const int col = c0 + chalf * 16;
+      const int o0 = n0 + col;
+      if (col < N && p_ok && o0 < g.C_out) {
+        float v[16];
+        lds_f(stg + ((uint32_t)lrow * EPI_PITCH + (uint32_t)chalf * 16u) * 4u, v);
+        tc_store16<false>(a, p, o0, v);
+      }
+    }
+  }
 }
 
 int tc_set_trace(void* buf) {
@@ -622,6 +752,17 @@ int tc_set_trace(void* buf) {
   return cudaMemcpyToSymbol(g_tc_trace, &p, sizeof(p)) == cudaSuccess ? CT_OK : CT_ERR_CUDA;
 }
 int tc_set_watch(void* mapped_host_buf) { return set_mbar_watch(mapped_host_buf); }
+
+// Plain bf16 convolutions whose K slices are whole 64-channel chunks of one tap take conv_tma_kernel when its 8 x 16
+// patches cover the output map with at most 15 % of padding rows; the others (C_in not a multiple of 64, maps such as
+// mot's 34 x 60 / 17 x 30, the bf16x3 engine) the register gather of conv_tc_kernel, whose 128-pixel tiles run across
+// image rows and images.
+static bool tc_uses_tma(const ct_conv_desc* d) {
+  if (d->engine != CT_ENGINE_TCGEN05 || d->a_mode != CT_A_CONV || d->C_in % 64 != 0 || d->stride < 1 || d->stride > 8)
+    return false;
+  const long long padded = (long long)((d->OW + 15) / 16) * ((d->OH + 7) / 8) * 128;
+  return (long long)d->OH * d->OW * 100 >= padded * 85;
+}
 
 // Configuration step: the launch arguments other than the pointers, and the launch configuration.  No CUDA call.
 static int tc_config(const ct_conv_desc* d, TcArgs& a, ConvConfig& c) {
@@ -656,6 +797,27 @@ static int tc_config(const ct_conv_desc* d, TcArgs& a, ConvConfig& c) {
   a.win_pw = 16 + 2 * a.win_m + 3;
   a.win_ph = 8 + 2 * a.win_m + 3;
   a.win_bytes = (uint32_t)(a.win_pw * a.win_ph * 128);
+  if (tc_uses_tma(d)) {
+    // as many stages (up to 4) as fit in the CTA's share of the SM: half of it at N <= 128 (two CTAs per SM)
+    const size_t stage = (size_t)A_STAGE_BYTES + (size_t)n_tile * 128;
+    const size_t limit = (n_tile <= 128 ? 113 : 227) * 1024;
+    auto smem_for = [&](int stg) { return (size_t)stg * stage + TMA_STAGING_BYTES + 2 * stg * 8 + 1024; };
+    int stages = 4;
+    while (stages > 2 && smem_for(stages) > limit) --stages;
+    if (smem_for(stages) > limit)
+      return fail(CT_ERR_UNSUPPORTED, "conv_tc: tile does not fit in shared memory%s (%ld)", "", (long)smem_for(stages));
+    a.stages = stages;
+    a.region0 = 0;
+    a.tiles_x = (g.OW + 15) / 16;
+    a.tiles_y = (g.OH + 7) / 8;
+    c.smem_bytes = (int32_t)smem_for(stages);
+    c.stages = stages;
+    c.tile_w = 16;
+    c.tile_h = 8;
+    c.ctas_per_sm = 0;
+    c.overlap = 0;
+    return CT_OK;
+  }
   const size_t stage_bytes = (size_t)(x3 ? 2 : 1) * (A_STAGE_BYTES + n_tile * 128);
   const size_t staging = (size_t)TC_BM * EPI_PITCH * 4;      // <= one stage (16 KB + n_tile x 128 B)
   auto region0_for = [&](int stg) { return ((size_t)stg * stage_bytes > staging ? (size_t)stg * stage_bytes : staging); };
@@ -725,9 +887,25 @@ int conv_forward_tc(const ct_conv_desc* d, cudaStream_t st) {
   const int n_tiles = (g.C_out + a.n_tile - 1) / a.n_tile;
   CUtensorMap tmap;
   memset(&tmap, 0, sizeof(tmap));
+  const cuuint64_t dims[4] = {(cuuint64_t)g.C_in, (cuuint64_t)g.W, (cuuint64_t)g.H, (cuuint64_t)g.B};
+  const cuuint64_t strides[3] = {(cuuint64_t)g.ld_in * 2, (cuuint64_t)g.W * g.ld_in * 2, (cuuint64_t)g.H * g.W * g.ld_in * 2};
+  if (tc_uses_tma(d)) {
+    // one K slice of an 8 x 16 output patch: 64 channels of 16 x 8 input pixels `stride` apart (the box counts elements
+    // before striding)
+    const cuuint32_t s = (cuuint32_t)g.stride;
+    const cuuint32_t box[4] = {64, 16 * s, 8 * s, 1};
+    const cuuint32_t estr[4] = {1, s, s, 1};
+    const int r = encode_tmap_bf16(&tmap, d->x, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, estr);
+    if (r != CT_OK) return r;
+    const int items = m_tiles * n_tiles;
+    const int per_sm = a.n_tile <= 128 ? 2 : 1;
+    const int grid = items < device_sm_count() * per_sm ? items : device_sm_count() * per_sm;
+    return dispatch_n_tile(a.n_tile, [&](auto n) {
+      constexpr int N = decltype(n)::value;
+      return launch_big_smem<conv_tma_kernel<N>>(dim3(grid), dim3(TMA_THREADS), c.smem_bytes, st, a, tmap);
+    });
+  }
   if (a.a_mode == CT_A_DCN_WIN) {                    // the TMA box of one patch's window
-    const cuuint64_t dims[4] = {(cuuint64_t)g.C_in, (cuuint64_t)g.W, (cuuint64_t)g.H, (cuuint64_t)g.B};
-    const cuuint64_t strides[3] = {(cuuint64_t)g.ld_in * 2, (cuuint64_t)g.W * g.ld_in * 2, (cuuint64_t)g.H * g.W * g.ld_in * 2};
     const cuuint32_t box[4] = {64, (cuuint32_t)a.win_pw, (cuuint32_t)a.win_ph, 1};
     const int r = encode_tmap_bf16(&tmap, d->x, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE);
     if (r != CT_OK) return r;

@@ -131,8 +131,6 @@ class DLA34Engine(object):
     self.dcn_window = bool(int(__import__('os').environ.get('CTB_DCN_WINDOW', '1')))
     # CTB_DCN_PERSIST=0: the 128 -> 128 DCN takes the global-memory gather instead of the window sampler
     self.dcn_window_all = bool(int(__import__('os').environ.get('CTB_DCN_PERSIST', '1')))
-    self.ntile_cap = int(__import__('os').environ.get('CTB_NTILE_CAP', '256'))
-    self.gather_128 = bool(int(__import__('os').environ.get('CTB_GATHER_128', '0')))   # experiment: level3's 3x3 on the gather engine
     self.depth_scale = float(depth_scale)
     self.has_pre_img = has_pre_img and ('base.pre_img_layer.0.weight' in self.sd)
     self.has_pre_hm = has_pre_hm and ('base.pre_hm_layer.0.weight' in self.sd)
@@ -263,23 +261,33 @@ class DLA34Engine(object):
       d.out, d.ld_out = out.ptr, out.ld
       self.named[name] = out
     n_tile = None
+    # plain bf16 layers the gather engine runs on its TMA-fed persistent kernel (csrc/conv_tc.cu, tc_uses_tma): the
+    # configuration of that kernel is the one with 16 x 8 patches
+    tma = False
+    if self.engine == L.CT_ENGINE_TCGEN05 and a_mode == L.CT_A_CONV and C_in % 64 == 0 and out_hw is None and \
+        out_mode != L.CT_OUT_NHWC_S2D:
+      d.engine, d.n_tile = self.engine, 16
+      c = L.conv_config(d)
+      tma = c is not None and (c.tile_w, c.tile_h) == (16, 8)
+    cpad = (C_out + 15) // 16 * 16
     if self.engine == L.CT_ENGINE_TCGEN05 and self.use_halo and a_mode == L.CT_A_CONV and stride == 1 and kh == kw and \
-        (C_in in (16, 32, 48, 64, 128, 192, 256) or (C_in == 8 and sum3)) and \
-        not (self.gather_128 and C_in == 128 and C_out == 128 and kh == 3):
+        (C_in in (16, 32, 48, 64, 128, 192, 256) or (C_in == 8 and sum3)):
       # stride-1 layer whose weights fit in smem: TMA halo tile + descriptor-shifted taps (csrc/conv_halo.cu)
-      cpad = (C_out + 15) // 16 * 16
       n_tile = self._first_fit(d, L.CT_ENGINE_TCGEN05_HALO, [48] if sum3 else [
           c for c in (128, 96, 80, 64, 48, 32, 16)
           if c <= cpad and (c == cpad or cpad % c == 0 or c >= 64) and (c >= 32 or cpad <= 16)])
+      if tma and n_tile is not None and n_tile <= 32 and n_tile < cpad:
+        # the halo engine's weights fit only 32 of the output channels (level3's 3x3 128 -> 128): it would re-fetch the
+        # halo per 32-channel tile with one m64n32 chain per warpgroup, bound by shared-memory operand reads
+        n_tile = None
     if n_tile is None:
       d.engine, d.n_tile = self.engine, 0
       if self.engine != L.CT_ENGINE_SIMT:
         cands = self._n_tile_cands(C_out)
         n_tile = self._pick_n_tile(P, C_out, cands)
-        if self.engine == L.CT_ENGINE_TCGEN05 and a_mode == L.CT_A_CONV and n_tile > self.ntile_cap:
-          # experiment knob (CTB_NTILE_CAP): 128-wide tiles with two co-resident CTAs measured SLOWER than one 256-wide
-          # CTA on levels 4-5 (conv_tc plain 1.81 vs 1.73 ms per 32-frame step), so the default cap is 256 = no cap
-          n_tile = self.ntile_cap
+        if tma and n_tile > 128:
+          # N <= 128 runs two CTAs per SM, so one CTA's epilogue overlaps the other's MMAs (DESIGN §3)
+          n_tile = 128
         # the widest tile not above that one whose stages fit in shared memory (the x3 DCN's do not at N = 256)
         if self._first_fit(d, self.engine, [c for c in cands if c <= n_tile]) is None:
           raise ValueError('%s: no N tile of %s fits in shared memory' % (name, cands))

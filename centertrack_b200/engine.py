@@ -262,10 +262,12 @@ class DLA34Engine(object):
       self.named[name] = out
     n_tile = None
     # plain bf16 layers the gather engine runs on its TMA-fed persistent kernel (csrc/conv_tc.cu, tc_uses_tma): the
-    # configuration of that kernel is the one with 16 x 8 patches
+    # configuration of that kernel is the one with 16 x 8 patches.  Not for a record without a launch: the fused head
+    # launch's 1x1 records read an intermediate that never exists, and at B = 64 on nuScenes' eight heads it would exceed
+    # the gather engine's 2^31-element limit, refusing a plan whose launches all fit.
     tma = False
     if self.engine == L.CT_ENGINE_TCGEN05 and a_mode == L.CT_A_CONV and C_in % 64 == 0 and out_hw is None and \
-        out_mode != L.CT_OUT_NHWC_S2D:
+        out_mode != L.CT_OUT_NHWC_S2D and not record_only:
       d.engine, d.n_tile = self.engine, 16
       c = L.conv_config(d)
       tma = c is not None and (c.tile_w, c.tile_h) == (16, 8)

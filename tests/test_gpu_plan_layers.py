@@ -14,15 +14,13 @@ import bounds as bd
 import ct_oracle as co
 from centertrack_b200 import _lib as L
 from helpers import HEAD_LAYOUTS
+from plan_rows import format_row, launch_row
 
 pytestmark = pytest.mark.gpu
 
 KERNEL = {L.CT_ENGINE_SIMT: 'simt', L.CT_ENGINE_TCGEN05: 'gather', L.CT_ENGINE_TCGEN05_X3: 'gather_x3',
           L.CT_ENGINE_TCGEN05_HALO: 'halo'}
 COEF = {'simt': bd.GAMMA_SIMT, 'gather': bd.ALPHA_BF16, 'gather_x3': bd.BETA_X3, 'halo': bd.ALPHA_BF16}
-A_MODE = {L.CT_A_CONV: 'conv', L.CT_A_DCN: 'dcn', L.CT_A_DCN_WIN: 'dcn_win'}
-OUT_MODE = {L.CT_OUT_NHWC: 'nhwc', L.CT_OUT_NHWC_F32: 'nhwc_f32', L.CT_OUT_NCHW_F32: 'nchw_f32',
-            L.CT_OUT_NHWC_S2D: 'nhwc_s2d'}
 HEAD_ACT = {L.CT_HEAD_NONE: 'none', L.CT_HEAD_SIGMOID: 'sigmoid', L.CT_HEAD_DEPTH: 'depth'}
 
 # (id, config, (H, W), B, precision, extra options, engine keyword arguments, environment)
@@ -36,6 +34,13 @@ CASES = [
     ('nuscenes_ddd_448x800_b2_bf16', 'nuscenes_ddd', (448, 800), 2, 'bf16', [], {}, {}),
     ('coco_pose_512_b2_bf16', 'coco_pose', (512, 512), 2, 'bf16', [], {}, {}),
     ('coco_pose_512_b2_bf16x3', 'coco_pose', (512, 512), 2, 'bf16x3', [], {}, {}),
+    # bench.py's batch: the 34 x 60 / 28 x 50 maps on the register gather at N = 256, the window DCN at N = 128 over 512
+    # channels, and in bf16x3 level5 and the global DCN at N = 128
+    ('mot_544x960_b32_bf16', 'mot', (544, 960), 32, 'bf16', [], {}, {}),
+    ('mot_544x960_b32_bf16x3', 'mot', (544, 960), 32, 'bf16x3', [], {}, {}),
+    ('nuscenes_ddd_448x800_b32_bf16', 'nuscenes_ddd', (448, 800), 32, 'bf16', [], {}, {}),
+    ('nuscenes_ddd_448x800_b32_bf16x3', 'nuscenes_ddd', (448, 800), 32, 'bf16x3', [], {}, {}),
+    ('coco_pose_512_b32_bf16', 'coco_pose', (512, 512), 32, 'bf16', [], {}, {}),
     ('dla_node_conv_64x96_b2_bf16', 'coco_tracking', (64, 96), 2, 'bf16', ['--dla_node', 'conv'], {}, {}),
     ('dla_node_gcn_64x96_b2_bf16', 'coco_tracking', (64, 96), 2, 'bf16', ['--dla_node', 'gcn'], {}, {}),
     ('coco_tracking_256_b2_bf16_no_halo', 'coco_tracking', (256, 256), 2, 'bf16', [], {'use_halo': False}, {}),
@@ -156,6 +161,9 @@ def _check_conv(eng, sp, bs):
   return r, use
 
 
+OTHER_KINDS = ('pack', 'pack32', 'pool', 'pool_s2d', 'up', 'stem')     # the kinds _check_other checks
+
+
 def _check_other(eng, sp, bs):
   """Non-conv ops: pack / pool exact, up (depthwise ConvT + skip) and the SIMT stem by the bound."""
   k = sp['kind']
@@ -226,18 +234,6 @@ def _build(cfg, hw, B, precision, extra, kw, monkeypatch, env):
   return eng
 
 
-def _coverage_row(eng, sp):
-  d = sp['desc']
-  kern = KERNEL[sp['engine']]
-  kh, kw = sp['k']
-  cfg = L.conv_config(d)             # the launch configuration the library picked for this op
-  assert cfg is not None, sp['name']
-  launch = ('%dx%d' % (cfg.tile_w, cfg.tile_h), cfg.stages, cfg.overlap) if kern != 'simt' else ('-', '-', '-')
-  return (kern, sp['n_tile'], d.C_in, '%dx%d' % (kh, kw), A_MODE[sp['a_mode']], OUT_MODE[sp['out_mode']],
-          int(sp['residual'] is not None), int(sp['out_mode'] == L.CT_OUT_NHWC_S2D or sp['name'] in eng.s2d_named),
-          int(bool(sp['sum3']))) + launch
-
-
 COVERAGE = {}
 
 
@@ -263,10 +259,12 @@ def test_plan_layers_within_bounds(case, monkeypatch):
       if use is not None:
         layer_use = max(layer_use, float(use.max()))
       del res, r, use
+    row = launch_row(eng, sp)
+    if row is not None:
+      COVERAGE.setdefault(row, set()).add(cid)
     if layer_at is None:
       continue
     if is_conv:
-      COVERAGE.setdefault(_coverage_row(eng, sp), set()).add(cid)
       key = (kern, 'fp32 out' if sp['out_mode'] in (L.CT_OUT_NHWC_F32, L.CT_OUT_NCHW_F32) or precision != 'bf16'
              else 'bf16 out')
     else:
@@ -287,10 +285,10 @@ def test_plan_layers_within_bounds(case, monkeypatch):
 
 
 def test_zz_plan_coverage_table():
-  """Print which (kernel, N, C_in, k, a_mode, out_mode, residual, s2d, sum3, tile, stages, overlap) the plans above
-  ran (runs after them in file order)."""
+  """Print the launch configuration rows (tests/plan_rows.py) the plans above ran (runs after them in file order):
+  conv rows are (kernel, N, C_in, k, stride, a_mode, out_mode, residual, s2d, sum3, tile, stages, overlap, work per
+  CTA)."""
   if not COVERAGE:
     pytest.skip('no plan audited in this session')
-  print('\nkernel     N   C_in k    a_mode  out_mode  res s2d sum3 tile   stages overlap  configs')
   for row in sorted(COVERAGE, key=lambda r: tuple(str(v) for v in r)):
-    print('%-9s %4d %5d %-4s %-7s %-9s %3d %3d %4d %-6s %6s %7s  %s' % (row + (','.join(sorted(COVERAGE[row])),)))
+    print('%-62s  %s' % (format_row(row), ','.join(sorted(COVERAGE[row]))))

@@ -137,6 +137,7 @@ EXPORTS = ['ct_packed_weight_bytes', 'ct_pack_weights', 'ct_conv_forward', 'ct_c
            'ct_pack_stem_input', 'ct_pack_stem_input_f32', 'ct_maxpool2', 'ct_maxpool2_s2d', 'ct_upsample_add', 'ct_decode_workspace_bytes', 'ct_decode',
            'ct_render_pre_hm', 'ct_track_smem_bytes', 'ct_track_step', 'ct_track_assoc_smem_bytes',
            'ct_track_step_assoc', 'ct_track_payload_smem_bytes', 'ct_track_step_payload', 'ct_track_start',
+           'ct_track_restore',
            'ct_render_tracks', 'ct_track_step_mapped', 'ct_render_tracks_mapped', 'ct_post_process', 'ct_flip_merge', 'ct_flip_merge_heads', 'ct_mirror_x',
            'ct_warp_affine_normalize', 'ct_pack_stem_frames', 'ct_pack_stem_frames_flip', 'ct_pack_stem_frames_dev',
            'ct_pack_stem_frames_flip_dev', 'ct_warp_frames_normalize', 'ct_stage_frames', 'ct_last_error',
@@ -216,6 +217,8 @@ def lib():
   L.ct_track_step_payload.argtypes = [C.POINTER(TrackDesc), C.POINTER(TrackAssoc), C.POINTER(TrackPayload), C.c_void_p]
   L.ct_track_start.argtypes = [C.POINTER(TrackDesc), C.POINTER(TrackPayload), C.c_void_p, C.c_int32, C.c_void_p,
                                C.c_void_p]
+  L.ct_track_restore.argtypes = [C.POINTER(TrackDesc), C.POINTER(TrackPayload), C.c_void_p, C.c_int32, C.c_void_p,
+                                 C.c_void_p, C.c_void_p]
   L.ct_render_tracks.argtypes = [C.c_void_p, C.c_int32, C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p]
   L.ct_track_step_mapped.argtypes = [C.POINTER(TrackDesc), C.POINTER(TrackAssoc), C.POINTER(TrackPayload), C.c_void_p,
                                      C.c_int32, C.c_void_p]

@@ -7,6 +7,7 @@
 //                    the pose / 3D / velocity / attribute fields of generic_post_process (post_process.py:55-89) in a
 //                    payload table beside the track table, and the amodal centre on 3D head sets
 //   ct_render_tracks the gaussian max-splat of those boxes into pre_hm (image.py:128-154)
+//   ct_track_start / ct_track_restore   a stream's table reset and seeded, or restored verbatim from an exported one
 //   ct_track_step_mapped / ct_render_tracks_mapped   the same two on a compacted batch of live streams (image i =
 //                    stream streams[i]), for StreamRunner's idle streams
 //   ct_post_process  Detector.post_process + merge_outputs (detector.py:356-377) for runners without a tracker: the
@@ -582,22 +583,29 @@ track_step_kernel(const TrackArgs a) {
 // and payload rows are cleared, its starts[e][1] seed rows (already filtered and numbered on the host) written, and its
 // render boxes computed from them by the same code as the track step's.  One CTA per started stream; the seeds of
 // entry e follow those of entries 0..e-1 in `seeds`.
+// RESTORE (ct_track_restore): entries are (stream, n, id_count), the rows are an exported stream's verbatim (ids, ages
+// and active kept) with their payload rows in `pay_rows`, and counts = (n, id_count).  A template parameter so that
+// ct_track_start's instantiation stays as it was.
+template <bool RESTORE = false>
 __global__ void __launch_bounds__(TRK_THREADS)
 track_start_kernel(const ct_track_desc d, float* __restrict__ payload, int Wp, const int* __restrict__ starts,
-                   const float* __restrict__ seeds) {
+                   const float* __restrict__ seeds, const float* __restrict__ pay_rows = nullptr) {
+  constexpr int S = RESTORE ? 3 : 2;                          // int32 per entry
   const int e = blockIdx.x, tid = threadIdx.x, T = d.max_tracks;
-  const int b = starts[2 * e];
+  const int b = starts[S * e];
   if (b < 0 || b >= d.B) return;
   auto clamp_n = [&](int n) { return seeds == nullptr ? 0 : (n < 0 ? 0 : (n > T ? T : n)); };
   size_t off = 0;
-  for (int k = 0; k < e; ++k) off += (size_t)clamp_n(starts[2 * k + 1]);
-  const int n = clamp_n(starts[2 * e + 1]);
+  for (int k = 0; k < e; ++k) off += (size_t)clamp_n(starts[S * k + 1]);
+  const int n = clamp_n(starts[S * e + 1]);
   float* trk = d.tracks + (size_t)b * T * TF;
   const float* src = seeds ? seeds + off * TF : nullptr;
   for (int i = tid; i < T * TF; i += TRK_THREADS) trk[i] = i < n * TF ? src[i] : 0.f;
-  if (payload)
-    for (int i = tid; i < T * Wp; i += TRK_THREADS) payload[(size_t)b * T * Wp + i] = 0.f;
-  if (tid == 0) { d.counts[b * 2 + 0] = n; d.counts[b * 2 + 1] = n; }
+  if (payload) {
+    const float* psrc = RESTORE && pay_rows ? pay_rows + off * Wp : nullptr;
+    for (int i = tid; i < T * Wp; i += TRK_THREADS) payload[(size_t)b * T * Wp + i] = psrc && i < n * Wp ? psrc[i] : 0.f;
+  }
+  if (tid == 0) { d.counts[b * 2 + 0] = n; d.counts[b * 2 + 1] = RESTORE ? starts[S * e + 2] : n; }
   __syncthreads();     // the seed rows written above are re-read below by other threads
   __threadfence_block();
   track_boxes(d, b, trk, n, tid);
@@ -1232,6 +1240,20 @@ extern "C" int ct_track_start(const ct_track_desc* d, const ct_track_payload* p,
   if (n_starts == 0) return CT_OK;
   track_start_kernel<<<n_starts, TRK_THREADS, 0, (cudaStream_t)stream>>>(*d, p ? p->payload : nullptr, p ? p->width : 0,
                                                                           starts, seeds);
+  return after_launch();
+}
+
+extern "C" int ct_track_restore(const ct_track_desc* d, const ct_track_payload* p, const int32_t* entries,
+                                int32_t n_entries, const float* rows, const float* payload_rows, void* stream) {
+  CT_REQUIRE(d && d->tracks && d->counts, "null pointer");
+  CT_REQUIRE(d->B > 0 && d->max_tracks > 0, "bad shape");
+  CT_REQUIRE(d->boxes == nullptr || (d->trans_input != nullptr && d->inp_h > 0 && d->inp_w > 0), "boxes need trans_input");
+  CT_REQUIRE(n_entries >= 0 && n_entries <= d->B, "n_entries outside [0, B]");
+  CT_REQUIRE(n_entries == 0 || entries, "null entry list");
+  CT_REQUIRE(!p || (p->payload && p->width > 0), "payload table needs payload and width > 0");
+  if (n_entries == 0) return CT_OK;
+  track_start_kernel<true><<<n_entries, TRK_THREADS, 0, (cudaStream_t)stream>>>(
+      *d, p ? p->payload : nullptr, p ? p->width : 0, entries, rows, payload_rows);
   return after_launch();
 }
 

@@ -239,6 +239,14 @@ class DeviceTracker(object):
     L.check(L.lib().ct_track_start(C.byref(self.desc), C.byref(self.pay) if self.pay is not None else None,
                                    L.ptr(start_list), n_starts, L.ptr(seeds), L.stream_ptr()), 'ct_track_start')
 
+  def restore_device(self, entries, n_entries, rows=None, payload_rows=None):
+    """ct_track_restore on device buffers: entries int32 [>= n_entries, 3] rows (stream, rows n, id_count), rows fp32
+    [sum of n, CT_TRK_FLOATS] and payload_rows fp32 [sum of n, Wp] in entries' order (None when every n is 0).  The
+    rows are written as they are, and each stream's boxes rendered from them with its own index and trans_input."""
+    L.check(L.lib().ct_track_restore(C.byref(self.desc), C.byref(self.pay) if self.pay is not None else None,
+                                     L.ptr(entries), n_entries, L.ptr(rows), L.ptr(payload_rows), L.stream_ptr()),
+            'ct_track_restore')
+
   def public_buffers(self):
     """Zeroed device buffers of the shape step() takes with --public_det: public_ct [B,P,2] fp32, public_n [B] int32."""
     return (torch.zeros((self.B, self.max_public, 2), dtype=torch.float32, device=self.device),

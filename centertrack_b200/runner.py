@@ -66,7 +66,14 @@ Every launch runs at that batch; the track step and the prior heat-map render ma
 device maps (ct_track_step_mapped, ct_render_tracks_mapped), uploaded with the slot's descriptors when they change.
 One CUDA graph per (slot, batch).  pre_images must not depend on an image index, so the fp32 and bf16x3 engines warp
 the previous slot's frames again (the bf16 engine's pack already does).  An idle stream's tables, frame region and
-camera rows are left as they are; it comes back with a video start.
+camera rows are left as they are; it comes back with a video start, or continues its video (`resume=`): its last frame
+is still in its region of the slot where it last had a frame (`last_slot`), and when that is not the previous slot one
+ct_stage_frames on the copy stream copies it there before the step's upload, so the step reads it as pre_images.
+
+Moving a video (`stream_state(b)`, `step_frames(..., restore={b: state})`, capacity runners): a StreamState holds a
+stream's last frame, camera and track rows; restoring it into a stream of this or another runner is a video start at the
+state's frame size and camera whose prologue stages that frame as pre_images and writes the rows verbatim
+(ct_track_restore) instead of seeding them.
 """
 import ctypes as C
 
@@ -219,6 +226,30 @@ def device_frame_source(x, fmt, layout, device, what='frame'):
   return (h, w), src
 
 
+def _ints(streams):
+  """The integer entries of a stream list, as a set (the others are refused by the list's own check)."""
+  return {int(s) for s in streams if isinstance(s, (int, np.integer)) and not isinstance(s, (bool, np.bool_))}
+
+
+class StreamState(object):
+  """One stream of a capacity runner after the last step in which it had a frame (StreamRunner.stream_state), what
+  step_frames(restore=) needs to continue its video on another stream or runner.
+    frame            device uint8 tensor of that frame in frame_format's layout ([h, w, 3], or [3h/2, w] in 4:2:0)
+    size             its (h, w)
+    calib            float32 [3, 4] camera matrix
+    tracks, counts, payload   tracking runners: the track rows [n, CT_TRK_FLOATS] (device), (n, id_count), and the
+                     payload rows [n, Wp] (device) on head sets with payload fields; None otherwise
+    input_size, record_layout, payload_layout, max_tracks, frame_format   the layout facts the importer checks
+  A copy: the exporting runner may go on using the stream."""
+
+  def __init__(self, frame, size, calib, tracks, counts, payload, input_size, record_layout, payload_layout, max_tracks,
+               frame_format):
+    self.frame, self.size, self.calib = frame, tuple(size), calib
+    self.tracks, self.counts, self.payload = tracks, counts, payload
+    self.input_size, self.record_layout, self.payload_layout = tuple(input_size), record_layout, payload_layout
+    self.max_tracks, self.frame_format = max_tracks, frame_format
+
+
 class StreamRunner(object):
 
   frame_format = 'bgr'
@@ -324,6 +355,8 @@ class StreamRunner(object):
     self.tracker = None
     self.device_tracking = device_tracking
     self._starts = [None] * NS                               # per slot: the streams whose frame starts a video
+    self._restores = [None] * NS                             # per slot: {stream: StreamState} restored in its step
+    self.last_slot = [None] * B                              # per stream: the slot of its last step with a frame
     self._start_bytes = 0                                    # start list + seed rows uploaded by the last step
     self.h_start = None                                      # per slot start list / seed staging, made on first use
     self.h_geo = None                                        # per slot camera geometry rows staging, made on first use
@@ -705,6 +738,7 @@ class StreamRunner(object):
 
   def reset_tracking(self):
     self.t = 0
+    self.last_slot = [None] * self.B
     if self.idle_g is not None:
       self._was_idle = set()
     if self.tracker is not None:
@@ -830,50 +864,94 @@ class StreamRunner(object):
     self._start_bytes = self._upload_starts(slot, plan, non_blocking=False) + \
         self._upload_geometry(slot, rows, non_blocking=False)
 
-  def _start_prologue(self, slot, streams):
-    """A step whose frames start new videos on `streams`, before the step itself (graph replay or eager), on the same
-    stream: first-frame pre_images and the tracker start.  Outside the graphs: they stay the same for every step."""
+  def _start_prologue(self, slot, streams, restores=None):
+    """A step whose frames start new videos on `streams` or continue restored ones ({stream: StreamState}), before the
+    step itself (graph replay or eager), on the same stream: first-frame pre_images, the restored streams' frames as
+    theirs, and the tracker start and restore.  Outside the graphs: they stay the same for every step.  In the first
+    step (t = 0) with restores, the step runs as a later one, so every other stream's frame is copied as a start's."""
+    restores = restores or {}
+    prev = (slot - 1) % NS
     if self.t > 0:
+      own = list(streams)
+    elif restores:
+      live = self._live[self.t & 1] if self.idle_g is not None else range(self.B)
+      own = [b for b in live if b not in restores]
+    else:
+      own = []
+    if restores:
+      # pre_images of a restored stream = the state's frame, staged into its region of the previous slot; safe as a
+      # start's copy below: the region is read by step t-1 as its images, which comes first on this stream
+      self._stage_states(prev, restores)
+    for b in own + sorted(restores):
       # pre_images of a started stream = its own frame: overwrite its part of the previous slot, which holds step t-1's
       # images.  Safe: that slot is read only by this step (as pre_images), after this prologue on the same stream, and
       # it is next written by the upload of step t+2, which waits for ev_done[prev], recorded after this step.
-      prev = (slot - 1) % NS
-      for b in streams:
-        # the pack kernel (or, on an idle-streams runner, the pre_images warp) reads u8[prev] again
-        if self.frames_mode and (self.eng.use_halo or self.idle_g is not None):
+      src = (self.u8[slot] if b in own else self.u8[prev]) if self.frames_mode else None
+      # the pack kernel (or, on an idle-streams runner, the pre_images warp) reads u8[prev] again
+      if self.frames_mode and (self.eng.use_halo or self.idle_g is not None):
+        if b in own:
           f = self.frames[b]
           o, n = f.offset, frame_layout(self.frame_format, f.h, f.w)[1]
           self.u8[prev][o:o + n].copy_(self.u8[slot][o:o + n])
-          continue
-        if self.frames_mode and self.frame_format != 'bgr':  # through the slot's device descriptor, which has the format
-          L.check(L.lib().ct_warp_frames_normalize(
-              L.ptr(self.u8[slot]), C.c_void_p(self.d_frames[slot].data_ptr() + b * C.sizeof(L.Frame)), 1,
-              self.slot_bytes, C.c_void_p(self.mean.ctypes.data), C.c_void_p(self.std.ctypes.data),
-              L.ptr(self.img[prev][b]), self.H, self.W, L.stream_ptr()), 'ct_warp_frames_normalize')
-        elif self.frames_mode:                               # the plan reads img[prev]: warp this frame into it
-          f = self.frames[b]
-          # a capacity runner's minv: the slot's device descriptor of this frame (its new geometry after a size change)
-          minv = L.ptr(self.minv[b]) if self.cap is None else \
-              C.c_void_p(self.d_frames[slot].data_ptr() + b * C.sizeof(L.Frame) + L.Frame.minv.offset)
-          L.check(L.lib().ct_warp_affine_normalize(
-              C.c_void_p(self.u8[slot].data_ptr() + f.offset), 1, f.h, f.w, f.step, minv,
-              C.c_void_p(self.mean.ctypes.data), C.c_void_p(self.std.ctypes.data), L.ptr(self.img[prev][b]), self.H,
-              self.W, L.stream_ptr()), 'ct_warp_affine_normalize')
-        else:
-          self.img[prev][b].copy_(self.img[slot][b])
-        if self.flip:                                        # --flip_test: pre_images is the (frame, mirror) pair
-          self._mirror(self.img[prev], b, 1)
+        continue
+      if self.frames_mode and self.frame_format != 'bgr':  # through the slot's device descriptor, which has the format
+        L.check(L.lib().ct_warp_frames_normalize(
+            L.ptr(src), C.c_void_p(self.d_frames[slot].data_ptr() + b * C.sizeof(L.Frame)), 1,
+            self.slot_bytes, C.c_void_p(self.mean.ctypes.data), C.c_void_p(self.std.ctypes.data),
+            L.ptr(self.img[prev][b]), self.H, self.W, L.stream_ptr()), 'ct_warp_frames_normalize')
+      elif self.frames_mode:                               # the plan reads img[prev]: warp this frame into it
+        f = self.frames[b]
+        # a capacity runner's minv: the slot's device descriptor of this frame (its new geometry after a size change)
+        minv = L.ptr(self.minv[b]) if self.cap is None else \
+            C.c_void_p(self.d_frames[slot].data_ptr() + b * C.sizeof(L.Frame) + L.Frame.minv.offset)
+        L.check(L.lib().ct_warp_affine_normalize(
+            C.c_void_p(src.data_ptr() + f.offset), 1, f.h, f.w, f.step, minv,
+            C.c_void_p(self.mean.ctypes.data), C.c_void_p(self.std.ctypes.data), L.ptr(self.img[prev][b]), self.H,
+            self.W, L.stream_ptr()), 'ct_warp_affine_normalize')
+      else:
+        self.img[prev][b].copy_(self.img[slot][b])
+      if self.flip:                                        # --flip_test: pre_images is the (frame, mirror) pair
+        self._mirror(self.img[prev], b, 1)
     geo, self._geo[slot] = self._geo[slot], None
     if geo:                                                  # new cameras: before the seeds' boxes are rendered
       self._geo_tables().set_geometry(geo, self.d_geo_in[slot], self.d_geo_out[slot])
-    if self.tracker is not None:                             # reset + seeds + boxes: the step's render splats them
+    if self.tracker is not None and streams:                 # reset + seeds + boxes: the step's render splats them
       self.tracker.start_device(self.d_start[slot], len(streams), self.d_seed[slot])
+    if self.tracker is not None and restores:                # the exported rows, boxes at this stream and camera
+      self._restore_tracks(restores)
+
+  def _on_device(self, t):
+    """t on the runner's device; a tensor of another device is copied over (on the current stream)."""
+    if t.device != self.u8[0].device:
+      return t.to(self.u8[0].device)
+    t.record_stream(torch.cuda.current_stream(self.device))  # the caller may drop the state once step_frames returns
+    return t
+
+  def _stage_states(self, dst_slot, restores):
+    """The restored streams' frames -> their regions of u8[dst_slot] (one ct_stage_frames), on the current stream."""
+    bs = sorted(restores)
+    frames = [self._on_device(restores[b].frame) for b in bs]
+    srcs = (L.FrameSrc * len(bs))(*[device_frame_source(x, self.frame_format, 'bgr', x.device)[1] for x in frames])
+    dst = (L.Frame * len(bs))(*[self.frames[b] for b in bs])
+    L.check(L.lib().ct_stage_frames(srcs, dst, len(bs), L.ptr(self.u8[dst_slot]), self.slot_bytes, L.stream_ptr()),
+            'ct_stage_frames')
+
+  def _restore_tracks(self, restores):
+    """ct_track_restore of the restored streams' rows, on the current stream."""
+    bs = sorted(restores)
+    ent = torch.tensor([[b, restores[b].counts[0], restores[b].counts[1]] for b in bs], dtype=torch.int32)
+    rows = [restores[b].tracks for b in bs if restores[b].counts[0]]
+    pay = [restores[b].payload for b in bs if restores[b].counts[0]] if self.tracker.payload is not None else []
+    rows = torch.cat([self._on_device(r) for r in rows]) if rows else None
+    pay = torch.cat([self._on_device(p) for p in pay]) if pay else None
+    self.tracker.restore_device(ent.to(self.device), len(bs), rows, pay)
 
   def _launch(self, slot):
     streams, self._starts[slot] = self._starts[slot], None
-    if streams:
-      self._start_prologue(slot, streams)
-    if self.t == 0:
+    restores, self._restores[slot] = self._restores[slot], None
+    if streams or restores:
+      self._start_prologue(slot, streams or [], restores)
+    if self.t == 0 and not restores:
       self._eager(slot, first=True)                          # first frame of the streams: pre_images = images
     elif self.use_graph:
       self._graph(slot).replay()
@@ -1045,8 +1123,139 @@ class StreamRunner(object):
                        '(starts=)' % back)
     return live
 
+  def _streams_arg(self, what, streams):
+    """A list of distinct stream indices in [0, B) (None: empty); ValueError otherwise."""
+    out = []
+    for s in streams or ():
+      if isinstance(s, (bool, np.bool_)) or not isinstance(s, (int, np.integer)):
+        raise ValueError('%s: stream indices must be integers, got %r' % (what, s))
+      s = int(s)
+      if not 0 <= s < self.B:
+        raise ValueError('%s: stream %d out of range [0, %d)' % (what, s, self.B))
+      if s in out:
+        raise ValueError('%s: stream %d given twice' % (what, s))
+      out.append(s)
+    return out
+
+  def _check_resume(self, resume, started, idle, restored):
+    """resume (streams idle in the last step whose frame in this step continues their video) -> the streams, ascending.
+    ValueError before anything is enqueued: resume on a runner without idle_streams, a stream that is also started,
+    restored or idle, one that was live in the last step, or one without a frame since the runner was built or reset.
+    (A frame of another size than the stream's last is refused by _check_sizes.)"""
+    out = self._streams_arg('resume', resume)
+    if not out:
+      return []
+    if self.idle_g is None:
+      raise ValueError('resume: this runner was built without idle_streams (its streams are never idle)')
+    for what, other in (('start a video (starts=)', started), ('are idle (idle=)', idle or ()),
+                        ('are restored (restore=)', restored)):
+      both = sorted(set(out) & _ints(other))
+      if both:
+        raise ValueError('resume: stream(s) %s also %s in this step' % (both, what))
+    live = sorted(set(out) - self._was_idle)
+    if live:
+      raise ValueError('resume: stream(s) %s were live in the last step; resume continues a stream that was idle' %
+                       live)
+    new = [b for b in out if self.last_slot[b] is None]
+    if new:
+      raise ValueError('resume: stream(s) %s have had no frame since the runner was built or reset; they come back with '
+                       'a video start' % new)
+    return sorted(out)
+
+  def _plan_resume(self, slot, live, resumed):
+    """Host bookkeeping of step t = self.t in `slot`: the copies that put each resumed stream's last frame where this
+    step reads pre_images -- [(stream, source slot, destination slot, byte offset, bytes)] for the streams whose last
+    slot is not the previous slot (t-1) % 3 -- and then last_slot of this step's live streams (every stream when live is
+    None) <- slot."""
+    dst = (self.t - 1) % NS
+    out = []
+    for b in resumed:
+      if self.last_slot[b] != dst:
+        f = self.frames[b]
+        out.append((b, self.last_slot[b], dst, f.offset, frame_layout(self.frame_format, f.h, f.w)[1]))
+    if self.cap is not None:
+      for b in (range(self.B) if live is None else live):
+        self.last_slot[b] = slot
+    return out
+
+  def _copy_resumed(self, copies):
+    """One ct_stage_frames of the resumed streams' last frames (_resume_copies) from their last slots into the previous
+    slot, on the current (copy) stream, before this step's frames are written."""
+    srcs, dsts = (L.FrameSrc * len(copies))(), (L.Frame * len(copies))()
+    for i, (b, s, _, o, n) in enumerate(copies):
+      f = self.frames[b]
+      view = self.u8[s][o:o + n].view(frame_layout(self.frame_format, f.h, f.w)[0])
+      srcs[i], dsts[i] = device_frame_source(view, self.frame_format, 'bgr', view.device)[1], f
+    L.check(L.lib().ct_stage_frames(srcs, dsts, len(copies), L.ptr(self.u8[copies[0][2]]), self.slot_bytes,
+                                    L.stream_ptr()), 'ct_stage_frames')
+
+  def _check_restore(self, restore, started, idle):
+    """restore ({stream: StreamState}) -> {stream: StreamState}.  ValueError before anything is enqueued: a runner
+    without max_frame_size, a stream out of range, also started or idle, or a state whose network input, record or
+    payload layout, tracker or frame_format differ from this runner's, with more rows than the track table, or whose
+    frame does not fit the capacity region or map to (H, W)."""
+    if not restore:
+      return {}
+    if self.cap is None:
+      raise ValueError('restore: needs a capacity frames runner (frame_sizes and max_frame_size)')
+    out = {}
+    for s in self._streams_arg('restore', list(restore)):
+      st = restore[s]
+      if not isinstance(st, StreamState):
+        raise ValueError('restore[%d]: expected a StreamState (stream_state()), got %s' % (s, type(st).__name__))
+      out[s] = st
+    for what, other in (('start a video (starts=)', started), ('are idle (idle=)', idle or ())):
+      both = sorted(set(out) & _ints(other))
+      if both:
+        raise ValueError('restore: stream(s) %s also %s in this step' % (both, what))
+    pay = self.tracker.payload_layout if self.tracker is not None else None
+    for s, st in sorted(out.items()):
+      if st.input_size != (self.H, self.W):
+        raise ValueError('restore[%d]: network input %s, the runner\'s is %s' % (s, st.input_size, (self.H, self.W)))
+      if st.record_layout != self.layout:
+        raise ValueError('restore[%d]: record layout %s differs from the runner\'s %s' % (s, st.record_layout,
+                                                                                         self.layout))
+      if st.frame_format != self.frame_format:
+        raise ValueError('restore[%d]: frame_format %r, the runner\'s is %r' % (s, st.frame_format, self.frame_format))
+      if (st.tracks is None) != (self.tracker is None):
+        raise ValueError('restore[%d]: the state %s track table and the runner %s a tracker' %
+                         (s, 'has no' if st.tracks is None else 'has a', 'has' if self.tracker else 'has no'))
+      if st.payload_layout != pay:
+        raise ValueError('restore[%d]: payload layout %s differs from the runner\'s %s' % (s, st.payload_layout, pay))
+      if self.tracker is not None and not 0 <= st.counts[0] <= self.tracker.T:
+        raise ValueError('restore[%d]: %d track rows, more than the %d of the track table' % (s, st.counts[0],
+                                                                                            self.tracker.T))
+      self._size_geometry('restore[%d]' % s, *st.size)
+    return out
+
+  def stream_state(self, b):
+    """Waits like fetch(), then returns stream b's StreamState after the last submitted step in which it had a frame:
+    that frame (a device copy), its size and camera, and on a tracking runner its track rows, counts and payload rows.
+    step_frames(restore={s: state}) on this or another runner continues the video on stream s from its next frame.
+    ValueError on a runner without max_frame_size, or a stream that has had no frame since the runner was built or
+    reset."""
+    if self.cap is None:
+      raise ValueError('stream_state: needs a capacity frames runner (frame_sizes and max_frame_size)')
+    b = self._streams_arg('stream_state', [b])[0]
+    s = self.last_slot[b]
+    if s is None:
+      raise ValueError('stream_state: stream %d has had no frame since the runner was built or reset' % b)
+    self.compute.synchronize()
+    f = self.frames[b]
+    shape, n, _ = frame_layout(self.frame_format, f.h, f.w)
+    trk = self.tracker
+    counts = tuple(int(v) for v in trk.counts[b].cpu()) if trk is not None else None
+    with torch.cuda.stream(self.compute):
+      frame = self.u8[s][f.offset:f.offset + n].clone().view(shape)
+      tracks = trk.tracks[b, :counts[0]].clone() if trk is not None else None
+      pay = trk.payload[b, :counts[0]].clone() if trk is not None and trk.payload is not None else None
+    self.compute.synchronize()
+    return StreamState(frame, (f.h, f.w), np.array(self._meta[b]['calib'], np.float32).reshape(3, 4), tracks, counts,
+                       pay, (self.H, self.W), dict(self.layout), trk.payload_layout if trk is not None else None,
+                       trk.T if trk is not None else None, self.frame_format)
+
   def step_frames(self, frames, pre_hms=None, public_dets=None, starts=None, pre_dets=None, calibs=None, idle=None,
-                  layout='bgr'):
+                  layout='bgr', resume=None, restore=None):
     """frames: B uint8 [h_b, w_b, 3] BGR arrays of the sizes given as frame_sizes (with frame_format 'nv12' / 'i420':
     [3h_b/2, w_b] arrays in that layout), or None when they were written through frame_buffers(), or B device frames
     (below).  pre_hms, public_dets, starts, pre_dets, calibs and the return value as in step_host;
@@ -1057,8 +1266,15 @@ class StreamRunner(object):
     with frame_sizes.
     idle (runners built with idle_streams): the streams without a frame in this step; their frames and public_dets
     entries are ignored (and may be None), their tables, camera and frame region are left as they are, and their
-    records come back zero and their fetch_results() entries None.  A stream idle in one step comes back only with a
-    video start.
+    records come back zero and their fetch_results() entries None.  A stream idle in one step comes back with a video
+    start, or in `resume`: its frame continues its video, and its records, tracks (ids, ages) and payload are those of
+    the stream fed only the frames it delivered, one after the other (tracks age per frame, not per step).  A resumed
+    frame has the size of the stream's last one.
+    restore ({stream: StreamState}, capacity runners): each listed stream continues the video of the state
+    (stream_state() of this or another runner, on any device) with this step's frame, of the state's size: a video start
+    at the state's size and camera whose pre_images is the state's frame and whose tracker gets the state's rows as they
+    are (ids, ages, id counter).  Refused, before anything is enqueued, together with starts, resume or idle for the
+    same stream, or for a state of another network input, head set, track table or frame_format.
     Device frames (what GPU decoders hand out): uint8 CUDA tensors on the runner's device instead of arrays, for every
     stream with a frame in this step (a step never mixes the two).  A BGR runner takes [h, w, 3] with layout 'bgr' or
     'rgb', or [3, h, w] with layout 'rgb_planar'; an NV12 runner one [3h/2, w] tensor in cv2's layout or the planes
@@ -1074,10 +1290,13 @@ class StreamRunner(object):
       raise ValueError('step_frames: the runner was not built with frame_sizes (use step_host)')
     plan = self._check_starts(starts, pre_dets)
     started = plan[0] if plan else ()
-    live = self._check_idle(idle, started, pre_hms)
+    rest = self._check_restore(restore, started, idle)
+    resumed = self._check_resume(resume, started, idle, rest)
+    live = self._check_idle(idle, list(started) + sorted(rest) + resumed, pre_hms)
     gone = () if live is None else set(range(self.B)) - set(live)
     pub = self._check_public(public_dets, gone)
     cal = self._check_calibs(calibs, started)
+    cal.update((b, np.asarray(st.calib, np.float32)) for b, st in rest.items())   # a restore: the state's camera
     dev = None                                       # device frames: [(stream, ct_frame_src, tensors)]
     if frames is not None and self._device_step(frames, gone):
       sizes, dev = self._device_sources(frames, gone, layout)
@@ -1085,10 +1304,16 @@ class StreamRunner(object):
       if layout != 'bgr':
         raise ValueError("layout=%r: applies to device frames; arrays are in the runner's frame_format" % (layout,))
       sizes = self._frame_sizes_of(frames, gone)
-    changed = self._check_sizes(sizes, started)
+    for b, st in sorted(rest.items()):
+      if tuple(sizes[b]) != st.size:
+        raise ValueError('restore[%d]: the frame of this step is %s, the state\'s video %s' % (b, tuple(sizes[b]),
+                                                                                             st.size))
+    changed = self._check_sizes(sizes, list(started) + sorted(rest))
     slot = self.t % NS
     self._pending_sizes = None
     desc, rows = self._plan_geometry(slot, changed, cal, live)
+    copies = self._plan_resume(slot, live, resumed)
+    self._restores[slot] = rest or None
     maps = None
     if live is not None:
       self._was_idle = set(gone)
@@ -1115,6 +1340,8 @@ class StreamRunner(object):
     caller = torch.cuda.current_stream(self.device)
     with torch.cuda.stream(self.copy):
       self.copy.wait_event(self.ev_done[slot])       # slot's old contents were last read as pre_images of step t-2
+      if copies:                                     # resumed streams' last frames -> pre_images, before any frame of
+        self._copy_resumed(copies)                   # this step is written (a source may be this slot: DESIGN §5)
       if dev is not None:                            # staged from the caller's tensors once its stream has written them
         self.copy.wait_stream(caller)
         self._stage_frames(slot, dev)
@@ -1139,7 +1366,7 @@ class StreamRunner(object):
         self.pub[slot][0].copy_(self.h_pub[slot][0], non_blocking=True)
         self.pub[slot][1].copy_(self.h_pub[slot][1], non_blocking=True)
       self._start_bytes = self._upload_starts(slot, plan, non_blocking=True) + \
-          self._upload_geometry(slot, rows, non_blocking=True)
+          self._upload_geometry(slot, rows, non_blocking=True) + (12 * len(rest) if self.tracker is not None else 0)
       self.ev_in[slot].record(self.copy)
     return self._submit(slot)
 

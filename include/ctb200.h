@@ -24,7 +24,8 @@
  *                     ct_track_step_assoc adds --hungarian and --public_det association (tracker.py:52-72,83-103);
  *                     ct_track_step_payload adds the pose / 3D / velocity / attribute fields (post_process.py:55-89).
  *                     ct_track_start: reset_tracking + Tracker.init_track(pre_dets) on some streams alone
- *                     (detector.py:97-103, utils/tracker.py:11-22).
+ *                     (detector.py:97-103, utils/tracker.py:11-22); ct_track_restore continues an exported stream's
+ *                     tracks on another stream or runner.
  *   ct_post_process   Detector.post_process + merge_outputs (detector.py:356-377) on the device for runners without a
  *                     tracker: each stream's kept detections in its source pixels, with ct_track_step's arithmetic.
  *   ct_flip_merge     Detector._flip_output, detector.py:311-332 (flip_tensor / flip_lr / flip_lr_off, model/utils.py:28-50);
@@ -352,6 +353,17 @@ int ct_track_step_payload(const ct_track_desc* d, const ct_track_assoc* a, const
  * Only d->B, max_tracks, pre_thresh, inp_h, inp_w, trans_input, tracks, counts and boxes are read. */
 int ct_track_start(const ct_track_desc* d, const ct_track_payload* p, const int32_t* starts, int32_t n_starts,
                    const float* seeds, void* stream);
+/* Continue a video exported from another stream (of this or another table) on some streams: ct_track_start with the
+ * rows kept as they are.  For each of the n_entries entries of `entries` (device int32 [n_entries][3] = (stream, rows n,
+ * id_count), distinct streams in [0, B)), the stream's T track rows, counts and (p != NULL) payload rows are zeroed, its
+ * n rows written verbatim (fp32 [n][CT_TRK_FLOATS]: ids, ages and active as exported) with its n payload rows (fp32
+ * [n][p->width], when p != NULL and payload_rows != NULL), counts = (n, id_count), and its T render boxes computed from
+ * them as ct_track_step computes them, with this stream's index and trans_input.  `rows` and `payload_rows` (device) hold
+ * the rows of entry 0, then entry 1, ...; rows may be NULL when every n is 0.  n is clamped to [0, T] and entries with a
+ * stream outside [0, B) are skipped on the device.  Every other stream is left untouched.  One CTA per entry;
+ * n_entries == 0 launches nothing.  Reads what ct_track_start reads. */
+int ct_track_restore(const ct_track_desc* d, const ct_track_payload* p, const int32_t* entries, int32_t n_entries,
+                     const float* rows, const float* payload_rows, void* stream);
 /* pre_hm (fp32 [B,1,H,W], zeroed here) <- max-splat of boxes [n,5] (rows with radius < 0 skipped); n is the grid size,
  * so the launch shape does not depend on the data (CUDA-graph capturable). */
 int ct_render_tracks(const float* boxes, int32_t n, float* pre_hm, int32_t B, int32_t H, int32_t W, void* stream);

@@ -13,7 +13,14 @@ The row depends on the batch and the SM count (n_sm = 132 on the CPU, the H100 S
 kernels at other batches.  tests/test_plan_rows.py checks that every row of every PRODUCT_PLANS plan is audited by a
 test_gpu_plan_layers.CASES plan or by an op named in TARGETED; tests/test_gpu_plan_rows.py audits the TARGETED ops.
 
-`python tests/plan_rows.py` prints the rows no audit reaches and the TARGETED entries that would cover them.
+A row says nothing about the size of the tensors, and the engines index memory with 32-bit offsets, guarded by host
+checks (the gather engines refuse an input of 2^31 elements).  So for every row that has an operand of at least 2^31
+bytes in some product plan, the op with the largest operand in that row (op_extents) must be named in EXTENT_TARGETED;
+tests/test_gpu_plan_rows.py runs those at their full batch and compares every image with the same launch on 4-image
+slices.
+
+`python tests/plan_rows.py` prints the rows no audit reaches and the TARGETED entries that would cover them, then the
+same for the large launches and EXTENT_TARGETED.
 """
 import contextlib
 import os
@@ -91,6 +98,22 @@ TARGETED = {
 }
 
 
+# product plan id -> the ops tests/test_gpu_plan_rows.py runs at their full size, image by image: for each row with an
+# operand of at least LARGE bytes in some product plan, the op of the largest extent in that row (op_extents,
+# `python tests/plan_rows.py`)
+EXTENT_TARGETED = {
+    # bf16x3: the stem's 48-channel fp32 output, and the 1x1 heads reading 256-channel slices of the 1024- / 1792-channel
+    # fp32 head intermediate (mot's is 99.6 % of the gather engine's 2^31-element limit)
+    'coco_pose_512x512_b64_bf16x3': ['hm_hp', 'hps'],
+    'coco_tracking_512x512_b64_bf16x3': ['hm'],
+    'mot_544x960_b64_bf16x3': ['stem48', 'base.level0', 'heads.0', 'hm'],
+    # the SIMT engine: eight heads' 2048-channel intermediate, 2.9e9 elements
+    'nuscenes_ddd_448x800_b64_fp32': ['heads.0', 'hm'],
+}
+
+LARGE = 1 << 31          # bytes: an operand this large has elements (or bytes) past a 32-bit signed offset
+
+
 def _conv_work(eng, d, kern, cfg):
   """'one' / 'several' work items per CTA of the persistent kernels, '-' for the others (conv_tc.cu / conv_halo.cu)."""
   if kern == 'gather' and d.a_mode == L.CT_A_CONV and (cfg.tile_w, cfg.tile_h) == (16, 8):   # tc_uses_tma
@@ -145,6 +168,65 @@ def plan_rows(eng):
     if r is not None:
       rows.setdefault(r, []).append(sp['name'])
   return rows
+
+
+OPERANDS = ('x', 'residual', 'om', 'skip', 'out')
+
+
+def op_extents(eng):
+  """{op name: {operand: (elements, bytes)}} of every op a launch of the plan computes, for each operand it reads or
+  writes: a channel slice by the whole NHWC buffer it lies in (B H W ld), a tensor (the offset / mask map, the fp32 NCHW
+  head planes B C_out OH OW) by itself.  Leaves out the fused head launch's records (heads.0 and the 1x1s that read its
+  intermediate, which never exists); its outputs are the same planes those 1x1 records describe."""
+  from centertrack_b200.engine import DeferredTV, TV
+  res = {}
+  for sp in eng.specs:
+    if isinstance(sp.get('x'), DeferredTV) or launch_row(eng, sp) is None:
+      continue
+    ext = {}
+    for k in OPERANDS:
+      t = sp.get(k)
+      if t is None:
+        continue
+      b = t.buf if isinstance(t, TV) else t
+      ext[k] = (b.numel(), b.numel() * b.element_size())
+    d = sp['desc']
+    if d is not None:                # what the gather engine's guard counts: the whole buffer x lies in
+      assert ext['x'][0] == d.B * d.H * d.W * d.ld_in, sp['name']
+      if d.out_mode == L.CT_OUT_NCHW_F32:
+        assert ext['out'][0] == d.B * d.C_out * d.OH * d.OW, sp['name']
+    res[sp['name']] = ext
+  return res
+
+
+def largest_operand(ext):
+  """(bytes, elements, operand) of the largest operand of an op_extents entry."""
+  return max((b, n, k) for k, (n, b) in ext.items())
+
+
+def large_launches():
+  """{row: (plan id, op, bytes, elements, operand)}: for every row with an operand of at least LARGE bytes in a
+  (buildable) PRODUCT_PLANS plan, the op with the largest operand in that row, at the first plan that has it."""
+  big = {}
+  for pid, cfg, hw, B, precision in PRODUCT_PLANS:
+    if pid in REFUSED:
+      continue
+    eng = cpu_plan(cfg, hw, B, precision)
+    rows = {sp['name']: launch_row(eng, sp) for sp in eng.specs}
+    for name, ext in op_extents(eng).items():
+      nbytes, n, k = largest_operand(ext)
+      row = rows[name]
+      if row not in big or nbytes > big[row][2]:
+        big[row] = (pid, name, nbytes, n, k)
+    del eng
+  return {r: v for r, v in big.items() if v[2] >= LARGE}
+
+
+def extent_unaudited(targeted, large=None):
+  """[(row, (plan id, op, bytes, elements, operand))] of the large launches (large_launches(), or `large`) whose op
+  targeted does not name in its plan."""
+  large = large_launches() if large is None else large
+  return [(r, v) for r, v in large.items() if v[1] not in targeted.get(v[0], ())]
 
 
 def format_row(row):
@@ -221,6 +303,16 @@ if __name__ == '__main__':
     print('%-36s %-12s %s' % (pid, names[0], format_row(r)))
     add.setdefault(pid, []).append(names[0])
   print('\n%d rows unaudited; TARGETED entries that cover them:' % len(missing))
+  for pid, _, _, _, _ in PRODUCT_PLANS:
+    if pid in add:
+      print('    %r: %r,' % (pid, add[pid]))
+  big = extent_unaudited(EXTENT_TARGETED)
+  add = {}
+  print()
+  for r, (pid, name, nbytes, n, k) in big:
+    print('%-36s %-12s %-8s %13d elements %6.2f GB  %s' % (pid, name, k, n, nbytes / 1e9, format_row(r)))
+    add.setdefault(pid, []).append(name)
+  print('\n%d launches with an operand of >= 2^31 bytes unaudited; EXTENT_TARGETED entries that cover them:' % len(big))
   for pid, _, _, _, _ in PRODUCT_PLANS:
     if pid in add:
       print('    %r: %r,' % (pid, add[pid]))

@@ -91,6 +91,27 @@ def test_bad_shapes_get_the_status_and_message_of_ct_conv_forward(built_lib, cas
   assert _forward(_desc(**kw)) == (rc, msg)
 
 
+# The gather engines' 32-bit element offsets: B H W ld_in < 2^31.  2^31 - 8 = 120 x 1247 x 113 x 127, the largest
+# input a multiple of 8 channels wide can have (tests/test_gpu_conv.py runs a launch of that size).
+EDGE_ACCEPTED = dict(B=1247, H=113, W=127, ld_in=120)
+EDGE_REFUSED = dict(B=4096, H=64, W=64, ld_in=128)
+
+
+@pytest.mark.parametrize('engine', [L.CT_ENGINE_TCGEN05, L.CT_ENGINE_TCGEN05_X3], ids=['bf16', 'x3'])
+@pytest.mark.parametrize('k', [1, 3])
+def test_gather_input_size_limit(built_lib, engine, k):
+  for shape, n in ((EDGE_ACCEPTED, (1 << 31) - 8), (EDGE_REFUSED, 1 << 31)):
+    d = _desc(engine=engine, C_in=40, C_out=16, k=k, n_tile=16, H=shape['H'], W=shape['W'])
+    d.B, d.ld_in = shape['B'], shape['ld_in']
+    assert d.B * d.H * d.W * d.ld_in == n
+    rc, msg, _ = _config(d)
+    if n < 1 << 31:
+      assert rc == L.CT_OK, msg
+    else:
+      assert rc == L.CT_ERR_INVALID and b'input tensor exceeds 2^31 elements' in msg, msg
+      assert _forward(d) == (rc, msg)
+
+
 def test_inconsistent_output_size_is_invalid(built_lib):
   d = _desc(engine=L.CT_ENGINE_TCGEN05)
   d.OH += 1

@@ -389,3 +389,82 @@ def test_conv_argument_validation():
   d = L.ConvDesc()
   assert lib.ct_conv_forward(C.byref(d), None) == -1
   assert b'null pointer' in lib.ct_last_error()
+
+
+# ---- the 32-bit edge: launches at the largest input an engine accepts -------------------------------------------------
+# (id, engine, dtype, B, H, W, C_in, ld_in, k, C_out, out_mode).  The gather engines: B H W ld_in = 2^31 - 8, the largest
+# input below their 2^31-element limit (tests/test_conv_config.py), C_in = 40 on the register gather (C_in = 64 takes the
+# TMA-fed kernel); the channels sit at the top of each pixel, so the last 16-byte load of the last image ends at element
+# 2^31 - 8 of the buffer.  The SIMT engine, which has no such limit: a 1x1 head reading the last 256 channels of nuScenes'
+# 2048-channel head intermediate at B = 64 (2.9e9 elements).
+EDGE = [('gather_1x1', L.CT_ENGINE_TCGEN05, L.CT_BF16, 1247, 113, 127, 40, 120, 1, 16, L.CT_OUT_NCHW_F32),
+        ('gather_3x3', L.CT_ENGINE_TCGEN05, L.CT_BF16, 1247, 113, 127, 40, 120, 3, 16, L.CT_OUT_NHWC),
+        ('gather_tma_3x3', L.CT_ENGINE_TCGEN05, L.CT_BF16, 1247, 113, 127, 64, 120, 3, 16, L.CT_OUT_NHWC),
+        ('x3_1x1', L.CT_ENGINE_TCGEN05_X3, L.CT_F32, 1247, 113, 127, 40, 120, 1, 16, L.CT_OUT_NCHW_F32),
+        ('x3_3x3', L.CT_ENGINE_TCGEN05_X3, L.CT_F32, 1247, 113, 127, 40, 120, 3, 16, L.CT_OUT_NHWC),
+        ('simt_1x1_nuscenes_heads', L.CT_ENGINE_SIMT, L.CT_F32, 64, 112, 200, 256, 2048, 1, 10, L.CT_OUT_NCHW_F32)]
+
+
+def _edge_out(B, C_out, H, W, act, out_mode):
+  shape = (B, C_out, H, W) if out_mode == L.CT_OUT_NCHW_F32 else (B, H, W, C_out)
+  return torch.full(shape, float('nan'), dtype=torch.float32 if out_mode == L.CT_OUT_NCHW_F32 else act, device='cuda')
+
+
+@pytest.mark.parametrize('case', EDGE, ids=[c[0] for c in EDGE])
+def test_largest_input_last_image(case):
+  """One launch over the whole input: its last image within the fp64 bound and bit-identical to a B = 1 launch on that
+  image alone, whose offsets stay small.  The channels outside the slice are NaN, so a read of them shows too."""
+  import ctypes as C
+  import gc
+  from gpu_helpers import packed_weights
+  name, engine, dtype, B, H, W, Cin, ld, k, Cout, out_mode = case
+  act = torch.bfloat16 if dtype == L.CT_BF16 else torch.float32
+  gc.collect()
+  torch.cuda.empty_cache()
+  torch.cuda.reset_peak_memory_stats()
+  free, _ = torch.cuda.mem_get_info()
+  need = B * H * W * (ld + Cout) * torch.finfo(act).bits // 8 * 2
+  if free < need:
+    pytest.skip('needs about %.1f GB of device memory, %.1f GB free' % (need / 1e9, free / 1e9))
+  off = ld - Cin
+  g = torch.Generator(device='cuda').manual_seed(len(name))
+  x = torch.full((B, H, W, ld), float('nan'), dtype=act, device='cuda')
+  x[..., off:].normal_(generator=g)
+  gw = torch.Generator().manual_seed(7)
+  w = torch.randn(Cout, Cin, k, k, generator=gw) * (2.0 / (Cin * k * k)) ** 0.5
+  b = torch.randn(Cout, generator=gw) * 0.1
+  n_tile = 16 if engine != L.CT_ENGINE_SIMT else 0
+  wp, sh = packed_weights(engine, w, n_tile), b.cuda()
+  d = L.ConvDesc()
+  d.engine, d.dtype, d.a_mode = engine, dtype, L.CT_A_CONV
+  d.B, d.H, d.W, d.C_in, d.ld_in, d.C_out = B, H, W, Cin, ld, Cout
+  d.KH = d.KW = k
+  d.stride, d.pad, d.OH, d.OW = 1, k // 2, H, W
+  d.out_mode, d.relu, d.sig_from, d.depth_scale, d.n_tile = out_mode, int(k == 3), 1 << 30, 1.0, n_tile
+  d.x, d.w, d.shift = x.data_ptr() + off * x.element_size(), wp.data_ptr(), sh.data_ptr()
+  out = _edge_out(B, Cout, H, W, act, out_mode)
+  d.out, d.ld_out = out.data_ptr(), 0 if out_mode == L.CT_OUT_NCHW_F32 else Cout
+  n_in = d.B * d.H * d.W * d.ld_in
+  assert n_in > (1 << 31) if engine == L.CT_ENGINE_SIMT else n_in == (1 << 31) - 8
+  lib = L.lib()
+  L.check(lib.ct_conv_forward(C.byref(d), L.stream_ptr()), name)
+  one = _edge_out(1, Cout, H, W, act, out_mode)
+  d1 = L.ConvDesc.from_buffer_copy(d)
+  d1.B, d1.x, d1.out = 1, d.x + (B - 1) * H * W * ld * x.element_size(), one.data_ptr()
+  L.check(lib.ct_conv_forward(C.byref(d1), L.stream_ptr()), name + ' B = 1')
+  torch.cuda.synchronize()
+  last = out[B - 1:]
+  bits = torch.int16 if last.element_size() == 2 else torch.int32
+  assert torch.equal(last.view(bits), one.view(bits)), '%s: the last image differs from a B = 1 launch on it' % name
+  xq = x[B - 1:, ..., off:].permute(0, 3, 1, 2).double()
+  wq = (w.bfloat16() if engine == L.CT_ENGINE_TCGEN05 else w).double().cuda()    # as ct_pack_weights rounds it
+  p = k // 2
+  ref, mag = bd.conv_ref(xq, wq, b, pad=(p, p, p, p))
+  got = last if out_mode == L.CT_OUT_NCHW_F32 else last.permute(0, 3, 1, 2)
+  m = _check(got.float(), ref, mag, engine, dtype, '%s, image %d' % (name, B - 1), 'relu' if k == 3 else 'none',
+             out_f32=out_mode == L.CT_OUT_NCHW_F32)
+  print('\n[%s] B H W ld_in = %d elements; image %d: worst |err| / bound %.3f, bit-identical to B = 1; peak %.1f GB' % (
+      name, n_in, B - 1, m, torch.cuda.max_memory_allocated() / 1e9))
+  del x, out, one
+  gc.collect()
+  torch.cuda.empty_cache()

@@ -3,7 +3,9 @@
 Every row of every PRODUCT_PLANS plan -- bench.py's configs at their resolutions, bf16 / bf16x3 / fp32, B = 1 ... 64,
 built on the CPU with the H100 SXM's 132 SMs -- must be run by a plan of test_gpu_plan_layers.CASES or by an op that
 plan_rows.TARGETED names (audited by tests/test_gpu_plan_rows.py).  A planner or library change that makes a product
-plan pick a configuration nothing audits fails here, listing the rows and the ops that run them."""
+plan pick a configuration nothing audits fails here, listing the rows and the ops that run them.  Likewise every row
+with an operand of >= 2^31 bytes must have its largest launch named in plan_rows.EXTENT_TARGETED, which
+tests/test_gpu_plan_rows.py runs at full size."""
 import pytest
 
 import plan_rows as pr
@@ -38,6 +40,48 @@ def test_every_product_row_is_audited(audit):
   assert not missing, '%d launch configurations of the product plans are audited by no CASES plan and no TARGETED ' \
       'op (plan, ops that run it, row):\n  %s' % (len(missing), '\n  '.join(
           '%s  %s  %s' % (pid, ','.join(names), pr.format_row(r)) for pid, r, names in missing))
+
+
+@pytest.fixture(scope='module')
+def large(built_lib):
+  return pr.large_launches()
+
+
+def test_every_large_launch_is_audited_at_its_size(large):
+  """The op with the largest operand of every row that reaches 2^31 bytes runs, at its plan's batch, in
+  tests/test_gpu_plan_rows.py: a planner change that makes a bigger launch fails here until EXTENT_TARGETED names it."""
+  missing = pr.extent_unaudited(pr.EXTENT_TARGETED, large)
+  assert not missing, '%d launches with an operand of >= 2^31 bytes are audited at no batch that large; add to ' \
+      'plan_rows.EXTENT_TARGETED (plan, op, its largest operand, row):\n  %s' % (len(missing), '\n  '.join(
+          '%s  %s  %s %d elements, %.2f GB  %s' % (pid, name, k, n, nbytes / 1e9, pr.format_row(r))
+          for r, (pid, name, nbytes, n, k) in missing))
+
+
+def test_extent_targeted_ops_are_the_largest_conv_launches(large):
+  """No stale entry: each EXTENT_TARGETED op is the largest launch of its row, and a convolution (which the GPU test
+  slices by images)."""
+  want = {(pid, name) for pid, name, _, _, _ in large.values()}
+  for pid, names in pr.EXTENT_TARGETED.items():
+    for n in names:
+      assert (pid, n) in want, '%s: %s is not the largest launch of a row with an operand of >= 2^31 bytes' % (pid, n)
+  for r in large:
+    assert r[0] in ('simt', 'gather', 'gather_x3', 'halo'), r
+
+
+def test_op_extents_count_whole_buffers(built_lib):
+  """A channel slice counts its whole NHWC buffer (ld, not C); the fp32 head planes B C_out OH OW; the fused head
+  launch's records are left out."""
+  eng = pr.cpu_plan('mot', pr.BENCH_SHAPES['mot'], 2, 'bf16x3')
+  ext = pr.op_extents(eng)
+  H, W = pr.BENCH_SHAPES['mot']
+  px4, px8 = (H // 4) * (W // 4), (H // 8) * (W // 8)
+  mid = 256 * len(eng.heads)                            # the heads' fp32 intermediate; hm reads channels 0 .. 255
+  assert ext['hm']['x'] == (2 * px4 * mid, 2 * px4 * mid * 4)
+  assert ext['hm']['out'] == (2 * eng.heads['hm'] * px4, 2 * eng.heads['hm'] * px4 * 4)
+  assert ext['base.level3.tree1']['x'] == (2 * px8 * 256, 2 * px8 * 256 * 4)      # level3.tree1's [x2 | x1] buffer
+  assert ext['base.level3.tree1']['out'][0] == 2 * px8 * (3 * 128 + 64)           # a slice of level3's root input
+  fused = pr.op_extents(pr.cpu_plan('mot', pr.BENCH_SHAPES['mot'], 2, 'bf16'))
+  assert 'heads.0' not in fused and 'hm' not in fused and 'base.level0' in fused
 
 
 def test_targeted_ops_exist_and_have_a_checker(audit):

@@ -139,8 +139,8 @@ EXPORTS = ['ct_packed_weight_bytes', 'ct_pack_weights', 'ct_conv_forward', 'ct_c
            'ct_track_step_assoc', 'ct_track_payload_smem_bytes', 'ct_track_step_payload', 'ct_track_start',
            'ct_track_restore',
            'ct_render_tracks', 'ct_track_step_mapped', 'ct_render_tracks_mapped', 'ct_post_process', 'ct_flip_merge', 'ct_flip_merge_heads', 'ct_mirror_x',
-           'ct_warp_affine_normalize', 'ct_pack_stem_frames', 'ct_pack_stem_frames_flip', 'ct_pack_stem_frames_dev',
-           'ct_pack_stem_frames_flip_dev', 'ct_warp_frames_normalize', 'ct_stage_frames', 'ct_last_error',
+           'ct_warp_affine_normalize', 'ct_pack_stem_frames_dev', 'ct_pack_stem_frames_flip_dev',
+           'ct_warp_frames_normalize', 'ct_stage_frames', 'ct_last_error',
            'ct_abi_version', 'ct_launch_count', 'ct_reset_launch_count', 'ct_debug_trace', 'ct_debug_watch']
 
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17', '-Xcompiler', '-fPIC']
@@ -229,9 +229,6 @@ def lib():
   L.ct_warp_affine_normalize.argtypes = [C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 4 + [C.c_int32] * 2 + [C.c_void_p]
   L.ct_flip_merge_heads.argtypes = [C.POINTER(FlipHead)] + [C.c_int32] * 4 + [C.c_void_p]
   L.ct_mirror_x.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p]
-  L.ct_pack_stem_frames.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(Frame), C.c_int32] + [C.c_void_p] * 4 + \
-      [C.c_int32] * 2 + [C.c_void_p]
-  L.ct_pack_stem_frames_flip.argtypes = L.ct_pack_stem_frames.argtypes
   L.ct_pack_stem_frames_dev.argtypes = [C.c_void_p] * 3 + [C.c_int32, C.c_int64] + [C.c_void_p] * 4 + \
       [C.c_int32] * 2 + [C.c_void_p]
   L.ct_pack_stem_frames_flip_dev.argtypes = L.ct_pack_stem_frames_dev.argtypes
@@ -242,7 +239,7 @@ def lib():
   L.ct_reset_launch_count.restype = None
   L.ct_debug_trace.argtypes = [C.c_void_p]
   L.ct_debug_watch.argtypes = [C.c_void_p]
-  if L.ct_abi_version() != 1:
+  if L.ct_abi_version() != 2:
     raise RuntimeError('libctb200 ABI mismatch')
   _lib = L
   return L

@@ -17,10 +17,11 @@
 //   ct_mirror_x      the mirrored half of a --flip_test batch (detector.py:225-226,285-286)
 //   ct_warp_affine_normalize   Detector.pre_process's cv2.warpAffine(INTER_LINEAR) + (x/255 - mean)/std + HWC->CHW
 //                    (detector.py:207-226), cv2's fixed-point bilinear restated
-//   ct_pack_stem_frames        the same warp + normalise of B ragged uint8 frames (and of their previous frames),
-//                    written straight as the tensor-core stem's packed bf16 input; ct_pack_stem_frames_flip also
-//                    writes each stream's mirror image (--flip_test); the device-descriptor forms also take NV12 /
-//                    I420 frames, cv2.cvtColor(COLOR_YUV2BGR_NV12 / _I420) applied to each bilinear tap
+//   ct_pack_stem_frames_dev    the same warp + normalise of B ragged uint8 frames (and of their previous frames) that
+//                    device-resident descriptors describe, written straight as the tensor-core stem's packed bf16
+//                    input; ct_pack_stem_frames_flip_dev also writes each stream's mirror image (--flip_test);
+//                    ct_warp_frames_normalize the same frames into an fp32 image.  BGR, NV12 or I420 frames, the
+//                    latter two with cv2.cvtColor(COLOR_YUV2BGR_NV12 / _I420) applied to each bilinear tap
 //   ct_stage_frames  B frames already in device memory (a GPU decoder's) copied into a frame slot in its layout
 // All HBM-bound byte/index work: one pass over the data, coalesced, no tensor cores.
 #include <math_constants.h>
@@ -703,8 +704,8 @@ __device__ __forceinline__ void yuv_to_bgr(int Y, int U, int V, int bgr[3]) {
 }
 
 // The warped uint8 BGR value of output pixel (x, y): src uint8 [sh, sw, 3] with row pitch sstep bytes, M the inverted
-// (dst -> src) map.  The one copy of the per-pixel warp arithmetic: ct_warp_affine_normalize and ct_pack_stem_frames
-// both call it, so that the fused stem input is byte-identical to the fp32 image packed afterwards.
+// (dst -> src) map.  The one copy of the per-pixel warp arithmetic: ct_warp_affine_normalize and the frames kernels
+// all call it, so that the fused stem input is byte-identical to the fp32 image packed afterwards.
 // FMT = CT_FRAME_NV12 / CT_FRAME_I420: src is the [3sh/2, sw] 4:2:0 frame (luma pitch sstep) and each tap inside the
 // frame is converted to BGR first, so the result is the warp of cv2.cvtColor's BGR image; taps outside read BGR 0.
 template <int FMT = CT_FRAME_BGR>
@@ -799,19 +800,11 @@ __global__ void warp_affine_norm_kernel(const unsigned char* __restrict__ src, i
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// Where a frames kernel finds stream b's ct_frame.  ParamFrames: in the kernel parameters, CT_FRAMES_PER_LAUNCH per
-// launch (a captured graph keeps them by value).  DeviceFrames: a device array [B] that may change between graph
-// replays; each CTA copies its stream's descriptor to shared memory once and checks it against the buffer size, since
-// the host cannot: an invalid one yields zeros and no read of the frame buffers.
+// Where a frames kernel finds stream b's ct_frame: a device array [B] that may change between graph replays.  Each CTA
+// copies its stream's descriptor to shared memory once and checks it against the buffer size, since the host cannot:
+// an invalid one yields zeros and no read of the frame buffers.
 // ------------------------------------------------------------------------------------------------------------------
-// kFormats: the descriptors may name any CT_FRAME_* format (the host checks the by-value ones to be BGR).
-struct ParamFrames {
-  static constexpr bool kFormats = false;
-  ct_frame f[CT_FRAMES_PER_LAUNCH];
-};
-
 struct DeviceFrames {
-  static constexpr bool kFormats = true;
   const ct_frame* f;
   long long buf_bytes;
 };
@@ -830,29 +823,19 @@ __device__ __forceinline__ bool frame_in_buffer(const ct_frame& f, long long buf
   return (long long)f.step >= row_bytes && (rows - 1) * f.step + row_bytes <= buf_bytes - f.offset;
 }
 
-// The warped BGR pixel (x, y) of the frame f describes at src (its first byte), in f's format `fmt`.  Frames without
-// formats compile the BGR sampler alone.
-template <class Frames>
+// The warped BGR pixel (x, y) of the frame f describes at src (its first byte), in f's format `fmt`.
 __device__ __forceinline__ void warp_frame_u8(const unsigned char* __restrict__ src, const ct_frame& f, int fmt, int x,
                                               int y, int p8[3]) {
-  if constexpr (Frames::kFormats) {
-    if (fmt == CT_FRAME_NV12) return warp_bilinear_u8<CT_FRAME_NV12>(src, f.h, f.w, f.step, f.minv, x, y, p8);
-    if (fmt == CT_FRAME_I420) return warp_bilinear_u8<CT_FRAME_I420>(src, f.h, f.w, f.step, f.minv, x, y, p8);
-  }
+  if (fmt == CT_FRAME_NV12) return warp_bilinear_u8<CT_FRAME_NV12>(src, f.h, f.w, f.step, f.minv, x, y, p8);
+  if (fmt == CT_FRAME_I420) return warp_bilinear_u8<CT_FRAME_I420>(src, f.h, f.w, f.step, f.minv, x, y, p8);
   warp_bilinear_u8(src, f.h, f.w, f.step, f.minv, x, y, p8);
 }
 
-// -> this CTA's descriptor (stream b0 + blockIdx.y) and whether it may be read; ends with __syncthreads()
-__device__ __forceinline__ const ct_frame& cta_frame(const ParamFrames& fs, int b0, ct_frame*, bool& ok) {
-  ok = true;
-  __syncthreads();
-  return fs.f[blockIdx.y];
-}
-
-__device__ __forceinline__ const ct_frame& cta_frame(const DeviceFrames& fs, int b0, ct_frame* s_f, bool& ok) {
+// -> this CTA's descriptor (stream blockIdx.y) and whether it may be read; ends with __syncthreads()
+__device__ __forceinline__ const ct_frame& cta_frame(const DeviceFrames& fs, ct_frame* s_f, bool& ok) {
   __shared__ int s_ok;
   if (threadIdx.x == 0) {
-    *s_f = fs.f[b0 + blockIdx.y];
+    *s_f = fs.f[blockIdx.y];
     s_ok = frame_in_buffer(*s_f, fs.buf_bytes);
   }
   __syncthreads();
@@ -865,7 +848,7 @@ __global__ void warp_frames_norm_kernel(const unsigned char* __restrict__ src, c
                                         float* __restrict__ dst, int oh, int ow, float3 mean, float3 stdv) {
   __shared__ ct_frame s_f;
   bool ok;
-  const ct_frame& f = cta_frame(fs, 0, &s_f, ok);
+  const ct_frame& f = cta_frame(fs, &s_f, ok);
   const int fmt = f.format;
   const size_t plane = (size_t)oh * ow;
   float* o = dst + (size_t)blockIdx.y * 3 * plane;
@@ -873,7 +856,7 @@ __global__ void warp_frames_norm_kernel(const unsigned char* __restrict__ src, c
     const int y = (int)(r / ow), x = (int)(r - (size_t)y * ow);
     if (ok) {
       int p8[3];
-      warp_frame_u8<DeviceFrames>(src + f.offset, f, fmt, x, y, p8);
+      warp_frame_u8(src + f.offset, f, fmt, x, y, p8);
       store_norm_pixel(p8, o + r, plane, mean, stdv);
     } else {
       o[r] = o[r + plane] = o[r + 2 * plane] = 0.f;
@@ -882,12 +865,11 @@ __global__ void warp_frames_norm_kernel(const unsigned char* __restrict__ src, c
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// ct_pack_stem_frames: the tensor-core stem's input [B,H,W,8] bf16 = (norm(warp(cur_b)) x3, norm(warp(prev_b)) x3,
-// pre_hm, 0) straight from each stream's uint8 frame.  blockIdx.y = stream (its descriptor read once, from the kernel
-// parameters or, in the _dev forms, from device memory: Frames), one 16-byte output pixel per thread and iteration.
-// The normalisation depends on the 8-bit value only: a 3 x 256 table built per CTA with normalize_u8 gives the same
-// floats without a per-pixel fp64 divide.
-// FLIP (ct_pack_stem_frames_flip): out is [2B,H,W,8] and image B+b is image b mirrored.  The mirrored packed pixel
+// ct_pack_stem_frames_dev: the tensor-core stem's input [B,H,W,8] bf16 = (norm(warp(cur_b)) x3, norm(warp(prev_b)) x3,
+// pre_hm, 0) straight from each stream's uint8 frame.  blockIdx.y = stream (its descriptor read once from device
+// memory), one 16-byte output pixel per thread and iteration.  The normalisation depends on the 8-bit value only: a
+// 3 x 256 table built per CTA with normalize_u8 gives the same floats without a per-pixel fp64 divide.
+// FLIP (ct_pack_stem_frames_flip_dev): out is [2B,H,W,8] and image B+b is image b mirrored.  The mirrored packed pixel
 // (y, W-1-x) equals the original's (y, x) in all 8 channels (frame, previous frame and pre_hm are all mirrored), so each
 // pixel is warped once and its 16-byte vector stored twice.
 // ------------------------------------------------------------------------------------------------------------------
@@ -932,43 +914,8 @@ __device__ __forceinline__ void pack_pixels(const unsigned char* __restrict__ sr
   }
 }
 
-template <bool FLIP, class Frames>
-__device__ __forceinline__ void pack_stem_frames_body(const unsigned char* __restrict__ cur,
-                                                      const unsigned char* __restrict__ prev, const Frames& fs, int b0,
-                                                      int B, float3 mean, float3 stdv, const float* __restrict__ hm,
-                                                      uint4* __restrict__ out, int H, int W) {
-  __shared__ float tab[3][256];
-  __shared__ ct_frame s_f;
-  for (int i = threadIdx.x; i < 3 * 256; i += PACK_THREADS) {
-    const int c = i >> 8, v = i & 255;
-    tab[c][v] = normalize_u8(v, c == 0 ? mean.x : (c == 1 ? mean.y : mean.z), c == 0 ? stdv.x : (c == 1 ? stdv.y : stdv.z));
-  }
-  bool ok;
-  const ct_frame& f = cta_frame(fs, b0, &s_f, ok);
-  const int b = b0 + blockIdx.y;
-  const unsigned char* src = cur + f.offset;
-  const unsigned char* psrc = prev ? prev + f.offset : nullptr;
-  const size_t base = (size_t)blockIdx.x * PACK_THREADS * PACK_PIX_PER_THREAD + threadIdx.x;
-  if constexpr (Frames::kFormats) {
-    const int fmt = f.format;
-    if (fmt == CT_FRAME_NV12)
-      return pack_pixels<FLIP, CT_FRAME_NV12>(src, psrc, f, ok, tab, b, B, base, hm, out, H, W);
-    if (fmt == CT_FRAME_I420)
-      return pack_pixels<FLIP, CT_FRAME_I420>(src, psrc, f, ok, tab, b, B, base, hm, out, H, W);
-  }
-  pack_pixels<FLIP, CT_FRAME_BGR>(src, psrc, f, ok, tab, b, B, base, hm, out, H, W);
-}
-
-template <bool FLIP>
-__global__ void __launch_bounds__(PACK_THREADS)
-pack_stem_frames_kernel(const unsigned char* __restrict__ cur, const unsigned char* __restrict__ prev,
-                        const __grid_constant__ ParamFrames fs, int b0, int B, float3 mean, float3 stdv,
-                        const float* __restrict__ hm, uint4* __restrict__ out, int H, int W) {
-  pack_stem_frames_body<FLIP>(cur, prev, fs, b0, B, mean, stdv, hm, out, H, W);
-}
-
-// The device-descriptor forms: 6 CTAs per SM, at most 40 registers -- the occupancy of the BGR-only sampler's 36
-// (allocated in steps of 8); without the bound the YUV samplers take the flip form to 48 registers and 5 CTAs.
+// 6 CTAs per SM, at most 40 registers -- the occupancy of the BGR-only sampler's 36 (allocated in steps of 8); without
+// the bound the YUV samplers take the flip form to 48 registers and 5 CTAs.
 constexpr int PACK_DEV_MIN_CTAS = 6;
 
 template <bool FLIP>
@@ -976,7 +923,24 @@ __global__ void __launch_bounds__(PACK_THREADS, PACK_DEV_MIN_CTAS)
 pack_stem_frames_dev_kernel(const unsigned char* __restrict__ cur, const unsigned char* __restrict__ prev,
                             const __grid_constant__ DeviceFrames fs, float3 mean, float3 stdv,
                             const float* __restrict__ hm, uint4* __restrict__ out, int H, int W) {
-  pack_stem_frames_body<FLIP>(cur, prev, fs, 0, gridDim.y, mean, stdv, hm, out, H, W);
+  __shared__ float tab[3][256];
+  __shared__ ct_frame s_f;
+  for (int i = threadIdx.x; i < 3 * 256; i += PACK_THREADS) {
+    const int c = i >> 8, v = i & 255;
+    tab[c][v] = normalize_u8(v, c == 0 ? mean.x : (c == 1 ? mean.y : mean.z), c == 0 ? stdv.x : (c == 1 ? stdv.y : stdv.z));
+  }
+  bool ok;
+  const ct_frame& f = cta_frame(fs, &s_f, ok);
+  const int b = blockIdx.y, B = gridDim.y;
+  const unsigned char* src = cur + f.offset;
+  const unsigned char* psrc = prev ? prev + f.offset : nullptr;
+  const size_t base = (size_t)blockIdx.x * PACK_THREADS * PACK_PIX_PER_THREAD + threadIdx.x;
+  const int fmt = f.format;
+  if (fmt == CT_FRAME_NV12)
+    return pack_pixels<FLIP, CT_FRAME_NV12>(src, psrc, f, ok, tab, b, B, base, hm, out, H, W);
+  if (fmt == CT_FRAME_I420)
+    return pack_pixels<FLIP, CT_FRAME_I420>(src, psrc, f, ok, tab, b, B, base, hm, out, H, W);
+  pack_pixels<FLIP, CT_FRAME_BGR>(src, psrc, f, ok, tab, b, B, base, hm, out, H, W);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1307,48 +1271,6 @@ extern "C" int ct_warp_affine_normalize(const uint8_t* src, int32_t B, int32_t s
       src, src_h, src_w, src_step, dst, B, out_h, out_w, minv, make_float3(mean[0], mean[1], mean[2]),
       make_float3(std[0], std[1], std[2]));
   return after_launch();
-}
-
-template <bool FLIP>
-static int pack_stem_frames(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames, int32_t B,
-                            const float* mean, const float* std, const float* pre_hm, void* out, int32_t H, int32_t W,
-                            void* stream) {
-  CT_REQUIRE(cur && frames && mean && std && out, "null pointer");
-  CT_REQUIRE(B > 0 && H > 0 && W > 0, "bad shape");
-  for (int32_t b = 0; b < B; ++b) {
-    CT_REQUIRE(frames[b].format == CT_FRAME_BGR,
-               "by-value frame descriptors take CT_FRAME_BGR only (YUV frames: the _dev entry points)");
-    CT_REQUIRE(frames[b].offset >= 0 && frames[b].h > 0 && frames[b].w > 0 && frames[b].step >= 3 * frames[b].w,
-               "bad frame descriptor (offset >= 0, h > 0, w > 0, step >= 3 w)");
-  }
-  const size_t plane = (size_t)H * W;
-  const size_t per_cta = (size_t)PACK_THREADS * PACK_PIX_PER_THREAD;
-  CT_REQUIRE((plane + per_cta - 1) / per_cta <= 0x7fffffffu, "output too large");
-  const float3 m = make_float3(mean[0], mean[1], mean[2]), s = make_float3(std[0], std[1], std[2]);
-  // descriptors travel in the kernel parameters (captured by value in a CUDA graph): CT_FRAMES_PER_LAUNCH per launch
-  for (int32_t b0 = 0; b0 < B; b0 += CT_FRAMES_PER_LAUNCH) {
-    const int n = B - b0 < CT_FRAMES_PER_LAUNCH ? B - b0 : CT_FRAMES_PER_LAUNCH;
-    ParamFrames fa = {};
-    memcpy(fa.f, frames + b0, sizeof(ct_frame) * n);
-    dim3 grid((unsigned)((plane + per_cta - 1) / per_cta), (unsigned)n);
-    pack_stem_frames_kernel<FLIP><<<grid, PACK_THREADS, 0, (cudaStream_t)stream>>>(
-        cur, prev, fa, b0, B, m, s, pre_hm, (uint4*)out, H, W);
-    const int rc = after_launch();
-    if (rc != CT_OK) return rc;
-  }
-  return CT_OK;
-}
-
-extern "C" int ct_pack_stem_frames(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames, int32_t B,
-                                   const float* mean, const float* std, const float* pre_hm, void* out, int32_t H,
-                                   int32_t W, void* stream) {
-  return pack_stem_frames<false>(cur, prev, frames, B, mean, std, pre_hm, out, H, W, stream);
-}
-
-extern "C" int ct_pack_stem_frames_flip(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames, int32_t B,
-                                        const float* mean, const float* std, const float* pre_hm, void* out, int32_t H,
-                                        int32_t W, void* stream) {
-  return pack_stem_frames<true>(cur, prev, frames, B, mean, std, pre_hm, out, H, W, stream);
 }
 
 template <bool FLIP>

@@ -77,7 +77,7 @@ def frame_geometry(opt, height, width):
   """Geometry of one height x width source frame at scale 1 (hazard H5: the reference never forwards `scale`), as
   Detector.pre_process_device and StreamRunner's frames mode use it: (meta, minv) with meta = pre_process's meta
   without `calib`, and minv fp64 [6] = meta['trans_input'] inverted exactly as cv::warpAffine inverts it (the dst -> src
-  map ct_warp_affine_normalize / ct_pack_stem_frames sample with)."""
+  map ct_warp_affine_normalize / ct_pack_stem_frames_dev sample with)."""
   _, c, s, inp_w, inp_h = input_geometry(opt, height, width, 1)
   out_w, out_h = inp_w // opt.down_ratio, inp_h // opt.down_ratio
   to_input = get_affine_transform(c, s, 0, [inp_w, inp_h])

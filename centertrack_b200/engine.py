@@ -421,7 +421,7 @@ class DLA34Engine(object):
       # three stems) whose epilogue applies ReLU per stem and sums them (dla.py:307-311)
       x8 = TV(self._buf(H, W, 8), 0, 8)
       self._op('pack', x8, 'stem.pack', out=x8)
-      self.stem_input = x8.buf                            # what forward_packed reads (ct_pack_stem_frames writes it)
+      self.stem_input = x8.buf                            # what forward_packed reads (ct_pack_stem_frames_dev writes it)
       w48 = torch.zeros((48, 8, 7, 7), dtype=torch.float64)
       for si, (c0, cn) in enumerate(((0, 3), (3, 3), (6, 1))):
         w48[16 * si:16 * si + 16, c0:c0 + cn] = wst[:, c0:c0 + cn, :].reshape(7, 7, cn, 16).permute(3, 2, 0, 1)
@@ -752,7 +752,7 @@ class DLA34Engine(object):
 
   def forward_packed(self, has_pre, has_hm, n=None):
     """The plan without its pack op, on a stem input the caller wrote into `stem_input` (bf16 NHWC [B,H,W,8],
-    ct_pack_stem_input's layout, e.g. by ct_pack_stem_frames): has_pre / has_hm say whether its pre_img / pre_hm
+    ct_pack_stem_input's layout, e.g. by ct_pack_stem_frames_dev): has_pre / has_hm say whether its pre_img / pre_hm
     channels are present, as forward's pre_images / pre_hms being given does.  n: the batch, as in forward.  bf16
     tensor-core plan only."""
     if not self.use_halo:

@@ -29,14 +29,15 @@ The end-to-end form (`step_host`) takes HOST frames: pinned staging, H2D on a co
 with the previous step's compute, graph replay, D2H of the records (and tracks).
 
 Frames mode (`frame_sizes`, `step_frames`) takes the raw uint8 BGR camera frames instead, one source size per stream:
-the three slots hold the B frames ragged (16-byte aligned offsets) in pinned and device memory, and the step warps and
-normalises them on the device exactly as Detector.pre_process_device does (cv2's fixed-point bilinear).  On the bf16
-engine ct_pack_stem_frames writes the stem's packed bf16 input straight from slot t (images) and slot t-1 (pre_images,
-warped again: no fp32 copy is kept); the fp32 and bf16x3 engines warp each stream into the fp32 image slot with
-ct_warp_affine_normalize and run their plan unchanged.  The tracker gets each stream's (c, s) and default calib, so
-tracks, public detections and 3D boxes are in that camera's pixels.  With max_frame_size, stream b's frame lives at
-b * cap in every slot and each slot's descriptors are a device array (ct_pack_stem_frames_dev, ct_warp_frames_normalize),
-so a stream may take a frame of another size, and a new camera, when it starts a video, without recapturing a graph.
+the three slots hold the B frames ragged (16-byte aligned offsets) in pinned and device memory, each slot's ct_frame
+descriptors are a device array beside them, and the step warps and normalises the frames on the device exactly as
+Detector.pre_process_device does (cv2's fixed-point bilinear).  On the bf16 engine ct_pack_stem_frames_dev writes the
+stem's packed bf16 input straight from slot t (images) and slot t-1 (pre_images, warped again: no fp32 copy is kept);
+the fp32 and bf16x3 engines warp every stream into the fp32 image slot with one ct_warp_frames_normalize and run their
+plan unchanged.  The tracker gets each stream's (c, s) and default calib, so tracks, public detections and 3D boxes are
+in that camera's pixels.  With max_frame_size, stream b's frame lives at b * cap in every slot, so a stream may take a
+frame of another size, and a new camera, when it starts a video: the step uploads the slot's changed descriptors, and
+a replayed graph reads them, without a recapture.
 A capacity runner may take NV12 or I420 frames instead (`frame_format`, what video decoders emit): each [3h/2, w] frame
 is uploaded as it is, half the bytes of BGR, and the device-descriptor kernels convert each bilinear tap to BGR with
 cv2.cvtColor's fixed-point arithmetic, so the stream computes what it computes on the cv2-converted BGR frame.
@@ -55,7 +56,7 @@ Flip test (`opt.flip_test`, detector.py:225-226,285-286,311-332): the network ru
 [0, B) and their mirrors [B, 2B), inside the same step.  pre_images is the previous step's 2B images, so the previous
 frame's mirror comes free (detector.py:148).  Uploads, the device tracker's render and a caller's pre_hm fill the first
 B images; ct_mirror_x writes the second half in the graph, or, in frames mode on the bf16 engine,
-ct_pack_stem_frames_flip stores every packed pixel at its mirrored position too.  One ct_flip_merge_heads launch
+ct_pack_stem_frames_flip_dev stores every packed pixel at its mirrored position too.  One ct_flip_merge_heads launch
 averages the flipped heads into [B] buffers; decode and tracking then run at B on those and on the first half of the
 other heads.  Records, tracks, uploads and downloads are the same size as without the flip.
 
@@ -262,10 +263,10 @@ class StreamRunner(object):
     frame (more raise ValueError; none is ever dropped).  calibs: with device_tracking on a 3D head set, one [3,4]
     camera matrix per stream (DeviceTracker's default otherwise; in frames mode Detector._get_default_calib of the
     stream's source size).  frame_sizes: B (height, width) source sizes to feed raw uint8 frames with step_frames; each
-    must map to the network input (H, W) under opt's resolution policy (ValueError otherwise).  Without
-    max_frame_size they are fixed for the runner's lifetime.  max_frame_size (h, w): every stream gets a frame region
-    of h * w * 3 bytes in each slot, and may bring a frame of any size that fits it and maps to (H, W) when it starts
-    a video (frame_sizes are then the first sizes); the descriptors of the frames live on the device.
+    must map to the network input (H, W) under opt's resolution policy (ValueError otherwise); the descriptors of the
+    frames live on the device.  Without max_frame_size they are fixed for the runner's lifetime.  max_frame_size
+    (h, w): every stream gets a frame region of h * w * 3 bytes in each slot, and may bring a frame of any size that
+    fits it and maps to (H, W) when it starts a video (frame_sizes are then the first sizes).
     opt.flip_test: every stream's frame runs with its mirror (2B images per step) and the averaged heads are merged
     before decode, as Detector.process does; inputs and outputs keep their B shapes.
     idle_streams g >= 1, or True for g = IDLE_GRANULE (capacity frames runners only): step_frames(idle=) may leave
@@ -325,13 +326,12 @@ class StreamRunner(object):
     if self.frames_mode:      # frame slots: B uint8 frames at 16-byte aligned offsets, pinned staging + device
       self.u8 = [torch.zeros(self.slot_bytes, dtype=torch.uint8, device=self.device) for _ in range(NS)]
       self.h_u8 = [torch.zeros(self.slot_bytes, dtype=torch.uint8).pin_memory() for _ in range(NS)]
-      if self.cap is None:
-        self.minv = torch.from_numpy(np.stack([f.minv[:] for f in self.frames])).to(self.device)
-      else:                  # per slot: the device descriptors of its frames, their pinned staging and a host mirror
-        desc = torch.from_numpy(np.frombuffer(bytes(self.frames), np.uint8).copy())
-        self.h_frames = [desc.clone().pin_memory() for _ in range(NS)]
-        self.d_frames = [desc.to(self.device) for _ in range(NS)]
-        self._desc_mirror = [bytes(self.frames)] * NS
+      # per slot: the device descriptors of its frames, their pinned staging and a host mirror.  The graphs read
+      # d_frames[slot], so it is written in place and never reallocated.
+      desc = torch.from_numpy(np.frombuffer(bytes(self.frames), np.uint8).copy())
+      self.h_frames = [desc.clone().pin_memory() for _ in range(NS)]
+      self.d_frames = [desc.to(self.device) for _ in range(NS)]
+      self._desc_mirror = [bytes(self.frames)] * NS
     if self.idle_g is not None:  # per slot: streams [B] (image -> stream) then image_of [B] (stream -> image), int32
       ident = torch.arange(B, dtype=torch.int32).repeat(2)
       self.h_map = [ident.clone().pin_memory() for _ in range(NS)]
@@ -364,7 +364,7 @@ class StreamRunner(object):
     self._frame_bytes = 0                                    # frame (+ descriptor) bytes of the last upload
     self._ev_read = None                                     # recorded after the last staging of device frames
     if self.frames_mode:
-      self._frame_bytes = self.slot_bytes if self.cap is None else sum(e - a for a, e in self._upload_runs())
+      self._frame_bytes = sum(e - a for a, e in self._upload_runs())
     self._eager(0, first=True)                               # sizes the record buffer
     if device_tracking:
       assert self.opt is not None, 'device tracking needs opt (thresholds, max_age)'
@@ -397,14 +397,12 @@ class StreamRunner(object):
       if self.post.payload is not None:
         self.h_det_pay = [torch.zeros_like(self.post.payload, device='cpu').pin_memory() for _ in range(2)]
     # launches of one step: the network plan + decode (+ memset-free: render + track step); frames mode: the pack op
-    # becomes ct_pack_stem_frames (one launch per CT_FRAMES_PER_LAUNCH streams), or B warps come before the plan.
+    # becomes ct_pack_stem_frames_dev, or one ct_warp_frames_normalize comes before the plan.
     # --flip_test: + the merge, + the mirrors of the images and pre_hm unless the flip pack writes them;
     # device_post_process: + ct_post_process
     self.launches_per_step = self.eng.n_launches + 1 + (2 if device_tracking else 0) + (1 if self.post else 0)
-    if self.frames_mode and self.cap is not None:           # device descriptors: one pack or one warp for all B
+    if self.frames_mode:
       self.launches_per_step += 0 if self.eng.use_halo else 1
-    elif self.frames_mode:
-      self.launches_per_step += (-(-B // L.CT_FRAMES_PER_LAUNCH) - 1) if self.eng.use_halo else B
     if self.flip:
       self.launches_per_step += 1 + (0 if self._pack_mirror else 1 + int(self.eng.has_pre_hm))
     if self.idle_g is not None and not self.eng.use_halo and self.eng.has_pre_img:   # + the pre_images warp (+ mirror)
@@ -549,20 +547,21 @@ class StreamRunner(object):
       c, s = default_geometry(self.H, self.W)
       rows = [(b, c, s, k) for b, k in sorted(calibs.items())]
     desc = None
-    if self.cap is not None:
+    if self.frames_mode:
       now = bytes(self.frames) if live is None else bytes(self._image_frames(live))
       if now != self._desc_mirror[slot]:
         desc = self._desc_mirror[slot] = now
     return desc, rows
 
   def _upload_runs(self, live=None):
-    """Maximal runs [start, end) of the slot bytes this step's frames use: stream b's frame, padded to 16 bytes, at
-    b * cap, for every stream or the `live` ones.  One run of slot_bytes when every stream is at capacity."""
+    """Maximal runs [start, end) of the slot bytes this step's frames use: stream b's frame, padded to 16 bytes, at its
+    offset, for every stream or the `live` ones.  One run of slot_bytes on a fixed runner (its frames are contiguous)
+    and on a capacity runner whose streams are all at capacity."""
     runs = []
     for b, f in enumerate(self.frames):
       if live is not None and b not in live:
         continue
-      a, e = b * self.cap, b * self.cap + (frame_layout(self.frame_format, f.h, f.w)[1] + 15) // 16 * 16
+      a, e = f.offset, f.offset + (frame_layout(self.frame_format, f.h, f.w)[1] + 15) // 16 * 16
       if runs and runs[-1][1] == a:
         runs[-1][1] = e
       else:
@@ -604,12 +603,9 @@ class StreamRunner(object):
       cur, pre = L.ptr(self.u8[slot]), L.ptr(self.u8[prev] if eng.has_pre_img else None)
       ms = (C.c_void_p(self.mean.ctypes.data), C.c_void_p(self.std.ctypes.data),
             L.ptr(self.hm[slot] if eng.has_pre_hm else None), L.ptr(eng.stem_input), self.H, self.W, L.stream_ptr())
-      if self.cap is None:
-        pack = L.lib().ct_pack_stem_frames_flip if self.flip else L.lib().ct_pack_stem_frames
-        L.check(pack(cur, pre, self.frames, self.B, *ms), 'ct_pack_stem_frames')
-      else:                  # the slot's device descriptors: a replayed graph reads the geometry the slot holds
-        pack = L.lib().ct_pack_stem_frames_flip_dev if self.flip else L.lib().ct_pack_stem_frames_dev
-        L.check(pack(cur, pre, L.ptr(self.d_frames[slot]), n, self.slot_bytes, *ms), 'ct_pack_stem_frames_dev')
+      # the slot's device descriptors: a replayed graph reads the geometry the slot holds
+      pack = L.lib().ct_pack_stem_frames_flip_dev if self.flip else L.lib().ct_pack_stem_frames_dev
+      L.check(pack(cur, pre, L.ptr(self.d_frames[slot]), n, self.slot_bytes, *ms), 'ct_pack_stem_frames_dev')
       out = dict(eng.forward_packed(eng.has_pre_img, eng.has_pre_hm, n=NBn))
     else:
       if self.frames_mode:
@@ -668,21 +664,14 @@ class StreamRunner(object):
     L.check(L.lib().ct_mirror_x(L.ptr(x[b]), L.ptr(x[half + b]), n, c, h, w, L.stream_ptr()), 'ct_mirror_x')
 
   def _warp_frames(self, slot, src=None, dst=None):
-    """fp32 and bf16x3 engines: the slot's frames -> its fp32 image, one ct_warp_affine_normalize per stream (one
-    ct_warp_frames_normalize for all of them from the device descriptors on a capacity runner, at the step's batch).
-    src / dst (capacity runners): another frame slot through this slot's descriptors, into another image buffer."""
-    lib, st = L.lib(), L.stream_ptr()
-    src = (self.u8[slot] if src is None else src).data_ptr()
+    """fp32 and bf16x3 engines: the slot's frames -> its fp32 image, one ct_warp_frames_normalize for all of them from
+    the slot's device descriptors, at the step's batch.  src / dst: another frame slot through this slot's descriptors,
+    into another image buffer."""
+    src = self.u8[slot] if src is None else src
     dst = self.img[slot] if dst is None else dst
-    if self.cap is not None:
-      L.check(lib.ct_warp_frames_normalize(C.c_void_p(src), L.ptr(self.d_frames[slot]), self._n, self.slot_bytes,
-                                           C.c_void_p(self.mean.ctypes.data), C.c_void_p(self.std.ctypes.data),
-                                           L.ptr(dst), self.H, self.W, st), 'ct_warp_frames_normalize')
-      return
-    for b, f in enumerate(self.frames):
-      L.check(lib.ct_warp_affine_normalize(C.c_void_p(src + f.offset), 1, f.h, f.w, f.step, L.ptr(self.minv[b]),
-                                           C.c_void_p(self.mean.ctypes.data), C.c_void_p(self.std.ctypes.data),
-                                           L.ptr(dst[b]), self.H, self.W, st), 'ct_warp_affine_normalize')
+    L.check(L.lib().ct_warp_frames_normalize(L.ptr(src), L.ptr(self.d_frames[slot]), self._n, self.slot_bytes,
+                                             C.c_void_p(self.mean.ctypes.data), C.c_void_p(self.std.ctypes.data),
+                                             L.ptr(dst), self.H, self.W, L.stream_ptr()), 'ct_warp_frames_normalize')
 
   def _graph(self, slot):
     if self.idle_g is not None:                              # one graph per (slot, batch), captured on first use
@@ -894,20 +883,11 @@ class StreamRunner(object):
           o, n = f.offset, frame_layout(self.frame_format, f.h, f.w)[1]
           self.u8[prev][o:o + n].copy_(self.u8[slot][o:o + n])
         continue
-      if self.frames_mode and self.frame_format != 'bgr':  # through the slot's device descriptor, which has the format
+      if self.frames_mode:   # the plan reads img[prev]: warp this frame into it through the slot's device descriptor
         L.check(L.lib().ct_warp_frames_normalize(
             L.ptr(src), C.c_void_p(self.d_frames[slot].data_ptr() + b * C.sizeof(L.Frame)), 1,
             self.slot_bytes, C.c_void_p(self.mean.ctypes.data), C.c_void_p(self.std.ctypes.data),
             L.ptr(self.img[prev][b]), self.H, self.W, L.stream_ptr()), 'ct_warp_frames_normalize')
-      elif self.frames_mode:                               # the plan reads img[prev]: warp this frame into it
-        f = self.frames[b]
-        # a capacity runner's minv: the slot's device descriptor of this frame (its new geometry after a size change)
-        minv = L.ptr(self.minv[b]) if self.cap is None else \
-            C.c_void_p(self.d_frames[slot].data_ptr() + b * C.sizeof(L.Frame) + L.Frame.minv.offset)
-        L.check(L.lib().ct_warp_affine_normalize(
-            C.c_void_p(src.data_ptr() + f.offset), 1, f.h, f.w, f.step, minv,
-            C.c_void_p(self.mean.ctypes.data), C.c_void_p(self.std.ctypes.data), L.ptr(self.img[prev][b]), self.H,
-            self.W, L.stream_ptr()), 'ct_warp_affine_normalize')
       else:
         self.img[prev][b].copy_(self.img[slot][b])
       if self.flip:                                        # --flip_test: pre_images is the (frame, mirror) pair
@@ -1173,9 +1153,8 @@ class StreamRunner(object):
       if self.last_slot[b] != dst:
         f = self.frames[b]
         out.append((b, self.last_slot[b], dst, f.offset, frame_layout(self.frame_format, f.h, f.w)[1]))
-    if self.cap is not None:
-      for b in (range(self.B) if live is None else live):
-        self.last_slot[b] = slot
+    for b in (range(self.B) if live is None else live):
+      self.last_slot[b] = slot
     return out
 
   def _copy_resumed(self, copies):
@@ -1345,21 +1324,16 @@ class StreamRunner(object):
       if dev is not None:                            # staged from the caller's tensors once its stream has written them
         self.copy.wait_stream(caller)
         self._stage_frames(slot, dev)
-      if self.cap is None:
-        if dev is None:
-          self.u8[slot].copy_(self.h_u8[slot], non_blocking=True)
-        self._frame_bytes = 0 if dev is not None else self.slot_bytes
-      else:                                          # the used bytes only, and the descriptors when they changed
-        self._frame_bytes = 0
-        for a, e in (self._upload_runs(live) if dev is None else ()):
-          self.u8[slot][a:e].copy_(self.h_u8[slot][a:e], non_blocking=True)
-          self._frame_bytes += e - a
-        if desc is not None:
-          self.d_frames[slot].copy_(self.h_frames[slot], non_blocking=True)
-          self._frame_bytes += len(desc)
-        if maps is not None:
-          self.d_map[slot].copy_(self.h_map[slot], non_blocking=True)
-          self._frame_bytes += len(maps)
+      self._frame_bytes = 0                          # the used bytes only, and the descriptors when they changed
+      for a, e in (self._upload_runs(live) if dev is None else ()):
+        self.u8[slot][a:e].copy_(self.h_u8[slot][a:e], non_blocking=True)
+        self._frame_bytes += e - a
+      if desc is not None:
+        self.d_frames[slot].copy_(self.h_frames[slot], non_blocking=True)
+        self._frame_bytes += len(desc)
+      if maps is not None:
+        self.d_map[slot].copy_(self.h_map[slot], non_blocking=True)
+        self._frame_bytes += len(maps)
       if use_hm:
         self.hm[slot][:self.B].copy_(src_hm, non_blocking=True)
       if pub is not None:

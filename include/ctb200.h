@@ -32,11 +32,12 @@
  *                     ct_flip_merge_heads merges every head of B pairs at once, ct_mirror_x mirrors the --flip_test
  *                     batch's second half (detector.py:225-226,285-286).
  *   ct_warp_affine_normalize   Detector.pre_process's cv2.warpAffine + normalise + HWC->CHW, detector.py:207-226.
- *   ct_pack_stem_frames        the same for B ragged uint8 frames and their previous frames, written as the packed
- *                     input of the tensor-core stem (no fp32 image in between); ct_pack_stem_frames_flip also writes
- *                     each stream's mirror image for --flip_test.  The _dev forms and ct_warp_frames_normalize read
- *                     the descriptors from device memory (frame sizes that change between graph replays), and take
- *                     NV12 / I420 frames too: cv2.cvtColor(COLOR_YUV2BGR_NV12 / _I420) fused into the warp's taps.
+ *   ct_pack_stem_frames_dev    the same for B ragged uint8 frames and their previous frames, written as the packed
+ *                     input of the tensor-core stem (no fp32 image in between); ct_pack_stem_frames_flip_dev also
+ *                     writes each stream's mirror image for --flip_test; ct_warp_frames_normalize warps them into an
+ *                     fp32 image.  The descriptors live in device memory (frame sizes that change between graph
+ *                     replays), and may name NV12 / I420 frames: cv2.cvtColor(COLOR_YUV2BGR_NV12 / _I420) fused into
+ *                     the warp's taps.
  *   ct_stage_frames            copies B decoder frames already in device memory (BGR / RGB / planar RGB, NV12, I420
  *                     planes at any pitch) into a frame slot in that slot's layout, so the kernels above read them as
  *                     uploaded frames.
@@ -50,7 +51,7 @@
 extern "C" {
 #endif
 
-#define CTB200_ABI_VERSION 1
+#define CTB200_ABI_VERSION 2
 
 typedef enum {
   CT_OK = 0,
@@ -455,37 +456,29 @@ typedef struct {
   int64_t offset;             /* byte offset of the frame in the buffer (StreamRunner aligns it to 16 bytes) */
   int32_t h, w, step;         /* source rows, columns, row pitch in bytes (BGR: >= 3 w; YUV: the luma pitch, >= w,
                                  the chroma rows start at offset + h step) */
-  int32_t format;             /* CT_FRAME_*; the by-value entry points take CT_FRAME_BGR only */
+  int32_t format;             /* CT_FRAME_* */
   double  minv[6];            /* dst -> src map, inverted exactly as cv::warpAffine inverts it (see above) */
 } ct_frame;
 
-/* Streams per kernel launch of ct_pack_stem_frames (the descriptors travel in the kernel parameters). */
+/* Streams per kernel launch of the entry points that take a HOST array of descriptors (ct_stage_frames): they travel
+ * in the kernel parameters. */
 #define CT_FRAMES_PER_LAUNCH 48
 
 /* out bf16 NHWC [B,H,W,8] = (norm(warp(cur_b)) x3, norm(warp(prev_b)) x3, pre_hm_b, 0): the tensor-core stem's input,
  * byte-identical to ct_warp_affine_normalize of each stream followed by ct_pack_stem_input.  cur / prev: device buffers
- * holding each stream's frame at frames[b].offset (the same descriptor is used for both); prev == NULL or
- * pre_hm == NULL (fp32 [B,1,H,W]) give zeros.  frames: HOST array [B] of CT_FRAME_BGR frames (another format is
- * CT_ERR_INVALID), read during the call and passed to the kernels by value (a captured CUDA graph keeps them); one
- * launch per CT_FRAMES_PER_LAUNCH streams.  mean / std host fp32[3]. */
-int ct_pack_stem_frames(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames, int32_t B, const float* mean,
-                        const float* std, const float* pre_hm, void* out, int32_t H, int32_t W, void* stream);
-/* --flip_test: ct_pack_stem_frames into out [2B,H,W,8] whose image B+b is image b mirrored along W (out[B+b][y][W-1-x]
- * = out[b][y][x]), as if frame, previous frame and pre_hm had all been mirrored.  Same arguments; pre_hm stays [B,1,H,W]
- * (un-mirrored). */
-int ct_pack_stem_frames_flip(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames, int32_t B,
-                             const float* mean, const float* std, const float* pre_hm, void* out, int32_t H, int32_t W,
-                             void* stream);
-
-/* Device-resident descriptors: the output of ct_pack_stem_frames(_flip), byte for byte, with frames_dev a DEVICE array
- * ct_frame[B] read by the kernel (a replayed CUDA graph reads whatever geometry it holds then) in one launch.  cur and
- * prev are buf_bytes long each.  Each descriptor may have any CT_FRAME_* format (one launch may mix them); a YUV frame
- * gives exactly what its cv2.cvtColor BGR image gives, zero border included.  A descriptor with h <= 0, w <= 0,
- * offset < 0, an unknown format, step < 3 w (BGR) or < w (YUV), an odd h or w (YUV), or a frame extending past
- * buf_bytes gives zeros for its stream (in both images under _flip) and reads nothing of cur / prev. */
+ * of buf_bytes each, holding each stream's frame at frames_dev[b].offset (the same descriptor is used for both);
+ * prev == NULL or pre_hm == NULL (fp32 [B,1,H,W]) give zeros.  frames_dev: DEVICE array ct_frame[B], read by the
+ * kernel (a replayed CUDA graph reads whatever geometry it holds then); one launch.  Each descriptor may have any
+ * CT_FRAME_* format (one launch may mix them); a YUV frame gives exactly what its cv2.cvtColor BGR image gives, zero
+ * border included.  A descriptor with h <= 0, w <= 0, offset < 0, an unknown format, step < 3 w (BGR) or < w (YUV), an
+ * odd h or w (YUV), or a frame extending past buf_bytes gives zeros for its stream (in both images under _flip) and
+ * reads nothing of cur / prev.  mean / std host fp32[3]. */
 int ct_pack_stem_frames_dev(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames_dev, int32_t B,
                             int64_t buf_bytes, const float* mean, const float* std, const float* pre_hm, void* out,
                             int32_t H, int32_t W, void* stream);
+/* --flip_test: ct_pack_stem_frames_dev into out [2B,H,W,8] whose image B+b is image b mirrored along W
+ * (out[B+b][y][W-1-x] = out[b][y][x]), as if frame, previous frame and pre_hm had all been mirrored.  Same arguments;
+ * pre_hm stays [B,1,H,W] (un-mirrored). */
 int ct_pack_stem_frames_flip_dev(const uint8_t* cur, const uint8_t* prev, const ct_frame* frames_dev, int32_t B,
                                  int64_t buf_bytes, const float* mean, const float* std, const float* pre_hm, void* out,
                                  int32_t H, int32_t W, void* stream);

@@ -25,7 +25,7 @@ def test_library_exports_every_declared_symbol(built_lib):
   for name in _declared():
     assert hasattr(lib, name), 'libctb200.so does not export %s' % name
   lib.ct_abi_version.restype = ctypes.c_int
-  assert lib.ct_abi_version() == 1
+  assert lib.ct_abi_version() == 2
 
 
 def test_python_binding_lists_match_header(built_lib):

@@ -19,8 +19,7 @@ def _runner(sizes, H=544, W=960, max_frame_size=(1080, 1920), cfg='mot'):
   r.B, r.H, r.W, r.opt = len(sizes), H, W, make_opt(cfg)
   r.frames_mode, r.tracker, r.t = True, None, 0
   r._frame_geometry(sizes, None, max_frame_size)
-  if r.cap is not None:
-    r._desc_mirror = [bytes(r.frames)] * 3
+  r._desc_mirror = [bytes(r.frames)] * 3
   return r
 
 
@@ -106,6 +105,9 @@ def test_slot_layout_and_upload_runs():
   assert full._upload_runs() == [(0, fixed.slot_bytes)]     # at capacity: the fixed runner's one copy
   odd = _runner([(301, 457), (301, 457)], max_frame_size=(301, 457))   # padded to 16 bytes: still one run
   assert odd.cap % 16 == 0 and odd._upload_runs() == [(0, 2 * odd.cap)]
+  ragged = _runner([(1080, 1920), (301, 457), (480, 640)], max_frame_size=None)   # fixed: contiguous ragged frames
+  assert [f.offset for f in ragged.frames] == [0, cap, cap + (301 * 457 * 3 + 15) // 16 * 16]
+  assert ragged._upload_runs() == [(0, ragged.slot_bytes)]
 
 
 def test_descriptors_upload_only_when_a_slot_changes():
@@ -118,6 +120,8 @@ def test_descriptors_upload_only_when_a_slot_changes():
     uploads.append(desc is not None)
   # the change at step 2 reaches slots 2, 0, 1 once each; steady state uploads nothing; step 6 changes slot 0 again
   assert uploads == [False, False, True, True, True, False, True]
+  fixed = _runner(MOT, max_frame_size=None)                 # its descriptors never change: never uploaded
+  assert all(fixed._plan_geometry(t % 3, {}, {})[0] is None for t in range(6))
 
 
 def test_meta_and_previous_meta_follow_each_frame():

@@ -1,6 +1,6 @@
 """-m gpu: --flip_test in StreamRunner -- each stream's frame and its mirror in one batched step of 2B images, merged on
 the device.  The kernels against their one-pair / unfused forms bit for bit (ct_flip_merge_heads, ct_mirror_x,
-ct_pack_stem_frames_flip); each stream of a flip runner against Detector.process with --flip_test, bit for bit; the
+ct_pack_stem_frames_flip_dev); each stream of a flip runner against Detector.process with --flip_test, bit for bit; the
 closed loop against the host pipeline; video starts against a fresh flip runner."""
 import ctypes as C
 
@@ -104,11 +104,13 @@ def _pack_flip_check(opt, cur, prev, frames, nb, hh, ww, hm):
   std = np.ascontiguousarray(ds.std, np.float32).reshape(3)
   ms = C.c_void_p(mean.ctypes.data), C.c_void_p(std.ctypes.data)
   lib, st = L.lib(), L.stream_ptr()
+  fdev = torch.frombuffer(bytearray(bytes(frames)), dtype=torch.uint8).to(DEV)
+  args = L.ptr(fdev), nb, cur.numel()
   for name, pv, h in (('first', cur, hm), ('no_prev', None, hm), ('no_hm', prev, None), ('both', prev, hm)):
     ref = torch.full((nb, hh, ww, 8), 7.0, dtype=torch.bfloat16, device=DEV)
     got = torch.full((2 * nb, hh, ww, 8), -7.0, dtype=torch.bfloat16, device=DEV)
-    L.check(lib.ct_pack_stem_frames(L.ptr(cur), L.ptr(pv), frames, nb, *ms, L.ptr(h), L.ptr(ref), hh, ww, st))
-    L.check(lib.ct_pack_stem_frames_flip(L.ptr(cur), L.ptr(pv), frames, nb, *ms, L.ptr(h), L.ptr(got), hh, ww, st))
+    L.check(lib.ct_pack_stem_frames_dev(L.ptr(cur), L.ptr(pv), *args, *ms, L.ptr(h), L.ptr(ref), hh, ww, st))
+    L.check(lib.ct_pack_stem_frames_flip_dev(L.ptr(cur), L.ptr(pv), *args, *ms, L.ptr(h), L.ptr(got), hh, ww, st))
     torch.cuda.synchronize()
     want = torch.cat((ref, ref.flip(2)), 0)
     eq = _bits(got) == _bits(want)
@@ -116,9 +118,9 @@ def _pack_flip_check(opt, cur, prev, frames, nb, hh, ww, hm):
 
 
 @pytest.mark.parametrize('out_hw', [(544, 960), (384, 1280)])
-def test_flip_pack_equals_pack_then_mirror_byte_for_byte(out_hw):
-  """ct_pack_stem_frames_flip == ct_pack_stem_frames followed by a flip of each packed [H, W, 8] image along W, on the
-  ragged streams of the unfused-pack test (odd width, padded pitch), with and without prev / pre_hm."""
+def test_dev_flip_pack_equals_dev_pack_then_mirror_byte_for_byte(out_hw):
+  """ct_pack_stem_frames_flip_dev == ct_pack_stem_frames_dev followed by a flip of each packed [H, W, 8] image along
+  W, on the ragged streams of the unfused-pack test (odd width, padded pitch), with and without prev / pre_hm."""
   hh, ww = out_hw
   opt = make_opt('mot', ['--input_h', str(hh), '--input_w', str(ww)])
   streams = [(1080, 1920, 5760), (480, 640, 1920), (375, 1242, 3726), (544, 960, 2880), (301, 457, 1392)]
@@ -127,11 +129,11 @@ def test_flip_pack_equals_pack_then_mirror_byte_for_byte(out_hw):
   _pack_flip_check(opt, cur, prev, frames, len(streams), hh, ww, hm)
 
 
-def test_flip_pack_over_several_launches():
-  """B = CT_FRAMES_PER_LAUNCH + 5 streams (two launches of the descriptors), odd output width."""
+def test_flip_pack_of_many_streams():
+  """B = 53 streams of small ragged frames, odd output width."""
   hh, ww = 48, 77
   opt = make_opt('mot', ['--input_h', str(hh), '--input_w', str(ww)])
-  nb = L.CT_FRAMES_PER_LAUNCH + 5
+  nb = 53
   streams = [((40, 66, 198), (31, 57, 176), (48, 77, 231))[b % 3] for b in range(nb)]
   cur, prev, frames, _ = _ragged(opt, streams, 23)
   hm = torch.rand((nb, 1, hh, ww), device=DEV)

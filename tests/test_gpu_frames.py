@@ -1,5 +1,5 @@
 """-m gpu: StreamRunner's frames mode -- raw uint8 camera frames of per-stream sizes warped, normalised and packed on the
-device (ct_pack_stem_frames on the bf16 engine, ct_warp_affine_normalize per stream on the others), tracks in each
+device (ct_pack_stem_frames_dev on the bf16 engine, ct_warp_frames_normalize on the others), tracks in each
 stream's source pixels.  Against the unfused kernels byte for byte, against a runner fed the fp32 images of the host
 pre_process (cv2) bit for bit, and closed-loop against the host pipeline."""
 import ctypes as C
@@ -61,7 +61,7 @@ def _ragged(opt, streams, seed):
 
 
 @pytest.mark.parametrize('out_hw', [(544, 960), (384, 1280)])
-def test_pack_stem_frames_equals_warp_then_pack_byte_for_byte(out_hw):
+def test_dev_pack_equals_warp_then_pack_byte_for_byte(out_hw):
   """Ragged streams in one call -- 1080x1920, 480x640, KITTI's 375x1242 (zero border), 544x960 (the identity map at
   544x960), an odd width with a padded row pitch -- against ct_warp_affine_normalize per stream + ct_pack_stem_input,
   for the first frame (prev = cur), no previous frame, no pre_hm, and both present."""
@@ -86,12 +86,14 @@ def test_pack_stem_frames_equals_warp_then_pack_byte_for_byte(out_hw):
     return img
 
   img_cur, img_prev = warped(cur), warped(prev)
+  frames_dev = torch.frombuffer(bytearray(bytes(frames)), dtype=torch.uint8).to(DEV)
   for name, pv, pre_img, h in (('first', cur, img_cur, hm), ('no_prev', None, None, hm),
                                ('no_hm', prev, img_prev, None), ('both', prev, img_prev, hm)):
     ref = torch.full((B, H, W, 8), 7.0, dtype=torch.bfloat16, device=DEV)
     got = torch.full((B, H, W, 8), -7.0, dtype=torch.bfloat16, device=DEV)
     L.check(lib.ct_pack_stem_input(L.ptr(img_cur), L.ptr(pre_img), L.ptr(h), L.ptr(ref), B, H, W, st))
-    L.check(lib.ct_pack_stem_frames(L.ptr(cur), L.ptr(pv), frames, B, *ms, L.ptr(h), L.ptr(got), H, W, st))
+    L.check(lib.ct_pack_stem_frames_dev(L.ptr(cur), L.ptr(pv), L.ptr(frames_dev), B, cur.numel(), *ms, L.ptr(h),
+                                        L.ptr(got), H, W, st))
     torch.cuda.synchronize()
     eq = got.view(torch.int16) == ref.view(torch.int16)
     assert bool(eq.all()), (name, int((~eq).sum()), [int((~eq[b]).sum()) for b in range(B)])
@@ -126,7 +128,7 @@ def test_frames_mode_records_equal_the_fp32_image_runner(precision, graph):
   ref = StreamRunner(model, B, H, W, **kw)
   for r in (fr, ref):
     r.warm()
-  want_launches = ref.launches_per_step + (0 if precision == 'bf16' else B)
+  want_launches = ref.launches_per_step + (0 if precision == 'bf16' else 1)
   assert fr.launches_per_step == want_launches
   assert fr.h2d_bytes_per_step == sum((h * w * 3 + 15) // 16 * 16 for h, w in SIZES) + B * H * W * 4
   for t in range(5):

@@ -1,7 +1,7 @@
 """-m gpu: the device pre_process and prior heat-map against the CPU oracle with no tolerance.
 
 Every entry point of the one warp (`warp_bilinear_u8`) -- ct_warp_affine_normalize, ct_warp_frames_normalize,
-ct_pack_stem_frames, ct_pack_stem_frames_flip and their _dev forms -- on every resolution policy over camera frame sizes
+ct_pack_stem_frames_dev and ct_pack_stem_frames_flip_dev -- on every resolution policy over camera frame sizes
 and on adversarial inverse maps, against ct_oracle.warp_affine_u8 (itself equal to cv2.warpAffine byte for byte:
 tests/test_warp_oracle.py): fp32 compared as int32 bits, bf16 as int16 bits.  Both splats, ct_render_pre_hm and
 ct_render_tracks, against draw_umich_gaussian into an fp32 map; the render boxes ct_track_start and ct_track_step write
@@ -99,8 +99,8 @@ def test_warp_affine_normalize_batch_with_a_map_per_image():
 
 # ------------------------------------------------------------------- ragged frames: the pack and frames entry points
 def _ragged(streams, seed):
-  """streams: [(image (h, w), row pitch, minv)] -> (cur, prev device buffers, host ct_frame array, device ct_frame
-  array, buffer bytes, [cur image], [prev image])."""
+  """streams: [(image (h, w), row pitch, minv)] -> (cur, prev device buffers, device ct_frame array, buffer bytes,
+  [cur image], [prev image])."""
   frames = (L.Frame * len(streams))()
   bufs, cur, prev = [bytearray(), bytearray()], [], []
   for b, ((h, w), pitch, minv) in enumerate(streams):
@@ -113,7 +113,7 @@ def _ragged(streams, seed):
     f.minv[:] = [float(v) for v in minv]
   dev = [torch.frombuffer(bytearray(bb), dtype=torch.uint8).to(DEV) for bb in bufs]
   fdev = torch.frombuffer(bytearray(bytes(frames)), dtype=torch.uint8).to(DEV)
-  return dev[0], dev[1], frames, fdev, len(bufs[0]), cur, prev
+  return dev[0], dev[1], fdev, len(bufs[0]), cur, prev
 
 
 def _mot_streams(opt):
@@ -135,13 +135,13 @@ def _group(name):
 
 
 @pytest.mark.parametrize('group', GROUPS)
-def test_frame_entry_points_equal_the_oracle(group):
+def test_device_descriptor_entry_points_equal_the_oracle(group):
   """Ragged buffers mixing camera sizes (odd and padded pitches, 1 x N and N x 1 frames) or the adversarial maps given
-  through ct_frame.minv, one descriptor per stream: ct_warp_frames_normalize, ct_pack_stem_frames (with and without
-  the previous frame and pre_hm), ct_pack_stem_frames_flip (both halves) and the two _dev packs."""
+  through ct_frame.minv, one descriptor per stream: ct_warp_frames_normalize, ct_pack_stem_frames_dev (with and
+  without the previous frame and pre_hm) and ct_pack_stem_frames_flip_dev (both halves)."""
   streams, (H, W) = _group(group)
   B = len(streams)
-  cur, prev, frames, fdev, nbytes, cur_imgs, prev_imgs = _ragged(streams, 500)
+  cur, prev, fdev, nbytes, cur_imgs, prev_imgs = _ragged(streams, 500)
   want_cur = [_want_chw(im, s[2], H, W) for im, s in zip(cur_imgs, streams)]
   want_prev = [_want_chw(im, s[2], H, W) for im, s in zip(prev_imgs, streams)]
   hm = torch.rand((B, 1, H, W), device=DEV)
@@ -153,45 +153,40 @@ def test_frame_entry_points_equal_the_oracle(group):
   for b in range(B):
     _check_bits(img[b], want_cur[b], (group, 'warp_frames', b))
 
-  def packed(fn, flip, pv, h, dev_desc):
+  def packed(fn, flip, pv, h):
     out = torch.full(((2 if flip else 1) * B, H, W, 8), -7.0, dtype=torch.bfloat16, device=DEV)
-    if dev_desc:
-      L.check(fn(L.ptr(cur), L.ptr(pv), L.ptr(fdev), B, nbytes, *MS, L.ptr(h), L.ptr(out), H, W, st))
-    else:
-      L.check(fn(L.ptr(cur), L.ptr(pv), frames, B, *MS, L.ptr(h), L.ptr(out), H, W, st))
+    L.check(fn(L.ptr(cur), L.ptr(pv), L.ptr(fdev), B, nbytes, *MS, L.ptr(h), L.ptr(out), H, W, st))
     return out
 
-  for fname, flip, dev_desc in (('ct_pack_stem_frames', False, False), ('ct_pack_stem_frames_flip', True, False),
-                                ('ct_pack_stem_frames_dev', False, True), ('ct_pack_stem_frames_flip_dev', True, True)):
-    out = packed(getattr(lib, fname), flip, prev, hm, dev_desc)
+  for fname, flip in (('ct_pack_stem_frames_dev', False), ('ct_pack_stem_frames_flip_dev', True)):
+    out = packed(getattr(lib, fname), flip, prev, hm)
     for b in range(B):
       want = co.stem_pixels(want_cur[b], want_prev[b], hm_np[b, 0], flip=flip)
       _check_bits(out[b], want[0] if flip else want, (group, fname, b))
       if flip:
         _check_bits(out[B + b], want[1], (group, fname, 'mirror', b))
-  out = packed(lib.ct_pack_stem_frames, False, None, None, False)
+  out = packed(lib.ct_pack_stem_frames_dev, False, None, None)
   for b in range(B):
     _check_bits(out[b], co.stem_pixels(want_cur[b], None, None), (group, 'no prev, no pre_hm', b))
 
 
 @pytest.mark.parametrize('B', [49, 97])
-def test_by_value_packs_across_launch_chunks(B):
-  """More streams than CT_FRAMES_PER_LAUNCH (48) descriptors per launch: the by-value packs split the batch into
-  launches of 48; every stream of every launch, small ragged frames, 32 x 48 output."""
+def test_dev_packs_of_many_ragged_streams(B):
+  """Many streams of small ragged frames in one launch of each _dev pack: every stream, 32 x 48 output."""
   from centertrack_b200.detector import frame_geometry
-  assert L.CT_FRAMES_PER_LAUNCH == 48
   opt = make_opt('coco_tracking', ['--input_h', '32', '--input_w', '48'])
   sizes = [(5, 7), (17, 23), (31, 40), (1, 1), (1, 9), (12, 1), (40, 64), (33, 47), (20, 30), (48, 32), (9, 61)]
   streams = [(hw, 3 * hw[1] + (b % 3) * 5, frame_geometry(opt, *hw)[1])
              for b, hw in ((b, sizes[b % len(sizes)]) for b in range(B))]
-  cur, prev, frames, _, _, cur_imgs, prev_imgs = _ragged(streams, 900 + B)
+  cur, prev, fdev, nbytes, cur_imgs, prev_imgs = _ragged(streams, 900 + B)
   H, W = 32, 48
   hm = torch.rand((B, 1, H, W), device=DEV)
   hm_np = hm.cpu().numpy()
   lib, st = L.lib(), L.stream_ptr()
-  for fname, flip in (('ct_pack_stem_frames', False), ('ct_pack_stem_frames_flip', True)):
+  for fname, flip in (('ct_pack_stem_frames_dev', False), ('ct_pack_stem_frames_flip_dev', True)):
     out = torch.full(((2 if flip else 1) * B, H, W, 8), -7.0, dtype=torch.bfloat16, device=DEV)
-    L.check(getattr(lib, fname)(L.ptr(cur), L.ptr(prev), frames, B, *MS, L.ptr(hm), L.ptr(out), H, W, st))
+    L.check(getattr(lib, fname)(L.ptr(cur), L.ptr(prev), L.ptr(fdev), B, nbytes, *MS, L.ptr(hm), L.ptr(out), H, W,
+                                st))
     for b, (_, _, minv) in enumerate(streams):
       want = co.stem_pixels(_want_chw(cur_imgs[b], minv, H, W), _want_chw(prev_imgs[b], minv, H, W), hm_np[b, 0],
                             flip=flip)

@@ -1,6 +1,5 @@
 """NV12 / I420 camera frames in StreamRunner, on the host (no GPU): the YUV reference against cv2.cvtColor byte for
-byte, a 4:2:0 runner's frame shapes, slot layout, upload runs and staging views, its argument checks, and the by-value
-entry points' refusal of a YUV descriptor."""
+byte, a 4:2:0 runner's frame shapes, slot layout, upload runs and staging views, and its argument checks."""
 import ctypes as C
 
 import cv2
@@ -169,19 +168,3 @@ def test_track_videos_sizes_4_2_0_frames():
   assert set(seen) == {A, Bs}
   with pytest.raises(ValueError, match='not a NV12 frame'):
     list(track_videos(Fake([A, A], 10 ** 6), [dict(id='bgr', frames=[np.zeros((12, 20, 3), np.uint8)])]))
-
-
-# ------------------------------------------------------------------------------------------ entry point checks
-def test_by_value_entry_points_refuse_yuv_descriptors_without_a_gpu(built_lib):
-  lib = L.lib()
-  p = C.c_void_p(256)
-  mean, std = np.zeros(3, np.float32), np.ones(3, np.float32)
-  ms = C.c_void_p(mean.ctypes.data), C.c_void_p(std.ctypes.data)
-  for fmt in (L.CT_FRAME_NV12, L.CT_FRAME_I420, 7):
-    frames = (L.Frame * 2)()
-    for f in frames:
-      f.h, f.w, f.step = 4, 4, 12
-    frames[1].format = fmt
-    for fn in (lib.ct_pack_stem_frames, lib.ct_pack_stem_frames_flip):
-      rc = fn(p, None, frames, 2, *ms, None, p, 8, 8, None)
-      assert rc == L.CT_ERR_INVALID and b'CT_FRAME_BGR only' in lib.ct_last_error(), lib.ct_last_error()

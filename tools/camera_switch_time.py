@@ -1,9 +1,8 @@
 """Cost and benefit of StreamRunner streams that change frame size at a video start (max_frame_size):
     python tools/camera_switch_time.py [--B 32] [--steps 40] [--rounds 7] [--videos 64] [--min_len 100] [--max_len 400]
 
-1. device time per call of ct_pack_stem_frames_dev (descriptors in device memory) against ct_pack_stem_frames
-   (descriptors in the kernel parameters), B streams, mot 1920x1080 -> 544x960 and KITTI 1242x375 ->
-   384x1280, CUDA events around 50 calls, alternating rounds, medians;
+1. device time per call of ct_pack_stem_frames_dev, B streams, mot 1920x1080 -> 544x960 and KITTI 1242x375 ->
+   384x1280, CUDA events around 50 calls, medians over rounds;
 2. steady-state frames/s of a capacity runner (max_frame_size = 1080x1920) against a fixed runner, B uniform 1920x1080
    streams, --config mot, bf16, device tracking, graphs; alternating rounds of `steps` steps, medians and the spread;
 3. a MOT17-style schedule through track_videos: `videos` synthetic videos of min_len..max_len frames, a quarter of them
@@ -55,24 +54,23 @@ def pack_times(cfg, B, rounds, n=50):
   std = np.ascontiguousarray(ds.std, np.float32).reshape(3)
   ms = C.c_void_p(mean.ctypes.data), C.c_void_p(std.ctypes.data)
   lib = L.lib()
-  arms = {'by_value': lambda: L.check(lib.ct_pack_stem_frames(L.ptr(cur), L.ptr(prev), frames, B, *ms, L.ptr(hm),
-                                                              L.ptr(out), H, W, L.stream_ptr())),
-          'device': lambda: L.check(lib.ct_pack_stem_frames_dev(L.ptr(cur), L.ptr(prev), L.ptr(dfr), B, cur.numel(),
-                                                                *ms, L.ptr(hm), L.ptr(out), H, W, L.stream_ptr()))}
-  for fn in arms.values():
-    fn()
+
+  def pack():
+    L.check(lib.ct_pack_stem_frames_dev(L.ptr(cur), L.ptr(prev), L.ptr(dfr), B, cur.numel(), *ms, L.ptr(hm),
+                                        L.ptr(out), H, W, L.stream_ptr()))
+
+  pack()
   torch.cuda.synchronize()
-  t = {k: [] for k in arms}
+  t = []
   for _ in range(rounds):
-    for k, fn in arms.items():
-      e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-      e0.record()
-      for _ in range(n):
-        fn()
-      e1.record()
-      torch.cuda.synchronize()
-      t[k].append(e0.elapsed_time(e1) / n)
-  return {'source': [h, w], 'input': [H, W], 'ms_per_call': {k: float(np.median(v)) for k, v in t.items()}}
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(n):
+      pack()
+    e1.record()
+    torch.cuda.synchronize()
+    t.append(e0.elapsed_time(e1) / n)
+  return {'source': [h, w], 'input': [H, W], 'ms_per_call': float(np.median(t))}
 
 
 def steady_state(model, opt, B, steps, rounds):
@@ -166,8 +164,8 @@ def main():
   print('card:', dev)
   res = {'card': dev, 'B': a.B, 'pack': {cfg: pack_times(cfg, a.B, a.rounds) for cfg in KERNEL_CASES}}
   for cfg, r in res['pack'].items():
-    print('%s %s -> %s, B=%d: ct_pack_stem_frames %.3f ms, ct_pack_stem_frames_dev %.3f ms per call' %
-          (cfg, r['source'], r['input'], a.B, r['ms_per_call']['by_value'], r['ms_per_call']['device']))
+    print('%s %s -> %s, B=%d: ct_pack_stem_frames_dev %.3f ms per call' % (cfg, r['source'], r['input'], a.B,
+                                                                          r['ms_per_call']))
   opt, model, _ = make_model('mot')
   model = model.cuda()
   res['steady'] = steady_state(model, opt, a.B, a.steps, a.rounds)

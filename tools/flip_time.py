@@ -6,7 +6,7 @@ mot: 1920x1080 sources into 544x960), bf16 engine, device tracking, frames writt
 1. end-to-end frames/s of a flip runner (2B images per step) against a runner without the flip, timed alternately,
    `rounds` rounds of `steps` steps each (host clock around steps that end in a sync).  B is --B, or the largest
    halving of it whose runners fit in device memory;
-2. device time per call of ct_pack_stem_frames_flip against ct_pack_stem_frames on the same slot data, and of one
+2. device time per call of ct_pack_stem_frames_flip_dev against ct_pack_stem_frames_dev on the same slot data, and of one
    ct_flip_merge_heads launch against the per-head, per-pair ct_flip_merge launches it replaces, CUDA events around
    50 calls, alternating rounds.
 Prints the card and its power limit with the numbers, and one JSON line.  Needs a GPU."""
@@ -98,10 +98,11 @@ def kernel_times(fl, rounds):
         L.check(lib.ct_flip_merge(L.ptr(t[b]), L.ptr(one[h]), t.shape[2], t.shape[3], t.shape[4], L.ptr(perm),
                                   L.ptr(sign), L.stream_ptr()))
 
-  fns = {'ct_pack_stem_frames_flip': lambda: L.check(lib.ct_pack_stem_frames_flip(
-             L.ptr(cur), L.ptr(prev), fl.frames, B, *ms, L.ptr(hm), L.ptr(stem), H, W, L.stream_ptr())),
-         'ct_pack_stem_frames': lambda: L.check(lib.ct_pack_stem_frames(
-             L.ptr(cur), L.ptr(prev), fl.frames, B, *ms, L.ptr(hm), L.ptr(stem), H, W, L.stream_ptr())),
+  desc = L.ptr(fl.d_frames[1]), B, fl.slot_bytes
+  fns = {'ct_pack_stem_frames_flip_dev': lambda: L.check(lib.ct_pack_stem_frames_flip_dev(
+             L.ptr(cur), L.ptr(prev), *desc, *ms, L.ptr(hm), L.ptr(stem), H, W, L.stream_ptr())),
+         'ct_pack_stem_frames_dev': lambda: L.check(lib.ct_pack_stem_frames_dev(
+             L.ptr(cur), L.ptr(prev), *desc, *ms, L.ptr(hm), L.ptr(stem), H, W, L.stream_ptr())),
          'ct_flip_merge_heads (1 launch)': lambda: flip_output(outs, fl.flip_plan, fl.merged),
          'ct_flip_merge (%d launches)' % (len(fl.flip_plan) * B): per_head}
   return events(fns, rounds)

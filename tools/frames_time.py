@@ -1,16 +1,16 @@
 """Cost of StreamRunner's frames mode (raw uint8 camera frames in, the warp + normalise + stem packing on the device):
-    python tools/frames_time.py [--config mot coco_tracking] [--B 32] [--steps 40] [--rounds 3]
+    python tools/frames_time.py [--config mot coco_tracking] [--B 32] [--steps 40] [--rounds 3] [--precision bf16]
 
-Per config (mot: 1920x1080 sources into the 544x960 input; coco_tracking: 640x480 sources into 512x512), bf16 engine,
-device tracking, B streams, one graph replay per step:
+Per config (mot: 1920x1080 sources into the 544x960 input; coco_tracking: 640x480 sources into 512x512), the bf16
+engine (or --precision's), device tracking, B streams, one graph replay per step:
 1. end-to-end frames/s of step_frames -- with the frames passed as arrays (copied into the pinned staging) and written
    in place through frame_buffers() -- against step_host fed the already pre-processed fp32 frames (pinned), the
    runners timed alternately, `rounds` rounds of `steps` steps each (host clock around steps that end in a sync);
 2. host CPU time (process time, every thread) of Detector.pre_process (cv2.warpAffine + normalise + HWC->CHW) per
    source frame, for context;
-3. device time per call of ct_pack_stem_frames against B x ct_warp_affine_normalize + ct_pack_stem_input (the unfused
-   path of the fp32-image runner, whose previous image is already warped), CUDA events around 50 calls, alternating
-   rounds.
+3. bf16: device time per call of ct_pack_stem_frames_dev against ct_warp_frames_normalize + ct_pack_stem_input (the
+   unfused path of the fp32-image runner, whose previous image is already warped); bf16x3 and fp32: of the runner's
+   ct_warp_frames_normalize.  CUDA events around 50 calls, alternating rounds.
 Prints the card and its power limit with the numbers, and one JSON line.  Needs a GPU."""
 import argparse
 import ctypes as C
@@ -71,26 +71,28 @@ def time_steps(fn, steps, runner):
 
 
 def kernel_times(runner, rounds, n=50):
-  """ms per call: fused ct_pack_stem_frames vs B x ct_warp_affine_normalize + ct_pack_stem_input, same slot data."""
+  """ms per call, same slot data.  bf16: the fused ct_pack_stem_frames_dev vs ct_warp_frames_normalize +
+  ct_pack_stem_input; bf16x3 and fp32: the runner's ct_warp_frames_normalize."""
   lib, eng, B, H, W = L.lib(), runner.eng, runner.B, runner.H, runner.W
   ms = C.c_void_p(runner.mean.ctypes.data), C.c_void_p(runner.std.ctypes.data)
   cur, prev, hm = runner.u8[1], runner.u8[0], runner.hm[1]
   img, pre = runner.img[1], runner.img[0]
 
   def fused():
-    L.check(lib.ct_pack_stem_frames(L.ptr(cur), L.ptr(prev), runner.frames, B, *ms, L.ptr(hm), L.ptr(eng.stem_input),
-                                    H, W, L.stream_ptr()))
+    L.check(lib.ct_pack_stem_frames_dev(L.ptr(cur), L.ptr(prev), L.ptr(runner.d_frames[1]), B, runner.slot_bytes, *ms,
+                                        L.ptr(hm), L.ptr(eng.stem_input), H, W, L.stream_ptr()))
 
   def unfused():
     runner._warp_frames(1)
     L.check(lib.ct_pack_stem_input(L.ptr(img), L.ptr(pre), L.ptr(hm), L.ptr(eng.stem_input), B, H, W, L.stream_ptr()))
 
-  out = {'fused': [], 'unfused': []}
-  for fn in (fused, unfused):
+  arms = (('fused', fused), ('unfused', unfused)) if eng.use_halo else (('warp', lambda: runner._warp_frames(1)),)
+  out = {name: [] for name, _ in arms}
+  for _, fn in arms:
     fn()
   torch.cuda.synchronize()
   for _ in range(rounds):
-    for name, fn in (('fused', fused), ('unfused', unfused)):
+    for name, fn in arms:
       e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
       e0.record()
       for _ in range(n):
@@ -101,7 +103,7 @@ def kernel_times(runner, rounds, n=50):
   return {k: float(np.median(v)) for k, v in out.items()}
 
 
-def run_config(cfg, B, steps, rounds):
+def run_config(cfg, B, steps, rounds, precision):
   from centertrack_b200.runner import StreamRunner
   h, w = SOURCES[cfg]
   opt, model, _ = make_model(cfg)
@@ -109,7 +111,7 @@ def run_config(cfg, B, steps, rounds):
   H, W = opt.input_h, opt.input_w
   sizes = [(h, w)] * B
   frames = [frame(h, w, 10 + b) for b in range(B)]
-  kw = dict(K=100, precision='bf16', device='cuda', opt=opt, device_tracking=True)
+  kw = dict(K=100, precision=precision, device='cuda', opt=opt, device_tracking=True)
   fr = StreamRunner(model, B, H, W, frame_sizes=sizes, **kw)
   hr = StreamRunner(model, B, H, W, **kw)
   for r in (fr, hr):
@@ -139,7 +141,7 @@ def run_config(cfg, B, steps, rounds):
   kern = kernel_times(fr, rounds)
   src_mb = h * w * 3 / 1e6
   img_mb = 3 * H * W * 4 / 1e6
-  res = {'config': cfg, 'B': B, 'source': [h, w], 'input': [H, W], 'frames_per_s': fps,
+  res = {'config': cfg, 'precision': precision, 'B': B, 'source': [h, w], 'input': [H, W], 'frames_per_s': fps,
          'pre_process_host_cpu_ms_per_frame': pre_ms, 'kernel_ms': kern,
          'h2d_mb_per_frame': {'uint8 source': src_mb, 'fp32 image': img_mb},
          'h2d_bytes_per_step': {'frames': fr.h2d_bytes_per_step, 'fp32 images': hr.h2d_bytes_per_step},
@@ -153,21 +155,25 @@ def main():
   ap.add_argument('--B', type=int, default=32)
   ap.add_argument('--steps', type=int, default=40)
   ap.add_argument('--rounds', type=int, default=3)
+  ap.add_argument('--precision', default='bf16', choices=['bf16', 'bf16x3', 'fp32'])
   a = ap.parse_args()
   assert torch.cuda.is_available(), 'frames_time.py needs a GPU'
   dev = card()
   print('card:', dev)
   out = []
   for cfg in a.config:
-    r = run_config(cfg, a.B, a.steps, a.rounds)
+    r = run_config(cfg, a.B, a.steps, a.rounds, a.precision)
     out.append(r)
-    print('%s: B=%d, %dx%d sources -> %dx%d input' % (cfg, a.B, r['source'][0], r['source'][1], r['input'][0],
-                                                       r['input'][1]))
+    print('%s, %s: B=%d, %dx%d sources -> %dx%d input' % (cfg, a.precision, a.B, r['source'][0], r['source'][1],
+                                                           r['input'][0], r['input'][1]))
     for k, v in r['frames_per_s'].items():
       print('  %-28s %8.1f frames/s' % (k, v))
     print('  Detector.pre_process host CPU  %8.2f ms per frame' % r['pre_process_host_cpu_ms_per_frame'])
-    print('  ct_pack_stem_frames            %8.3f ms per call' % r['kernel_ms']['fused'])
-    print('  B x warp + ct_pack_stem_input  %8.3f ms per call' % r['kernel_ms']['unfused'])
+    if 'fused' in r['kernel_ms']:
+      print('  ct_pack_stem_frames_dev        %8.3f ms per call' % r['kernel_ms']['fused'])
+      print('  warp + ct_pack_stem_input      %8.3f ms per call' % r['kernel_ms']['unfused'])
+    else:
+      print('  ct_warp_frames_normalize       %8.3f ms per call' % r['kernel_ms']['warp'])
     print('  H2D per frame: uint8 %.2f MB, fp32 %.2f MB' % (r['h2d_mb_per_frame']['uint8 source'],
                                                            r['h2d_mb_per_frame']['fp32 image']))
   print(json.dumps({'card': dev, 'results': out}))

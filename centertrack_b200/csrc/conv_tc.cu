@@ -640,8 +640,12 @@ conv_tc_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
 // warpgroups finish the current one; at N <= 128 two CTAs share an SM and one CTA's epilogue runs under the other's MMAs.
 // (A separate producer warp would make 9 warps per CTA: the register file of an SM sub-partition then holds two such
 // CTAs only at 96 registers, where N = 128 spills.)
+// The epilogue stages 16 accumulator columns at a time (10 KB for both warpgroups instead of 18 KB for 32 columns): that
+// is what lets N = 128 hold 3 stages and N <= 64 hold 4 within the 113 KB of a CTA at two CTAs per SM.
 constexpr int TMA_THREADS = 256;
-constexpr int TMA_STAGING_BYTES = 2 * 64 * EPI_PITCH * 4;     // per warpgroup: 64 rows x 32 columns of fp32
+constexpr int TMA_EPI_COLS = 16;
+constexpr int TMA_EPI_PITCH = TMA_EPI_COLS + 4;               // floats per staging row: 16-byte reads conflict-free
+constexpr int TMA_STAGING_BYTES = 2 * 64 * TMA_EPI_PITCH * 4; // per warpgroup: 64 rows x 16 columns of fp32
 
 template <int N>
 __global__ void __launch_bounds__(TMA_THREADS, N <= 128 ? 2 : 1)
@@ -652,7 +656,7 @@ conv_tma_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int S = a.stages;
   constexpr uint32_t b_bytes = (uint32_t)N * 128u;
-  // smem: [A stages][B stages][staging 2 x 64 x EPI_PITCH fp32][full[S], empty[S]]
+  // smem: [A stages][B stages][staging 2 x 64 x TMA_EPI_PITCH fp32][full[S], empty[S]]
   const uint32_t sA = smem_u32(smem);
   const uint32_t sB = sA + S * A_STAGE_BYTES;
   const uint32_t sStg = sB + S * b_bytes;
@@ -698,7 +702,7 @@ conv_tma_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
   const int wg = warp >> 2, w4 = warp & 3;
   const int lrow = 32 * (w4 & 1) + lane;           // epilogue: row of this warpgroup's 64, 16-column half chalf
   const int chalf = w4 >> 1;
-  const uint32_t stg = sStg + (uint32_t)wg * (64u * EPI_PITCH * 4u);
+  const uint32_t stg = sStg + (uint32_t)wg * (64u * TMA_EPI_PITCH * 4u);
   float acc[N / 2];
   int it = 0;
   for (int item = blockIdx.x; item < items; item += gridDim.x) {
@@ -727,22 +731,24 @@ conv_tma_kernel(const TcArgs a, const __grid_constant__ CUtensorMap tmap) {
     if (lane == 0) mbar_arrive(empty_bar((it - 1) % S));
     if (tid == 0) load_next();
 
-    // ---- epilogue of this warpgroup's 64 rows, 32 accumulator columns at a time through its staging tile
+    // ---- epilogue of this warpgroup's 64 rows, 32 accumulator columns at a time: the two 16-column halves pass in turn
+    // through the staging tile, half h read by the threads with chalf == h, then every thread stores its 16 columns
     const int p = tc_pixel(a, mt, 64 * wg + lrow);
     const bool p_ok = p < g.P_out;
     const int n0 = nt * N;
 #pragma unroll
     for (int c0 = 0; c0 < N; c0 += 32) {
-      named_sync(1 + wg, 128);                     // the previous chunk's readers are done with the staging tile
-      stage_acc_chunk(acc, c0, stg, 0);
-      named_sync(1 + wg, 128);
+      float v[16];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        named_sync(1 + wg, 128);                   // the previous half's readers are done with the staging tile
+        stage_acc_chunk<N / 2, TMA_EPI_COLS, TMA_EPI_PITCH>(acc, c0 + h * TMA_EPI_COLS, stg, 0);
+        named_sync(1 + wg, 128);
+        if (chalf == h) lds_f(stg + (uint32_t)lrow * TMA_EPI_PITCH * 4u, v);
+      }
       const int col = c0 + chalf * 16;
       const int o0 = n0 + col;
-      if (col < N && p_ok && o0 < g.C_out) {
-        float v[16];
-        lds_f(stg + ((uint32_t)lrow * EPI_PITCH + (uint32_t)chalf * 16u) * 4u, v);
-        tc_store16<false>(a, p, o0, v);
-      }
+      if (col < N && p_ok && o0 < g.C_out) tc_store16<false>(a, p, o0, v);
     }
   }
 }

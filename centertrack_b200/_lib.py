@@ -99,6 +99,13 @@ class TrackPayload(C.Structure):
   ]
 
 
+class TrackOpts(C.Structure):
+  _fields_ = [
+      ('out_thresh', C.c_float), ('new_thresh', C.c_float), ('pre_thresh', C.c_float), ('max_age', C.c_int32),
+      ('hungarian', C.c_int32), ('public_det', C.c_int32), ('reserved', C.c_int32 * 2),
+  ]
+
+
 CT_DET_FLOATS = 10
 
 
@@ -138,7 +145,8 @@ EXPORTS = ['ct_packed_weight_bytes', 'ct_pack_weights', 'ct_conv_forward', 'ct_c
            'ct_render_pre_hm', 'ct_track_smem_bytes', 'ct_track_step', 'ct_track_assoc_smem_bytes',
            'ct_track_step_assoc', 'ct_track_payload_smem_bytes', 'ct_track_step_payload', 'ct_track_start',
            'ct_track_restore',
-           'ct_render_tracks', 'ct_track_step_mapped', 'ct_render_tracks_mapped', 'ct_post_process', 'ct_flip_merge', 'ct_flip_merge_heads', 'ct_mirror_x',
+           'ct_render_tracks', 'ct_track_step_mapped', 'ct_render_tracks_mapped', 'ct_post_process',
+           'ct_track_step_opts', 'ct_track_start_opts', 'ct_track_restore_opts', 'ct_post_process_opts', 'ct_flip_merge', 'ct_flip_merge_heads', 'ct_mirror_x',
            'ct_warp_affine_normalize', 'ct_pack_stem_frames_dev', 'ct_pack_stem_frames_flip_dev',
            'ct_warp_frames_normalize', 'ct_stage_frames', 'ct_last_error',
            'ct_abi_version', 'ct_launch_count', 'ct_reset_launch_count', 'ct_debug_trace', 'ct_debug_watch']
@@ -225,6 +233,14 @@ def lib():
   L.ct_render_tracks_mapped.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p] + [C.c_int32] * 3 + \
       [C.c_void_p]
   L.ct_post_process.argtypes = [C.POINTER(DetDesc), C.POINTER(TrackPayload), C.c_void_p, C.c_int32, C.c_void_p]
+  L.ct_track_step_opts.argtypes = [C.POINTER(TrackDesc), C.POINTER(TrackAssoc), C.POINTER(TrackPayload), C.c_void_p,
+                                   C.c_void_p, C.c_int32, C.c_void_p]
+  L.ct_track_start_opts.argtypes = [C.POINTER(TrackDesc), C.POINTER(TrackPayload), C.c_void_p, C.c_void_p, C.c_int32,
+                                    C.c_void_p, C.c_void_p]
+  L.ct_track_restore_opts.argtypes = [C.POINTER(TrackDesc), C.POINTER(TrackPayload), C.c_void_p, C.c_void_p,
+                                      C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+  L.ct_post_process_opts.argtypes = [C.POINTER(DetDesc), C.POINTER(TrackPayload), C.c_void_p, C.c_void_p, C.c_int32,
+                                     C.c_void_p]
   L.ct_flip_merge.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p, C.c_void_p, C.c_void_p]
   L.ct_warp_affine_normalize.argtypes = [C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 4 + [C.c_int32] * 2 + [C.c_void_p]
   L.ct_flip_merge_heads.argtypes = [C.POINTER(FlipHead)] + [C.c_int32] * 4 + [C.c_void_p]

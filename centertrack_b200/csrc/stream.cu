@@ -85,6 +85,8 @@ struct TrackArgs {
   int pay_smem;            // byte offset of the staged payload rows in dynamic shared memory
   const int* streams;      // ct_track_step_mapped: CTA i runs stream streams[i] on records[i]; NULL = identity
   int n_streams;           // rows of every per-stream array when streams != NULL
+  const ct_track_opts* opts;   // ct_track_step_opts: stream b's settings are opts[b]; NULL = `dflt`
+  ct_track_opts dflt;      // the descriptor's scalars and the assoc modes (the entry points without opts)
 };
 
 // bytes of the greedy layout before the association scratch (a multiple of 8: the scratch starts with fp64 arrays)
@@ -343,7 +345,8 @@ __device__ __forceinline__ void det_payload(const ct_track_payload& p, const flo
 // Boxes of the NEXT frame's prior heat-map (detector.py:254-290) from stream b's first `total` track rows `trk`: image
 // -> input coords, clip, radius, centre; rows past `total` and tracks that are not splatted get radius -1.  The one copy
 // of this arithmetic: the track step and ct_track_start both end with it.  Called by all TRK_THREADS threads.
-__device__ __forceinline__ void track_boxes(const ct_track_desc& d, int b, const float* trk, int total, int tid) {
+__device__ __forceinline__ void track_boxes(const ct_track_desc& d, int b, const float* trk, int total, float pre_thresh,
+                                            int tid) {
   if (!d.boxes) return;
   const int T = d.max_tracks;
   const double* ti = d.trans_input + b * 6;
@@ -352,7 +355,7 @@ __device__ __forceinline__ void track_boxes(const ct_track_desc& d, int b, const
     float radius = -1.f, cxo = 0.f, cyo = 0.f;
     if (r < total) {
       const float* t = trk + (size_t)r * TF;
-      if (!(t[CT_TRK_SCORE] < d.pre_thresh) && t[CT_TRK_ACTIVE] != 0.f) {
+      if (!(t[CT_TRK_SCORE] < pre_thresh) && t[CT_TRK_ACTIVE] != 0.f) {
         const float wmax = (float)(d.inp_w - 1), hmax = (float)(d.inp_h - 1);
         float x0 = (float)aff_f64(ti, (double)t[CT_TRK_BBOX], (double)t[CT_TRK_BBOX + 1]);
         float y0 = (float)aff_f64(ti + 3, (double)t[CT_TRK_BBOX], (double)t[CT_TRK_BBOX + 1]);
@@ -409,6 +412,9 @@ track_step_kernel(const TrackArgs a) {
   __shared__ float red_v[TRK_THREADS / 32];
   __shared__ int red_j[TRK_THREADS / 32];
   __shared__ int s_n, s_total, s_ids, s_nclaim;
+  // the stream's settings, read once per CTA and kept in shared memory (held in registers across the association they
+  // pushed the payload instantiation into spills)
+  __shared__ ct_track_opts so;
 
   int M = d.counts[b * 2 + 0];
   if (M > T) M = T;
@@ -421,14 +427,17 @@ track_step_kernel(const TrackArgs a) {
   float* s_oldp = reinterpret_cast<float*>(tsm + a.pay_smem);  // [T][Wp]
   if constexpr (PAY)
     for (int i = tid; i < M * Wp; i += TRK_THREADS) s_oldp[i] = pay[i];
-  if (tid == 0) s_n = 0;
+  if (tid == 0) {
+    s_n = 0;
+    so = a.opts ? a.opts[b] : a.dflt;
+  }
   __syncthreads();
 
   // ---- detections of this frame: generic_post_process (post_process.py:21-91), merge_outputs (detector.py:371-377)
   const float* rec = d.records + (size_t)(MAP ? (int)blockIdx.x : b) * K * d.F;
   const float* to = d.trans_out_inv + b * 6;
   int cnt = 0;
-  for (int i = tid; i < K; i += TRK_THREADS) cnt += rec[(size_t)i * d.F + CT_REC_SCORE] > d.out_thresh ? 1 : 0;
+  for (int i = tid; i < K; i += TRK_THREADS) cnt += rec[(size_t)i * d.F + CT_REC_SCORE] > so.out_thresh ? 1 : 0;
   atomicAdd(&s_n, cnt);
   __syncthreads();
   const int N = s_n;                     // records are sorted by score: the kept detections are a prefix
@@ -450,7 +459,9 @@ track_step_kernel(const TrackArgs a) {
   }
   __syncthreads();
 
-  const bool hung = a.as.hungarian != 0, pub = a.as.public_det != 0;
+  // a stream runs --public_det only where the launch has the public detections (as.public_det); the association
+  // scratch is present whenever a stream may run either mode
+  const bool hung = so.hungarian != 0, pub = so.public_det != 0 && a.as.public_det != 0;
   if (hung || pub) {
     for (int i = tid; i < N; i += TRK_THREADS) s_rej[i] = -1;
     __syncthreads();
@@ -510,6 +521,8 @@ track_step_kernel(const TrackArgs a) {
   //      coasting walk the reference's `unmatched` lists: the naturally unmatched ascending, then the detections /
   //      tracks of rejected (forced through a blocked cell) Hungarian pairs in pair order
   if (tid == 0) {
+    const float new_thresh = so.new_thresh;
+    const int max_age = so.max_age;
     int pos = 0, ids = id_count;
     for (int i = 0; i < N; ++i) {
       s_pos_det[i] = -1;
@@ -522,7 +535,7 @@ track_step_kernel(const TrackArgs a) {
     }
     auto birth = [&](int i) {
       float* o = s_det + (size_t)i * TF;
-      if (o[CT_TRK_SCORE] > d.new_thresh) {
+      if (o[CT_TRK_SCORE] > new_thresh) {
         ++ids;
         o[CT_TRK_ID] = (float)ids; o[CT_TRK_AGE] = 1.f; o[CT_TRK_ACTIVE] = 1.f;
         if (pos < T) s_pos_det[i] = pos++;
@@ -530,7 +543,7 @@ track_step_kernel(const TrackArgs a) {
     };
     auto coast = [&](int j) {
       float* t = s_old + (size_t)j * TF;
-      if (t[CT_TRK_AGE] < (float)d.max_age) {
+      if (t[CT_TRK_AGE] < (float)max_age) {
         t[CT_TRK_AGE] += 1.f; t[CT_TRK_ACTIVE] = 0.f;
         if (pos < T) s_pos_trk[j] = pos++;
       }
@@ -577,7 +590,7 @@ track_step_kernel(const TrackArgs a) {
   if (tid == 0) { d.counts[b * 2 + 0] = total; d.counts[b * 2 + 1] = s_ids; }
   __syncthreads();     // the table rows written above are re-read below by other threads
   __threadfence_block();
-  track_boxes(d, b, trk, total, tid);
+  track_boxes(d, b, trk, total, so.pre_thresh, tid);
 }
 
 // ct_track_start: stream starts[e][0] begins a new video -- Tracker.reset + init_track(seeds): its T track rows, counts
@@ -586,11 +599,13 @@ track_step_kernel(const TrackArgs a) {
 // entry e follow those of entries 0..e-1 in `seeds`.
 // RESTORE (ct_track_restore): entries are (stream, n, id_count), the rows are an exported stream's verbatim (ids, ages
 // and active kept) with their payload rows in `pay_rows`, and counts = (n, id_count).  A template parameter so that
-// ct_track_start's instantiation stays as it was.
+// ct_track_start's instantiation stays as it was.  opts (_opts entry points): the boxes use opts[b].pre_thresh; NULL =
+// the descriptor's.
 template <bool RESTORE = false>
 __global__ void __launch_bounds__(TRK_THREADS)
 track_start_kernel(const ct_track_desc d, float* __restrict__ payload, int Wp, const int* __restrict__ starts,
-                   const float* __restrict__ seeds, const float* __restrict__ pay_rows = nullptr) {
+                   const float* __restrict__ seeds, const float* __restrict__ pay_rows,
+                   const ct_track_opts* __restrict__ opts) {
   constexpr int S = RESTORE ? 3 : 2;                          // int32 per entry
   const int e = blockIdx.x, tid = threadIdx.x, T = d.max_tracks;
   const int b = starts[S * e];
@@ -609,7 +624,7 @@ track_start_kernel(const ct_track_desc d, float* __restrict__ payload, int Wp, c
   if (tid == 0) { d.counts[b * 2 + 0] = n; d.counts[b * 2 + 1] = RESTORE ? starts[S * e + 2] : n; }
   __syncthreads();     // the seed rows written above are re-read below by other threads
   __threadfence_block();
-  track_boxes(d, b, trk, n, tid);
+  track_boxes(d, b, trk, n, opts ? opts[b].pre_thresh : d.pre_thresh, tid);
 }
 
 // splat of the boxes written by track_step_kernel; rows with radius < 0 are skipped.  grid = B*T (fixed: graph-capturable)
@@ -651,6 +666,7 @@ struct DetArgs {
   ct_track_payload p;      // read by the payload instantiation only
   const int* streams;      // NULL = identity
   int n_streams;
+  const ct_track_opts* opts;   // ct_post_process_opts: stream b keeps score > opts[b].out_thresh; NULL = d.out_thresh
 };
 
 template <bool PAY>
@@ -663,8 +679,9 @@ __global__ void __launch_bounds__(DET_THREADS) post_process_kernel(const DetArgs
   __syncthreads();
   const int K = d.K, F = d.F;
   const float* rec = d.records + (size_t)blockIdx.x * K * F;
+  const float out_thresh = a.opts ? a.opts[b].out_thresh : d.out_thresh;
   int cnt = 0;
-  for (int i = threadIdx.x; i < K; i += DET_THREADS) cnt += rec[(size_t)i * F + CT_REC_SCORE] > d.out_thresh ? 1 : 0;
+  for (int i = threadIdx.x; i < K; i += DET_THREADS) cnt += rec[(size_t)i * F + CT_REC_SCORE] > out_thresh ? 1 : 0;
   atomicAdd(&s_n, cnt);
   __syncthreads();
   const int N = s_n;
@@ -1138,9 +1155,11 @@ static int payload_check(const ct_track_payload* p, int32_t F) {
   return CT_OK;
 }
 
-// One track step launch: CTA i on records[i] and stream streams[i] (streams == NULL: stream i of d->B).
+// One track step launch: CTA i on records[i] and stream streams[i] (streams == NULL: stream i of d->B).  opts == NULL:
+// every stream runs the descriptor's scalars with as's modes; else stream b runs opts[b], the association scratch is
+// always present, and as->public_det says whether the launch has public detections.
 static int track_step_launch(const ct_track_desc* d, const ct_track_assoc* as, const ct_track_payload* p,
-                             const int32_t* streams, int32_t n_streams, void* stream) {
+                             const ct_track_opts* opts, const int32_t* streams, int32_t n_streams, void* stream) {
   CT_REQUIRE(d && as && d->records && d->trans_out_inv && d->tracks && d->counts, "null pointer");
   CT_REQUIRE(d->B > 0 && d->K > 0 && d->F >= CT_REC_HEADS && d->max_tracks >= d->K, "bad shape");
   CT_REQUIRE(d->rec_tracking < 0 || d->rec_tracking + 2 <= d->F, "tracking offset outside the record");
@@ -1151,7 +1170,7 @@ static int track_step_launch(const ct_track_desc* d, const ct_track_assoc* as, c
     const int rc = payload_check(p, d->F);
     if (rc != CT_OK) return rc;
   }
-  const bool scratch = as->hungarian || as->public_det;
+  const bool scratch = opts || as->hungarian || as->public_det;
   const size_t smem = (size_t)ct_track_payload_smem_bytes(d->K, d->max_tracks, p ? p->width : 0, scratch);
   CT_REQUIRE(smem <= 200 * 1024, "track table does not fit in shared memory (lower max_tracks)");
   auto kernel = streams ? (p ? track_step_kernel<true, true> : track_step_kernel<false, true>)
@@ -1167,13 +1186,15 @@ static int track_step_launch(const ct_track_desc* d, const ct_track_assoc* as, c
                               : 0));
   a.streams = streams;
   a.n_streams = n_streams;
+  a.opts = opts;
+  a.dflt = {d->out_thresh, d->new_thresh, d->pre_thresh, d->max_age, as->hungarian, as->public_det, {0, 0}};
   kernel<<<d->B, TRK_THREADS, smem, (cudaStream_t)stream>>>(a);
   return after_launch();
 }
 
 extern "C" int ct_track_step_payload(const ct_track_desc* d, const ct_track_assoc* as, const ct_track_payload* p,
                                      void* stream) {
-  return track_step_launch(d, as, p, nullptr, 0, stream);
+  return track_step_launch(d, as, p, nullptr, nullptr, 0, stream);
 }
 
 extern "C" int ct_track_step_mapped(const ct_track_desc* d, const ct_track_assoc* as, const ct_track_payload* p,
@@ -1181,7 +1202,16 @@ extern "C" int ct_track_step_mapped(const ct_track_desc* d, const ct_track_assoc
   CT_REQUIRE(streams, "null stream map");
   CT_REQUIRE(n_streams > 0, "n_streams <= 0");
   const ct_track_assoc greedy = {};
-  return track_step_launch(d, as ? as : &greedy, p, streams, n_streams, stream);
+  return track_step_launch(d, as ? as : &greedy, p, nullptr, streams, n_streams, stream);
+}
+
+extern "C" int ct_track_step_opts(const ct_track_desc* d, const ct_track_assoc* as, const ct_track_payload* p,
+                                  const ct_track_opts* opts, const int32_t* streams, int32_t n_streams, void* stream) {
+  CT_REQUIRE(opts, "null opts");
+  CT_REQUIRE(n_streams >= 0, "n_streams < 0");
+  CT_REQUIRE(!streams || n_streams > 0, "a stream map needs n_streams > 0");
+  const ct_track_assoc greedy = {};
+  return track_step_launch(d, as ? as : &greedy, p, opts, streams, n_streams, stream);
 }
 
 extern "C" int ct_track_step_assoc(const ct_track_desc* d, const ct_track_assoc* as, void* stream) {
@@ -1193,36 +1223,53 @@ extern "C" int ct_track_step(const ct_track_desc* d, void* stream) {
   return ct_track_step_assoc(d, &greedy, stream);
 }
 
-extern "C" int ct_track_start(const ct_track_desc* d, const ct_track_payload* p, const int32_t* starts,
-                              int32_t n_starts, const float* seeds, void* stream) {
+// ct_track_start / ct_track_restore (RESTORE) and their _opts forms: one CTA per entry.
+template <bool RESTORE>
+static int track_start_launch(const ct_track_desc* d, const ct_track_payload* p, const ct_track_opts* opts,
+                              const int32_t* entries, int32_t n, const float* rows, const float* payload_rows,
+                              void* stream) {
   CT_REQUIRE(d && d->tracks && d->counts, "null pointer");
   CT_REQUIRE(d->B > 0 && d->max_tracks > 0, "bad shape");
   CT_REQUIRE(d->boxes == nullptr || (d->trans_input != nullptr && d->inp_h > 0 && d->inp_w > 0), "boxes need trans_input");
-  CT_REQUIRE(n_starts >= 0 && n_starts <= d->B, "n_starts outside [0, B]");
-  CT_REQUIRE(n_starts == 0 || starts, "null start list");
+  if (RESTORE) {
+    CT_REQUIRE(n >= 0 && n <= d->B, "n_entries outside [0, B]");
+    CT_REQUIRE(n == 0 || entries, "null entry list");
+  } else {
+    CT_REQUIRE(n >= 0 && n <= d->B, "n_starts outside [0, B]");
+    CT_REQUIRE(n == 0 || entries, "null start list");
+  }
   CT_REQUIRE(!p || (p->payload && p->width > 0), "payload table needs payload and width > 0");
-  if (n_starts == 0) return CT_OK;
-  track_start_kernel<<<n_starts, TRK_THREADS, 0, (cudaStream_t)stream>>>(*d, p ? p->payload : nullptr, p ? p->width : 0,
-                                                                          starts, seeds);
+  if (n == 0) return CT_OK;
+  track_start_kernel<RESTORE><<<n, TRK_THREADS, 0, (cudaStream_t)stream>>>(
+      *d, p ? p->payload : nullptr, p ? p->width : 0, entries, rows, payload_rows, opts);
   return after_launch();
+}
+
+extern "C" int ct_track_start(const ct_track_desc* d, const ct_track_payload* p, const int32_t* starts,
+                              int32_t n_starts, const float* seeds, void* stream) {
+  return track_start_launch<false>(d, p, nullptr, starts, n_starts, seeds, nullptr, stream);
 }
 
 extern "C" int ct_track_restore(const ct_track_desc* d, const ct_track_payload* p, const int32_t* entries,
                                 int32_t n_entries, const float* rows, const float* payload_rows, void* stream) {
-  CT_REQUIRE(d && d->tracks && d->counts, "null pointer");
-  CT_REQUIRE(d->B > 0 && d->max_tracks > 0, "bad shape");
-  CT_REQUIRE(d->boxes == nullptr || (d->trans_input != nullptr && d->inp_h > 0 && d->inp_w > 0), "boxes need trans_input");
-  CT_REQUIRE(n_entries >= 0 && n_entries <= d->B, "n_entries outside [0, B]");
-  CT_REQUIRE(n_entries == 0 || entries, "null entry list");
-  CT_REQUIRE(!p || (p->payload && p->width > 0), "payload table needs payload and width > 0");
-  if (n_entries == 0) return CT_OK;
-  track_start_kernel<true><<<n_entries, TRK_THREADS, 0, (cudaStream_t)stream>>>(
-      *d, p ? p->payload : nullptr, p ? p->width : 0, entries, rows, payload_rows);
-  return after_launch();
+  return track_start_launch<true>(d, p, nullptr, entries, n_entries, rows, payload_rows, stream);
 }
 
-extern "C" int ct_post_process(const ct_det_desc* d, const ct_track_payload* p, const int32_t* streams,
-                               int32_t n_streams, void* stream) {
+extern "C" int ct_track_start_opts(const ct_track_desc* d, const ct_track_payload* p, const ct_track_opts* opts,
+                                   const int32_t* starts, int32_t n_starts, const float* seeds, void* stream) {
+  CT_REQUIRE(opts, "null opts");
+  return track_start_launch<false>(d, p, opts, starts, n_starts, seeds, nullptr, stream);
+}
+
+extern "C" int ct_track_restore_opts(const ct_track_desc* d, const ct_track_payload* p, const ct_track_opts* opts,
+                                     const int32_t* entries, int32_t n_entries, const float* rows,
+                                     const float* payload_rows, void* stream) {
+  CT_REQUIRE(opts, "null opts");
+  return track_start_launch<true>(d, p, opts, entries, n_entries, rows, payload_rows, stream);
+}
+
+static int post_process_launch(const ct_det_desc* d, const ct_track_payload* p, const ct_track_opts* opts,
+                               const int32_t* streams, int32_t n_streams, void* stream) {
   CT_REQUIRE(d && d->records && d->trans_out_inv && d->dets && d->counts, "null pointer");
   CT_REQUIRE(d->n > 0 && d->K > 0 && d->F >= CT_REC_HEADS, "bad shape (n > 0, K > 0, F >= CT_REC_HEADS)");
   CT_REQUIRE(d->rec_tracking < 0 || (d->rec_tracking >= CT_REC_HEADS && d->rec_tracking + 2 <= d->F),
@@ -1238,9 +1285,21 @@ extern "C" int ct_post_process(const ct_det_desc* d, const ct_track_payload* p, 
   if (p) a.p = *p;
   a.streams = streams;
   a.n_streams = n_streams;
+  a.opts = opts;
   auto kernel = p ? post_process_kernel<true> : post_process_kernel<false>;
   kernel<<<d->n, DET_THREADS, 0, (cudaStream_t)stream>>>(a);
   return after_launch();
+}
+
+extern "C" int ct_post_process(const ct_det_desc* d, const ct_track_payload* p, const int32_t* streams,
+                               int32_t n_streams, void* stream) {
+  return post_process_launch(d, p, nullptr, streams, n_streams, stream);
+}
+
+extern "C" int ct_post_process_opts(const ct_det_desc* d, const ct_track_payload* p, const ct_track_opts* opts,
+                                    const int32_t* streams, int32_t n_streams, void* stream) {
+  CT_REQUIRE(opts, "null opts");
+  return post_process_launch(d, p, opts, streams, n_streams, stream);
 }
 
 extern "C" int ct_render_tracks(const float* boxes, int32_t n, float* pre_hm, int32_t B, int32_t H, int32_t W,

@@ -12,7 +12,8 @@ import numpy as np
 import torch
 
 from . import _lib as L
-from .device_tracker import DeviceTracker, default_geometry, payload_layout
+from .device_tracker import POST_OPTION_KEYS, DeviceTracker, default_geometry, opts_records, payload_layout, \
+    resolve_options
 
 
 class DeviceDetections(object):
@@ -25,10 +26,21 @@ class DeviceDetections(object):
   _calibs = DeviceTracker._calibs
   geometry_rows = DeviceTracker.geometry_rows
 
-  def __init__(self, opt, B, K, rec_floats, layout, inp_h, inp_w, device, centers=None, scales=None, calibs=None):
+  opts_bytes = DeviceTracker.opts_bytes
+  _opts = DeviceTracker._opts
+
+  def __init__(self, opt, B, K, rec_floats, layout, inp_h, inp_w, device, centers=None, scales=None, calibs=None,
+               stream_opts=None):
     """centers/scales: per-stream (c, s) of the source rectangle; default = a source image of exactly the network
     input size.  calibs: per-stream [3,4] camera matrices for the 3D head sets (loc, rot_y); default as
-    DeviceTracker's."""
+    DeviceTracker's.  stream_opts: None, or B entries, each None (opt) or {'out_thresh': v}, the threshold stream b
+    keeps its records above (ct_post_process_opts on the device records d_opts)."""
+    self.per_stream = stream_opts is not None
+    if self.per_stream and len(stream_opts) != B:
+      raise ValueError('stream_opts: expected %d entries (one per stream, None or a dict), got %d' %
+                       (B, len(stream_opts)))
+    self.options = [resolve_options(opt, f, POST_OPTION_KEYS, 'stream_opts[%d]' % b)
+                    for b, f in enumerate(stream_opts if self.per_stream else [None] * B)]
     self.opt, self.B, self.K, self.F = opt, B, K, rec_floats
     self.inp_h, self.inp_w = inp_h, inp_w
     self.device = torch.device(device)
@@ -62,6 +74,17 @@ class DeviceDetections(object):
         self.calib = torch.from_numpy(self._calibs(opt, calibs, centers, inp_h, inp_w)).to(self.device)
         p.calib = self.calib.data_ptr()
       self.pay = p
+    self.d_opts = None
+    if self.per_stream:
+      self.d_opts = torch.frombuffer(bytearray(self.opts_bytes()), dtype=torch.uint8).to(self.device)
+
+  def check_options(self, flags, what='options', resolved=False):
+    """A stream's new setting ({'out_thresh': v}, or resolved as a StreamState carries it) -> the resolved setting;
+    ValueError for another key, a bad value, or a runner built without stream_opts."""
+    if not self.per_stream:
+      raise ValueError('%s: this runner was built without stream_opts: its streams all run opt (build it with '
+                       'stream_opts to give streams their own out_thresh)' % what)
+    return dict(flags) if resolved else resolve_options(self.opt, flags, POST_OPTION_KEYS, what)
 
   def set_geometry(self, streams, rows_in, rows_out):
     """trans_out_inv (and calib on 3D head sets) of `streams` <- rows_out (geometry_rows, device tensors), on the
@@ -71,24 +94,30 @@ class DeviceDetections(object):
       if self.calib is not None:
         self.calib[b].view(12).copy_(rows_out[i, 6:])
 
-  def _launch(self, records, streams):
+  def _launch(self, records, streams, opts=None):
     n = records.shape[0]
     assert records.is_cuda and records.dtype == torch.float32 and records.is_contiguous() and \
         tuple(records.shape) == (n, self.K, self.F) and 0 < n <= self.B
     self.desc.n, self.desc.records = n, records.data_ptr()
-    L.check(L.lib().ct_post_process(C.byref(self.desc), C.byref(self.pay) if self.pay is not None else None,
-                                    L.ptr(streams), self.B, L.stream_ptr()), 'ct_post_process')
+    pay = C.byref(self.pay) if self.pay is not None else None
+    if self.per_stream:
+      L.check(L.lib().ct_post_process_opts(C.byref(self.desc), pay, self._opts(opts), L.ptr(streams), self.B,
+                                           L.stream_ptr()), 'ct_post_process_opts')
+      return
+    L.check(L.lib().ct_post_process(C.byref(self.desc), pay, L.ptr(streams), self.B, L.stream_ptr()),
+            'ct_post_process')
 
-  def step(self, records):
+  def step(self, records, opts=None):
     """records [B,K,F] (ct_decode) -> dets, counts (and payload) of every stream, on the current stream.  The
-    descriptor points at the buffers of this call, so a CUDA graph captured around it keeps reading them."""
-    self._launch(records, None)
+    descriptor points at the buffers of this call, so a CUDA graph captured around it keeps reading them.  With
+    stream_opts: on `opts` (device ct_track_opts [B], default d_opts)."""
+    self._launch(records, None, opts)
 
-  def step_mapped(self, records, streams):
+  def step_mapped(self, records, streams, opts=None):
     """step() on a compacted batch: records [n,K,F], streams int32 [>= n] device map (image i is stream streams[i];
     < 0: a padding image, nothing is written).  Streams that are not listed keep their rows byte for byte."""
     assert streams.is_cuda and streams.dtype == torch.int32 and streams.numel() >= records.shape[0]
-    self._launch(records, streams)
+    self._launch(records, streams, opts)
 
   @property
   def d2h_bytes(self):

@@ -69,9 +69,75 @@ def seed_rows(items, new_thresh):
   return np.stack(rows) if rows else np.zeros((0, L.CT_TRK_FLOATS), np.float32)
 
 
+# The reference flags a StreamRunner stream may set for itself (stream_opts, options=): they act only in the per-stream
+# kernels.  A runner without a tracker (device_post_process) takes out_thresh alone.
+TRACK_OPTION_KEYS = ('track_thresh', 'out_thresh', 'pre_thresh', 'new_thresh', 'max_age', 'hungarian', 'public_det')
+POST_OPTION_KEYS = ('out_thresh',)
+
+
+def resolve_options(opt, flags, keys=TRACK_OPTION_KEYS, what='options'):
+  """The settings of opt_b = opt with a stream's flags ({name: value} of `keys`, or None) applied -> {out_thresh,
+  new_thresh, pre_thresh, max_age, hungarian, public_det}; None and {} give opt's own.  The one rule for every entry:
+  flags that set no threshold leave opt's thresholds as they are (its current attributes, whatever changed them after
+  opts().init).  A threshold flag (track_thresh, out_thresh, pre_thresh, new_thresh) re-derives all three as
+  opts.py:97-99 does on tracking tasks, max(track_thresh, threshold), from the thresholds opts was given (opt.thresh_args) while
+  those still derive to opt's current values -- so opt_b is opts().init of the runner's flags plus the stream's -- and
+  from opt's current thresholds once opt was changed after init (or has no thresh_args).  Only out_thresh, without the
+  derivation, when keys is POST_OPTION_KEYS.  ValueError naming the key for a key outside `keys` (such as K, flip_test,
+  pre_hm or a head option, which change the network or the records) or a value of the wrong type."""
+  flags = {} if flags is None else flags
+  if not isinstance(flags, dict):
+    raise ValueError('%s: expected a dict of per-stream flags or None, got %s' % (what, type(flags).__name__))
+  for k, v in flags.items():
+    if k not in keys:
+      raise ValueError('%s: %r cannot differ between the streams of a runner; a stream may set %s' %
+                       (what, k, ', '.join(keys)))
+    if k in ('hungarian', 'public_det'):
+      ok = isinstance(v, (bool, np.bool_))
+    elif k == 'max_age':
+      ok = isinstance(v, (int, np.integer)) and not isinstance(v, (bool, np.bool_))
+    else:
+      ok = isinstance(v, (int, float, np.integer, np.floating)) and not isinstance(v, (bool, np.bool_)) and \
+          np.isfinite(v)
+    if not ok:
+      raise ValueError('%s[%r]: bad value %r (%s)' % (what, k, v, 'a bool' if k in ('hungarian', 'public_det') else
+                                                     'an int' if k == 'max_age' else 'a finite number'))
+  if keys == POST_OPTION_KEYS:
+    return {'out_thresh': float(flags.get('out_thresh', opt.out_thresh))}
+  names = ('out_thresh', 'pre_thresh', 'new_thresh')
+  now = {k: getattr(opt, k) for k in names}
+  given = now
+  if any(k in flags for k in names + ('track_thresh',)):
+    tracking = 'tracking' in getattr(opt, 'task', 'tracking')
+    derive = lambda v, track: {k: max(track, x) for k, x in v.items()} if tracking else dict(v)
+    args = getattr(opt, 'thresh_args', None)
+    if args is not None and derive(args, opt.track_thresh) == now:
+      given = dict(args)                             # opt as opts().init left it: the thresholds as given
+    else:
+      given = dict(now)                              # opt changed after init: its current thresholds
+    given.update((k, flags[k]) for k in names if k in flags)
+    given = derive(given, flags.get('track_thresh', getattr(opt, 'track_thresh', 0.3)))
+  return {'out_thresh': float(given['out_thresh']), 'new_thresh': float(given['new_thresh']),
+          'pre_thresh': float(given['pre_thresh']), 'max_age': int(flags.get('max_age', opt.max_age)),
+          'hungarian': bool(flags.get('hungarian', getattr(opt, 'hungarian', False))),
+          'public_det': bool(flags.get('public_det', getattr(opt, 'public_det', False)))}
+
+
+def opts_records(resolved):
+  """Resolved settings (resolve_options), one per stream -> ct_track_opts [n] (ctypes array)."""
+  arr = (L.TrackOpts * len(resolved))()
+  for r, v in zip(arr, resolved):
+    r.out_thresh = v['out_thresh']
+    if 'max_age' in v:
+      r.new_thresh, r.pre_thresh, r.max_age = v['new_thresh'], v['pre_thresh'], v['max_age']
+      r.hungarian, r.public_det = int(v['hungarian']), int(v['public_det'])
+  return arr
+
+
 def plan_starts(B, T, new_thresh, has_payload, starts, pre_dets):
   """Checks one step's video starts and builds their seeds, before anything is enqueued.  starts: stream indices whose
-  frame is a video's first; pre_dets: {stream: list of result dicts} seeding some of them (or None).
+  frame is a video's first; pre_dets: {stream: list of result dicts} seeding some of them (or None).  new_thresh: one
+  threshold, or one per stream (each stream's seeds are filtered with its own).
   -> (streams list, [seed rows float32 [n_i, CT_TRK_FLOATS]] in the same order).  ValueError on a stream out of range
   or repeated, pre_dets for a stream that does not start, more kept seeds than the T rows of the track table, or
   pre_dets on a head set with payload fields (their seeds would need those fields)."""
@@ -94,7 +160,7 @@ def plan_starts(B, T, new_thresh, has_payload, starts, pre_dets):
                      'attributes); start those streams without pre_dets')
   seeds = []
   for s in streams:
-    rows = seed_rows(pre_dets.get(s, ()), new_thresh)
+    rows = seed_rows(pre_dets.get(s, ()), new_thresh[s] if isinstance(new_thresh, (list, tuple)) else new_thresh)
     if len(rows) > T:
       raise ValueError('pre_dets[%d]: %d seeds above new_thresh, more than the %d rows of the track table' %
                        (s, len(rows), T))
@@ -110,21 +176,32 @@ def default_geometry(inp_h, inp_w):
 class DeviceTracker(object):
 
   def __init__(self, opt, B, K, rec_floats, layout, inp_h, inp_w, device, centers=None, scales=None, max_tracks=None,
-               max_public_dets=512, calibs=None):
+               max_public_dets=512, calibs=None, stream_opts=None):
     """centers/scales: per-stream (c, s) of the source rectangle (Detector._input_geometry); default = a source image
     of exactly the network input size (the synthetic benchmark streams).  max_public_dets: with --public_det, the most
     public detections one stream may bring per frame (P, the row count of the public_ct buffers step() takes).
     calibs: per-stream [3,4] camera matrices for the 3D head sets (loc, rot_y); default = Detector._get_default_calib
-    of a source image centred on c, with --test_focal_length or the dataset's rest_focal_length."""
-    self.hungarian = bool(getattr(opt, 'hungarian', False))
-    self.public_det = bool(getattr(opt, 'public_det', False))
+    of a source image centred on c, with --test_focal_length or the dataset's rest_focal_length.
+    stream_opts: None (every stream runs opt), or B entries, each None (opt) or a dict of TRACK_OPTION_KEYS flags that
+    stream b runs with instead (resolve_options): its own thresholds, max_age, --hungarian and --public_det, through the
+    _opts entry points and the device records d_opts.  The table's T rows then come from the largest max_age, public
+    detections are staged when any stream has --public_det, and the Hungarian scratch is always allocated."""
+    self.per_stream = stream_opts is not None
+    if self.per_stream and len(stream_opts) != B:
+      raise ValueError('stream_opts: expected %d entries (one per stream, None or a dict), got %d' %
+                       (B, len(stream_opts)))
+    self.options = [resolve_options(opt, f, what='stream_opts[%d]' % b)
+                    for b, f in enumerate(stream_opts if self.per_stream else [None] * B)]
+    self.hungarian = any(o['hungarian'] for o in self.options)
+    self.public_det = any(o['public_det'] for o in self.options)
+    self.max_age = max(o['max_age'] for o in self.options)     # the table's coasting capacity
     self.max_public = int(max_public_dets)
     if self.public_det and self.max_public <= 0:
       raise ValueError('--public_det needs max_public_dets > 0')
     self.opt, self.B, self.K, self.F = opt, B, K, rec_floats
     self.inp_h, self.inp_w = inp_h, inp_w
     self.device = torch.device(device)
-    self.T = int(max_tracks or (K * (1 + max(0, int(opt.max_age)))))
+    self.T = int(max_tracks or (K * (1 + max(0, self.max_age))))
     self.T = max(self.T, K)
     c0, s0 = default_geometry(inp_h, inp_w)
     t_in, t_out = self._trans_rows([c0 if centers is None else centers[b] for b in range(B)],
@@ -165,9 +242,35 @@ class DeviceTracker(object):
         self.calib = torch.from_numpy(self._calibs(opt, calibs, centers, inp_h, inp_w)).to(self.device)
         p.calib = self.calib.data_ptr()
       self.pay = p
-    smem = L.lib().ct_track_payload_smem_bytes(K, self.T, self.Wp, int(self.hungarian or self.public_det))
+    smem = L.lib().ct_track_payload_smem_bytes(K, self.T, self.Wp, int(self.hungarian or self.public_det or
+                                                                         self.per_stream))
     if smem > 200 * 1024:
       raise ValueError('track table of %d rows does not fit in shared memory' % self.T)
+    self.d_opts = None
+    if self.per_stream:
+      self.d_opts = torch.frombuffer(bytearray(self.opts_bytes()), dtype=torch.uint8).to(self.device)
+
+  def opts_bytes(self):
+    """The ct_track_opts records of the streams' current settings, as bytes."""
+    return bytes(opts_records(self.options))
+
+  def check_options(self, flags, what='options', resolved=False):
+    """A stream's new settings (a dict of flags, resolved against opt; resolved=True: settings resolve_options already
+    gave, as a StreamState carries them) -> the resolved settings.  ValueError for what resolve_options refuses, on a tracker built without
+    stream_opts, for a max_age above the table's capacity, or --public_det on a tracker that stages no public
+    detections."""
+    if not self.per_stream:
+      raise ValueError('%s: this runner was built without stream_opts: its streams all run opt (build it with '
+                       'stream_opts to give streams their own tracker settings)' % what)
+    o = dict(flags) if resolved else resolve_options(self.opt, flags, what=what)
+    if o['max_age'] > self.max_age:
+      raise ValueError('%s: max_age %d is above the %d the track table was sized for (T = K (1 + max_age) = %d rows); '
+                       'give the runner a stream_opts entry with the largest max_age' % (what, o['max_age'],
+                                                                                          self.max_age, self.T))
+    if o['public_det'] and not self.public_det:
+      raise ValueError('%s: public_det on a runner that stages no public detections (neither opt nor any stream_opts '
+                       'entry has public_det)' % what)
+    return o
 
   def _calibs(self, opt, calibs, centers, inp_h, inp_w):
     if calibs is not None:
@@ -226,43 +329,60 @@ class DeviceTracker(object):
     stream: its tracks, counts and payload are cleared, the seeds written (seed_rows), and its boxes rendered from them,
     so that the next render() splats them.  seeds: {stream: list of result dicts} (pre_dets) or None.  ValueError as
     plan_starts."""
-    streams, rows = plan_starts(self.B, self.T, self.opt.new_thresh, self.payload is not None, streams, seeds)
+    streams, rows = plan_starts(self.B, self.T, [o['new_thresh'] for o in self.options], self.payload is not None,
+                                streams, seeds)
     if not streams:
       return
     lst = torch.tensor([[s, len(r)] for s, r in zip(streams, rows)], dtype=torch.int32).to(self.device)
     seed = torch.from_numpy(np.concatenate(rows)).to(self.device) if sum(map(len, rows)) else None
     self.start_device(lst, len(streams), seed)
 
-  def start_device(self, start_list, n_starts, seeds=None):
-    """ct_track_start on device buffers: start_list int32 [>= n_starts, 2] rows (stream, seed rows), seeds fp32
-    [sum of n, CT_TRK_FLOATS] in start_list's order (or None).  No checks of the contents: see plan_starts."""
-    L.check(L.lib().ct_track_start(C.byref(self.desc), C.byref(self.pay) if self.pay is not None else None,
-                                   L.ptr(start_list), n_starts, L.ptr(seeds), L.stream_ptr()), 'ct_track_start')
+  def _opts(self, opts):
+    """The device ct_track_opts records a launch reads: `opts` (a runner's per-slot copy), or d_opts."""
+    return L.ptr(self.d_opts if opts is None else opts)
 
-  def restore_device(self, entries, n_entries, rows=None, payload_rows=None):
+  def start_device(self, start_list, n_starts, seeds=None, opts=None):
+    """ct_track_start on device buffers: start_list int32 [>= n_starts, 2] rows (stream, seed rows), seeds fp32
+    [sum of n, CT_TRK_FLOATS] in start_list's order (or None).  No checks of the contents: see plan_starts.  With
+    stream_opts: ct_track_start_opts on `opts` (device ct_track_opts [B], default d_opts)."""
+    pay = C.byref(self.pay) if self.pay is not None else None
+    if self.per_stream:
+      L.check(L.lib().ct_track_start_opts(C.byref(self.desc), pay, self._opts(opts), L.ptr(start_list), n_starts,
+                                          L.ptr(seeds), L.stream_ptr()), 'ct_track_start_opts')
+      return
+    L.check(L.lib().ct_track_start(C.byref(self.desc), pay, L.ptr(start_list), n_starts, L.ptr(seeds),
+                                   L.stream_ptr()), 'ct_track_start')
+
+  def restore_device(self, entries, n_entries, rows=None, payload_rows=None, opts=None):
     """ct_track_restore on device buffers: entries int32 [>= n_entries, 3] rows (stream, rows n, id_count), rows fp32
     [sum of n, CT_TRK_FLOATS] and payload_rows fp32 [sum of n, Wp] in entries' order (None when every n is 0).  The
-    rows are written as they are, and each stream's boxes rendered from them with its own index and trans_input."""
-    L.check(L.lib().ct_track_restore(C.byref(self.desc), C.byref(self.pay) if self.pay is not None else None,
-                                     L.ptr(entries), n_entries, L.ptr(rows), L.ptr(payload_rows), L.stream_ptr()),
-            'ct_track_restore')
+    rows are written as they are, and each stream's boxes rendered from them with its own index and trans_input.
+    With stream_opts: ct_track_restore_opts on `opts`, as start_device."""
+    pay = C.byref(self.pay) if self.pay is not None else None
+    if self.per_stream:
+      L.check(L.lib().ct_track_restore_opts(C.byref(self.desc), pay, self._opts(opts), L.ptr(entries), n_entries,
+                                            L.ptr(rows), L.ptr(payload_rows), L.stream_ptr()), 'ct_track_restore_opts')
+      return
+    L.check(L.lib().ct_track_restore(C.byref(self.desc), pay, L.ptr(entries), n_entries, L.ptr(rows),
+                                     L.ptr(payload_rows), L.stream_ptr()), 'ct_track_restore')
 
   def public_buffers(self):
     """Zeroed device buffers of the shape step() takes with --public_det: public_ct [B,P,2] fp32, public_n [B] int32."""
     return (torch.zeros((self.B, self.max_public, 2), dtype=torch.float32, device=self.device),
             torch.zeros((self.B,), dtype=torch.int32, device=self.device))
 
-  def step(self, records, public_ct=None, public_n=None, steps=None):
+  def step(self, records, public_ct=None, public_n=None, steps=None, opts=None):
     """records [B,K,F] (ct_decode) -> updates tracks/counts/boxes in place, on the current stream.
     With --public_det: public_ct [B,P,2] fp32 (each stream's public detection centres, image coordinates, first
     public_n[b] rows used) and public_n [B] int32, device tensors (P = max_public_dets).  The descriptor points at
     the buffers of this call, so a CUDA graph captured around it keeps reading them.  steps: optional [B] int32
-    device tensor that receives the Dijkstra search steps of each stream's Hungarian solve."""
+    device tensor that receives the Dijkstra search steps of each stream's Hungarian solve.  With stream_opts: one
+    ct_track_step_opts on `opts` (device ct_track_opts [B], default d_opts)."""
     if self.public_det and (public_ct is None or public_n is None):
       raise ValueError('--public_det: step() needs the public detections (public_ct, public_n)')
     assert records.is_cuda and records.dtype == torch.float32 and tuple(records.shape) == (self.B, self.K, self.F)
     self.desc.records = records.data_ptr()
-    if self.pay is None and not (self.hungarian or self.public_det or steps is not None):
+    if self.pay is None and not (self.per_stream or self.hungarian or self.public_det or steps is not None):
       L.check(L.lib().ct_track_step(C.byref(self.desc), L.stream_ptr()), 'ct_track_step')
       return
     a = self.assoc
@@ -277,7 +397,10 @@ class DeviceTracker(object):
     if steps is not None:
       assert steps.is_cuda and steps.dtype == torch.int32 and tuple(steps.shape) == (self.B,)
     a.steps = steps.data_ptr() if steps is not None else None
-    if self.pay is not None:
+    if self.per_stream:
+      L.check(L.lib().ct_track_step_opts(C.byref(self.desc), C.byref(a), C.byref(self.pay) if self.pay is not None
+                                         else None, self._opts(opts), None, 0, L.stream_ptr()), 'ct_track_step_opts')
+    elif self.pay is not None:
       L.check(L.lib().ct_track_step_payload(C.byref(self.desc), C.byref(a), C.byref(self.pay), L.stream_ptr()),
               'ct_track_step_payload')
     else:
@@ -289,7 +412,7 @@ class DeviceTracker(object):
     L.check(L.lib().ct_render_tracks(L.ptr(self.boxes), self.B * self.T, L.ptr(pre_hm), self.B, self.inp_h,
                                      self.inp_w, L.stream_ptr()), 'ct_render_tracks')
 
-  def step_mapped(self, records, streams, public_ct=None, public_n=None):
+  def step_mapped(self, records, streams, public_ct=None, public_n=None, opts=None):
     """step() on a compacted batch: records [n,K,F], streams int32 [>= n] device map (image i is stream streams[i];
     < 0: a padding image, nothing is written).  Streams that are not listed keep their tables byte for byte.
     public_ct / public_n stay indexed by the stream, as in step()."""
@@ -305,8 +428,13 @@ class DeviceTracker(object):
     a.public_ct = a.public_n = a.steps = None
     if self.public_det:
       a.public_ct, a.public_n = public_ct.data_ptr(), public_n.data_ptr()
-    L.check(L.lib().ct_track_step_mapped(C.byref(d), C.byref(a), C.byref(self.pay) if self.pay is not None else None,
-                                         L.ptr(streams), self.B, L.stream_ptr()), 'ct_track_step_mapped')
+    pay = C.byref(self.pay) if self.pay is not None else None
+    if self.per_stream:
+      L.check(L.lib().ct_track_step_opts(C.byref(d), C.byref(a), pay, self._opts(opts), L.ptr(streams), self.B,
+                                         L.stream_ptr()), 'ct_track_step_opts')
+      return
+    L.check(L.lib().ct_track_step_mapped(C.byref(d), C.byref(a), pay, L.ptr(streams), self.B, L.stream_ptr()),
+            'ct_track_step_mapped')
 
   def render_mapped(self, pre_hm, image_of):
     """render() on a compacted batch: pre_hm [n,1,H,W] fp32 <- the tracks of stream s splatted into image

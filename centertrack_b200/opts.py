@@ -92,6 +92,8 @@ class opts(object):
     opt.lr_step = [int(i) for i in opt.lr_step.split(',')]
     opt.test_scales = [float(i) for i in opt.test_scales.split(',')]
     opt.pre_img = False
+    # the thresholds as given, before the derivation below: a StreamRunner stream's own flags are derived from them
+    opt.thresh_args = {'out_thresh': opt.out_thresh, 'pre_thresh': opt.pre_thresh, 'new_thresh': opt.new_thresh}
     if 'tracking' in opt.task:
       opt.tracking = True
       opt.out_thresh = max(opt.track_thresh, opt.out_thresh)

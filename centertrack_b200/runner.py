@@ -75,6 +75,13 @@ Moving a video (`stream_state(b)`, `step_frames(..., restore={b: state})`, capac
 stream's last frame, camera and track rows; restoring it into a stream of this or another runner is a video start at the
 state's frame size and camera whose prologue stages that frame as pre_images and writes the rows verbatim
 (ct_track_restore) instead of seeding them.
+
+Per-stream tracker settings (`stream_opts`, `options=` at a video start, a StreamState's options): each stream may run
+its own out_thresh / pre_thresh / new_thresh (derived from its track_thresh as opts.py derives them), max_age,
+--hungarian and --public_det, so that stream b computes what Detector(opt_b).run computes.  They act only in the
+per-stream kernels (ct_track_step_opts, ct_track_start_opts / _restore_opts, ct_post_process_opts), which read one
+ct_track_opts record per stream from the slot's device copy; a slot's records are uploaded with its frames when they
+changed, so the graphs are never recaptured.
 """
 import ctypes as C
 
@@ -240,15 +247,20 @@ class StreamState(object):
     calib            float32 [3, 4] camera matrix
     tracks, counts, payload   tracking runners: the track rows [n, CT_TRK_FLOATS] (device), (n, id_count), and the
                      payload rows [n, Wp] (device) on head sets with payload fields; None otherwise
+    options          the stream's resolved tracker settings (resolve_options: out_thresh, new_thresh, pre_thresh,
+                     max_age, hungarian, public_det; out_thresh alone without a tracker), which restore= applies on a
+                     runner built with stream_opts (one built without runs its own opt on every stream); None on a
+                     runner that neither tracks nor post-processes
     input_size, record_layout, payload_layout, max_tracks, frame_format   the layout facts the importer checks
   A copy: the exporting runner may go on using the stream."""
 
   def __init__(self, frame, size, calib, tracks, counts, payload, input_size, record_layout, payload_layout, max_tracks,
-               frame_format):
+               frame_format, options=None):
     self.frame, self.size, self.calib = frame, tuple(size), calib
     self.tracks, self.counts, self.payload = tracks, counts, payload
     self.input_size, self.record_layout, self.payload_layout = tuple(input_size), record_layout, payload_layout
     self.max_tracks, self.frame_format = max_tracks, frame_format
+    self.options = dict(options) if options is not None else None
 
 
 class StreamRunner(object):
@@ -258,7 +270,7 @@ class StreamRunner(object):
 
   def __init__(self, model, B, H, W, K=100, precision='bf16', device='cuda', use_graph=True, opt=None,
                device_tracking=False, max_public_dets=512, calibs=None, frame_sizes=None, max_frame_size=None,
-               idle_streams=None, frame_format='bgr', device_post_process=False):
+               idle_streams=None, frame_format='bgr', device_post_process=False, stream_opts=None):
     """max_public_dets: with device_tracking and --public_det, the most public detections a stream may bring per
     frame (more raise ValueError; none is ever dropped).  calibs: with device_tracking on a 3D head set, one [3,4]
     camera matrix per stream (DeviceTracker's default otherwise; in frames mode Detector._get_default_calib of the
@@ -279,7 +291,17 @@ class StreamRunner(object):
     device_post_process (runners without device_tracking): each step also post-processes its records on the device
     (ct_post_process, inside the graph) into each stream's detections in its source pixels -- Detector.post_process +
     merge_outputs -- and downloads them with the records: fetch_results() / previous_results() give the host path's
-    dicts, fetch_detections() the tables.  calibs then give the 3D head sets' cameras, as with device_tracking."""
+    dicts, fetch_detections() the tables.  calibs then give the 3D head sets' cameras, as with device_tracking.
+    stream_opts (device_tracking or device_post_process): None, every stream runs opt (the launches and bytes of a
+    runner without it), or B entries, each None (opt) or a dict of the flags stream b runs with instead --
+    track_thresh, out_thresh, pre_thresh, new_thresh, max_age, hungarian, public_det with a tracker (resolved against
+    opt by device_tracker.resolve_options), out_thresh alone with device_post_process.  A stream changes them only at
+    a video start (options= of step_host / step_frames / load_device_inputs) or with a restore.  The track table's
+    rows come from the largest max_age among opt and these entries, and public detections are staged when opt or any
+    entry has public_det."""
+    if stream_opts is not None and not (device_tracking or device_post_process):
+      raise ValueError('stream_opts: the per-stream settings act in the tracker or the device post-processing; build '
+                       'the runner with device_tracking or device_post_process')
     if device_post_process and device_tracking:
       raise ValueError('device_post_process is for runners without a tracker: device_tracking already post-processes '
                        'the detections (fetch_results() gives its tracks)')
@@ -372,14 +394,20 @@ class StreamRunner(object):
       if self.frames_mode:
         geo = dict(centers=[m['c'] for m in self._meta], scales=[m['s'] for m in self._meta])
       self.tracker = DeviceTracker(self.opt, B, K, self.rec.shape[2], self.layout, H, W, self.device,
-                                   max_public_dets=max_public_dets, calibs=calibs, **geo)
+                                   max_public_dets=max_public_dets, calibs=calibs, stream_opts=stream_opts, **geo)
     elif device_post_process:
       assert self.opt is not None, 'device post-processing needs opt (out_thresh)'
       geo = {}
       if self.frames_mode:
         geo = dict(centers=[m['c'] for m in self._meta], scales=[m['s'] for m in self._meta])
       self.post = DeviceDetections(self.opt, B, K, self.rec.shape[2], self.layout, H, W, self.device, calibs=calibs,
-                                   **geo)
+                                   stream_opts=stream_opts, **geo)
+    self.d_opts = None
+    tables = self._geo_tables()
+    if self._per_stream():                        # per slot: device ct_track_opts [B], pinned staging, host mirror
+      self.d_opts = [tables.d_opts.clone() for _ in range(NS)]
+      self.h_opts = [tables.d_opts.cpu().pin_memory() for _ in range(NS)]
+      self._opts_mirror = [tables.opts_bytes()] * NS
     self.public = self.tracker is not None and self.tracker.public_det
     if self.public:                                          # per slot: device (public_ct, public_n) + pinned staging
       self.pub = [self.tracker.public_buffers() for _ in range(NS)]
@@ -636,15 +664,60 @@ class StreamRunner(object):
     if self.tracker is not None:                             # tracks(t)
       pub = self.pub[slot] if self.public else ()
       if self.idle_g is None:
-        self.tracker.step(self.rec, *pub)
+        self.tracker.step(self.rec, *pub, opts=self._slot_opts(slot))
       else:
-        self.tracker.step_mapped(self.rec[:n], self.d_map[slot][:self.B], *pub)
+        self.tracker.step_mapped(self.rec[:n], self.d_map[slot][:self.B], *pub, opts=self._slot_opts(slot))
     if self.post is not None:                                # each stream's detections in its source pixels
       if self.idle_g is None:
-        self.post.step(self.rec)
+        self.post.step(self.rec, opts=self._slot_opts(slot))
       else:
-        self.post.step_mapped(self.rec[:n], self.d_map[slot][:self.B])
+        self.post.step_mapped(self.rec[:n], self.d_map[slot][:self.B], opts=self._slot_opts(slot))
     return res
+
+  def _slot_opts(self, slot):
+    """The device ct_track_opts records slot's step reads (stream_opts runners), or None."""
+    return self.d_opts[slot] if getattr(self, 'd_opts', None) is not None else None
+
+  def _check_options(self, options, streams):
+    """options ({stream: flags} of streams that start a video in this step) -> {stream: resolved settings}; ValueError
+    before anything is enqueued (a stream that does not start, or what check_options refuses)."""
+    out = {}
+    for s, flags in (options or {}).items():
+      if s not in streams:
+        raise ValueError('options: stream %r does not start a video in this step; a stream changes its tracker '
+                         'settings only at a video start (starts=) or a restore' % (s,))
+      tables = self._geo_tables()
+      if tables is None:
+        raise ValueError('options: the runner has neither device_tracking nor device_post_process, whose settings they '
+                         'are')
+      out[s] = tables.check_options(flags, 'options[%d]' % s)
+    return out
+
+  def _per_stream(self):
+    """Whether the runner was built with stream_opts."""
+    return getattr(self._geo_tables(), 'per_stream', False)
+
+  def _step_options(self, planned):
+    """Each stream's settings in this step (stream_opts runners; None otherwise): the current ones with `planned`
+    ({stream: resolved}) applied."""
+    if not self._per_stream():
+      return None
+    return [planned.get(b, o) for b, o in enumerate(self._geo_tables().options)]
+
+  def _plan_options(self, slot, planned):
+    """Applies planned settings to the host state; -> the slot's ct_track_opts bytes to upload when its device copy
+    differs (staged in h_opts[slot]), else None."""
+    if getattr(self, 'd_opts', None) is None:
+      return None
+    tables = self._geo_tables()
+    for b, o in planned.items():
+      tables.options[b] = o
+    now = tables.opts_bytes()
+    if now == self._opts_mirror[slot]:
+      return None
+    self._opts_mirror[slot] = now
+    self.h_opts[slot].numpy()[:] = np.frombuffer(now, np.uint8)
+    return now
 
   def _decode_ws(self, n):
     """The decode workspace of a batch n <= B.  ct_decode keeps n per-image counters at its start, which must be zero
@@ -733,10 +806,11 @@ class StreamRunner(object):
     if self.tracker is not None:
       self.tracker.reset()
 
-  def _check_public(self, public_dets, idle=()):
+  def _check_public(self, public_dets, idle=(), options=None):
     """public_dets: list of B arrays [P_b, 2] (the `ct` of each of the frame's public detections, image coordinates)
     -> list of B float32 arrays; ValueError when they are missing, unexpected, or more than max_public_dets.  The
-    entries of `idle` streams are ignored (and may be None)."""
+    entries of `idle` streams are ignored (and may be None).  options (stream_opts runners: each stream's settings in
+    this step): a stream whose public_det is off must have a None entry."""
     if not self.public:
       if public_dets is not None:
         raise ValueError('public detections are only read by device tracking with --public_det')
@@ -747,7 +821,11 @@ class StreamRunner(object):
       raise ValueError('public_dets: expected %d arrays (one per stream), got %d' % (self.B, len(public_dets)))
     out = []
     for b, p in enumerate(public_dets):
-      if b in idle:
+      private = options is not None and not options[b]['public_det']
+      if private and p is not None and b not in idle:
+        raise ValueError('public_dets[%d]: stream %d runs without public_det (its stream_opts / options); its entry '
+                         'must be None' % (b, b))
+      if b in idle or private:
         out.append(np.zeros((0, 2), np.float32))
         continue
       a = np.asarray(p, np.float32)
@@ -768,11 +846,12 @@ class StreamRunner(object):
       ct[b, :len(a)] = torch.from_numpy(a)
       n[b] = len(a)
 
-  def _check_starts(self, starts, pre_dets):
+  def _check_starts(self, starts, pre_dets, options=None):
     """starts (stream indices whose frame in this step is a video's first) and pre_dets ({stream: list of result
     dicts} seeding the tracker of some of them, in each stream's source pixels like the tracks) -> (streams, seed rows)
     or None.  ValueError (device_tracker.plan_starts) before anything is enqueued; without device tracking a start only
-    switches pre_images, and pre_dets are refused."""
+    switches pre_images, and pre_dets are refused.  options: each stream's settings in this step (stream_opts
+    runners), whose new_thresh filters its seeds."""
     if starts is None or len(starts) == 0:
       if pre_dets:
         raise ValueError('pre_dets: stream(s) %s do not start a video in this step' % sorted(pre_dets))
@@ -782,7 +861,8 @@ class StreamRunner(object):
         raise ValueError('pre_dets seed the device tracker: this runner was built without device_tracking')
       return plan_starts(self.B, 0, 0.0, False, starts, None)
     trk = self.tracker
-    return plan_starts(self.B, trk.T, self.opt.new_thresh, trk.payload is not None, starts, pre_dets)
+    nt = [o['new_thresh'] for o in options] if options is not None else self.opt.new_thresh
+    return plan_starts(self.B, trk.T, nt, trk.payload is not None, starts, pre_dets)
 
   def _stage_starts(self, slot, plan):
     """The pinned staging of slot's start list (stream, seeds) and seed rows <- plan; -> (entries, seed rows).  The
@@ -837,10 +917,14 @@ class StreamRunner(object):
     self._geo[slot] = list(streams)
     return n * (6 * 8 + 18 * 4)
 
-  def load_device_inputs(self, images, pre_hms, slot, public_dets=None, starts=None, pre_dets=None, calibs=None):
-    """Copies step_device's inputs into `slot` on the current stream; starts / pre_dets / calibs as in step_host."""
-    pub = self._check_public(public_dets)
-    plan = self._check_starts(starts, pre_dets)
+  def load_device_inputs(self, images, pre_hms, slot, public_dets=None, starts=None, pre_dets=None, calibs=None,
+                         options=None):
+    """Copies step_device's inputs into `slot` on the current stream; starts / pre_dets / calibs / options as in
+    step_host."""
+    planned = self._check_options(options, self._streams_arg('starts', starts) if options else ())
+    now = self._step_options(planned)
+    pub = self._check_public(public_dets, (), now)
+    plan = self._check_starts(starts, pre_dets, now)
     cal = self._check_calibs(calibs, plan[0] if plan else ())
     self.img[slot][:self.B].copy_(images)
     if pre_hms is not None:
@@ -850,8 +934,11 @@ class StreamRunner(object):
       self.pub[slot][0].copy_(self.h_pub[slot][0])
       self.pub[slot][1].copy_(self.h_pub[slot][1])
     _, rows = self._plan_geometry(slot, {}, cal)
+    ob = self._plan_options(slot, planned)
+    if ob is not None:
+      self.d_opts[slot].copy_(self.h_opts[slot])
     self._start_bytes = self._upload_starts(slot, plan, non_blocking=False) + \
-        self._upload_geometry(slot, rows, non_blocking=False)
+        self._upload_geometry(slot, rows, non_blocking=False) + (len(ob) if ob is not None else 0)
 
   def _start_prologue(self, slot, streams, restores=None):
     """A step whose frames start new videos on `streams` or continue restored ones ({stream: StreamState}), before the
@@ -896,9 +983,9 @@ class StreamRunner(object):
     if geo:                                                  # new cameras: before the seeds' boxes are rendered
       self._geo_tables().set_geometry(geo, self.d_geo_in[slot], self.d_geo_out[slot])
     if self.tracker is not None and streams:                 # reset + seeds + boxes: the step's render splats them
-      self.tracker.start_device(self.d_start[slot], len(streams), self.d_seed[slot])
+      self.tracker.start_device(self.d_start[slot], len(streams), self.d_seed[slot], opts=self._slot_opts(slot))
     if self.tracker is not None and restores:                # the exported rows, boxes at this stream and camera
-      self._restore_tracks(restores)
+      self._restore_tracks(restores, self._slot_opts(slot))
 
   def _on_device(self, t):
     """t on the runner's device; a tensor of another device is copied over (on the current stream)."""
@@ -916,7 +1003,7 @@ class StreamRunner(object):
     L.check(L.lib().ct_stage_frames(srcs, dst, len(bs), L.ptr(self.u8[dst_slot]), self.slot_bytes, L.stream_ptr()),
             'ct_stage_frames')
 
-  def _restore_tracks(self, restores):
+  def _restore_tracks(self, restores, opts=None):
     """ct_track_restore of the restored streams' rows, on the current stream."""
     bs = sorted(restores)
     ent = torch.tensor([[b, restores[b].counts[0], restores[b].counts[1]] for b in bs], dtype=torch.int32)
@@ -924,7 +1011,7 @@ class StreamRunner(object):
     pay = [restores[b].payload for b in bs if restores[b].counts[0]] if self.tracker.payload is not None else []
     rows = torch.cat([self._on_device(r) for r in rows]) if rows else None
     pay = torch.cat([self._on_device(p) for p in pay]) if pay else None
-    self.tracker.restore_device(ent.to(self.device), len(bs), rows, pay)
+    self.tracker.restore_device(ent.to(self.device), len(bs), rows, pay, opts=opts)
 
   def _launch(self, slot):
     streams, self._starts[slot] = self._starts[slot], None
@@ -945,7 +1032,7 @@ class StreamRunner(object):
     self.t += 1
     return self.rec
 
-  def step_host(self, images, pre_hms=None, public_dets=None, starts=None, pre_dets=None, calibs=None):
+  def step_host(self, images, pre_hms=None, public_dets=None, starts=None, pre_dets=None, calibs=None, options=None):
     """images [B,3,H,W] (and pre_hms [B,1,H,W] unless device_tracking): float32 HOST tensors (what
     Detector.pre_process / _get_additional_inputs produce); with --public_det, public_dets = B arrays [P_b, 2] (the
     `ct`s of each frame's public detections).  starts: the streams whose frame in this step is a new video's first
@@ -953,15 +1040,23 @@ class StreamRunner(object):
     empty, or from pre_dets = {stream: list of result dicts} as Tracker.init_track; the other streams are unaffected).
     calibs: {stream: [3, 4] camera matrix} of some started streams, their camera from this frame on (3D head sets:
     loc, rot_y); a started stream without one keeps its camera.
+    options: {stream: flags} of some started streams (runners built with stream_opts): their tracker settings from this
+    frame on, resolved against opt as the constructor's stream_opts entries are; a started stream without one keeps
+    its settings.  ValueError, before anything is enqueued, for a stream that does not start, a key or value
+    resolve_options refuses, a max_age above the track table's capacity, or public_det on a runner that stages no
+    public detections.
     Returns the records of the PREVIOUS call (None the first time) -- a one-step software pipeline: this step's H2D
     overlaps the previous step's compute."""
     if self.idle_g is not None:
       raise ValueError('step_host: a runner built with idle_streams takes raw frames (step_frames)')
-    pub = self._check_public(public_dets)
-    plan = self._check_starts(starts, pre_dets)
+    planned = self._check_options(options, self._streams_arg('starts', starts) if options else ())
+    now = self._step_options(planned)
+    pub = self._check_public(public_dets, (), now)
+    plan = self._check_starts(starts, pre_dets, now)
     cal = self._check_calibs(calibs, plan[0] if plan else ())
     slot = self.t % NS
     _, rows = self._plan_geometry(slot, {}, cal)
+    ob = self._plan_options(slot, planned)
     if pub is not None:        # the slot's staging was last read by step t-3's upload, which the last fetch() waited for
       self._fill_public(self.h_pub[slot], pub)
     use_hm = self.tracker is None and pre_hms is not None
@@ -981,9 +1076,17 @@ class StreamRunner(object):
         self.pub[slot][0].copy_(self.h_pub[slot][0], non_blocking=True)
         self.pub[slot][1].copy_(self.h_pub[slot][1], non_blocking=True)
       self._start_bytes = self._upload_starts(slot, plan, non_blocking=True) + \
-          self._upload_geometry(slot, rows, non_blocking=True)
+          self._upload_geometry(slot, rows, non_blocking=True) + self._upload_options(slot, ob)
       self.ev_in[slot].record(self.copy)
     return self._submit(slot)
+
+  def _upload_options(self, slot, ob):
+    """Uploads slot's staged ct_track_opts records (_plan_options) when they changed, on the current (copy) stream;
+    -> the bytes uploaded."""
+    if ob is None:
+      return 0
+    self.d_opts[slot].copy_(self.h_opts[slot], non_blocking=True)
+    return len(ob)
 
   def _submit(self, slot):
     """The step of the uploaded slot on the compute stream and the D2H of its results; -> the previous step's
@@ -1106,7 +1209,7 @@ class StreamRunner(object):
   def _streams_arg(self, what, streams):
     """A list of distinct stream indices in [0, B) (None: empty); ValueError otherwise."""
     out = []
-    for s in streams or ():
+    for s in (() if streams is None else streams):
       if isinstance(s, (bool, np.bool_)) or not isinstance(s, (int, np.integer)):
         raise ValueError('%s: stream indices must be integers, got %r' % (what, s))
       s = int(s)
@@ -1207,6 +1310,15 @@ class StreamRunner(object):
       self._size_geometry('restore[%d]' % s, *st.size)
     return out
 
+  def _restore_options(self, rest):
+    """{stream: resolved settings} the restored states carry, on a runner built with stream_opts; ValueError as
+    check_options.  A runner built without stream_opts runs its own opt on every stream, restored ones included."""
+    tables = self._geo_tables()
+    if not self._per_stream():
+      return {}
+    return {s: tables.check_options(st.options, 'restore[%d]' % s, resolved=True)
+            for s, st in sorted(rest.items()) if st.options is not None}
+
   def stream_state(self, b):
     """Waits like fetch(), then returns stream b's StreamState after the last submitted step in which it had a frame:
     that frame (a device copy), its size and camera, and on a tracking runner its track rows, counts and payload rows.
@@ -1231,10 +1343,11 @@ class StreamRunner(object):
     self.compute.synchronize()
     return StreamState(frame, (f.h, f.w), np.array(self._meta[b]['calib'], np.float32).reshape(3, 4), tracks, counts,
                        pay, (self.H, self.W), dict(self.layout), trk.payload_layout if trk is not None else None,
-                       trk.T if trk is not None else None, self.frame_format)
+                       trk.T if trk is not None else None, self.frame_format,
+                       self._geo_tables().options[b] if self._geo_tables() is not None else None)
 
   def step_frames(self, frames, pre_hms=None, public_dets=None, starts=None, pre_dets=None, calibs=None, idle=None,
-                  layout='bgr', resume=None, restore=None):
+                  layout='bgr', resume=None, restore=None, options=None):
     """frames: B uint8 [h_b, w_b, 3] BGR arrays of the sizes given as frame_sizes (with frame_format 'nv12' / 'i420':
     [3h_b/2, w_b] arrays in that layout), or None when they were written through frame_buffers(), or B device frames
     (below).  pre_hms, public_dets, starts, pre_dets, calibs and the return value as in step_host;
@@ -1258,7 +1371,8 @@ class StreamRunner(object):
     stream with a frame in this step (a step never mixes the two).  A BGR runner takes [h, w, 3] with layout 'bgr' or
     'rgb', or [3, h, w] with layout 'rgb_planar'; an NV12 runner one [3h/2, w] tensor in cv2's layout or the planes
     (Y [h, w], UV [h/2, w]); an I420 runner one [3h/2, w] tensor of rows of exactly w bytes or the planes
-    (Y [h, w], U [h/2, w/2], V [h/2, w/2]).  Rows may have any pitch (views of wider or taller surfaces); the innermost
+    (Y [h, w], U [h/2, w/2], V [h/2, w/2]).  options as in step_host; a restored stream takes the state's options.
+    Rows may have any pitch (views of wider or taller surfaces); the innermost
     stride must be 1 (device_frame_source).  One ct_stage_frames copies them into the slot on the runner's copy stream,
     after the work queued on the caller's current stream at this call (which writes the frames); nothing of them is
     uploaded, and the step computes bit for bit what it computes on the same frames given as arrays (RGB swapped to
@@ -1267,13 +1381,16 @@ class StreamRunner(object):
     has completed: make the decoder's stream wait on it."""
     if not self.frames_mode:
       raise ValueError('step_frames: the runner was not built with frame_sizes (use step_host)')
-    plan = self._check_starts(starts, pre_dets)
+    planned = self._check_options(options, self._streams_arg('starts', starts) if options else ())
+    rest = self._check_restore(restore, self._streams_arg('starts', starts), idle)
+    planned.update(self._restore_options(rest))
+    now = self._step_options(planned)
+    plan = self._check_starts(starts, pre_dets, now)
     started = plan[0] if plan else ()
-    rest = self._check_restore(restore, started, idle)
     resumed = self._check_resume(resume, started, idle, rest)
     live = self._check_idle(idle, list(started) + sorted(rest) + resumed, pre_hms)
     gone = () if live is None else set(range(self.B)) - set(live)
-    pub = self._check_public(public_dets, gone)
+    pub = self._check_public(public_dets, gone, now)
     cal = self._check_calibs(calibs, started)
     cal.update((b, np.asarray(st.calib, np.float32)) for b, st in rest.items())   # a restore: the state's camera
     dev = None                                       # device frames: [(stream, ct_frame_src, tensors)]
@@ -1291,6 +1408,7 @@ class StreamRunner(object):
     slot = self.t % NS
     self._pending_sizes = None
     desc, rows = self._plan_geometry(slot, changed, cal, live)
+    ob = self._plan_options(slot, planned)
     copies = self._plan_resume(slot, live, resumed)
     self._restores[slot] = rest or None
     maps = None
@@ -1340,7 +1458,8 @@ class StreamRunner(object):
         self.pub[slot][0].copy_(self.h_pub[slot][0], non_blocking=True)
         self.pub[slot][1].copy_(self.h_pub[slot][1], non_blocking=True)
       self._start_bytes = self._upload_starts(slot, plan, non_blocking=True) + \
-          self._upload_geometry(slot, rows, non_blocking=True) + (12 * len(rest) if self.tracker is not None else 0)
+          self._upload_geometry(slot, rows, non_blocking=True) + (12 * len(rest) if self.tracker is not None else 0) + \
+          self._upload_options(slot, ob)
       self.ev_in[slot].record(self.copy)
     return self._submit(slot)
 

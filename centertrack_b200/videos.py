@@ -24,11 +24,14 @@ class Video(object):
   has: Detector._get_default_calib of its frame size when that size differs from the stream's last one, otherwise the
   stream's current camera -- which may be the `calib` of the previous video on that stream.  When some videos of a
   dataset carry a calib, give every video one (e.g. detector.default_calib of its size) so that its camera does not
-  depend on the stream it lands on."""
+  depend on the stream it lands on.
+  `options`: the tracker flags the video runs with (StreamRunner's options= at its start: track_thresh, out_thresh,
+  pre_thresh, new_thresh, max_age, hungarian, public_det), on a runner built with stream_opts; on such a runner a video
+  without options runs the runner's opt, whichever stream it lands on."""
 
-  def __init__(self, id, frames, pre_dets=None, public_dets=None, calib=None):
+  def __init__(self, id, frames, pre_dets=None, public_dets=None, calib=None, options=None):
     self.id, self.frames, self.pre_dets, self.public_dets = id, frames, pre_dets, public_dets
-    self.calib = calib
+    self.calib, self.options = calib, options
 
 
 class _Playing(object):
@@ -55,6 +58,8 @@ def track_videos(runner, videos, layout='bgr'):
   if layout != 'bgr' and not runner.frames_mode:
     raise ValueError('track_videos: layout=%r needs a frames-mode runner' % (layout,))
   B = runner.B
+  tables = runner.tracker if runner.tracker is not None else runner.post
+  per_stream = getattr(tables, 'per_stream', False)
   capacity = runner.frames_mode and getattr(runner, 'max_frame_bytes', None) is not None
   idle_runner = getattr(runner, 'idle_g', None) is not None
   fmt = getattr(runner, 'frame_format', 'bgr')
@@ -160,13 +165,22 @@ def track_videos(runner, videos, layout='bgr'):
         last[b] = filler(sizes[b])
       frames.append(last[b])
     pre_dets = {b: playing[b].video.pre_dets for b in started if playing[b].video.pre_dets is not None}
+    options = {b: playing[b].video.options or {} for b in started} if per_stream else \
+        {b: playing[b].video.options for b in started if playing[b].video.options is not None}
+    step_opts = runner._step_options({b: tables.check_options(o, 'video %r: options' % (playing[b].video.id,))
+                                      for b, o in options.items()}) if per_stream else None
     public = None
     if runner.public:
       public = []
-      for p in playing:
+      for b, p in enumerate(playing):
         pd = p.video.public_dets if p is not None else None
+        if per_stream and not step_opts[b]['public_det']:      # a stream without --public_det takes None
+          public.append(None)
+          continue
         public.append(np.zeros((0, 2), np.float32) if pd is None else pd[p.index])
     kw = dict(public_dets=public, starts=started, pre_dets=pre_dets or None)
+    if options:
+      kw['options'] = options
     if idle_runner:
       kw['idle'] = [b for b, p in enumerate(playing) if p is None]
     calibs = {b: playing[b].video.calib for b in started if playing[b].video.calib is not None}

@@ -28,6 +28,9 @@
  *                     tracks on another stream or runner.
  *   ct_post_process   Detector.post_process + merge_outputs (detector.py:356-377) on the device for runners without a
  *                     tracker: each stream's kept detections in its source pixels, with ct_track_step's arithmetic.
+ *   ct_track_step_opts, ct_track_start_opts, ct_track_restore_opts, ct_post_process_opts   the same launches with each
+ *                     stream's own tracker settings (a ct_track_opts record per stream: thresholds, max_age,
+ *                     --hungarian, --public_det), as if each stream were its own Detector(opt_b).
  *   ct_flip_merge     Detector._flip_output, detector.py:311-332 (flip_tensor / flip_lr / flip_lr_off, model/utils.py:28-50);
  *                     ct_flip_merge_heads merges every head of B pairs at once, ct_mirror_x mirrors the --flip_test
  *                     batch's second half (detector.py:225-226,285-286).
@@ -365,6 +368,36 @@ int ct_track_start(const ct_track_desc* d, const ct_track_payload* p, const int3
  * n_entries == 0 launches nothing.  Reads what ct_track_start reads. */
 int ct_track_restore(const ct_track_desc* d, const ct_track_payload* p, const int32_t* entries, int32_t n_entries,
                      const float* rows, const float* payload_rows, void* stream);
+/* Per-stream tracker settings: what opt_b (the runner's opt with a stream's flags, derived as opts.py:97-99 derives
+ * them) gives the per-stream kernels.  32 bytes, read once per CTA. */
+typedef struct {
+  float out_thresh;           /* as ct_track_desc's (ct_post_process_opts reads only this field) */
+  float new_thresh;
+  float pre_thresh;
+  int32_t max_age;            /* <= the max_age the table's T rows were sized for (T = K (1 + max_age)) */
+  int32_t hungarian;          /* 1: --hungarian */
+  int32_t public_det;         /* 1: --public_det (only where the launch's ct_track_assoc has public_det set) */
+  int32_t reserved[2];
+} ct_track_opts;
+
+/* ct_track_step_payload / ct_track_step_mapped with per-stream settings: stream b (the CTA's stream, as in either form)
+ * runs opts[b] (device ct_track_opts [n_streams], or [d->B] when streams == NULL) in place of d's out_thresh,
+ * new_thresh, pre_thresh, max_age and a's hungarian / public_det.  Greedy and Hungarian, private and public births may be
+ * mixed in one launch; the association scratch is always allocated (ct_track_payload_smem_bytes(.., assoc = 1)).
+ * a (may be NULL: no public detections, no steps) supplies the buffers: a->public_det = 1 means the launch has
+ * public_ct / public_n (checked as ct_track_step_assoc checks them), and a stream runs --public_det only when both its
+ * record and a->public_det say so; a stream whose record has public_det = 0 ignores public_n.  p == NULL: no payload.
+ * streams == NULL: CTA i runs stream i of d->B.  CT_ERR_INVALID for NULL opts, n_streams < 0, a map with
+ * n_streams == 0, or what ct_track_step_payload refuses. */
+int ct_track_step_opts(const ct_track_desc* d, const ct_track_assoc* a, const ct_track_payload* p,
+                       const ct_track_opts* opts, const int32_t* streams, int32_t n_streams, void* stream);
+/* ct_track_start / ct_track_restore whose render boxes use opts[b].pre_thresh (device ct_track_opts [d->B]) for each
+ * entry's stream b.  CT_ERR_INVALID for NULL opts, or what ct_track_start / ct_track_restore refuse. */
+int ct_track_start_opts(const ct_track_desc* d, const ct_track_payload* p, const ct_track_opts* opts,
+                        const int32_t* starts, int32_t n_starts, const float* seeds, void* stream);
+int ct_track_restore_opts(const ct_track_desc* d, const ct_track_payload* p, const ct_track_opts* opts,
+                          const int32_t* entries, int32_t n_entries, const float* rows, const float* payload_rows,
+                          void* stream);
 /* pre_hm (fp32 [B,1,H,W], zeroed here) <- max-splat of boxes [n,5] (rows with radius < 0 skipped); n is the grid size,
  * so the launch shape does not depend on the data (CUDA-graph capturable). */
 int ct_render_tracks(const float* boxes, int32_t n, float* pre_hm, int32_t B, int32_t H, int32_t W, void* stream);
@@ -407,6 +440,10 @@ typedef struct {
  * a map, or a field outside the record / payload width / missing calib as ct_track_step_payload checks them. */
 int ct_post_process(const ct_det_desc* d, const ct_track_payload* p, const int32_t* streams, int32_t n_streams,
                     void* stream);
+/* ct_post_process with stream b keeping its records with score > opts[b].out_thresh (device ct_track_opts
+ * [n_streams]; the other fields are not read).  CT_ERR_INVALID for NULL opts, or what ct_post_process refuses. */
+int ct_post_process_opts(const ct_det_desc* d, const ct_track_payload* p, const ct_track_opts* opts,
+                         const int32_t* streams, int32_t n_streams, void* stream);
 
 /* out[c,y,x] = (in2[0,c,y,x] + sign[c] * in2[1,perm[c],y,W-1-x]) / 2;  in2 fp32 [2,C,H,W], out [1,C,H,W];
  * perm (int32 [C], device) / sign (fp32 [C], device) may be NULL (identity / +1). */

@@ -201,7 +201,9 @@ def test_batch_prefix_matches_full_batch_at_bench_shape():
   """mot 544x960 bf16 at B = 32 replayed once; then forward(n) on the first n images: every op's output on those images
   equals the full-batch run bit for bit (fused heads and space-to-depth buffers included), and not one byte of the other
   images changes -- they are filled with 0xff (a NaN in bf16 and fp32) before the run, inputs included, so a launch that
-  read them would also spoil the first n."""
+  read them would also spoil the first n.  Images < n are restored to the full-batch result before each run, so an
+  element of them that forward(n) leaves unwritten still passes: test_gpu_plan_fresh_state.py's
+  test_graph_eager_and_prefix_agree_from_poisoned_buffers poisons every image and restores nothing."""
   from helpers import make_model
   from centertrack_b200 import synthetic as syn
   B, (H, W) = 32, pr.BENCH_SHAPES['mot']

@@ -798,6 +798,9 @@ static int tc_config(const ct_conv_desc* d, TcArgs& a, ConvConfig& c) {
   const bool win = d->a_mode == CT_A_DCN_WIN;
   if (win && (x3 || g.C_in % 64 != 0))
     return fail(CT_ERR_INVALID, "conv_tc: CT_A_DCN_WIN needs the bf16 engine and C_in %% 64 == 0%s (%ld)", "", g.C_in);
+  // dcn_row reads a pixel's offset / mask row as 16-byte vectors: consecutive rows must stay 16 bytes apart
+  if (d->a_mode != CT_A_CONV && g.ld_om % 4 != 0)
+    return fail(CT_ERR_INVALID, "conv_tc: DCN needs ld_om %% 4 == 0 (16-byte offset / mask rows)%s (%ld)", "", g.ld_om);
   static const int win_margin = getenv("CTB_TC_DCN_MARGIN") ? atoi(getenv("CTB_TC_DCN_MARGIN")) : 2;
   a.win_m = win_margin < 0 ? 0 : (win_margin > 6 ? 6 : win_margin);
   a.win_pw = 16 + 2 * a.win_m + 3;
@@ -882,6 +885,8 @@ int conv_forward_tc(const ct_conv_desc* d, cudaStream_t st) {
   if (rc != CT_OK) return rc;
   if (((uintptr_t)d->x & 15) || ((uintptr_t)d->w & 15) || ((uintptr_t)d->out & 15) || ((uintptr_t)d->residual & 15))
     return fail(CT_ERR_INVALID, "conv_tc: x/w/out/residual must be 16-byte aligned%s", "");
+  if (d->a_mode != CT_A_CONV && ((uintptr_t)d->om & 15))
+    return fail(CT_ERR_INVALID, "conv_tc: DCN needs a 16-byte aligned om%s", "");
   a.x = (const __nv_bfloat16*)d->x;
   a.w = (const __nv_bfloat16*)d->w;
   a.shift = d->shift;

@@ -58,7 +58,12 @@ class DCN(nn.Module):
 
   def _pack(self, device, P):
     sms = torch.cuda.get_device_properties(device).multi_processor_count
-    key = (self.precision, str(device), P >= sms * 128)
+    # each parameter's storage and version counter: an in-place update of the parameter (mul_, copy_, nn.init) or a
+    # re-assigned .data repacks, as upstream DCNv2 reads self.weight on every call.  An in-place update THROUGH .data
+    # (p.data.mul_(2)) changes neither, so it is not seen until load_state_dict / reset_parameters: update the
+    # parameter itself under torch.no_grad() instead
+    params = (self.weight, self.bias, self.conv_offset_mask.weight, self.conv_offset_mask.bias)
+    key = (self.precision, str(device), P >= sms * 128) + tuple((p.data_ptr(), p._version) for p in params)
     if self._packed is not None and self._packed[0] == key:
       return self._packed[1]
     lib = L.lib()

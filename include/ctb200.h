@@ -135,7 +135,8 @@ typedef struct {
   int32_t head_act;      /* ct_head_act (CT_OUT_NCHW_F32 only) */
   int32_t sig_from;      /* CT_OUT_NHWC_F32: sigmoid applied to channels >= sig_from (DCN mask) */
   float   depth_scale;
-  int32_t ld_om;         /* CT_A_DCN: pixel stride of `om` (fp32 NHWC, >= 27) */
+  int32_t ld_om;         /* CT_A_DCN / CT_A_DCN_WIN: pixel stride of `om` (fp32 NHWC, >= 27).  The wgmma engines read
+                            each pixel's row as 16-byte vectors: there ld_om % 4 == 0 and om 16-byte aligned */
   int32_t n_tile;        /* wgmma engines: output-channel tile (multiple of 16, <= 256; required) */
   int32_t epilogue_sum3; /* HALO engine, C_out == 48: out16 = sum over present groups g (bit g set) of
                             relu(acc[16g..16g+15] + shift) -- the three DLA stems (dla.py:307-311) */

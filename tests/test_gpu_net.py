@@ -168,23 +168,112 @@ def test_module_surface_and_dcn_module():
   opt.model_output_list = True
   lst = model(img.cuda(), pre.cuda(), hm.cuda())[0]
   assert isinstance(lst, list) and len(lst) == len(opt.heads)
-  # DCN module: same parameter names as upstream, forward == oracle restatement
+  # DCN module: same parameter names as upstream (its values: the DCN module tests below)
   d = DCN(64, 128).cuda()
   assert sorted(k for k, _ in d.named_parameters()) == ['bias', 'conv_offset_mask.bias', 'conv_offset_mask.weight', 'weight']
-  g = torch.Generator().manual_seed(2)
-  with torch.no_grad():
-    d.conv_offset_mask.weight.copy_(torch.randn(27, 64, 3, 3, generator=g) * 0.02)
-    d.conv_offset_mask.bias.copy_(torch.randn(27, generator=g))
-    d.bias.copy_(torch.randn(128, generator=g))
-  x = torch.randn(2, 64, 12, 20, generator=g)
-  ref = co.dcn_v2_forward(x, d.weight.detach().cpu(), d.bias.detach().cpu(), d.conv_offset_mask.weight.detach().cpu(),
-                          d.conv_offset_mask.bias.detach().cpu())
-  d.precision = 'fp32'
-  assert (d(x.cuda()).cpu() - ref).abs().max() < 1e-4
-  d.precision = 'bf16'
-  assert (d(x.cuda()).cpu() - ref).abs().max() < 5e-2
   with pytest.raises(RuntimeError, match='no CPU fallback'):
-    d(x)
+    d(torch.zeros(1, 64, 8, 8))
+
+
+# The DeformConv layers of DLASeg (make_model('coco_tracking'): {dla_up.ida_*, ida_up}.{proj,node}_*.conv), as
+# (C_out, C_in, side of the map a 512 x 512 input gives them: 128 x 128 at 64 channels, halved per doubling).
+DCN_SHAPES = [(64, 64, 128), (64, 128, 64), (128, 128, 64), (128, 256, 32), (256, 256, 32), (256, 512, 16), (64, 256, 32)]
+
+
+def test_dcn_shapes_are_dlaseg_s():
+  _, _, sd = make_model('coco_tracking')
+  got = {tuple(v.shape[:2]) for k, v in sd.items() if k.startswith(('dla_up.ida_', 'ida_up.')) and
+         k.endswith('.conv.weight') and ('.proj_' in k or '.node_' in k)}
+  assert got == {(o, i) for o, i, _ in DCN_SHAPES}
+
+
+def _check_dcn_module(d, x, what):
+  """d(x) against the fp64 oracle of d's current parameters, per element (tests/bounds.py) the way test_dcn_v2 does
+  it: the offset / mask conv (the same launch the module makes) within its own bound, then the columns built from those
+  device offsets -- the bf16 sampler's rounding points emulated exactly -- and the GEMM's bound on the output."""
+  import bounds as bd
+  from centertrack_b200 import _lib as L
+  from gpu_helpers import run_conv
+  tc = d.precision == 'bf16'
+  engine, dtype, coef = (L.CT_ENGINE_TCGEN05, L.CT_BF16, bd.ALPHA_BF16) if tc else (L.CT_ENGINE_SIMT, L.CT_F32, bd.GAMMA_SIMT)
+  rq = (lambda t: t.detach().float().bfloat16().double()) if tc else (lambda t: t.detach().double())
+  with torch.no_grad():
+    got = d(x)
+  torch.cuda.synchronize()
+  xq = rq(x)
+  wo, bo = d.conv_offset_mask.weight.detach(), d.conv_offset_mask.bias.detach()
+  om_ref, om_mag = bd.conv_ref(xq, rq(wo), bo, pad=(1, 1, 1, 1))
+  om = run_conv(engine, dtype, x, wo.float().cpu(), bo.float().cpu(), 1, relu=False, out_mode=L.CT_OUT_NHWC_F32,
+                sig_from=18, n_tile=32)
+  bd.assert_bound(om[:, :18], om_ref[:, :18], om_mag[:, :18], coef, False, what + ' offsets')
+  bd.assert_bound(om[:, 18:27], om_ref[:, 18:27], om_mag[:, 18:27], coef, False, what + ' mask', 'sigmoid')
+  cols = co.dcn_sample_columns(xq, om[:, :18].contiguous(), om[:, 18:27].contiguous(), bf16_blend=tc)
+  B, C, _, H, W = cols.shape
+  wm, cm = rq(d.weight).reshape(-1, C * 9), cols.reshape(B, C * 9, H * W)
+  b = d.bias.detach().double().view(1, -1, 1, 1)
+  ref = torch.matmul(wm, cm).view(B, -1, H, W) + b
+  mag = torch.matmul(wm.abs(), cm.abs()).view(B, -1, H, W) + b.abs()
+  assert got.dtype == x.dtype and got.shape == ref.shape
+  return bd.assert_bound(got, ref, mag, coef, tc, what)
+
+
+def _random_dcn(cin, cout, seed):
+  from centertrack_b200.dcn import DCN
+  d = DCN(cin, cout).cuda()
+  g = torch.Generator().manual_seed(seed)
+  with torch.no_grad():
+    d.conv_offset_mask.weight.copy_(torch.randn(27, cin, 3, 3, generator=g) * (0.6 / (cin * 9) ** 0.5))
+    d.conv_offset_mask.bias.copy_(torch.randn(27, generator=g) * 1.5)
+    d.bias.copy_(torch.randn(cout, generator=g) * 0.1)
+  return d, g
+
+
+@pytest.mark.parametrize('B', [1, 2])
+@pytest.mark.parametrize('precision', ['bf16', 'fp32'])
+@pytest.mark.parametrize('shape', DCN_SHAPES, ids=['%d-%d-%dx%d' % (o, i, s, s) for o, i, s in DCN_SHAPES])
+def test_dcn_module_matches_oracle_at_dlaseg_shapes(shape, precision, B):
+  """Every DeformConv shape of DLASeg at its 512 x 512 map size, B = 1 and 2, both precisions (the module's wide
+  n-tile side, at C_out > 64 and large maps: test_dcn_module_n_tile_switch)."""
+  cout, cin, side = shape
+  d, g = _random_dcn(cin, cout, cin + cout)
+  d.precision = precision
+  x = torch.randn(B, cin, side, side, generator=g).cuda()
+  m = _check_dcn_module(d, x, 'DCN %d -> %d %dx%d B %d %s' % (cin, cout, side, side, B, precision))
+  print('\n[DCN %d -> %d %dx%d B %d %s] worst |err| / bound %.3f' % (cin, cout, side, side, B, precision, m))
+
+
+def test_dcn_module_n_tile_switch():
+  """The bf16 module packs its main weights at n_tile 64 below one 128-pixel tile per SM and at min(256, C_out) from
+  there on (C_out > 64): 128 -> 128 at 64 x 64 (a DLASeg shape) with the largest B below the switch and the smallest B
+  at it, on one module, back and forth -- each side repacked and within the bound."""
+  d, g = _random_dcn(128, 128, 21)
+  d.precision = 'bf16'
+  sms = torch.cuda.get_device_properties(torch.device('cuda')).multi_processor_count
+  b_lo = (sms * 128 - 1) // (64 * 64)
+  for B, n_main in ((b_lo, 64), (b_lo + 1, 128), (b_lo, 64)):
+    x = torch.randn(B, 128, 64, 64, generator=g).cuda()
+    m = _check_dcn_module(d, x, 'DCN 128 -> 128 64x64 B %d' % B)
+    assert d._packed[1]['n_main'] == n_main and d._packed[0][2] == (n_main == 128), (B, d._packed[0][:3])
+    print('\n[DCN 128 -> 128 64x64 B %d, n_tile %d] worst |err| / bound %.3f' % (B, n_main, m))
+
+
+def test_dcn_module_sees_in_place_parameter_updates():
+  """Upstream DCNv2 reads its parameters on every call: after an in-place mul_, copy_ or nn.init of any of them, the
+  next forward must use the new values (the module caches its packed weights)."""
+  d, g = _random_dcn(64, 64, 11)
+  x = torch.randn(2, 64, 16, 24, generator=g).cuda()
+  params = [('weight', d.weight), ('bias', d.bias), ('conv_offset_mask.weight', d.conv_offset_mask.weight),
+            ('conv_offset_mask.bias', d.conv_offset_mask.bias)]
+  for precision in ('bf16', 'fp32'):
+    d.precision = precision
+    _check_dcn_module(d, x, 'DCN %s before the updates' % precision)
+    for name, p in params:
+      edits = [('mul_', lambda: p.mul_(-1.5)), ('copy_', lambda: p.copy_(torch.randn(p.shape, generator=g) * float(p.std()))),
+               ('nn.init', lambda: torch.nn.init.uniform_(p, -float(p.abs().max()), float(p.abs().max())))]
+      for op, edit in edits:
+        with torch.no_grad():
+          edit()
+        _check_dcn_module(d, x, 'DCN %s after %s.%s' % (precision, name, op))
 
 
 def test_checkpoint_roundtrip_and_module_prefix(tmp_path):

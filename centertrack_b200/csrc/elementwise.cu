@@ -462,7 +462,9 @@ static inline int ew_blocks(size_t total) {
 extern "C" int ct_maxpool2(const void* x, void* out, int32_t dtype, int32_t B, int32_t H, int32_t W,
                            int32_t C, int32_t ld_in, int32_t ld_out, void* stream) {
   CT_REQUIRE(x && out, "null pointer");
+  CT_REQUIRE(B > 0 && H > 0 && W > 0 && C > 0, "bad shape");
   CT_REQUIRE(H % 2 == 0 && W % 2 == 0, "odd spatial size");
+  CT_REQUIRE(ld_in >= C && ld_out >= C, "ld_in, ld_out >= C");
   const int vecw = dtype == CT_F32 ? 4 : 8;
   CT_REQUIRE(C % vecw == 0 && ld_in % vecw == 0 && ld_out % vecw == 0, "channels / strides must be multiples of 16 bytes");
   const size_t total = (size_t)B * (H / 2) * (W / 2) * (C / vecw);
@@ -497,6 +499,8 @@ __global__ void maxpool2_s2d_kernel(const T* __restrict__ x, T* __restrict__ out
 extern "C" int ct_maxpool2_s2d(const void* x, void* out, int32_t dtype, int32_t B, int32_t H2, int32_t W2, int32_t C,
                                int32_t ld_in, int32_t ld_out, void* stream) {
   CT_REQUIRE(x && out, "null pointer");
+  CT_REQUIRE(B > 0 && H2 > 0 && W2 > 0 && C > 0, "bad shape");
+  CT_REQUIRE(ld_out >= C, "ld_out >= C");
   const int vecw = dtype == CT_F32 ? 4 : 8;
   CT_REQUIRE(C % vecw == 0 && ld_in % vecw == 0 && ld_out % vecw == 0 && ld_in >= 4 * C,
              "channels / strides must be multiples of 16 bytes, ld_in >= 4 C");
@@ -515,6 +519,8 @@ extern "C" int ct_upsample_add(const void* x, const void* skip, const float* w, 
                                int32_t ld_skip, int32_t ld_out, void* stream) {
   CT_REQUIRE(x && w && out, "null pointer");
   CT_REQUIRE(f == 2 || f == 4 || f == 8, "unsupported upsample factor");
+  CT_REQUIRE(B > 0 && H > 0 && W > 0 && C > 0, "bad shape");
+  CT_REQUIRE(ld_in >= C && ld_out >= C && (skip == nullptr || ld_skip >= C), "ld_in, ld_out, ld_skip >= C");
   const int vec = dtype == CT_F32 ? 4 : 8;
   CT_REQUIRE(C % vec == 0 && ld_in % vec == 0 && ld_out % vec == 0 && (skip == nullptr || ld_skip % vec == 0),
              "channels / strides must be multiples of the 16-byte vector width");

@@ -43,15 +43,39 @@ OUT_MODE = {L.CT_OUT_NHWC: 'nhwc', L.CT_OUT_NHWC_F32: 'nhwc_f32', L.CT_OUT_NCHW_
 BENCH_SHAPES = {'coco_tracking': (512, 512), 'mot': (544, 960), 'nuscenes_ddd': (448, 800), 'coco_pose': (512, 512)}
 PRECISIONS = ('bf16', 'bf16x3', 'fp32')
 BATCHES = (1, 2, 4, 8, 16, 32, 64)
+# the --keep_res sizes of the large cameras stop at B = 16: from B = 32 on, bf16x3 is refused (an input past 2^31
+# elements) and the fp32 plans alone hold 60 GB (928 x 1632) and 65 GB (1088 x 1920) of buffers at B = 32, 120 and
+# 131 GB at B = 64, so that neither they nor the full-size audit of their largest launches (tests/test_gpu_plan_rows.py)
+# fit an 80 GB H100
+KEEP_BATCHES = (1, 2, 4, 8, 16)
+
+# input sizes the product builds plans at beyond the bench: (name, config, (H, W), extra options, batches).  --keep_res
+# pads each camera's frame up to a multiple of 32 (detector.frame_geometry), a StreamRunner stream can switch to such a
+# camera at a video start, and --input_h / --input_w / --input_res / --fix_short take any multiple of 32.  The name
+# starts the plan id: the config's, or the dataset's where the options change the model.  Map-size-dependent choices
+# (TMA or register gather, N tile, halo stages, work items per persistent CTA) differ from the bench sizes', and the
+# partial edge patches, TMA boxes overhanging the map and the upsample's grid-stride carries depend on H and W.
+PRODUCT_SHAPES = [
+    ('mot', 'mot', (1088, 1920), [], KEEP_BATCHES),                   # a 1080p camera under --keep_res
+    ('nuscenes_ddd', 'nuscenes_ddd', (928, 1632), [], KEEP_BATCHES),  # nuScenes' 900 x 1600 under --keep_res
+    ('kitti_tracking', 'coco_tracking', (384, 1280), ['--num_classes', '3'], BATCHES),  # kitti(_tracking)'s default
+    ('kitti_tracking', 'coco_tracking', (384, 1248), ['--num_classes', '3'], BATCHES),  # KITTI's 375 x 1242, --keep_res
+    ('coco_tracking', 'coco_tracking', (480, 640), [], BATCHES),      # a VGA camera under --keep_res
+    ('coco_tracking', 'coco_tracking', (64, 1024), [], BATCHES),      # a wide strip: level 5 is 2 x 32
+    ('coco_tracking', 'coco_tracking', (32, 64), [], BATCHES),        # the smallest input: level 5 is 1 x 2
+]
 
 
 def plan_id(cfg, hw, B, precision):
   return '%s_%dx%d_b%d_%s' % (cfg, hw[0], hw[1], B, precision)
 
 
-# (id, config, (H, W), B, precision), in the order TARGETED was filled: batch, then config, then precision
-PRODUCT_PLANS = [(plan_id(cfg, BENCH_SHAPES[cfg], B, p), cfg, BENCH_SHAPES[cfg], B, p)
-                 for B in BATCHES for cfg in sorted(BENCH_SHAPES) for p in PRECISIONS]
+# (id, config, (H, W), B, precision, extra options), in the order TARGETED was filled: bench.py's shapes by batch, then
+# config, then precision; then PRODUCT_SHAPES by batch, then shape, then precision
+PRODUCT_PLANS = [(plan_id(cfg, BENCH_SHAPES[cfg], B, p), cfg, BENCH_SHAPES[cfg], B, p, [])
+                 for B in BATCHES for cfg in sorted(BENCH_SHAPES) for p in PRECISIONS] + \
+    [(plan_id(name, hw, B, p), cfg, hw, B, p, extra)
+     for B in BATCHES for name, cfg, hw, extra, batches in PRODUCT_SHAPES if B in batches for p in PRECISIONS]
 
 # product plans test_gpu_plan_layers.CASES audits whole, every op: bench.py's default batch in bf16 for every config,
 # and in bf16x3 for the three whose deep maps differ (coco_pose shares coco_tracking's backbone and neck)
@@ -59,8 +83,11 @@ WHOLE_PLANS = [plan_id(cfg, BENCH_SHAPES[cfg], 32, p) for cfg in sorted(BENCH_SH
                if not (cfg == 'coco_pose' and p == 'bf16x3')]
 
 # product plans the library refuses to build, -> what the refusal says.  nuScenes' two-pass heads at B = 64 in bf16x3:
-# the 1x1 heads read a 2048-channel intermediate of 2.9e9 elements, beyond the gather engine's 32-bit offsets.
-REFUSED = {plan_id('nuscenes_ddd', BENCH_SHAPES['nuscenes_ddd'], 64, 'bf16x3'): 'input tensor exceeds 2^31 elements'}
+# the 1x1 heads read a 2048-channel intermediate of 2.9e9 elements, beyond the gather engine's 32-bit offsets; under
+# --keep_res at 928 x 1632 the same from B = 16 (3.1e9 elements).  (At B = 32, which KEEP_BATCHES leaves out, mot at
+# 1088 x 1920 is refused too: its 1024-channel head intermediate has 4.3e9 elements.)
+REFUSED = {plan_id(cfg, hw, B, 'bf16x3'): 'input tensor exceeds 2^31 elements'
+           for cfg, hw, B in (('nuscenes_ddd', BENCH_SHAPES['nuscenes_ddd'], 64), ('nuscenes_ddd', (928, 1632), 16))}
 
 # product plan id -> the ops tests/test_gpu_plan_rows.py audits in it: for each row that no test_gpu_plan_layers.CASES
 # plan and no earlier entry runs, the first op of the plan that runs it (see `python tests/plan_rows.py`)
@@ -95,6 +122,11 @@ TARGETED = {
     'coco_pose_512x512_b64_bf16': ['base.level5.tree1.conv1', 'base.level5.tree1', 'base.level5.tree2.conv1',
                                    'base.level5', 'dla_up.ida_0.proj_1.offset', 'dla_up.ida_0.node_1.offset'],
     'mot_544x960_b64_bf16': ['dla_up.ida_0.proj_1'],
+    # PRODUCT_SHAPES: the rows test_gpu_plan_layers' cases at those sizes do not run
+    'coco_tracking_64x1024_b1_bf16x3': ['base.level1', 'heads.0'],
+    'mot_1088x1920_b2_bf16': ['dla_up.ida_0.node_1.offset'],
+    'coco_tracking_32x64_b4_bf16x3': ['stem48'],
+    'coco_tracking_32x64_b64_bf16': ['base.level3.tree1.tree1', 'base.level3.tree1.tree2.conv1'],
 }
 
 
@@ -103,15 +135,24 @@ TARGETED = {
 # `python tests/plan_rows.py`)
 EXTENT_TARGETED = {
     # bf16x3: the stem's 48-channel fp32 output, and the 1x1 heads reading 256-channel slices of the 1024- / 1792-channel
-    # fp32 head intermediate (mot's is 99.6 % of the gather engine's 2^31-element limit)
+    # fp32 head intermediate (mot's is 99.6 % of the gather engine's 2^31-element limit; coco_tracking's largest is
+    # at 480 x 640)
     'coco_pose_512x512_b64_bf16x3': ['hm_hp', 'hps'],
-    'coco_tracking_512x512_b64_bf16x3': ['hm'],
     'mot_544x960_b64_bf16x3': ['stem48', 'base.level0', 'heads.0', 'hm'],
-    # the SIMT engine: eight heads' 2048-channel intermediate, 2.9e9 elements
+    'coco_tracking_480x640_b64_bf16x3': ['hm'],
+    # the SIMT engine: eight heads' 2048-channel intermediate, 3.1e9 elements under nuScenes' --keep_res at B = 16
+    'nuscenes_ddd_928x1632_b16_fp32': ['heads.0', 'hm'],
+}
+
+# bench.py's own launches of rows whose largest launch EXTENT_TARGETED names at a PRODUCT_SHAPES size: also run at full
+# size by tests/test_gpu_plan_rows.py, being what the benchmarked configs run at B = 64 (each must still have an operand
+# of at least LARGE bytes, in a row of large_launches())
+EXTENT_BENCH = {
+    'coco_tracking_512x512_b64_bf16x3': ['hm'],
     'nuscenes_ddd_448x800_b64_fp32': ['heads.0', 'hm'],
 }
 
-LARGE = 1 << 31          # bytes: an operand this large has elements (or bytes) past a 32-bit signed offset
+LARGE =1 << 31          # bytes: an operand this large has elements (or bytes) past a 32-bit signed offset
 
 
 def _conv_work(eng, d, kern, cfg):
@@ -208,10 +249,10 @@ def large_launches():
   """{row: (plan id, op, bytes, elements, operand)}: for every row with an operand of at least LARGE bytes in a
   (buildable) PRODUCT_PLANS plan, the op with the largest operand in that row, at the first plan that has it."""
   big = {}
-  for pid, cfg, hw, B, precision in PRODUCT_PLANS:
+  for pid, cfg, hw, B, precision, extra in PRODUCT_PLANS:
     if pid in REFUSED:
       continue
-    eng = cpu_plan(cfg, hw, B, precision)
+    eng = cpu_plan(cfg, hw, B, precision, extra)
     rows = {sp['name']: launch_row(eng, sp) for sp in eng.specs}
     for name, ext in op_extents(eng).items():
       nbytes, n, k = largest_operand(ext)
@@ -278,10 +319,10 @@ def unaudited(cases, targeted):
   row once, at the first plan (PRODUCT_PLANS order) that runs it.  Also returns the product plans' rows."""
   audited = set(case_rows(cases))
   plans = {}
-  for pid, cfg, hw, B, precision in PRODUCT_PLANS:
+  for pid, cfg, hw, B, precision, extra in PRODUCT_PLANS:
     if pid in REFUSED:
       continue
-    rows = plan_rows(cpu_plan(cfg, hw, B, precision))
+    rows = plan_rows(cpu_plan(cfg, hw, B, precision, extra))
     plans[pid] = rows
     for r, names in rows.items():
       if set(names) & set(targeted.get(pid, ())):
@@ -303,7 +344,7 @@ if __name__ == '__main__':
     print('%-36s %-12s %s' % (pid, names[0], format_row(r)))
     add.setdefault(pid, []).append(names[0])
   print('\n%d rows unaudited; TARGETED entries that cover them:' % len(missing))
-  for pid, _, _, _, _ in PRODUCT_PLANS:
+  for pid, _, _, _, _, _ in PRODUCT_PLANS:
     if pid in add:
       print('    %r: %r,' % (pid, add[pid]))
   big = extent_unaudited(EXTENT_TARGETED)
@@ -313,6 +354,6 @@ if __name__ == '__main__':
     print('%-36s %-12s %-8s %13d elements %6.2f GB  %s' % (pid, name, k, n, nbytes / 1e9, format_row(r)))
     add.setdefault(pid, []).append(name)
   print('\n%d launches with an operand of >= 2^31 bytes unaudited; EXTENT_TARGETED entries that cover them:' % len(big))
-  for pid, _, _, _, _ in PRODUCT_PLANS:
+  for pid, _, _, _, _, _ in PRODUCT_PLANS:
     if pid in add:
       print('    %r: %r,' % (pid, add[pid]))

@@ -45,7 +45,8 @@ FRESH_CASES = ['coco_tracking_512_b32_bf16', 'coco_tracking_512_b32_bf16x3',
                'nuscenes_ddd_448x800_b32_bf16',
                'coco_pose_512_b2_bf16x3',               # two-pass heads
                'coco_tracking_512_b1_fp32',             # SIMT convs, ct_stem_forward, fp32 upsample
-               'coco_tracking_256_b2_bf16_dcn_global', 'coco_tracking_256_b2_bf16_no_halo']
+               'coco_tracking_256_b2_bf16_dcn_global', 'coco_tracking_256_b2_bf16_no_halo',
+               'kitti_tracking_384x1280_b2_bf16']       # a non-bench size: level 5's 12 x 40 ends in partial patches
 PREFIX_CASES = ['mot_544x960_b32_bf16', 'coco_tracking_512_b32_bf16x3']
 PDL_CASES = ['coco_tracking_512_b32_bf16', 'mot_544x960_b32_bf16x3']
 

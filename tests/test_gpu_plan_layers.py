@@ -45,6 +45,15 @@ CASES = [
     ('dla_node_gcn_64x96_b2_bf16', 'coco_tracking', (64, 96), 2, 'bf16', ['--dla_node', 'gcn'], {}, {}),
     ('coco_tracking_256_b2_bf16_no_halo', 'coco_tracking', (256, 256), 2, 'bf16', [], {'use_halo': False}, {}),
     ('coco_tracking_256_b2_bf16_dcn_global', 'coco_tracking', (256, 256), 2, 'bf16', [], {}, {'CTB_DCN_WINDOW': '0'}),
+    # input sizes beyond the bench (plan_rows.PRODUCT_SHAPES): kitti(_tracking)'s default, whose level 5 is 12 x 40 ...
+    ('kitti_tracking_384x1280_b2_bf16', 'coco_tracking', (384, 1280), 2, 'bf16', ['--num_classes', '3'], {}, {}),
+    ('kitti_tracking_384x1280_b2_bf16x3', 'coco_tracking', (384, 1280), 2, 'bf16x3', ['--num_classes', '3'], {}, {}),
+    # ... a 1080p camera under --keep_res: level 4's convs on the plain gather at N = 64 with several work items per CTA
+    ('mot_keep_1088x1920_b1_bf16', 'mot', (1088, 1920), 1, 'bf16', [], {}, {}),
+    # ... a 64 x 1024 strip: the bf16x3 gather at N = 16 on level 2 and the global DCN
+    ('wide_64x1024_b2_bf16x3', 'coco_tracking', (64, 1024), 2, 'bf16x3', [], {}, {}),
+    # ... and a VGA camera under --keep_res (level 5 is 15 x 20)
+    ('coco_keep_480x640_b2_bf16', 'coco_tracking', (480, 640), 2, 'bf16', [], {}, {}),
 ] + [  # the other output-head layouts (tests/helpers.py::HEAD_LAYOUTS); bf16x3 plans them all in two passes
     ('heads_%s_64x96_b2_%s' % (tag, precision), cfg, (64, 96), 2, precision, extra, {}, {})
     for tag, cfg, extra, plan in HEAD_LAYOUTS for precision in ('bf16', 'bf16x3')

@@ -6,9 +6,9 @@ plan_rows.TARGETED names, per product plan, the ops that run a configuration not
 each plan is built as the product builds it, replayed once on synthetic_inputs, and only those ops are recomputed in fp64
 and held to the bounds of tests/bounds.py, as test_gpu_plan_layers does for whole plans.
 
-plan_rows.EXTENT_TARGETED names the launches with operands of >= 2^31 bytes (B = 64): they are checked in fp64 on their
-first and last four images, and bit for bit on every image against the same launch on 4-image slices, so an offset
-that wraps past 32 bits anywhere in the batch fails."""
+plan_rows.EXTENT_TARGETED and EXTENT_BENCH name the launches with operands of >= 2^31 bytes (B = 64, or 16 under
+nuScenes' --keep_res): they are checked in fp64 on their first and last four images, and bit for bit on every image
+against the same launch on 4-image slices, so an offset that wraps past 32 bits anywhere in the batch fails."""
 import ctypes as C
 import gc
 import time
@@ -24,7 +24,7 @@ from centertrack_b200.engine import DeferredTV
 
 pytestmark = pytest.mark.gpu
 
-PLANS = {pid: (cfg, hw, B, p) for pid, cfg, hw, B, p in pr.PRODUCT_PLANS}
+PLANS = {pid: (cfg, hw, B, p, extra) for pid, cfg, hw, B, p, extra in pr.PRODUCT_PLANS}
 
 
 def _ops_within_bounds(eng, pid, names, chunks):
@@ -63,8 +63,8 @@ def _chunks(B):
 
 @pytest.mark.parametrize('pid', sorted(pr.TARGETED))
 def test_targeted_ops_within_bounds(pid, monkeypatch):
-  cfg, hw, B, precision = PLANS[pid]
-  eng = tpl._build(cfg, hw, B, precision, [], {}, monkeypatch, {})
+  cfg, hw, B, precision, extra = PLANS[pid]
+  eng = tpl._build(cfg, hw, B, precision, extra, {}, monkeypatch, {})
   tpl._assert_no_overlapping_writes(eng)
   failures, report = _ops_within_bounds(eng, pid, pr.TARGETED[pid], _chunks(eng.B))
   print('\n[%s] per audited op: worst |err| / bound, largest |err| / mag beyond the output rounding as a multiple of '
@@ -131,11 +131,11 @@ def _sliced_matches(eng, sp, n=tpl.CHUNK):
   return bad
 
 
-def _plan_need(cfg, hw, B, precision, names):
+def _plan_need(cfg, hw, B, precision, extra, names):
   """Device bytes the extent test needs for a plan: its buffers at batch B (the B = 1 plan's activations times B, plus
   weights), and twice the largest operand of the audited ops (the NaN-filled output copy, or the fp64 reference of
   4 images)."""
-  eng = pr.cpu_plan(cfg, hw, 1, precision)
+  eng = pr.cpu_plan(cfg, hw, 1, precision, extra)
   seen = {}
   for t in eng.keep + [eng.in_img, eng.in_pre, eng.in_hm] + list(eng.outputs.values()):
     seen[t.data_ptr()] = t.numel() * t.element_size() * (B if t.dim() == 4 else 1)
@@ -143,14 +143,18 @@ def _plan_need(cfg, hw, B, precision, names):
   return sum(seen.values()) + 2 * B * max(pr.largest_operand(ext[n])[0] for n in names)
 
 
-@pytest.mark.parametrize('pid', sorted(pr.EXTENT_TARGETED))
+EXTENT_RUN = dict(pr.EXTENT_TARGETED, **pr.EXTENT_BENCH)
+
+
+@pytest.mark.parametrize('pid', sorted(EXTENT_RUN))
 def test_largest_launches_at_full_size(pid, monkeypatch):
-  """The product's launches with operands of >= 2^31 bytes, at their plan's batch: each audited op within the fp64
-  bounds on its first and last 4-image chunk (the last holds the largest offsets), and bit-identical on every image to
-  the same launch issued on 4-image slices."""
-  cfg, hw, B, precision = PLANS[pid]
-  names = pr.EXTENT_TARGETED[pid]
-  need = _plan_need(cfg, hw, B, precision, names)
+  """The product's launches with operands of >= 2^31 bytes, at their plan's batch (plan_rows.EXTENT_TARGETED, and the
+  benchmarked configs' own such launches, plan_rows.EXTENT_BENCH): each audited op within the fp64 bounds on its first
+  and last 4-image chunk (the last holds the largest offsets), and bit-identical on every image to the same launch
+  issued on 4-image slices."""
+  cfg, hw, B, precision, extra = PLANS[pid]
+  names = EXTENT_RUN[pid]
+  need = _plan_need(cfg, hw, B, precision, extra, names)
   gc.collect()
   torch.cuda.empty_cache()
   free, total = torch.cuda.mem_get_info()
@@ -161,11 +165,17 @@ def test_largest_launches_at_full_size(pid, monkeypatch):
   t0 = time.time()
   eng = specs = None
   try:
-    eng = tpl._build(cfg, hw, B, precision, [], {}, monkeypatch, {})
+    eng = tpl._build(cfg, hw, B, precision, extra, {}, monkeypatch, {})
     tpl._assert_no_overlapping_writes(eng)
     specs = {sp['name']: sp for sp in eng.specs}
     ext = pr.op_extents(eng)
-    failures, report = _ops_within_bounds(eng, pid, names, [slice(0, tpl.CHUNK), slice(B - tpl.CHUNK, B)])
+    # the first and last CHUNK images, in passes as small as the fp64 reference needs: up to about twenty fp64 tensors
+    # the size of the largest operand's images are alive at once (nuScenes' 2048-channel head intermediate is 1.6 GB an
+    # image at 928 x 1632)
+    per_image = max(pr.largest_operand(ext[n])[1] for n in names) // B * 8
+    step = int(max(1, min(tpl.CHUNK, torch.cuda.mem_get_info()[0] // (24 * per_image))))
+    chunks = [slice(b, min(b + step, e)) for s, e in ((0, tpl.CHUNK), (B - tpl.CHUNK, B)) for b in range(s, e, step)]
+    failures, report = _ops_within_bounds(eng, pid, names, chunks)
     for name in names:
       failures += _sliced_matches(eng, specs[name])
       nbytes, n, k = pr.largest_operand(ext[name])

@@ -1,7 +1,7 @@
 """The launch configurations of the product plans (tests/plan_rows.py) are all audited on the GPU (no GPU needed here).
 
-Every row of every PRODUCT_PLANS plan -- bench.py's configs at their resolutions, bf16 / bf16x3 / fp32, B = 1 ... 64,
-built on the CPU with the H100 SXM's 132 SMs -- must be run by a plan of test_gpu_plan_layers.CASES or by an op that
+Every row of every PRODUCT_PLANS plan -- bench.py's configs at their resolutions and the product's other input sizes
+(plan_rows.PRODUCT_SHAPES), bf16 / bf16x3 / fp32, B = 1 ... 64, built on the CPU with the H100 SXM's 132 SMs -- must be run by a plan of test_gpu_plan_layers.CASES or by an op that
 plan_rows.TARGETED names (audited by tests/test_gpu_plan_rows.py).  A planner or library change that makes a product
 plan pick a configuration nothing audits fails here, listing the rows and the ops that run them.  Likewise every row
 with an operand of >= 2^31 bytes must have its largest launch named in plan_rows.EXTENT_TARGETED, which
@@ -22,9 +22,24 @@ def test_product_plans_cover_every_bench_config():
   assert set(pr.BENCH_SHAPES) == set(bench.CONFIGS)
   for cfg, (H, W) in pr.BENCH_SHAPES.items():
     assert bench.CONFIGS[cfg][:2] == (H, W), cfg
-  got = {(cfg, hw, B, p) for _, cfg, hw, B, p in pr.PRODUCT_PLANS}
+  got = {(cfg, hw, B, p) for _, cfg, hw, B, p, extra in pr.PRODUCT_PLANS if hw == pr.BENCH_SHAPES[cfg] and not extra}
   assert got == {(cfg, pr.BENCH_SHAPES[cfg], B, p) for cfg in bench.CONFIGS for B in (1, 2, 4, 8, 16, 32, 64)
                  for p in ('bf16', 'bf16x3', 'fp32')}
+  assert len({pid for pid, _, _, _, _, _ in pr.PRODUCT_PLANS}) == len(pr.PRODUCT_PLANS)
+
+
+def test_product_plans_cover_the_product_shapes():
+  """The sizes beyond the bench: the large cameras under --keep_res, KITTI's default and --keep_res sizes, VGA, a wide
+  strip and the smallest input, each at every precision and at least at the batches up to 16."""
+  got = {(cfg, hw, tuple(extra), B, p) for _, cfg, hw, B, p, extra in pr.PRODUCT_PLANS}
+  want = {('mot', (1088, 1920), ()), ('nuscenes_ddd', (928, 1632), ()),
+          ('coco_tracking', (384, 1280), ('--num_classes', '3')), ('coco_tracking', (384, 1248), ('--num_classes', '3')),
+          ('coco_tracking', (480, 640), ()), ('coco_tracking', (64, 1024), ()), ('coco_tracking', (32, 64), ())}
+  assert {(cfg, hw, tuple(extra)) for _, cfg, hw, extra, _ in pr.PRODUCT_SHAPES} == want
+  for cfg, hw, extra in want:
+    for B in (1, 2, 4, 8, 16):
+      for p in ('bf16', 'bf16x3', 'fp32'):
+        assert (cfg, hw, extra, B, p) in got, (cfg, hw, extra, B, p)
 
 
 def test_bench_plans_are_audited_whole():
@@ -68,6 +83,23 @@ def test_extent_targeted_ops_are_the_largest_conv_launches(large):
     assert r[0] in ('simt', 'gather', 'gather_x3', 'halo'), r
 
 
+def test_extent_bench_ops_are_large_bench_launches(large):
+  """Each EXTENT_BENCH op is a convolution of a benchmarked config's plan with an operand of >= 2^31 bytes, in a row
+  whose largest launch EXTENT_TARGETED names in another plan."""
+  plans = {pid: (cfg, hw, B, p, extra) for pid, cfg, hw, B, p, extra in pr.PRODUCT_PLANS}
+  assert not set(pr.EXTENT_BENCH) & set(pr.EXTENT_TARGETED)
+  for pid, names in pr.EXTENT_BENCH.items():
+    cfg, hw, B, p, extra = plans[pid]
+    assert hw == pr.BENCH_SHAPES[cfg] and not extra, pid
+    eng = pr.cpu_plan(cfg, hw, B, p, extra)
+    rows = {sp['name']: pr.launch_row(eng, sp) for sp in eng.specs}
+    ext = pr.op_extents(eng)
+    for n in names:
+      assert pr.largest_operand(ext[n])[0] >= pr.LARGE, (pid, n)
+      assert rows[n] in large and large[rows[n]][0] != pid, (pid, n, pr.format_row(rows[n]))
+    del eng
+
+
 def test_op_extents_count_whole_buffers(built_lib):
   """A channel slice counts its whole NHWC buffer (ld, not C); the fp32 head planes B C_out OH OW; the fused head
   launch's records are left out."""
@@ -92,16 +124,16 @@ def test_targeted_ops_exist_and_have_a_checker(audit):
     ran = {n: r for r, ns in plans[pid].items() for n in ns}
     for n in names:
       assert n in ran, '%s: no op %s runs a launch of the plan' % (pid, n)
-  for pid, cfg, hw, B, p in pr.PRODUCT_PLANS:
+  for pid, cfg, hw, B, p, extra in pr.PRODUCT_PLANS:
     if pid in pr.TARGETED:
-      eng = pr.cpu_plan(cfg, hw, B, p)
+      eng = pr.cpu_plan(cfg, hw, B, p, extra)
       kinds = {sp['name']: sp['kind'] for sp in eng.specs}
       for n in pr.TARGETED[pid]:
         assert kinds[n] == 'conv' or kinds[n] in OTHER_KINDS, (pid, n, kinds[n])
 
 
 def test_refused_product_plans_say_why(built_lib):
-  for pid, cfg, hw, B, p in pr.PRODUCT_PLANS:
+  for pid, cfg, hw, B, p, extra in pr.PRODUCT_PLANS:
     if pid in pr.REFUSED:
       with pytest.raises(RuntimeError, match=pr.REFUSED[pid].replace('^', r'\^')):
-        pr.cpu_plan(cfg, hw, B, p)
+        pr.cpu_plan(cfg, hw, B, p, extra)

@@ -49,7 +49,7 @@ class ConvDesc(C.Structure):
 
 class ConvConfig(C.Structure):
   _fields_ = [('smem_bytes', C.c_int32), ('stages', C.c_int32), ('tile_w', C.c_int32), ('tile_h', C.c_int32),
-              ('ctas_per_sm', C.c_int32), ('overlap', C.c_int32)]
+              ('ctas_per_sm', C.c_int32), ('overlap', C.c_int32), ('pixel_major', C.c_int32)]
 
 
 class DecodeHead(C.Structure):

@@ -158,6 +158,7 @@ extern "C" int ct_conv_config(const ct_conv_desc* d, struct ct_conv_config* out)
   CT_REQUIRE(d && out, "null pointer");
   const int r = check_conv_desc(d);
   if (r != CT_OK) return r;
+  *out = ConvConfig{};
   if (d->engine == CT_ENGINE_SIMT) return conv_config_simt(d, out);
   if (d->engine == CT_ENGINE_TCGEN05_HALO) return d->n_heads ? conv_config_heads(d, out) : conv_config_halo(d, out);
   return conv_config_tc(d, out);

@@ -20,6 +20,14 @@
 // 32 columns at a time -> row-per-thread stores).  Warp 8 is the TMA producer.  Two CTAs per SM where shared memory
 // allows, so one CTA's epilogue overlaps the other's MMAs; where only one fits and 64 <= N <= 128, the two warpgroups
 // take turns on the tensor cores instead (ping-pong), so one warpgroup's epilogue overlaps the other's MMAs.
+//
+// Pixel-major flavour (n_tile == C_out == 64, NHWC bf16 output): an m64n64k16 reads 2 KB of A and 2 KB of B from shared
+// memory per 32 tensor-core cycles, the whole shared-memory bandwidth.  There the operands swap: A = the weights of the
+// K16 block (64 output channels, the same packed blocks through the same descriptor B uses otherwise), B = the item's
+// 128 halo pixel rows (the pixel-row descriptor above, whole tile: N = 128 is 16 core-matrix groups at SBO = pitch),
+// one m64n128k16 per block, 96 B/cycle.  A warpgroup then takes whole items (warpgroup w: items w, w + 2, ...), its
+// accumulator is [64 channels][128 pixels], and its epilogue transposes it through the staging tile 32 pixels at a
+// time.  The walk (ky, kx, chunk, K-step) is a compile-time PxWalk, so the chain unrolls.
 #include "conv_common.cuh"
 #include "wgmma.cuh"
 #include <cuda.h>
@@ -65,11 +73,28 @@ struct HaloArgs {
   // A-descriptor walk of one work item (all in 16-byte units, warp-uniform): for ky, kx|pair, chunk, kstep
   int m_nky, m_nkx, m_nc, m_nq;
   uint32_t m_sky, m_skx, m_sc, m_sq, m_alo, m_ahi;
+  int px;                               // != 0: pixel-major flavour, the PX_WALKS entry (1-based) of its walk
 };
+
+// Compile-time walk of the pixel-major chain: KY x KX taps, NC 64-channel chunks, NQ K16 steps per chunk
+template <int KY, int KX, int NC, int NQ>
+struct PxWalk {
+  static constexpr bool on = true;
+  static constexpr int ky = KY, kx = KX, nc = NC, nq = NQ;
+};
+struct NoPx {
+  static constexpr bool on = false;
+  static constexpr int ky = 0, kx = 0, nc = 0, nq = 0;
+};
+// (KH, KW, C_in) of the 64 -> 64-channel layers of the shipped plans: level0 and the level2 3x3s (3x3, 64),
+// level2.tree1.conv1 on level1's space-to-depth output (2x2, 128), level2.project (1x1, 32) and level2's root (1x1, 128)
+constexpr int PX_WALKS[][3] = {{3, 3, 64}, {2, 2, 128}, {1, 1, 32}, {1, 1, 128}};
+constexpr int PX_PITCH = 68;      // floats per pixel row of the pixel-major staging tile (32 x 64 channels + pad)
 
 // OVERLAP: the flavour for launches that get one CTA per SM (64 <= N <= 128): the warpgroups' MMA chains alternate (see
 // the item loop) and the register cap is that of one CTA.
-template <int N, bool OVERLAP>
+// PX: the pixel-major flavour's walk (N == 64), or NoPx.
+template <int N, bool OVERLAP, class PX = NoPx>
 __global__ void __launch_bounds__(H_THREADS, (N <= 128 && !OVERLAP) ? 2 : 1)
 conv_halo_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
   extern __shared__ __align__(1024) unsigned char hsm_dyn[];
@@ -95,7 +120,8 @@ conv_halo_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
   pdl_trigger();                       // the next kernel of the stream may start its own prologue now
   if (tid == 0) {
     mbar_init(w_full, 1);
-    for (int s = 0; s < S; ++s) { mbar_init(halo_full(s), 1); mbar_init(halo_empty(s), H_MMA_WARPS); }
+    // a halo stage is read by both warpgroups, or (pixel-major) by the one whose item it holds
+    for (int s = 0; s < S; ++s) { mbar_init(halo_full(s), 1); mbar_init(halo_empty(s), PX::on ? 4 : H_MMA_WARPS); }
     mbar_init_fence();
   }
   // folded-BN shift / bias of this CTA's output-channel tile, staged once (read as float4 broadcasts)
@@ -147,6 +173,123 @@ conv_halo_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
         h_stamp(trace, it, 1);
       }
     }
+  } else if constexpr (PX::on) {
+    // ===================== pixel-major MMA + epilogue warpgroups (see the top of the file) =====================
+    const int wg = warp >> 2, w4 = warp & 3;
+    const bool lead = (tid & 127) == 0;          // stamps the trace of this warpgroup's items
+    const uint32_t stg = base + off_stg + (uint32_t)wg * (64u * EPI_PITCH * 4u);
+    // A (weights, K-major no-swizzle): LBO = next 8 k (64 x 16 B), SBO = next 8 channels (128 B); 64 x 32 B per block
+    const uint64_t w_desc0 = wg_desc(sW, 64u * 16u, 128u, 0u);
+    const uint64_t h_hi = (uint64_t)a.m_ahi << 32;
+    // epilogue pass j (pixels 32j .. 32j + 31 of the item): thread = pixel 32j + lane, channels 16 w4 .. 16 w4 + 15
+    const int gy = lane >> 3, rx = lane & 7;     // pixel 32j + lane = (tile row 4j + gy, x rx)
+    // passes whose residual is prefetched (2 x 16 B of registers each): all four under the one-CTA register cap, none
+    // under the two-CTA one (the accumulator alone is 64 registers)
+    constexpr int PF = OVERLAP ? 4 : 0;
+    uint4 rq[PF > 0 ? PF : 1][2];
+    const bool use_res = a.residual != nullptr;
+    auto prefetch_residual = [&](int sp_n) {
+      const int bn = sp_n / per_img, rn = sp_n - bn * per_img;
+      const int tyn = rn / a.tiles_x, txn = rn - tyn * a.tiles_x;
+      const int oxn = txn * HT_W + rx;
+#pragma unroll
+      for (int j = 0; j < PF; ++j) {
+        const int oyn = tyn * HT_H + 4 * j + gy;
+        rq[j][0] = make_uint4(0, 0, 0, 0); rq[j][1] = make_uint4(0, 0, 0, 0);
+        if (oyn < g.OH && oxn < g.OW) {
+          const uint4* rp = reinterpret_cast<const uint4*>(
+              a.residual + (((size_t)bn * g.OH + oyn) * g.OW + oxn) * g.ld_res + 16 * w4);
+          rq[j][0] = __ldg(rp); rq[j][1] = __ldg(rp + 1);
+        }
+      }
+    };
+    const int sp_first = sp0 + wg * sp_stride, sp_step = 2 * sp_stride;
+    if (PF > 0 && use_res && sp_first < sp_total) prefetch_residual(sp_first);
+    // folded-BN shifts of this thread's two accumulator rows (channels 16 w4 + lane / 4, + 8)
+    const float sh0 = s_shift[16 * w4 + (lane >> 2)], sh1 = s_shift[16 * w4 + (lane >> 2) + 8];
+    mbar_wait(w_full, 0, 2, 0);
+    // OVERLAP: the chains take turns in item order (warpgroup 0's item 0, warpgroup 1's item 1, ...), on the named
+    // barriers of the other flavour; after the loop the warpgroup that did not run the last item consumes the last
+    // arrival.
+    const int n_items = sp0 < sp_total ? (sp_total - sp0 - 1) / sp_stride + 1 : 0;
+    if constexpr (OVERLAP)
+      if (wg == 1 && n_items > 0) named_arrive(3, 256);
+    float acc[64];
+    int it = wg;
+    for (int sp = sp_first; sp < sp_total; sp += sp_step, it += 2) {
+      const int s = it % S;
+      const uint32_t ph = (uint32_t)(it / S) & 1u;
+      if constexpr (OVERLAP) named_sync(3 + wg, 256);
+      mbar_wait(halo_full(s), ph, 3, it);
+      if (lead) h_stamp(trace, it, 2);
+      const uint32_t h_lo0 = a.m_alo + (sH >> 4) + ((uint32_t)s * halo_bytes >> 4);
+      wg_fence();
+#pragma unroll
+      for (int ky = 0; ky < PX::ky; ++ky)
+#pragma unroll
+        for (int kx = 0; kx < PX::kx; ++kx)
+#pragma unroll
+          for (int c = 0; c < PX::nc; ++c)
+#pragma unroll
+            for (int qq = 0; qq < PX::nq; ++qq) {
+              const int blk = ((ky * PX::kx + kx) * PX::nc + c) * PX::nq + qq;
+              const uint32_t h_lo = h_lo0 + (uint32_t)ky * a.m_sky + (uint32_t)kx * a.m_skx + (uint32_t)c * a.m_sc +
+                                    (uint32_t)qq * a.m_sq;
+              Wgmma<128>::mma(acc, w_desc0 + (uint64_t)(blk * 128), h_hi | h_lo, blk > 0 ? 1u : 0u);
+            }
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_operand(acc);
+      if constexpr (OVERLAP) named_arrive(3 + (wg ^ 1), 256);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(halo_empty(s));     // this warp's MMAs no longer read the halo stage
+      if (lead) h_stamp(trace, it, 4);
+
+      // ---- epilogue: acc[4 i + 2 h + e] = channel 16 w4 + lane / 4 + 8 h, pixel 8 i + 2 (lane % 4) + e
+      const int b = sp / per_img, r = sp - b * per_img;
+      const int ty = r / a.tiles_x, tx = r - ty * a.tiles_x;
+      const int ox = tx * HT_W + rx;
+      if (lead) h_stamp(trace, it, 5);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        named_sync(1 + wg, 128);                   // the previous pass's readers are done with the staging tile
+        // + shift, transposed into the staging tile [32 pixels][PX_PITCH]
+#pragma unroll
+        for (int i = 4 * j; i < 4 * j + 4; ++i)
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const uint32_t px = (uint32_t)(8 * (i - 4 * j) + 2 * (lane & 3) + e);
+              const uint32_t ch = (uint32_t)(16 * w4 + (lane >> 2) + 8 * h);
+              const float v = acc[4 * i + 2 * h + e] + (h ? sh1 : sh0);
+              sts32(stg + (px * PX_PITCH + ch) * 4u, __float_as_uint(v));
+            }
+        named_sync(1 + wg, 128);
+        const int oy = ty * HT_H + 4 * j + gy;
+        if (oy >= g.OH || ox >= g.OW) continue;
+        const size_t p = a.out_s2d ? ((((size_t)b * (g.OH >> 1) + (oy >> 1)) * (g.OW >> 1) + (ox >> 1)) << 2) + (((oy & 1) << 1) | (ox & 1))
+                                   : ((size_t)b * g.OH + oy) * g.OW + ox;
+        float v[16];
+        lds_f(stg + ((uint32_t)lane * PX_PITCH + 16u * w4) * 4u, v);
+        if (use_res) {
+          uint4 ra, rb;
+          if (j < PF) {
+            ra = rq[j < PF ? j : 0][0]; rb = rq[j < PF ? j : 0][1];
+          } else {
+            const uint4* rp = reinterpret_cast<const uint4*>(a.residual + p * g.ld_res + 16 * w4);
+            ra = __ldg(rp); rb = __ldg(rp + 1);
+          }
+          add_residual_bf16(v, ra, rb);
+        }
+        relu16(v, g.relu);
+        store_bf16x16(reinterpret_cast<__nv_bfloat16*>(a.out) + p * g.ld_out + 16 * w4, v);
+      }
+      if (PF > 0 && use_res && sp + sp_step < sp_total) prefetch_residual(sp + sp_step);
+      if (lead) h_stamp(trace, it, 6);
+    }
+    if constexpr (OVERLAP)
+      if (n_items > 0 && wg != ((n_items - 1) & 1)) named_sync(3 + wg, 256);
   } else {
     // ===================== MMA + epilogue warpgroups =====================
     const int wg = warp >> 2, w4 = warp & 3;
@@ -389,6 +532,11 @@ static int halo_config(const ct_conv_desc* d, HaloArgs& a, ConvConfig& c) {
     a.m_alo = ((uint32_t)a.plane_bytes >> 4) << 16;       // LBO = plane stride
     a.m_ahi = (uint32_t)a.pw;
   }
+  // pixel-major: the 64 -> 64-channel layers with NHWC bf16 output, for the walks PX_WALKS instantiates
+  a.px = 0;
+  if (n_tile == 64 && g.C_out == 64 && g.out_mode == CT_OUT_NHWC && !a.sum3 && a.swz && !a.pair_taps && a.tw == HT_W)
+    for (int i = 0; i < (int)(sizeof(PX_WALKS) / sizeof(PX_WALKS[0])); ++i)
+      if (g.KH == PX_WALKS[i][0] && g.KW == PX_WALKS[i][1] && g.C_in == PX_WALKS[i][2]) a.px = i + 1;
   a.tiles_x = (g.OW + a.tw - 1) / a.tw;
   a.tiles_y = (g.OH + a.th - 1) / a.th;
   a.tiles_total = g.B * a.tiles_x * a.tiles_y;
@@ -423,6 +571,7 @@ static int halo_config(const ct_conv_desc* d, HaloArgs& a, ConvConfig& c) {
   c.tile_h = a.th;
   c.ctas_per_sm = per_sm;
   c.overlap = overlap_env && per_sm == 1 && n_tile >= 64 && n_tile <= 128;
+  c.pixel_major = a.px != 0;
   return CT_OK;
 }
 
@@ -470,6 +619,22 @@ int conv_forward_halo(const ct_conv_desc* d, cudaStream_t st) {
   if (groups < 1) groups = 1;
   if (groups > a.tiles_total) groups = a.tiles_total;
   const int grid = (int)(groups * a.n_tiles_n);
+  if (a.px) {
+    auto launch_px = [&](auto px) {
+      using PX = decltype(px);
+      if (a.m_nky != PX::ky || a.m_nkx != PX::kx || a.m_nc != PX::nc || a.m_nq != PX::nq)
+        return fail(CT_ERR_INVALID, "conv_halo: pixel-major walk does not match the layer%s", "");
+      return c.overlap ? launch_big_smem<conv_halo_kernel<64, true, PX>>(dim3(grid), dim3(H_THREADS), c.smem_bytes, st, a, tmap)
+                       : launch_big_smem<conv_halo_kernel<64, false, PX>>(dim3(grid), dim3(H_THREADS), c.smem_bytes, st, a, tmap);
+    };
+    static_assert(sizeof(PX_WALKS) / sizeof(PX_WALKS[0]) == 4, "one case per walk");
+    switch (a.px) {
+      case 1: return launch_px(PxWalk<3, 3, 1, 4>{});
+      case 2: return launch_px(PxWalk<2, 2, 2, 4>{});
+      case 3: return launch_px(PxWalk<1, 1, 1, 2>{});
+      default: return launch_px(PxWalk<1, 1, 2, 4>{});
+    }
+  }
   return dispatch_n_tile(a.n_tile, [&](auto n) {
     constexpr int NT = decltype(n)::value;
     if constexpr (NT >= 64 && NT <= 128)

@@ -179,6 +179,7 @@ struct ct_conv_config {
                             consecutive pixels (gather engines) */
   int32_t ctas_per_sm;   /* HALO: CTAs per SM the persistent grid is sized for; 0 for the other engines */
   int32_t overlap;       /* HALO: 1 = the one-CTA-per-SM flavour whose two warpgroups take turns on the tensor cores */
+  int32_t pixel_major;   /* HALO: 1 = the 64-channel flavour: weights on wgmma M, the item's 128 pixels on N (m64n128) */
 };
 /* The configuration step of ct_conv_forward alone: validates the descriptor's shape and fills `out`, with no CUDA
  * call.  Returns the status and ct_last_error() message ct_conv_forward would return for this shape

@@ -16,6 +16,7 @@ lib = L.lib()
 import os as _os
 cases = [('stem 7x7 8->48 sum3 512x512', 16, 8, 48, 512, 512, 7, False, 48),
          ('level0 16->16 512x512', 16, 16, 16, 512, 512, 3, False, 16),
+         ('level0 64->64 256x256 (space-to-depth grid)', 16, 64, 64, 256, 256, 3, False, 64),
          ('heads.0 64->1024 nt128 128x128', 16, 64, 1024, 128, 128, 3, False, 128),
          ('level2 64->64 +res 128x128', 16, 64, 64, 128, 128, 3, True, 64),
          ('level3 128->128 +res nt32 64x64', 16, 128, 128, 64, 64, 3, True, 32),

@@ -132,6 +132,13 @@ class FrameSrc(C.Structure):
   _fields_ = [('plane', C.c_void_p * 3), ('pitch', C.c_int64 * 3), ('layout', C.c_int32), ('reserved', C.c_int32)]
 
 
+class CropDesc(C.Structure):
+  _fields_ = [('buf', C.c_void_p), ('buf_bytes', C.c_int64), ('frames', C.c_void_p), ('rows', C.c_void_p),
+              ('row_floats', C.c_int32), ('rows_per_stream', C.c_int32), ('counts', C.c_void_p),
+              ('counts_stride', C.c_int32), ('active_col', C.c_int32), ('K', C.c_int32), ('out_h', C.c_int32),
+              ('out_w', C.c_int32), ('out', C.c_void_p), ('out_counts', C.c_void_p)]
+
+
 CT_FLIP_MAX_HEADS = 12
 
 
@@ -148,7 +155,7 @@ EXPORTS = ['ct_packed_weight_bytes', 'ct_pack_weights', 'ct_conv_forward', 'ct_c
            'ct_render_tracks', 'ct_track_step_mapped', 'ct_render_tracks_mapped', 'ct_post_process',
            'ct_track_step_opts', 'ct_track_start_opts', 'ct_track_restore_opts', 'ct_post_process_opts', 'ct_flip_merge', 'ct_flip_merge_heads', 'ct_mirror_x',
            'ct_warp_affine_normalize', 'ct_pack_stem_frames_dev', 'ct_pack_stem_frames_flip_dev',
-           'ct_warp_frames_normalize', 'ct_stage_frames', 'ct_last_error',
+           'ct_warp_frames_normalize', 'ct_stage_frames', 'ct_crop_boxes', 'ct_last_error',
            'ct_abi_version', 'ct_launch_count', 'ct_reset_launch_count', 'ct_debug_trace', 'ct_debug_watch']
 
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17', '-Xcompiler', '-fPIC']
@@ -251,6 +258,7 @@ def lib():
   L.ct_warp_frames_normalize.argtypes = [C.c_void_p] * 2 + [C.c_int32, C.c_int64] + [C.c_void_p] * 3 + \
       [C.c_int32] * 2 + [C.c_void_p]
   L.ct_stage_frames.argtypes = [C.POINTER(FrameSrc), C.POINTER(Frame), C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]
+  L.ct_crop_boxes.argtypes = [C.POINTER(CropDesc), C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
   L.ct_launch_count.restype = C.c_int64
   L.ct_reset_launch_count.restype = None
   L.ct_debug_trace.argtypes = [C.c_void_p]

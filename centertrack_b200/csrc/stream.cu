@@ -23,6 +23,8 @@
 //                    ct_warp_frames_normalize the same frames into an fp32 image.  BGR, NV12 or I420 frames, the
 //                    latter two with cv2.cvtColor(COLOR_YUV2BGR_NV12 / _I420) applied to each bilinear tap
 //   ct_stage_frames  B frames already in device memory (a GPU decoder's) copied into a frame slot in its layout
+//   ct_crop_boxes    each stream's active tracks (or kept detections) cropped out of its frame slot: cv2.warpAffine
+//                    of the box stretched to a fixed crop size, the frames kernels' bilinear taps
 // All HBM-bound byte/index work: one pass over the data, coalesced, no tensor cores.
 #include <math_constants.h>
 
@@ -1075,6 +1077,103 @@ stage_frames_kernel(const __grid_constant__ StageArgs a, unsigned char* __restri
   }
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// ct_crop_boxes: crop k of stream b = cv2.warpAffine(frame_b, M, (out_w, out_h), INTER_LINEAR | WARP_INVERSE_MAP,
+// BORDER_CONSTANT 0) with the box's dst -> src map M = [sx, 0, (x0 - .5) + .5 sx, 0, sy, (y0 - .5) + .5 sy],
+// sx = (x1 - x0) / out_w, sy = (y1 - y0) / out_h in fp64, each step rounded on its own (no FMA contraction).  The taps
+// are warp_bilinear_u8's, so a 4:2:0 frame gives the crop of its cv2.cvtColor BGR image.
+// grid (pixel chunks, K, n): CTA (., k, i) writes crop k of image i's stream and exits when k is past its count, so the
+// launch shape depends on n, K and the crop size alone.  A CTA's CROP_PIX * CROP_THREADS consecutive crop pixels are
+// warped with adjacent pixels on adjacent lanes (their taps are neighbours: coalesced loads), staged as bytes in shared
+// memory, and stored as 16-byte vectors on adjacent lanes where the crop is 16-byte aligned.  Its time goes to the
+// taps, not to the writes (DESIGN §5).
+// ------------------------------------------------------------------------------------------------------------------
+constexpr int CROP_THREADS = 128;
+constexpr int CROP_PIX = 16;                // pixels per thread
+constexpr int CROP_CTA_BYTES = 3 * CROP_PIX * CROP_THREADS;
+constexpr float CROP_MAX_COORD = 16384.f;   // beyond it cv2's int16 source map would saturate: the crop is zeros
+
+struct CropArgs {
+  ct_crop_desc d;
+  const int* streams;      // NULL = identity
+  int n_streams;
+};
+
+// The CTA's pixels [p0, p0 + CROP_PIX * CROP_THREADS) of the crop -> s_px (3 bytes each); zero = the box failed the
+// guard (an all-zero crop).
+template <int FMT>
+__device__ __forceinline__ void crop_pixels(const unsigned char* __restrict__ src, const ct_frame& f, const double* M,
+                                            bool zero, int out_w, size_t total, size_t p0, unsigned char* s_px) {
+#pragma unroll 4
+  for (int q = 0; q < CROP_PIX; ++q) {
+    const int j = q * CROP_THREADS + (int)threadIdx.x;
+    const size_t p = p0 + j;
+    if (p >= total) break;
+    int p8[3] = {0, 0, 0};
+    if (!zero) {
+      const int y = (int)(p / out_w), x = (int)(p - (size_t)y * out_w);
+      warp_bilinear_u8<FMT>(src, f.h, f.w, f.step, M, x, y, p8);
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) s_px[3 * j + c] = (unsigned char)p8[c];
+  }
+}
+
+__global__ void __launch_bounds__(CROP_THREADS) crop_boxes_kernel(const __grid_constant__ CropArgs a) {
+  const ct_crop_desc& d = a.d;
+  const int i = blockIdx.z, k = blockIdx.y;
+  const int b = a.streams ? a.streams[i] : i;
+  if (b < 0 || b >= a.n_streams) return;                    // a padding image, or no stream: nothing is written
+  __shared__ ct_frame s_f;
+  __shared__ int s_cnt, s_first;
+  const int RF = d.row_floats;
+  const float* rows = d.rows + (size_t)b * d.rows_per_stream * RF;
+  if (threadIdx.x == 0) {
+    s_f = d.frames[i];
+    int n = d.counts[(size_t)b * d.counts_stride];
+    n = max(0, min(n, min(d.K, d.rows_per_stream)));
+    s_cnt = s_first = frame_in_buffer(s_f, d.buf_bytes) ? n : 0;   // an invalid frame: no crop, nothing read
+  }
+  __syncthreads();
+  int n = s_cnt;
+  if (d.active_col >= 0) {                                  // track tables: the leading active rows
+    for (int r = threadIdx.x; r < n; r += CROP_THREADS)
+      if (rows[(size_t)r * RF + d.active_col] == 0.f) atomicMin(&s_first, r);
+    __syncthreads();
+    n = s_first;
+  }
+  if (blockIdx.x == 0 && k == 0 && threadIdx.x == 0) d.out_counts[b] = n;
+  if (k >= n) return;
+  const float* bx = rows + (size_t)k * RF + CT_TRK_BBOX;
+  const float x0 = bx[0], y0 = bx[1], x1 = bx[2], y1 = bx[3];
+  const bool zero = !(fabsf(x0) <= CROP_MAX_COORD && fabsf(y0) <= CROP_MAX_COORD && fabsf(x1) <= CROP_MAX_COORD &&
+                      fabsf(y1) <= CROP_MAX_COORD);            // non-finite or too far out
+  const double sx = __ddiv_rn(__dsub_rn((double)x1, (double)x0), (double)d.out_w);
+  const double sy = __ddiv_rn(__dsub_rn((double)y1, (double)y0), (double)d.out_h);
+  const double M[6] = {sx, 0.0, __dadd_rn(__dsub_rn((double)x0, 0.5), __dmul_rn(0.5, sx)),
+                       0.0, sy, __dadd_rn(__dsub_rn((double)y0, 0.5), __dmul_rn(0.5, sy))};
+  const size_t total = (size_t)d.out_h * d.out_w;
+  const size_t p0 = (size_t)blockIdx.x * CROP_THREADS * CROP_PIX;
+  if (p0 >= total) return;
+  __shared__ __align__(16) unsigned char s_px[CROP_CTA_BYTES];
+  const ct_frame& f = s_f;
+  const unsigned char* src = d.buf + f.offset;
+  if (f.format == CT_FRAME_NV12) crop_pixels<CT_FRAME_NV12>(src, f, M, zero, d.out_w, total, p0, s_px);
+  else if (f.format == CT_FRAME_I420) crop_pixels<CT_FRAME_I420>(src, f, M, zero, d.out_w, total, p0, s_px);
+  else crop_pixels<CT_FRAME_BGR>(src, f, M, zero, d.out_w, total, p0, s_px);
+  __syncthreads();
+  const size_t nbytes = (total - p0 < (size_t)CROP_PIX * CROP_THREADS ? total - p0 : (size_t)CROP_PIX * CROP_THREADS) * 3;
+  unsigned char* dst = d.out + (((size_t)b * d.K + k) * total + p0) * 3;
+  if (aligned16(dst)) {                                     // p0 * 3 is a multiple of 16: aligned when the crop is
+    const int vec = (int)(nbytes >> 4);
+    for (int j = threadIdx.x; j < vec; j += CROP_THREADS)
+      reinterpret_cast<uint4*>(dst)[j] = reinterpret_cast<const uint4*>(s_px)[j];
+    for (int j = (vec << 4) + threadIdx.x; j < (int)nbytes; j += CROP_THREADS) dst[j] = s_px[j];
+  } else {
+    for (int j = threadIdx.x; j < (int)nbytes; j += CROP_THREADS) dst[j] = s_px[j];
+  }
+}
+
 }  // namespace ctb
 
 using namespace ctb;
@@ -1375,6 +1474,28 @@ extern "C" int ct_warp_frames_normalize(const uint8_t* src, const ct_frame* fram
   const DeviceFrames fs = {frames_dev, (long long)buf_bytes};
   warp_frames_norm_kernel<<<dim3((unsigned)nx, (unsigned)B), 256, 0, (cudaStream_t)stream>>>(
       src, fs, dst, out_h, out_w, make_float3(mean[0], mean[1], mean[2]), make_float3(std[0], std[1], std[2]));
+  return after_launch();
+}
+
+extern "C" int ct_crop_boxes(const ct_crop_desc* d, const int32_t* streams, int32_t n, int32_t n_streams,
+                             void* stream) {
+  CT_REQUIRE(d && d->buf && d->frames && d->rows && d->counts && d->out && d->out_counts, "null pointer");
+  CT_REQUIRE(n > 0 && n <= 65535 && n_streams > 0, "bad batch (0 < n <= 65535, n_streams > 0)");
+  CT_REQUIRE(d->K > 0 && d->K <= 65535 && d->out_h > 0 && d->out_w > 0, "bad shape (0 < K <= 65535, out_h, out_w > 0)");
+  CT_REQUIRE(d->rows_per_stream > 0 && d->counts_stride > 0 && d->buf_bytes >= 0,
+             "bad table (rows_per_stream > 0, counts_stride > 0, buf_bytes >= 0)");
+  CT_REQUIRE(d->row_floats >= CT_TRK_BBOX + 4 && d->active_col >= -1 && d->active_col < d->row_floats,
+             "row width does not contain the bbox or active column");
+  CT_REQUIRE(streams || n <= n_streams, "without a stream map every image needs a stream (n <= n_streams)");
+  const size_t total = (size_t)d->out_h * d->out_w;
+  const size_t per_cta = (size_t)CROP_THREADS * CROP_PIX;
+  CT_REQUIRE((total + per_cta - 1) / per_cta <= 0x7fffffffu, "crop too large");
+  CropArgs a = {};
+  a.d = *d;
+  a.streams = streams;
+  a.n_streams = n_streams;
+  const dim3 grid((unsigned)((total + per_cta - 1) / per_cta), (unsigned)d->K, (unsigned)n);
+  crop_boxes_kernel<<<grid, CROP_THREADS, 0, (cudaStream_t)stream>>>(a);
   return after_launch();
 }
 

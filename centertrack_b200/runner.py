@@ -82,6 +82,13 @@ its own out_thresh / pre_thresh / new_thresh (derived from its track_thresh as o
 per-stream kernels (ct_track_step_opts, ct_track_start_opts / _restore_opts, ct_post_process_opts), which read one
 ct_track_opts record per stream from the slot's device copy; a slot's records are uploaded with its frames when they
 changed, so the graphs are never recaptured.
+
+Crops (`crop_size=(out_h, out_w)`, frames runners with device_tracking or device_post_process): the last launch of each
+step, inside its graph, crops every active track (or kept detection) of every stream out of the frame slot the step
+read -- one ct_crop_boxes, cv2.warpAffine of each box stretched to out_h x out_w, with the warp's taps and so 4:2:0
+frames converted as cv2.cvtColor converts them -- into that slot's uint8 BGR crop buffer [B, K, out_h, out_w, 3].  The
+graphs have fixed pointers, so there is one crop buffer per input slot: a step's crops stay put until its slot is
+reused three steps later.  Only the crop counts [B] travel to the host, with the tables (fetch_crops).
 """
 import ctypes as C
 
@@ -234,6 +241,24 @@ def device_frame_source(x, fmt, layout, device, what='frame'):
   return (h, w), src
 
 
+def check_crop_size(crop_size, frames_mode, tables):
+  """crop_size of StreamRunner -> (out_h, out_w), or None when off.  ValueError for a size that is not two integers
+  >= 1, or a runner without frames (frame_sizes) or without a tracker or device post-processing (tables), whose boxes
+  and frames the crops come from."""
+  if crop_size is None:
+    return None
+  hw = tuple(crop_size) if isinstance(crop_size, (tuple, list)) else None
+  if hw is None or len(hw) != 2 or any(isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or v < 1
+                                       for v in hw):
+    raise ValueError('crop_size: expected (out_h, out_w), two integers >= 1, got %r' % (crop_size,))
+  if not frames_mode:
+    raise ValueError('crop_size: crops are cut from the camera frames; build the runner with frame_sizes (frames mode)')
+  if not tables:
+    raise ValueError('crop_size: crops are cut at the tracks or detections of the device tables; build the runner with '
+                     'device_tracking or device_post_process')
+  return int(hw[0]), int(hw[1])
+
+
 def _ints(streams):
   """The integer entries of a stream list, as a set (the others are refused by the list's own check)."""
   return {int(s) for s in streams if isinstance(s, (int, np.integer)) and not isinstance(s, (bool, np.bool_))}
@@ -267,10 +292,11 @@ class StreamRunner(object):
 
   frame_format = 'bgr'
   post = None                                                # device_post_process: DeviceDetections
+  crop = None                                                # crop_size: (out_h, out_w)
 
   def __init__(self, model, B, H, W, K=100, precision='bf16', device='cuda', use_graph=True, opt=None,
                device_tracking=False, max_public_dets=512, calibs=None, frame_sizes=None, max_frame_size=None,
-               idle_streams=None, frame_format='bgr', device_post_process=False, stream_opts=None):
+               idle_streams=None, frame_format='bgr', device_post_process=False, stream_opts=None, crop_size=None):
     """max_public_dets: with device_tracking and --public_det, the most public detections a stream may bring per
     frame (more raise ValueError; none is ever dropped).  calibs: with device_tracking on a 3D head set, one [3,4]
     camera matrix per stream (DeviceTracker's default otherwise; in frames mode Detector._get_default_calib of the
@@ -298,13 +324,18 @@ class StreamRunner(object):
     opt by device_tracker.resolve_options), out_thresh alone with device_post_process.  A stream changes them only at
     a video start (options= of step_host / step_frames / load_device_inputs) or with a restore.  The track table's
     rows come from the largest max_age among opt and these entries, and public detections are staged when opt or any
-    entry has public_det."""
+    entry has public_det.
+    crop_size (out_h, out_w): frames runners with device_tracking or device_post_process; each step also crops every
+    stream's active tracks (or kept detections) out of its frame on the device (fetch_crops, previous_crops).  None:
+    off, the launches and bytes of a runner without it."""
     if stream_opts is not None and not (device_tracking or device_post_process):
       raise ValueError('stream_opts: the per-stream settings act in the tracker or the device post-processing; build '
                        'the runner with device_tracking or device_post_process')
     if device_post_process and device_tracking:
       raise ValueError('device_post_process is for runners without a tracker: device_tracking already post-processes '
                        'the detections (fetch_results() gives its tracks)')
+    self.crop_size = check_crop_size(crop_size, frame_sizes is not None, device_tracking or device_post_process)
+    self.crop = None                                         # crop_size once the tables exist (_eager launches it)
     self.B, self.H, self.W, self.K = B, H, W, K
     self.device = torch.device(device)
     self.model = model
@@ -402,6 +433,12 @@ class StreamRunner(object):
         geo = dict(centers=[m['c'] for m in self._meta], scales=[m['s'] for m in self._meta])
       self.post = DeviceDetections(self.opt, B, K, self.rec.shape[2], self.layout, H, W, self.device, calibs=calibs,
                                    stream_opts=stream_opts, **geo)
+    if self.crop_size is not None:   # per input slot: the slot's graphs write its crops; the counts go to the host
+      self.crops = [torch.zeros((B, K) + self.crop_size + (3,), dtype=torch.uint8, device=self.device)
+                    for _ in range(NS)]
+      self.crop_counts = torch.zeros((B,), dtype=torch.int32, device=self.device)
+      self.h_crop_cnt = [torch.zeros((B,), dtype=torch.int32).pin_memory() for _ in range(2)]
+      self.crop = self.crop_size
     self.d_opts = None
     tables = self._geo_tables()
     if self._per_stream():                        # per slot: device ct_track_opts [B], pinned staging, host mirror
@@ -427,8 +464,9 @@ class StreamRunner(object):
     # launches of one step: the network plan + decode (+ memset-free: render + track step); frames mode: the pack op
     # becomes ct_pack_stem_frames_dev, or one ct_warp_frames_normalize comes before the plan.
     # --flip_test: + the merge, + the mirrors of the images and pre_hm unless the flip pack writes them;
-    # device_post_process: + ct_post_process
-    self.launches_per_step = self.eng.n_launches + 1 + (2 if device_tracking else 0) + (1 if self.post else 0)
+    # device_post_process: + ct_post_process; crop_size: + ct_crop_boxes
+    self.launches_per_step = self.eng.n_launches + 1 + (2 if device_tracking else 0) + (1 if self.post else 0) + \
+        (1 if self.crop else 0)
     if self.frames_mode:
       self.launches_per_step += 0 if self.eng.use_halo else 1
     if self.flip:
@@ -672,7 +710,26 @@ class StreamRunner(object):
         self.post.step(self.rec, opts=self._slot_opts(slot))
       else:
         self.post.step_mapped(self.rec[:n], self.d_map[slot][:self.B], opts=self._slot_opts(slot))
+    if self.crop is not None:                                # the boxes just written, cut from the frames just read
+      self._crop(slot)
     return res
+
+  def _crop(self, slot):
+    """ct_crop_boxes of this step's tables from u8[slot] through the slot's device descriptors into crops[slot], at the
+    step's batch (image i = stream d_map[slot][i] on an idle-streams runner), on the current stream."""
+    d = L.CropDesc()
+    d.buf, d.buf_bytes, d.frames = self.u8[slot].data_ptr(), self.slot_bytes, self.d_frames[slot].data_ptr()
+    if self.tracker is not None:                             # the active prefix of each stream's track rows
+      trk = self.tracker
+      d.rows, d.row_floats, d.rows_per_stream = trk.tracks.data_ptr(), L.CT_TRK_FLOATS, trk.T
+      d.counts, d.counts_stride, d.active_col = trk.counts.data_ptr(), 2, L.CT_TRK_ACTIVE
+    else:                                                    # each stream's kept detections
+      d.rows, d.row_floats, d.rows_per_stream = self.post.dets.data_ptr(), L.CT_DET_FLOATS, self.K
+      d.counts, d.counts_stride, d.active_col = self.post.counts.data_ptr(), 1, -1
+    d.K, d.out_h, d.out_w = self.K, self.crop[0], self.crop[1]
+    d.out, d.out_counts = self.crops[slot].data_ptr(), self.crop_counts.data_ptr()
+    streams = L.ptr(self.d_map[slot][:self.B]) if self.idle_g is not None else None
+    L.check(L.lib().ct_crop_boxes(C.byref(d), streams, self._n, self.B, L.stream_ptr()), 'ct_crop_boxes')
 
   def _slot_opts(self, slot):
     """The device ct_track_opts records slot's step reads (stream_opts runners), or None."""
@@ -1109,6 +1166,8 @@ class StreamRunner(object):
         self.h_det_cnt[self.t & 1].copy_(self.post.counts, non_blocking=True)
         if self.post.payload is not None:
           self.h_det_pay[self.t & 1].copy_(self.post.payload, non_blocking=True)
+      if self.crop is not None:
+        self.h_crop_cnt[self.t & 1].copy_(self.crop_counts, non_blocking=True)
       # this step's pre_images slot may be overwritten once this step is done
       self.ev_done[(slot - 1) % NS].record(self.compute)
     self.t += 1
@@ -1589,6 +1648,33 @@ class StreamRunner(object):
       raise ValueError('previous_results(): fewer than two steps submitted')
     return self._results(self.t - 2)
 
+  def fetch_crops(self):
+    """(crops, counts) of the last submitted step (crop_size runners); waits as fetch_results() does.  crops: the
+    device uint8 view [B, K, out_h, out_w, 3] of that step's crop buffer, BGR, crop k of stream b being the box of
+    fetch_results()[b][k]; counts: numpy int32 [B], 0 for a stream that was idle in that step.  Crops at or beyond
+    counts[b] are stale.  The view is not a copy: a step's crops stay unchanged until its input slot is reused, by the
+    step submitted three steps later, whose graph rewrites them: they stay valid while the next two steps are submitted,
+    and work the caller queues on its own stream that reads them must have finished before the third is."""
+    if self.crop is None:
+      raise ValueError('fetch_crops(): the runner was built without crop_size')
+    if self.t < 1:
+      raise ValueError('fetch_crops(): no step submitted')
+    self.compute.synchronize()
+    return self._crops_of(self.t - 1)
+
+  def previous_crops(self):
+    """After a step_frames call: fetch_crops() of the step before it, without a wait (as previous_results())."""
+    if self.crop is None:
+      raise ValueError('previous_crops(): the runner was built without crop_size')
+    if self.t < 2:
+      raise ValueError('previous_crops(): fewer than two steps submitted')
+    return self._crops_of(self.t - 2)
+
+  def _crops_of(self, t):
+    cnt = self.h_crop_cnt[t & 1].numpy().copy()
+    cnt[sorted(self._idle_of(t))] = 0
+    return self.crops[t % NS], cnt
+
   @property
   def h2d_bytes_per_step(self):
     """Bytes uploaded per step: the frames (and pre_hm / public detections); a step that starts videos with device
@@ -1606,7 +1692,7 @@ class StreamRunner(object):
   @property
   def d2h_bytes_per_step(self):
     tables = self._geo_tables()
-    return self.rec.numel() * 4 + (tables.d2h_bytes if tables is not None else 0)
+    return self.rec.numel() * 4 + (tables.d2h_bytes if tables is not None else 0) + (self.B * 4 if self.crop else 0)
 
   def views(self, rec_np):
     from .decode import views_from_records

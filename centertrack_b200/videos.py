@@ -45,16 +45,24 @@ def _as_video(v):
   return v if isinstance(v, Video) else Video(**v)
 
 
-def track_videos(runner, videos, layout='bgr'):
+def track_videos(runner, videos, layout='bgr', crops=False):
   """runner: a StreamRunner with device tracking, or with device_post_process (detection models: each frame's
   detections, and no video may bring pre_dets); videos: an iterable of Video (or dicts of its fields).  Yields
   (video id, frame index, results) for every frame of every video exactly once, as its tracks come back; results is the
   list of dicts fetch_results() gives for that stream (in source pixels in frames mode).  layout: step_frames' layout of
   device frames.  ValueError for a video whose frame size no stream can take, a video whose frames are of another kind
   (device tensors or arrays) than the first video's, or a runner with neither device tracking nor device
-  post-processing."""
+  post-processing.
+  crops=True (a runner built with crop_size): yields (video id, frame index, results, crops) instead, crops being that
+  stream's device uint8 view [n, out_h, out_w, 3] of the frame's crops (StreamRunner.fetch_crops), n being the number
+  of active tracks (the leading entries of results; every detection without a tracker) and crop k the box of
+  results[k].  A step's items come after the next step is submitted, and the step submitted three steps
+  later rewrites its crops: a view stays valid while the items of the next step are pulled, and becomes invalid when
+  the first item of the step after that is pulled.  Copy (or consume) a crop before then."""
   if runner.tracker is None and getattr(runner, 'post', None) is None:
     raise ValueError('track_videos: the runner needs device_tracking=True or device_post_process=True')
+  if crops and getattr(runner, 'crop', None) is None:
+    raise ValueError('track_videos: crops=True needs a runner built with crop_size')
   if layout != 'bgr' and not runner.frames_mode:
     raise ValueError('track_videos: layout=%r needs a frames-mode runner' % (layout,))
   B = runner.B
@@ -194,9 +202,10 @@ def track_videos(runner, videos, layout='bgr'):
       runner.step_host(torch.stack([torch.as_tensor(f, dtype=torch.float32).reshape(sizes[0]) for f in frames]), **kw)
     if fed is not None:
       res = runner.previous_results()
+      cut = runner.previous_crops() if crops else None
       for b, key in enumerate(fed):
         if key is not None:
-          yield key + (res[b],)
+          yield key + (res[b],) + ((cut[0][b, :cut[1][b]],) if crops else ())
     fed = now
     for b, p in enumerate(playing):   # advance; a finished video frees its stream for the next step
       if p is not None:
@@ -207,6 +216,7 @@ def track_videos(runner, videos, layout='bgr'):
           p.frame, p.index = nxt, p.index + 1
   if fed is not None:
     res = runner.fetch_results()
+    cut = runner.fetch_crops() if crops else None
     for b, key in enumerate(fed):
       if key is not None:
-        yield key + (res[b],)
+        yield key + (res[b],) + ((cut[0][b, :cut[1][b]],) if crops else ())

@@ -44,6 +44,9 @@
  *   ct_stage_frames            copies B decoder frames already in device memory (BGR / RGB / planar RGB, NV12, I420
  *                     planes at any pitch) into a frame slot in that slot's layout, so the kernels above read them as
  *                     uploaded frames.
+ *   ct_crop_boxes              crops every active track (or kept detection) of each stream out of its frame at a fixed
+ *                     size, cv2.warpAffine of the box (the frames kernels' taps): appearance, attribute or thumbnail
+ *                     inputs without a frame download.
  */
 #ifndef CTB200_H_
 #define CTB200_H_
@@ -557,6 +560,44 @@ typedef struct {
  * destination regions must not overlap each other or the sources. */
 int ct_stage_frames(const ct_frame_src* srcs, const ct_frame* dst, int32_t n, uint8_t* buf, int64_t buf_bytes,
                     void* stream);
+
+/* ---- crops of each stream's boxes from its frame ------------------------------------------------------------------
+ * Which rows: with a track table (active_col = CT_TRK_ACTIVE) the leading rows of stream b's first counts[b] rows
+ * whose active column is != 0 -- Tracker.step orders its rows matched, new, then coasting (active = 0), so these are
+ * the active tracks and crop k is the box of result k; with a detection table (active_col = -1) its first counts[b]
+ * rows.  Never more than K or rows_per_stream.
+ * The crop of box (x0, y0, x1, y1) (fp32 columns CT_TRK_BBOX.. of the row, widened to fp64) is
+ *   cv2.warpAffine(frame, M, (out_w, out_h), flags = INTER_LINEAR | WARP_INVERSE_MAP, BORDER_CONSTANT 0),
+ *   sx = (x1 - x0) / out_w,  sy = (y1 - y0) / out_h,  M = [sx, 0, (x0 - 0.5) + 0.5 sx, 0, sy, (y0 - 0.5) + 0.5 sy]
+ * each operation an fp64 rounding of its own, left to right: pixel centres map to pixel centres and the box is
+ * stretched to the crop (an inverted box gives the mirrored crop).  Of a 4:2:0 frame, the crop of its cv2.cvtColor BGR
+ * image.  A box with a non-finite coordinate or one of magnitude above 16384 px gives an all-zero crop (it still
+ * counts): within that bound cv2's int16 source map does not saturate. */
+typedef struct {
+  const uint8_t* buf;         /* the frames' buffer (a frame slot), buf_bytes long */
+  int64_t buf_bytes;
+  const ct_frame* frames;     /* DEVICE ct_frame [n]: image i's frame (minv is not read) */
+  const float* rows;          /* [n_streams, rows_per_stream, row_floats]: a track or detection table */
+  int32_t row_floats;         /* CT_TRK_FLOATS or CT_DET_FLOATS (>= CT_TRK_BBOX + 4, > active_col) */
+  int32_t rows_per_stream;
+  const int32_t* counts;      /* stream b's row count at counts[b * counts_stride]: track counts [B,2] (stride 2), or
+                                 detection counts [B] (stride 1) */
+  int32_t counts_stride;
+  int32_t active_col;         /* CT_TRK_ACTIVE, or -1: every counted row is cropped */
+  int32_t K;                  /* crops per stream */
+  int32_t out_h, out_w;       /* crop size */
+  uint8_t* out;               /* out uint8 BGR [n_streams, K, out_h, out_w, 3] */
+  int32_t* out_counts;        /* out int32 [n_streams]: the crops written for each stream */
+} ct_crop_desc;
+
+/* Crops of image i's stream b = i, or streams[i] when streams (device int32 [n]) is not NULL, written to out[b][0 ..
+ * out_counts[b]); an entry outside [0, n_streams) writes nothing.  Crops at or beyond out_counts[b], and streams no
+ * image maps to, are left untouched.  A frame descriptor that ct_pack_stem_frames_dev would read as invalid gives
+ * out_counts[b] = 0 and reads nothing.  One launch whose shape depends on n, K, out_h and out_w alone (CUDA-graph
+ * capturable).  CT_ERR_INVALID before any launch for a null pointer, n, K, out_h, out_w, n_streams, rows_per_stream or
+ * counts_stride <= 0, n or K above 65535, a row width that does not contain the bbox (or active) column, or
+ * n > n_streams without a map. */
+int ct_crop_boxes(const ct_crop_desc* d, const int32_t* streams, int32_t n, int32_t n_streams, void* stream);
 
 /* ---- misc --------------------------------------------------------------------------- */
 const char* ct_last_error(void);

@@ -139,6 +139,15 @@ class CropDesc(C.Structure):
               ('out_w', C.c_int32), ('out', C.c_void_p), ('out_counts', C.c_void_p)]
 
 
+CT_CROP_F32, CT_CROP_F16, CT_CROP_BF16 = 0, 1, 2
+CT_CROP_RGB, CT_CROP_BGR = 0, 1
+
+
+class CropTensor(C.Structure):
+  _fields_ = [('type', C.c_int32), ('order', C.c_int32), ('mean', C.c_float * 3), ('std', C.c_float * 3),
+              ('rows_cap', C.c_int64), ('out', C.c_void_p), ('out_offsets', C.c_void_p)]
+
+
 CT_FLIP_MAX_HEADS = 12
 
 
@@ -155,7 +164,8 @@ EXPORTS = ['ct_packed_weight_bytes', 'ct_pack_weights', 'ct_conv_forward', 'ct_c
            'ct_render_tracks', 'ct_track_step_mapped', 'ct_render_tracks_mapped', 'ct_post_process',
            'ct_track_step_opts', 'ct_track_start_opts', 'ct_track_restore_opts', 'ct_post_process_opts', 'ct_flip_merge', 'ct_flip_merge_heads', 'ct_mirror_x',
            'ct_warp_affine_normalize', 'ct_pack_stem_frames_dev', 'ct_pack_stem_frames_flip_dev',
-           'ct_warp_frames_normalize', 'ct_stage_frames', 'ct_crop_boxes', 'ct_last_error',
+           'ct_warp_frames_normalize', 'ct_stage_frames', 'ct_crop_boxes', 'ct_crop_boxes_tensor',
+           'ct_last_error',
            'ct_abi_version', 'ct_launch_count', 'ct_reset_launch_count', 'ct_debug_trace', 'ct_debug_watch']
 
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17', '-Xcompiler', '-fPIC']
@@ -259,6 +269,8 @@ def lib():
       [C.c_int32] * 2 + [C.c_void_p]
   L.ct_stage_frames.argtypes = [C.POINTER(FrameSrc), C.POINTER(Frame), C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]
   L.ct_crop_boxes.argtypes = [C.POINTER(CropDesc), C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
+  L.ct_crop_boxes_tensor.argtypes = [C.POINTER(CropDesc), C.POINTER(CropTensor), C.c_void_p, C.c_int32, C.c_int32,
+                                     C.c_void_p]
   L.ct_launch_count.restype = C.c_int64
   L.ct_reset_launch_count.restype = None
   L.ct_debug_trace.argtypes = [C.c_void_p]

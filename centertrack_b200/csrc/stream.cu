@@ -24,9 +24,13 @@
 //                    latter two with cv2.cvtColor(COLOR_YUV2BGR_NV12 / _I420) applied to each bilinear tap
 //   ct_stage_frames  B frames already in device memory (a GPU decoder's) copied into a frame slot in its layout
 //   ct_crop_boxes    each stream's active tracks (or kept detections) cropped out of its frame slot: cv2.warpAffine
-//                    of the box stretched to a fixed crop size, the frames kernels' bilinear taps
+//                    of the box stretched to a fixed crop size, the frames kernels' bilinear taps;
+//                    ct_crop_boxes_tensor the same crops as one packed, normalised fp32 / fp16 / bf16 NCHW batch
 // All HBM-bound byte/index work: one pass over the data, coalesced, no tensor cores.
+#include <cuda_fp16.h>
 #include <math_constants.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -1097,7 +1101,26 @@ struct CropArgs {
   ct_crop_desc d;
   const int* streams;      // NULL = identity
   int n_streams;
+  ct_crop_tensor t;        // ct_crop_boxes_tensor's output (the tensor forms)
 };
+
+// Output forms of crop_boxes_kernel: ct_crop_boxes' uint8 BGR crops, or ct_crop_boxes_tensor's packed NCHW rows of
+// one ct_crop_type.
+constexpr int CROP_U8 = -1;
+
+// Which rows of stream b image i's crops come from, shared by both entry points: the first counts[b] rows, clamped to
+// [0, min(K, rows_per_stream)], none for an invalid frame (nothing is read); with a track table, cut at the first of
+// them whose active column is 0 (crop_row_inactive).
+__device__ __forceinline__ int crop_row_limit(const ct_crop_desc& d, const ct_frame& f, int b) {
+  const int n = d.counts[(size_t)b * d.counts_stride];
+  return frame_in_buffer(f, d.buf_bytes) ? max(0, min(n, min(d.K, d.rows_per_stream))) : 0;
+}
+__device__ __forceinline__ const float* crop_rows(const ct_crop_desc& d, int b) {
+  return d.rows + (size_t)b * d.rows_per_stream * d.row_floats;
+}
+__device__ __forceinline__ bool crop_row_inactive(const ct_crop_desc& d, const float* rows, int r) {
+  return rows[(size_t)r * d.row_floats + d.active_col] == 0.f;
+}
 
 // The CTA's pixels [p0, p0 + CROP_PIX * CROP_THREADS) of the crop -> s_px (3 bytes each); zero = the box failed the
 // guard (an all-zero crop).
@@ -1119,6 +1142,69 @@ __device__ __forceinline__ void crop_pixels(const unsigned char* __restrict__ sr
   }
 }
 
+// The CTA's npx staged pixels s_px -> the uint8 BGR crop at dst (crop pixel p0).
+__device__ __forceinline__ void crop_store_u8(const unsigned char* s_px, unsigned char* dst, int npx) {
+  const int nbytes = 3 * npx;
+  if (aligned16(dst)) {                                     // p0 * 3 is a multiple of 16: aligned when the crop is
+    const int vec = nbytes >> 4;
+    for (int j = threadIdx.x; j < vec; j += CROP_THREADS)
+      reinterpret_cast<uint4*>(dst)[j] = reinterpret_cast<const uint4*>(s_px)[j];
+    for (int j = (vec << 4) + threadIdx.x; j < nbytes; j += CROP_THREADS) dst[j] = s_px[j];
+  } else {
+    for (int j = threadIdx.x; j < nbytes; j += CROP_THREADS) dst[j] = s_px[j];
+  }
+}
+
+// The element bits of value v in the output type TYPE (round to nearest even), in the low bits of a word.
+template <int TYPE>
+__device__ __forceinline__ uint32_t crop_elem_bits(float v) {
+  if constexpr (TYPE == CT_CROP_F32) return __float_as_uint(v);
+  else if constexpr (TYPE == CT_CROP_F16) return __half_as_ushort(__float2half_rn(v));
+  else return __bfloat16_as_ushort(__float2bfloat16_rn(v));
+}
+
+// The CTA's npx staged pixels s_px -> row's three channel planes (row: out + row index * 3 * total elements), from
+// crop pixel p0.  Element (c, byte u) = ((float)u / 255 - mean[c]) / std[c], each operation an fp32 rounding of its
+// own, then rounded into TYPE: a table of the 3 x 256 values per CTA, so the pixels cost one shared load each.  Each
+// plane's run is stored as 16-byte vectors from its first 16-byte boundary on, the elements around them one by one.
+template <int TYPE>
+__device__ __forceinline__ void crop_store_tensor(const ct_crop_tensor& t, const unsigned char* s_px, void* row,
+                                                  size_t total, size_t p0, int npx) {
+  using T = typename std::conditional<TYPE == CT_CROP_F32, uint32_t, uint16_t>::type;
+  constexpr int V = 16 / (int)sizeof(T);
+  __shared__ uint32_t s_lut[3][256];
+  for (int j = threadIdx.x; j < 3 * 256; j += CROP_THREADS) {
+    const int c = j >> 8;
+    s_lut[c][j & 255] = crop_elem_bits<TYPE>(__fdiv_rn(__fsub_rn(__fdiv_rn((float)(j & 255), 255.f), t.mean[c]), t.std[c]));
+  }
+  __syncthreads();
+#pragma unroll 1
+  for (int c = 0; c < 3; ++c) {
+    const int sc = t.order == CT_CROP_RGB ? 2 - c : c;    // the staged pixels are BGR
+    const uint32_t* lut = s_lut[c];
+    const unsigned char* px = s_px + sc;
+    T* dst = reinterpret_cast<T*>(row) + (size_t)c * total + p0;
+    const int head = min(npx, (int)(((16 - ((uintptr_t)dst & 15)) & 15) / sizeof(T)));
+    const int vec = (npx - head) / V;
+    for (int j = threadIdx.x; j < head; j += CROP_THREADS) dst[j] = (T)lut[px[3 * j]];
+    for (int j = threadIdx.x; j < vec; j += CROP_THREADS) {
+      const int q = head + j * V;
+      uint32_t w[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        if constexpr (V == 4) w[e] = lut[px[3 * (q + e)]];
+        else w[e] = lut[px[3 * (q + 2 * e)]] | (lut[px[3 * (q + 2 * e + 1)]] << 16);
+      }
+      *reinterpret_cast<uint4*>(dst + q) = make_uint4(w[0], w[1], w[2], w[3]);
+    }
+    for (int j = head + vec * V + threadIdx.x; j < npx; j += CROP_THREADS) dst[j] = (T)lut[px[3 * j]];
+  }
+}
+
+// FORM CROP_U8 (ct_crop_boxes): crop k of stream b -> out[b][k], its count -> out_counts[b] (the row selection here).
+// FORM a ct_crop_type (ct_crop_boxes_tensor): the stream's rows and count come from t.out_offsets, which
+// crop_offsets_kernel wrote with the same row selection just before; crop k -> row out_offsets[b] + k of t.out.
+template <int FORM>
 __global__ void __launch_bounds__(CROP_THREADS) crop_boxes_kernel(const __grid_constant__ CropArgs a) {
   const ct_crop_desc& d = a.d;
   const int i = blockIdx.z, k = blockIdx.y;
@@ -1126,25 +1212,33 @@ __global__ void __launch_bounds__(CROP_THREADS) crop_boxes_kernel(const __grid_c
   if (b < 0 || b >= a.n_streams) return;                    // a padding image, or no stream: nothing is written
   __shared__ ct_frame s_f;
   __shared__ int s_cnt, s_first;
-  const int RF = d.row_floats;
-  const float* rows = d.rows + (size_t)b * d.rows_per_stream * RF;
-  if (threadIdx.x == 0) {
-    s_f = d.frames[i];
-    int n = d.counts[(size_t)b * d.counts_stride];
-    n = max(0, min(n, min(d.K, d.rows_per_stream)));
-    s_cnt = s_first = frame_in_buffer(s_f, d.buf_bytes) ? n : 0;   // an invalid frame: no crop, nothing read
-  }
-  __syncthreads();
-  int n = s_cnt;
-  if (d.active_col >= 0) {                                  // track tables: the leading active rows
-    for (int r = threadIdx.x; r < n; r += CROP_THREADS)
-      if (rows[(size_t)r * RF + d.active_col] == 0.f) atomicMin(&s_first, r);
+  const float* rows = crop_rows(d, b);
+  int n;
+  if constexpr (FORM == CROP_U8) {
+    if (threadIdx.x == 0) {
+      s_f = d.frames[i];
+      s_cnt = s_first = crop_row_limit(d, s_f, b);          // an invalid frame: no crop, nothing read
+    }
     __syncthreads();
-    n = s_first;
+    n = s_cnt;
+    if (d.active_col >= 0) {                                // track tables: the leading active rows
+      for (int r = threadIdx.x; r < n; r += CROP_THREADS)
+        if (crop_row_inactive(d, rows, r)) atomicMin(&s_first, r);
+      __syncthreads();
+      n = s_first;
+    }
+    if (blockIdx.x == 0 && k == 0 && threadIdx.x == 0) d.out_counts[b] = n;
+  } else {
+    if (threadIdx.x == 0) {
+      s_f = d.frames[i];
+      s_first = a.t.out_offsets[b];
+      s_cnt = a.t.out_offsets[b + 1] - s_first;
+    }
+    __syncthreads();
+    n = s_cnt;
   }
-  if (blockIdx.x == 0 && k == 0 && threadIdx.x == 0) d.out_counts[b] = n;
   if (k >= n) return;
-  const float* bx = rows + (size_t)k * RF + CT_TRK_BBOX;
+  const float* bx = rows + (size_t)k * d.row_floats + CT_TRK_BBOX;
   const float x0 = bx[0], y0 = bx[1], x1 = bx[2], y1 = bx[3];
   const bool zero = !(fabsf(x0) <= CROP_MAX_COORD && fabsf(y0) <= CROP_MAX_COORD && fabsf(x1) <= CROP_MAX_COORD &&
                       fabsf(y1) <= CROP_MAX_COORD);            // non-finite or too far out
@@ -1162,15 +1256,70 @@ __global__ void __launch_bounds__(CROP_THREADS) crop_boxes_kernel(const __grid_c
   else if (f.format == CT_FRAME_I420) crop_pixels<CT_FRAME_I420>(src, f, M, zero, d.out_w, total, p0, s_px);
   else crop_pixels<CT_FRAME_BGR>(src, f, M, zero, d.out_w, total, p0, s_px);
   __syncthreads();
-  const size_t nbytes = (total - p0 < (size_t)CROP_PIX * CROP_THREADS ? total - p0 : (size_t)CROP_PIX * CROP_THREADS) * 3;
-  unsigned char* dst = d.out + (((size_t)b * d.K + k) * total + p0) * 3;
-  if (aligned16(dst)) {                                     // p0 * 3 is a multiple of 16: aligned when the crop is
-    const int vec = (int)(nbytes >> 4);
-    for (int j = threadIdx.x; j < vec; j += CROP_THREADS)
-      reinterpret_cast<uint4*>(dst)[j] = reinterpret_cast<const uint4*>(s_px)[j];
-    for (int j = (vec << 4) + threadIdx.x; j < (int)nbytes; j += CROP_THREADS) dst[j] = s_px[j];
+  const int npx = (int)(total - p0 < (size_t)CROP_PIX * CROP_THREADS ? total - p0 : (size_t)CROP_PIX * CROP_THREADS);
+  if constexpr (FORM == CROP_U8) {
+    crop_store_u8(s_px, d.out + (((size_t)b * d.K + k) * total + p0) * 3, npx);
   } else {
-    for (int j = threadIdx.x; j < (int)nbytes; j += CROP_THREADS) dst[j] = s_px[j];
+    const size_t row = (size_t)s_first + k;
+    char* out = static_cast<char*>(a.t.out) + row * 3 * total * (FORM == CT_CROP_F32 ? 4 : 2);
+    crop_store_tensor<FORM>(a.t, s_px, out, total, p0, npx);
+  }
+}
+
+// ct_crop_boxes_tensor's row offsets, one CTA: stream b's crop count (crop_row_limit, cut at the first inactive row by
+// one warp's ballots) -> out_counts[b], then the exclusive prefix over streams 0 .. n_streams -> t.out_offsets (a
+// stream no image maps to counts 0).  Images sharing a stream are not supported (as in ct_crop_boxes).
+constexpr int CROP_OFF_THREADS = 1024;
+
+__global__ void __launch_bounds__(CROP_OFF_THREADS) crop_offsets_kernel(const __grid_constant__ CropArgs a, int n) {
+  const ct_crop_desc& d = a.d;
+  int* off = a.t.out_offsets;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int b = threadIdx.x; b <= a.n_streams; b += CROP_OFF_THREADS) off[b] = 0;
+  __syncthreads();
+  for (int i = warp; i < n; i += CROP_OFF_THREADS / 32) {   // one warp per image; every branch is warp-uniform
+    const int b = a.streams ? a.streams[i] : i;
+    if (b < 0 || b >= a.n_streams) continue;
+    int cnt = crop_row_limit(d, d.frames[i], b);
+    if (d.active_col >= 0) {
+      const float* rows = crop_rows(d, b);
+      for (int r0 = 0; r0 < cnt; r0 += 32) {
+        const unsigned m = __ballot_sync(0xffffffffu, r0 + lane < cnt && crop_row_inactive(d, rows, r0 + lane));
+        if (m) {
+          cnt = r0 + __ffs(m) - 1;
+          break;
+        }
+      }
+    }
+    if (lane == 0) off[b] = d.out_counts[b] = cnt;
+  }
+  __syncthreads();
+  __shared__ int s_warp[CROP_OFF_THREADS / 32];
+  int carry = 0;
+  for (int b0 = 0; b0 <= a.n_streams; b0 += CROP_OFF_THREADS) {
+    const int b = b0 + threadIdx.x;
+    const int v = b <= a.n_streams ? off[b] : 0;
+    int x = v;                                              // inclusive scan: lanes, then warps
+#pragma unroll
+    for (int s = 1; s < 32; s <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, x, s);
+      if (lane >= s) x += y;
+    }
+    if (lane == 31) s_warp[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+      int w = s_warp[lane];
+#pragma unroll
+      for (int s = 1; s < 32; s <<= 1) {
+        const int y = __shfl_up_sync(0xffffffffu, w, s);
+        if (lane >= s) w += y;
+      }
+      s_warp[lane] = w;
+    }
+    __syncthreads();
+    if (b <= a.n_streams) off[b] = carry + (warp ? s_warp[warp - 1] : 0) + x - v;
+    carry += s_warp[CROP_OFF_THREADS / 32 - 1];
+    __syncthreads();
   }
 }
 
@@ -1477,9 +1626,9 @@ extern "C" int ct_warp_frames_normalize(const uint8_t* src, const ct_frame* fram
   return after_launch();
 }
 
-extern "C" int ct_crop_boxes(const ct_crop_desc* d, const int32_t* streams, int32_t n, int32_t n_streams,
-                             void* stream) {
-  CT_REQUIRE(d && d->buf && d->frames && d->rows && d->counts && d->out && d->out_counts, "null pointer");
+// What ct_crop_boxes and ct_crop_boxes_tensor both refuse (the uint8 out is ct_crop_boxes' alone).
+static int crop_desc_ok(const ct_crop_desc* d, const int32_t* streams, int32_t n, int32_t n_streams, bool u8_out) {
+  CT_REQUIRE(d && d->buf && d->frames && d->rows && d->counts && (d->out || !u8_out) && d->out_counts, "null pointer");
   CT_REQUIRE(n > 0 && n <= 65535 && n_streams > 0, "bad batch (0 < n <= 65535, n_streams > 0)");
   CT_REQUIRE(d->K > 0 && d->K <= 65535 && d->out_h > 0 && d->out_w > 0, "bad shape (0 < K <= 65535, out_h, out_w > 0)");
   CT_REQUIRE(d->rows_per_stream > 0 && d->counts_stride > 0 && d->buf_bytes >= 0,
@@ -1490,12 +1639,49 @@ extern "C" int ct_crop_boxes(const ct_crop_desc* d, const int32_t* streams, int3
   const size_t total = (size_t)d->out_h * d->out_w;
   const size_t per_cta = (size_t)CROP_THREADS * CROP_PIX;
   CT_REQUIRE((total + per_cta - 1) / per_cta <= 0x7fffffffu, "crop too large");
+  return CT_OK;
+}
+
+static dim3 crop_grid(const ct_crop_desc* d, int32_t n) {
+  const size_t total = (size_t)d->out_h * d->out_w;
+  const size_t per_cta = (size_t)CROP_THREADS * CROP_PIX;
+  return dim3((unsigned)((total + per_cta - 1) / per_cta), (unsigned)d->K, (unsigned)n);
+}
+
+extern "C" int ct_crop_boxes(const ct_crop_desc* d, const int32_t* streams, int32_t n, int32_t n_streams,
+                             void* stream) {
+  if (const int e = crop_desc_ok(d, streams, n, n_streams, true)) return e;
   CropArgs a = {};
   a.d = *d;
   a.streams = streams;
   a.n_streams = n_streams;
-  const dim3 grid((unsigned)((total + per_cta - 1) / per_cta), (unsigned)d->K, (unsigned)n);
-  crop_boxes_kernel<<<grid, CROP_THREADS, 0, (cudaStream_t)stream>>>(a);
+  crop_boxes_kernel<CROP_U8><<<crop_grid(d, n), CROP_THREADS, 0, (cudaStream_t)stream>>>(a);
+  return after_launch();
+}
+
+extern "C" int ct_crop_boxes_tensor(const ct_crop_desc* d, const ct_crop_tensor* t, const int32_t* streams, int32_t n,
+                                    int32_t n_streams, void* stream) {
+  if (const int e = crop_desc_ok(d, streams, n, n_streams, false)) return e;
+  CT_REQUIRE(t && t->out && t->out_offsets, "null pointer");
+  CT_REQUIRE(t->type == CT_CROP_F32 || t->type == CT_CROP_F16 || t->type == CT_CROP_BF16, "unknown element type");
+  CT_REQUIRE(t->order == CT_CROP_RGB || t->order == CT_CROP_BGR, "unknown channel order");
+  for (int c = 0; c < 3; ++c)
+    CT_REQUIRE(isfinite(t->mean[c]) && isfinite(t->std[c]) && t->std[c] != 0.f, "mean and std must be finite, std != 0");
+  const int64_t rows = (int64_t)n * d->K;
+  CT_REQUIRE(rows <= 0x7fffffff, "n * K above 2^31 - 1 (int32 offsets)");
+  CT_REQUIRE(t->rows_cap >= rows, "rows_cap < n * K");
+  CT_REQUIRE(((uintptr_t)t->out & (t->type == CT_CROP_F32 ? 3 : 1)) == 0, "out not aligned to its element size");
+  CropArgs a = {};
+  a.d = *d;
+  a.streams = streams;
+  a.n_streams = n_streams;
+  a.t = *t;
+  crop_offsets_kernel<<<1, CROP_OFF_THREADS, 0, (cudaStream_t)stream>>>(a, n);
+  if (const int e = after_launch()) return e;
+  const dim3 grid = crop_grid(d, n);
+  if (t->type == CT_CROP_F32) crop_boxes_kernel<CT_CROP_F32><<<grid, CROP_THREADS, 0, (cudaStream_t)stream>>>(a);
+  else if (t->type == CT_CROP_F16) crop_boxes_kernel<CT_CROP_F16><<<grid, CROP_THREADS, 0, (cudaStream_t)stream>>>(a);
+  else crop_boxes_kernel<CT_CROP_BF16><<<grid, CROP_THREADS, 0, (cudaStream_t)stream>>>(a);
   return after_launch();
 }
 

@@ -89,6 +89,11 @@ read -- one ct_crop_boxes, cv2.warpAffine of each box stretched to out_h x out_w
 frames converted as cv2.cvtColor converts them -- into that slot's uint8 BGR crop buffer [B, K, out_h, out_w, 3].  The
 graphs have fixed pointers, so there is one crop buffer per input slot: a step's crops stay put until its slot is
 reused three steps later.  Only the crop counts [B] travel to the host, with the tables (fetch_crops).
+With crop_format as well, the crops are written instead as the batch an embedding or classifier network reads: one
+ct_crop_boxes_tensor (an offsets pass, then the crop pass) packs every stream's crops, stream after stream, into that
+slot's [B * K, 3, out_h, out_w] tensor of the format's dtype, channel order and Normalize(mean, std), beside the slot's
+row offsets [B + 1]; the uint8 buffers are not allocated.  In fp16 at B = 32, K = 100 and 256 x 128 crops a slot's batch
+is 629 MB (1.9 GB for the three slots).
 """
 import ctypes as C
 
@@ -259,6 +264,43 @@ def check_crop_size(crop_size, frames_mode, tables):
   return int(hw[0]), int(hw[1])
 
 
+CROP_DTYPES = {torch.float32: L.CT_CROP_F32, torch.float16: L.CT_CROP_F16, torch.bfloat16: L.CT_CROP_BF16}
+CROP_ORDERS = {'rgb': L.CT_CROP_RGB, 'bgr': L.CT_CROP_BGR}
+
+
+def check_crop_format(crop_format, crop_size):
+  """crop_format of StreamRunner -> {'dtype', 'channels', 'mean', 'std'} with mean and std as fp32 tuples, or None when
+  off.  ValueError without crop_size, for a value that is not a dict of exactly these keys, a dtype other than
+  torch.float16 / bfloat16 / float32, channels other than 'rgb' / 'bgr', or a mean or std that is not three real
+  numbers finite in fp32, or a std with an entry that is 0 in fp32 (torchvision's Normalize refuses it too)."""
+  if crop_format is None:
+    return None
+  if crop_size is None:
+    raise ValueError('crop_format: it describes the crops of crop_size; build the runner with crop_size too')
+  keys = ('dtype', 'channels', 'mean', 'std')
+  if not isinstance(crop_format, dict) or sorted(crop_format) != sorted(keys):
+    raise ValueError('crop_format: expected a dict of exactly %s, got %r' % (', '.join(keys), crop_format))
+  if not any(crop_format['dtype'] is t for t in CROP_DTYPES):
+    raise ValueError('crop_format: dtype must be torch.float16, torch.bfloat16 or torch.float32, got %r' %
+                     (crop_format['dtype'],))
+  if not isinstance(crop_format['channels'], str) or crop_format['channels'] not in CROP_ORDERS:
+    raise ValueError("crop_format: channels must be 'rgb' or 'bgr', got %r" % (crop_format['channels'],))
+  out = dict(dtype=crop_format['dtype'], channels=crop_format['channels'])
+  for key in ('mean', 'std'):
+    v = crop_format[key]
+    v = tuple(v) if isinstance(v, (tuple, list, np.ndarray)) else None
+    if v is None or len(v) != 3 or any(isinstance(x, (bool, np.bool_)) or not isinstance(x, (int, float, np.integer,
+                                                                                             np.floating)) for x in v):
+      raise ValueError('crop_format: %s must be three real numbers, got %r' % (key, crop_format[key]))
+    with np.errstate(over='ignore'):
+      f32 = tuple(np.float32(x) for x in v)
+    if not all(np.isfinite(f32)) or (key == 'std' and any(x == 0 for x in f32)):
+      raise ValueError('crop_format: %s must be finite in fp32%s, got %r' % (key, ' and != 0' if key == 'std' else '',
+                                                                            crop_format[key]))
+    out[key] = tuple(float(x) for x in f32)
+  return out
+
+
 def _ints(streams):
   """The integer entries of a stream list, as a set (the others are refused by the list's own check)."""
   return {int(s) for s in streams if isinstance(s, (int, np.integer)) and not isinstance(s, (bool, np.bool_))}
@@ -293,10 +335,12 @@ class StreamRunner(object):
   frame_format = 'bgr'
   post = None                                                # device_post_process: DeviceDetections
   crop = None                                                # crop_size: (out_h, out_w)
+  crop_format = None                                         # crop_format: check_crop_format's dict
 
   def __init__(self, model, B, H, W, K=100, precision='bf16', device='cuda', use_graph=True, opt=None,
                device_tracking=False, max_public_dets=512, calibs=None, frame_sizes=None, max_frame_size=None,
-               idle_streams=None, frame_format='bgr', device_post_process=False, stream_opts=None, crop_size=None):
+               idle_streams=None, frame_format='bgr', device_post_process=False, stream_opts=None, crop_size=None,
+               crop_format=None):
     """max_public_dets: with device_tracking and --public_det, the most public detections a stream may bring per
     frame (more raise ValueError; none is ever dropped).  calibs: with device_tracking on a 3D head set, one [3,4]
     camera matrix per stream (DeviceTracker's default otherwise; in frames mode Detector._get_default_calib of the
@@ -327,7 +371,11 @@ class StreamRunner(object):
     entry has public_det.
     crop_size (out_h, out_w): frames runners with device_tracking or device_post_process; each step also crops every
     stream's active tracks (or kept detections) out of its frame on the device (fetch_crops, previous_crops).  None:
-    off, the launches and bytes of a runner without it."""
+    off, the launches and bytes of a runner without it.
+    crop_format (with crop_size): {'dtype': torch.float16 | torch.bfloat16 | torch.float32, 'channels': 'rgb' | 'bgr',
+    'mean': (m0, m1, m2), 'std': (s0, s1, s2)}, mean and std in output-channel order; the crops come as one packed
+    batch of that dtype, torchvision's Normalize(mean, std)(ToTensor()(crop)).to(dtype) of each crop in that channel
+    order (fetch_crops).  None: the uint8 BGR crops."""
     if stream_opts is not None and not (device_tracking or device_post_process):
       raise ValueError('stream_opts: the per-stream settings act in the tracker or the device post-processing; build '
                        'the runner with device_tracking or device_post_process')
@@ -335,6 +383,7 @@ class StreamRunner(object):
       raise ValueError('device_post_process is for runners without a tracker: device_tracking already post-processes '
                        'the detections (fetch_results() gives its tracks)')
     self.crop_size = check_crop_size(crop_size, frame_sizes is not None, device_tracking or device_post_process)
+    self.crop_format = check_crop_format(crop_format, crop_size)
     self.crop = None                                         # crop_size once the tables exist (_eager launches it)
     self.B, self.H, self.W, self.K = B, H, W, K
     self.device = torch.device(device)
@@ -434,8 +483,13 @@ class StreamRunner(object):
       self.post = DeviceDetections(self.opt, B, K, self.rec.shape[2], self.layout, H, W, self.device, calibs=calibs,
                                    stream_opts=stream_opts, **geo)
     if self.crop_size is not None:   # per input slot: the slot's graphs write its crops; the counts go to the host
-      self.crops = [torch.zeros((B, K) + self.crop_size + (3,), dtype=torch.uint8, device=self.device)
-                    for _ in range(NS)]
+      if self.crop_format is None:
+        self.crops = [torch.zeros((B, K) + self.crop_size + (3,), dtype=torch.uint8, device=self.device)
+                      for _ in range(NS)]
+      else:                          # the packed batch [B * K rows] and its row offsets [B + 1]
+        self.crops = [torch.zeros((B * K, 3) + self.crop_size, dtype=self.crop_format['dtype'], device=self.device)
+                      for _ in range(NS)]
+        self.crop_offsets = [torch.zeros((B + 1,), dtype=torch.int32, device=self.device) for _ in range(NS)]
       self.crop_counts = torch.zeros((B,), dtype=torch.int32, device=self.device)
       self.h_crop_cnt = [torch.zeros((B,), dtype=torch.int32).pin_memory() for _ in range(2)]
       self.crop = self.crop_size
@@ -464,9 +518,9 @@ class StreamRunner(object):
     # launches of one step: the network plan + decode (+ memset-free: render + track step); frames mode: the pack op
     # becomes ct_pack_stem_frames_dev, or one ct_warp_frames_normalize comes before the plan.
     # --flip_test: + the merge, + the mirrors of the images and pre_hm unless the flip pack writes them;
-    # device_post_process: + ct_post_process; crop_size: + ct_crop_boxes
+    # device_post_process: + ct_post_process; crop_size: + ct_crop_boxes, or with crop_format ct_crop_boxes_tensor's two
     self.launches_per_step = self.eng.n_launches + 1 + (2 if device_tracking else 0) + (1 if self.post else 0) + \
-        (1 if self.crop else 0)
+        ((2 if self.crop_format else 1) if self.crop else 0)
     if self.frames_mode:
       self.launches_per_step += 0 if self.eng.use_halo else 1
     if self.flip:
@@ -715,8 +769,9 @@ class StreamRunner(object):
     return res
 
   def _crop(self, slot):
-    """ct_crop_boxes of this step's tables from u8[slot] through the slot's device descriptors into crops[slot], at the
-    step's batch (image i = stream d_map[slot][i] on an idle-streams runner), on the current stream."""
+    """ct_crop_boxes (ct_crop_boxes_tensor with crop_format, its offsets into crop_offsets[slot]) of this step's tables
+    from u8[slot] through the slot's device descriptors into crops[slot], at the step's batch (image i = stream
+    d_map[slot][i] on an idle-streams runner), on the current stream."""
     d = L.CropDesc()
     d.buf, d.buf_bytes, d.frames = self.u8[slot].data_ptr(), self.slot_bytes, self.d_frames[slot].data_ptr()
     if self.tracker is not None:                             # the active prefix of each stream's track rows
@@ -727,9 +782,19 @@ class StreamRunner(object):
       d.rows, d.row_floats, d.rows_per_stream = self.post.dets.data_ptr(), L.CT_DET_FLOATS, self.K
       d.counts, d.counts_stride, d.active_col = self.post.counts.data_ptr(), 1, -1
     d.K, d.out_h, d.out_w = self.K, self.crop[0], self.crop[1]
-    d.out, d.out_counts = self.crops[slot].data_ptr(), self.crop_counts.data_ptr()
+    d.out_counts = self.crop_counts.data_ptr()
     streams = L.ptr(self.d_map[slot][:self.B]) if self.idle_g is not None else None
-    L.check(L.lib().ct_crop_boxes(C.byref(d), streams, self._n, self.B, L.stream_ptr()), 'ct_crop_boxes')
+    if self.crop_format is None:
+      d.out = self.crops[slot].data_ptr()
+      L.check(L.lib().ct_crop_boxes(C.byref(d), streams, self._n, self.B, L.stream_ptr()), 'ct_crop_boxes')
+      return
+    fmt, t = self.crop_format, L.CropTensor()
+    t.type, t.order = CROP_DTYPES[fmt['dtype']], CROP_ORDERS[fmt['channels']]
+    t.mean[:], t.std[:] = fmt['mean'], fmt['std']
+    t.rows_cap, t.out, t.out_offsets = self.crops[slot].shape[0], self.crops[slot].data_ptr(), \
+        self.crop_offsets[slot].data_ptr()
+    L.check(L.lib().ct_crop_boxes_tensor(C.byref(d), C.byref(t), streams, self._n, self.B, L.stream_ptr()),
+            'ct_crop_boxes_tensor')
 
   def _slot_opts(self, slot):
     """The device ct_track_opts records slot's step reads (stream_opts runners), or None."""
@@ -1654,7 +1719,10 @@ class StreamRunner(object):
     fetch_results()[b][k]; counts: numpy int32 [B], 0 for a stream that was idle in that step.  Crops at or beyond
     counts[b] are stale.  The view is not a copy: a step's crops stay unchanged until its input slot is reused, by the
     step submitted three steps later, whose graph rewrites them: they stay valid while the next two steps are submitted,
-    and work the caller queues on its own stream that reads them must have finished before the third is."""
+    and work the caller queues on its own stream that reads them must have finished before the third is.
+    With crop_format: (batch, counts), batch being the device view [N, 3, out_h, out_w] of that step's packed batch in
+    the format's dtype, N = counts.sum(): stream b's crops are batch[counts[:b].sum():counts[:b + 1].sum()], in the
+    order above.  The same lifetime."""
     if self.crop is None:
       raise ValueError('fetch_crops(): the runner was built without crop_size')
     if self.t < 1:
@@ -1673,6 +1741,8 @@ class StreamRunner(object):
   def _crops_of(self, t):
     cnt = self.h_crop_cnt[t & 1].numpy().copy()
     cnt[sorted(self._idle_of(t))] = 0
+    if self.crop_format is not None:                         # the idle streams have no rows in the batch
+      return self.crops[t % NS][:int(cnt.sum())], cnt
     return self.crops[t % NS], cnt
 
   @property

@@ -45,6 +45,15 @@ def _as_video(v):
   return v if isinstance(v, Video) else Video(**v)
 
 
+def _stream_crops(runner, cut, b):
+  """Stream b's crops of fetch_crops()' (crops, counts): its rows of the packed batch with crop_format."""
+  crops, counts = cut
+  if getattr(runner, 'crop_format', None) is not None:
+    start = int(counts[:b].sum())
+    return crops[start:start + int(counts[b])]
+  return crops[b, :counts[b]]
+
+
 def track_videos(runner, videos, layout='bgr', crops=False):
   """runner: a StreamRunner with device tracking, or with device_post_process (detection models: each frame's
   detections, and no video may bring pre_dets); videos: an iterable of Video (or dicts of its fields).  Yields
@@ -58,9 +67,14 @@ def track_videos(runner, videos, layout='bgr', crops=False):
   of active tracks (the leading entries of results; every detection without a tracker) and crop k the box of
   results[k].  A step's items come after the next step is submitted, and the step submitted three steps
   later rewrites its crops: a view stays valid while the items of the next step are pulled, and becomes invalid when
-  the first item of the step after that is pulled.  Copy (or consume) a crop before then."""
+  the first item of the step after that is pulled.  Copy (or consume) a crop before then.  With the runner's
+  crop_format, crops is instead that stream's slice [n, 3, out_h, out_w] of the step's packed batch, with the same
+  lifetime.  ValueError for crops other than True or False (the batch's format is the runner's crop_format)."""
   if runner.tracker is None and getattr(runner, 'post', None) is None:
     raise ValueError('track_videos: the runner needs device_tracking=True or device_post_process=True')
+  if crops not in (True, False):
+    raise ValueError('track_videos: crops must be True or False, got %r (build the runner with crop_format for a '
+                     'normalised batch)' % (crops,))
   if crops and getattr(runner, 'crop', None) is None:
     raise ValueError('track_videos: crops=True needs a runner built with crop_size')
   if layout != 'bgr' and not runner.frames_mode:
@@ -205,7 +219,7 @@ def track_videos(runner, videos, layout='bgr', crops=False):
       cut = runner.previous_crops() if crops else None
       for b, key in enumerate(fed):
         if key is not None:
-          yield key + (res[b],) + ((cut[0][b, :cut[1][b]],) if crops else ())
+          yield key + (res[b],) + ((_stream_crops(runner, cut, b),) if crops else ())
     fed = now
     for b, p in enumerate(playing):   # advance; a finished video frees its stream for the next step
       if p is not None:
@@ -219,4 +233,4 @@ def track_videos(runner, videos, layout='bgr', crops=False):
     cut = runner.fetch_crops() if crops else None
     for b, key in enumerate(fed):
       if key is not None:
-        yield key + (res[b],) + ((cut[0][b, :cut[1][b]],) if crops else ())
+        yield key + (res[b],) + ((_stream_crops(runner, cut, b),) if crops else ())

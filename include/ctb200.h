@@ -46,7 +46,8 @@
  *                     uploaded frames.
  *   ct_crop_boxes              crops every active track (or kept detection) of each stream out of its frame at a fixed
  *                     size, cv2.warpAffine of the box (the frames kernels' taps): appearance, attribute or thumbnail
- *                     inputs without a frame download.
+ *                     inputs without a frame download; ct_crop_boxes_tensor writes them as one packed, normalised
+ *                     fp32 / fp16 / bf16 NCHW batch.
  */
 #ifndef CTB200_H_
 #define CTB200_H_
@@ -598,6 +599,34 @@ typedef struct {
  * counts_stride <= 0, n or K above 65535, a row width that does not contain the bbox (or active) column, or
  * n > n_streams without a map. */
 int ct_crop_boxes(const ct_crop_desc* d, const int32_t* streams, int32_t n, int32_t n_streams, void* stream);
+
+/* The same crops as one packed batch an embedding or classifier network reads: element (c, y, x) of a crop is
+ *   ((float)u8 / 255 - mean[c]) / std[c],  u8 the crop's byte of output channel c (RGB or BGR order),
+ * each operation an IEEE fp32 rounding of its own, then rounded to nearest even into the element type: torchvision's
+ * Normalize(mean, std)(ToTensor()(crop)).to(dtype) on the CPU. */
+typedef enum { CT_CROP_F32 = 0, CT_CROP_F16 = 1, CT_CROP_BF16 = 2 } ct_crop_type;
+typedef enum { CT_CROP_RGB = 0, CT_CROP_BGR = 1 } ct_crop_order;
+
+typedef struct {
+  int32_t type;               /* ct_crop_type */
+  int32_t order;              /* ct_crop_order */
+  float mean[3];              /* per output channel */
+  float std[3];               /* per output channel: finite, != 0 */
+  int64_t rows_cap;           /* rows of out (>= n * K) */
+  void* out;                  /* out [rows_cap, 3, out_h, out_w] of type, NCHW */
+  int32_t* out_offsets;       /* out int32 [n_streams + 1]: stream b's crops are rows [out_offsets[b], out_offsets[b + 1]) */
+} ct_crop_tensor;
+
+/* ct_crop_boxes' crops (same rows, map, zero guard, frame formats and invalid descriptors) packed into t->out: stream
+ * b's crops are rows out_offsets[b] .. out_offsets[b] + out_counts[b], in result order, streams in ascending order;
+ * a stream no image maps to contributes no rows (its out_counts entry is left untouched); out_offsets[n_streams] = N,
+ * the number of rows, and rows at or beyond N are not written.  d->out is not read (may be NULL).  Each stream at most
+ * once in streams.  Two launches, a one-CTA offsets pass and the crop pass, whose shapes depend on n, K, out_h and
+ * out_w alone (CUDA-graph capturable).  CT_ERR_INVALID before any launch for whatever ct_crop_boxes refuses, a null t,
+ * out or out_offsets, an unknown type or order, a non-finite mean or std or a std equal to 0, n * K above 2^31 - 1,
+ * rows_cap < n * K, or an out not aligned to its element size. */
+int ct_crop_boxes_tensor(const ct_crop_desc* d, const ct_crop_tensor* t, const int32_t* streams, int32_t n,
+                         int32_t n_streams, void* stream);
 
 /* ---- misc --------------------------------------------------------------------------- */
 const char* ct_last_error(void);
